@@ -2,11 +2,12 @@
 """Headline benchmark: BA observations/sec + descriptor-pairs/sec (BASELINE.json metric).
 
     python bench.py --gpus N --steps K --warmup W            # this engine (one rank per GPU)
+    python bench.py --gpus 1 --steps K --dump-outputs DIR    # + the last timed step's results as DIR/<name>.npy
     python bench.py --impl reference --gpus N ...            # the reference's CPU path, host cores
 
 Workload (config.workload): the synthetic cube scene of BASELINE.json configs[3],
 500 cameras / 200k points / 2M observations (exactly 10 observations per point), which fits
-one B200 and is the configuration the north-star target is quoted on.  One *step* is
+one H100 (80 GB) and is the configuration the north-star target is quoted on.  One *step* is
 
   BA     one full `bundle()` of that scene: Levenberg-Marquardt to convergence (SoftLOneLoss,
          cameras optimised, <= 100 iterations) from the seed-43 perturbed start;
@@ -69,10 +70,12 @@ def peaks():
         d = json.load(open(p))
         return dict(hbm=d["hbm_gbs"], bf16=d["bf16_tflops"], bf16_sustained=d.get("bf16_tflops_sustained", d["bf16_tflops"]),
                     source="measured (MEASURED_PEAKS.json)")
-    return dict(hbm=6650.0, bf16=1590.0, bf16_sustained=1400.0, source="fallback (B200_PROFILING.md)")
+    # NVIDIA H100 SXM data sheet (dense, 700 W card); a card with a lower power limit reaches less
+    return dict(hbm=3350.0, bf16=989.0, bf16_sustained=989.0, source="H100 SXM data sheet")
 
 
-FP64_TENSOR_PEAK_TFLOPS = 37.2   # scripts/bench_dmma.cu on this pool's B200 (DMMA = DFMA = 64 FMA/clk/SM); not in MEASURED_PEAKS
+FP64_TENSOR_PEAK_TFLOPS = 67.0   # H100 SXM data sheet, FP64 tensor core (dense)
+FP8_TENSOR_PEAK_TFLOPS = 1979.0  # H100 SXM data sheet, FP8 tensor core (dense)
 POPC_PER_CLK_PER_SM = 16.0       # CUDA programming guide, arithmetic-instruction throughput table (population count)
 
 
@@ -106,7 +109,7 @@ def config_of(w, pb, pairs, feats, world):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons during the timed region (read-only queries)."""
 
     Q = ("clocks.sm,clocks.max.sm,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -369,7 +372,7 @@ def run_extras(pk, clocks_mhz, with_cpu):
                      "(epipolar threshold 0.006), symmetric" % (n_img, n_desc, len(pairs)),
          "value": work / (tot * 1e-3), "unit": "descriptor-pairs/s", "device_ms": tot, "distance_kernel_ms": ker,
          "mask_and_finalize_ms": tot - ker, "matches": int(sum(len(v) for v in res["m"].values())),
-         "kernel": "bf_top2_tc<masked> + epi_mask_bits" if pm.last_kernel() == 2 else "bf_top2_f32_cv",
+         "kernel": "bf_top2_wg<L2, masked> + epi_mask_bits" if pm.last_kernel() == 2 else "bf_top2_f32_cv",
          "e2e": {"value": work / e2e_s, "unit": "descriptor-pairs/s",
                  "h2d_bytes_per_step": int(n_img * n_desc * (128 + 12)), "d2h_bytes_per_step": int(4 * n_desc * len(pairs))},
          "roofline": {"bound": "tensor", "achieved": 2.0 * 128 * work / (ker * 1e-3) / 1e12, "peak": pk["bf16_sustained"],
@@ -390,7 +393,8 @@ def run_extras(pk, clocks_mhz, with_cpu):
     n_img, n_desc = 8, 8000
     pairs8 = [(i, j) for i in range(n_img) for j in range(i + 1, n_img)][:16]
     work8 = 2 * len(pairs8) * n_desc * n_desc
-    sm_clock = (clocks_mhz or 1965.0) * 1e6
+    sm_clock = (clocks_mhz or torch.cuda.get_device_properties(0).clock_rate / 1e3) * 1e6
+    n_sms = torch.cuda.get_device_properties(0).multi_processor_count
 
     def simt(name, make, extra):
         pm = matching.PairMatcher()
@@ -404,8 +408,8 @@ def run_extras(pk, clocks_mhz, with_cpu):
         tot, ker = timed(pm, go)
         rec = {"workload": "%d images x %d descriptors, %d symmetric pairs" % (n_img, n_desc, len(pairs8)),
                "value": work8 / (tot * 1e-3), "unit": "descriptor-pairs/s", "distance_kernel_ms": ker,
-               "kernel": {1: "bf_top2_simt<u8>" if name != "float" else "bf_top2_f32_cv", 2: "bf_top2_tc",
-                          3: "bf_top2_tc_h8"}[pm.last_kernel()]}
+               "kernel": {1: "bf_top2_simt<u8>" if name != "float" else "bf_top2_f32_cv", 2: "bf_top2_wg<L2>",
+                          3: "bf_top2_wg<Hamming>"}[pm.last_kernel()]}
         rec.update(extra(ker, pm.last_kernel()))
         if with_cpu:
             f = [make(i) for i in range(n_img)]
@@ -417,24 +421,23 @@ def run_extras(pk, clocks_mhz, with_cpu):
     def popc_roof(words):
         def f(ker, kid):
             if kid == 3:
-                # +-1 fp8 contraction, K padded to 512 per descriptor pair; no measured fp8 figure in
-                # MEASURED_PEAKS.json -> the nominal dense fp8 peak (4.5 PFLOP/s), said so in the note
+                # +-1 fp8 contraction, K padded to 512 per descriptor pair, against the data-sheet dense fp8 peak
                 ach = 2.0 * 512 * work8 / (ker * 1e-3) / 1e12
-                return {"roofline": {"bound": "tensor", "achieved": ach, "peak": 4500.0, "unit": "TFLOP/s", "frac": ach / 4500.0,
-                                     "note": "fp8 (E4M3 +-1) tcgen05 kind::f8f6f4, K = 512 per pair (%d useful bits); peak = "
-                                             "nominal dense fp8; the epilogue (top-2 over 128x128 accumulators), not "
-                                             "the tensor pipe, bounds this kernel" % (words * 32)}}
+                return {"roofline": {"bound": "tensor", "achieved": ach, "peak": FP8_TENSOR_PEAK_TFLOPS, "unit": "TFLOP/s",
+                                     "frac": ach / FP8_TENSOR_PEAK_TFLOPS,
+                                     "note": "fp8 (E4M3 +-1) wgmma m64n128k32, K = 512 per pair (%d useful bits); peak = "
+                                             "H100 SXM data sheet dense fp8" % (words * 32)}}
             ach = work8 * words / (ker * 1e-3)
-            peak = 148 * POPC_PER_CLK_PER_SM * sm_clock
+            peak = n_sms * POPC_PER_CLK_PER_SM * sm_clock
             return {"roofline": {"bound": "alu-popc", "achieved": ach / 1e12, "peak": peak / 1e12, "unit": "Tpopc/s",
                                  "frac": ach / peak,
-                                 "note": "%d 32-bit XOR+POPC per descriptor pair; peak = 148 SMs x 16 POPC/clk x SM clock "
-                                         "(CUDA programming guide throughput table)" % words}}
+                                 "note": "%d 32-bit XOR+POPC per descriptor pair; peak = %d SMs x 16 POPC/clk x SM clock "
+                                         "(CUDA programming guide throughput table)" % (words, n_sms)}}
         return f
 
     def fp32_roof(ker, kid):
         ach = work8 * 128 * 3 / (ker * 1e-3)   # sub, mul, add per element: cv2's order forbids FMA
-        peak = 148 * 128 * sm_clock
+        peak = n_sms * 128 * sm_clock
         return {"roofline": {"bound": "alu-fp32", "achieved": ach / 1e12, "peak": peak / 1e12, "unit": "Tinst/s",
                              "frac": ach / peak, "note": "3 fp32 instructions per element (no FMA: bit-exact cv2 order)"}}
 
@@ -469,6 +472,39 @@ def run_extras(pk, clocks_mhz, with_cpu):
 # --------------------------------------------------------------------------------------
 # GPU arm
 # --------------------------------------------------------------------------------------
+DUMP_REPROJ_ROWS = 1 << 19   # seeded sample of the per-observation reprojection errors (12 MB as float64)
+DUMP_MATCH_PAIRS = 256       # seeded sample of image pairs whose full match lists are written
+
+
+def dump_outputs(out_dir, res, pairs, matches):
+    """What the timed path returned in its last step, as float64 .npy files (about 25 MB for c4): the BA solution
+    (cameras, rig instances, points, a fixed seeded sample of the reprojection errors) and the symmetric match
+    lists (the match count of every pair, and the (query, train) rows of a fixed seeded sample of pairs).
+    The samples depend only on the workload's sizes, so two builds are compared element for element."""
+    os.makedirs(out_dir, exist_ok=True)
+
+    def save(name, a):
+        np.save(os.path.join(out_dir, name + ".npy"), np.ascontiguousarray(a, dtype=np.float64))
+
+    save("ba_cam_params", res["cam_params"])
+    save("ba_rig_instances", res["inst"])
+    save("ba_points", res["points"])
+    rep = res["reprojection_errors"]
+    rows = np.arange(len(rep))
+    if len(rep) > DUMP_REPROJ_ROWS:
+        rows = np.sort(np.random.RandomState(0).choice(len(rep), DUMP_REPROJ_ROWS, replace=False))
+    save("ba_reprojection_errors_rows", rows)
+    save("ba_reprojection_errors", rep[rows])
+    save("ba_summary_costs", [res["summary"]["initial_cost"], res["summary"]["final_cost"], res["summary"]["iterations"]])
+    save("match_counts", [len(matches[p]) for p in pairs])
+    sel = np.arange(len(pairs))
+    if len(pairs) > DUMP_MATCH_PAIRS:
+        sel = np.sort(np.random.RandomState(1).choice(len(pairs), DUMP_MATCH_PAIRS, replace=False))
+    rows = [np.column_stack([np.full(len(matches[pairs[k]]), k), matches[pairs[k]]]) for k in sel]
+    save("match_sample_pairs", np.asarray([pairs[k] for k in sel]).reshape(-1, 2))
+    save("match_sample_rows", np.concatenate(rows) if rows else np.zeros((0, 3)))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -478,7 +514,11 @@ def main():
     ap.add_argument("--workload", default="c4", choices=sorted(WORKLOADS))
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-extras", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step computed (BA solution, match lists) as DIR/<name>.npy")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     args.warmup = max(args.warmup, 0)
 
     rank = int(os.environ.get("RANK", "0"))
@@ -569,6 +609,7 @@ def main():
     t_begin = time.perf_counter()
     ba_dev_ms, ba_wall, ba_run_s, ba_iters, ba_sum = 0.0, 0.0, 0.0, 0, None
     mt_dev_ms, mt_kernel_ms, mt_wall = 0.0, 0.0, 0.0
+    last_matches = None
     for _ in range(args.steps):
         res, dt = ba_step()
         s = res["summary"]
@@ -580,7 +621,7 @@ def main():
         tot, ker = match_resident()
         mt_dev_ms += tot
         mt_kernel_ms += ker
-        dte, _ = match_e2e()
+        dte, last_matches = match_e2e()
         mt_wall += dte
     barrier()
     t_total = time.perf_counter() - t_begin
@@ -618,22 +659,10 @@ def main():
         kern["ba_linearize"] = dict(bytes=per_launch, ms=dur * 1e3, share=s["time_linearize_ms"] / s["time_device_ms"])
     kern["pcg"] = dict(ms=s["time_pcg_ms"], share=s["time_pcg_ms"] / s["time_device_ms"],
                        iterations=s["pcg_iterations"], reduced_dim=s["reduced_dim"])
-    # DRAM traffic per launch from the committed `ncu --set full` capture of this command (scripts/extract_traffic.py)
-    traffic = {}
-    for tname in ("r02_traffic.json", "r01_traffic.json"):
-        tpath = os.path.join(ROOT, "profiles", tname)
-        if os.path.exists(tpath):
-            traffic = json.load(open(tpath))
-            break
-
-    def dram(*names):
-        vals = [traffic[n]["dram_bytes_per_launch"] for n in names if n in traffic]
-        return float(sum(vals)) if vals else None
-
     if "ba_schur" in kern:
         # the Schur phase: its arithmetic intensity (~ 22 flop/B against the planes) is above the fp64 machine
-        # balance (37.2 TFLOP/s / 6.57 TB/s = 5.7 flop/B): the fp64 tensor pipe is its roofline, the HBM figure
-        # is reported next to it
+        # balance (67 TFLOP/s / 3.35 TB/s = 20 flop/B on the H100 SXM data sheet): the fp64 tensor pipe is its
+        # roofline, the HBM figure is reported next to it
         npts = len(pb.points) // world
         kk = nloc / max(npts, 1)
         wc_ = s["jac_planes"] / 2.0 - 4.0  # jac_planes = nres * (wc + 4), nres = 2
@@ -644,18 +673,20 @@ def main():
         kern["ba_schur"]["fp64_peak_tflops"] = FP64_TENSOR_PEAK_TFLOPS
         kern["ba_schur"]["fp64_frac"] = tf / FP64_TENSOR_PEAK_TFLOPS
         kern["ba_schur"]["fp64_note"] = ("2*3*(k*wc)^2 flop per point, k = observations per point, wc = camera-side width "
-                                         "(full square); peak = DMMA/DFMA rate measured by scripts/bench_dmma.cu")
+                                         "(full square); peak = H100 SXM data sheet fp64 tensor core")
     dom = max((k for k in kern if "bytes" in kern[k]), key=lambda k: kern[k]["share"])
     ach = kern[dom]["bytes"] / (kern[dom]["ms"] * 1e-3) / 1e9
-    dom_traffic = dram("ba_point_blocks", "ba_schur_pipe<9, 0>", "ba_schur_pipe<0, 0>", "ba_schur_mma<9>", "ba_schur_mma<0>", "ba_schur") if dom == "ba_schur" else dram("ba_linearize<1, 5, 0>") or dram("ba_linearize<1, 3>") or dram("ba_linearize<1>")
     roofline = {"kernel": dom, "bound": "hbm", "achieved": ach, "peak": pk["hbm"], "unit": "GB/s",
-                "frac": ach / pk["hbm"], "traffic": dom_traffic, "peak_source": pk["source"], "kernels": kern}
+                "frac": ach / pk["hbm"], "peak_source": pk["source"], "kernels": kern}
     flops = 2.0 * 128.0 * my_pair_work * K
     tc_ach = flops / (mt_kernel_ms * 1e-3) / 1e12
-    mt_roof = {"kernel": "bf_top2_tc" if pm.last_kernel() == 2 else "bf_top2_f32_cv", "bound": "tensor",
+    mt_roof = {"kernel": "bf_top2_wg<L2>" if pm.last_kernel() == 2 else "bf_top2_f32_cv", "bound": "tensor",
                "achieved": tc_ach, "peak": pk["bf16_sustained"], "unit": "TFLOP/s", "frac": tc_ach / pk["bf16_sustained"],
-               "traffic": dram("bf_top2_tc<0>") or dram("bf_top2_tc", "bf_top2_tc<false>"), "peak_source": pk["source"] + ", sustained bf16",
+               "peak_source": pk["source"] + ", bf16 dense",
                "note": "2*128 flop per descriptor pair per direction (SURVEY 8d); kernel time = distance kernel only"}
+
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, res, pairs if world == 1 else my_pairs, last_matches)
 
     line = None
     if rank == 0:

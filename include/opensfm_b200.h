@@ -1,4 +1,4 @@
-/* opensfm_b200 — C ABI of the B200-native hot paths of OpenSfM.
+/* opensfm_b200 — C ABI of the H100-native hot paths of OpenSfM.
  *
  * Plain C, plain pointers and sizes; no torch / pybind types.  Every entry
  * point returns 0 on success and a non-zero code on failure; the message of
@@ -12,7 +12,7 @@
  *           opensfm/src/bundle/src/bundle_adjuster.cc) behind pybundle /
  *          sfm::BAHelpers (opensfm/src/sfm/src/ba_helpers.cc:117,408,581).
  *
- * There is no CPU fallback: every call needs a CUDA device (sm_100a).
+ * There is no CPU fallback: every call needs a CUDA device (H100, sm_90a).
  */
 #ifndef OPENSFM_B200_H_
 #define OPENSFM_B200_H_
@@ -100,10 +100,10 @@ int osfm_matcher_fetch_pairs(osfm_matcher* m, int64_t* offsets_out, int32_t* pai
                              int64_t* total_rows);
 /* Milliseconds spent on the device by the last batch (CUDA events on the matcher's stream). */
 int osfm_matcher_last_device_ms(osfm_matcher* m, float* ms_total, float* ms_distance_kernel);
-/* 0 = pick automatically, 1 = force the exact SIMT kernel, 2 = force the tcgen05 kernel
+/* 0 = pick automatically, 1 = force the exact SIMT kernel, 2 = force the tensor-core (wgmma) kernel
  * (fails at match time if the descriptors are not exactly representable). */
 int osfm_matcher_set_kernel(osfm_matcher* m, int which);
-/* Which distance kernel the last batch used: 1 = SIMT, 2 = tcgen05 (L2), 3 = tcgen05 fp8 (Hamming). */
+/* Which distance kernel the last batch used: 1 = SIMT, 2 = tensor cores bf16 (L2), 3 = tensor cores fp8 (Hamming). */
 int osfm_matcher_last_kernel(osfm_matcher* m);
 /* Device memory held by the matcher's descriptor slabs (bytes reserved / bytes in use by live sets). */
 int osfm_matcher_device_bytes(osfm_matcher* m, int64_t* reserved, int64_t* in_use);

@@ -1,6 +1,6 @@
-"""Builds the CUDA library in-tree for sm_100a (nvcc cross-compiles without a GPU).
+"""Builds the CUDA library in-tree for H100 (sm_90a); nvcc cross-compiles without a GPU.
 
-Output: opensfm_b200/lib/libopensfm_b200.so (git-ignored, travels to the GPU box).
+Output: opensfm_b200/lib/libopensfm_b200.so (git-ignored build product).
 """
 from __future__ import annotations
 
@@ -14,7 +14,8 @@ CSRC = os.path.join(HERE, "csrc")
 LIBDIR = os.path.join(HERE, "lib")
 LIB = os.path.join(LIBDIR, "libopensfm_b200.so")
 SOURCES = ["core.cu", "match.cu", "match_tc.cu", "words.cu", "ba.cu"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
+NVCC_FLAGS = ARCH + [ "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "-ccbin", "/usr/bin/g++"]
 
 
@@ -51,8 +52,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
 
     with ThreadPoolExecutor(max_workers=len(SOURCES)) as ex:
         objs = list(ex.map(compile_one, SOURCES))
-    cmd = [nvcc, "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_100a,code=sm_100a", "-ccbin", "/usr/bin/g++",
-                                                "-cudart", "static", "-ldl"]
+    cmd = [nvcc, "-shared", "-o", LIB] + objs + ARCH + ["-ccbin", "/usr/bin/g++", "-cudart", "static", "-ldl"]
     subprocess.check_call(cmd)
     return LIB
 

@@ -1,4 +1,4 @@
-// Bundle adjustment on B200 (sm_100a): Levenberg-Marquardt with Schur
+// Bundle adjustment on H100 (sm_90a): Levenberg-Marquardt with Schur
 // elimination of the points and PCG on the reduced camera system, all in fp64.
 //
 // Replaces bundle::BundleAdjuster::Run (opensfm/src/bundle/src/bundle_adjuster.cc:595-1121)
@@ -1006,7 +1006,7 @@ struct BA {
   PcgPipe pcg_pipe{};
   bool pcg_pipe_ok = false;
   int pcg_pipe_smem = 0, pcg_pipe_its = 0, pcg_fallbacks = 0;
-  int num_sms = 148;
+  int num_sms = 132;
   DevBuf<int> d_pr_cam_param, d_pr_cam_col, d_pr_cam_log, d_pr_pos_inst, d_pr_pos_axis, d_pr_pos_col;
   DevBuf<double> d_pr_cam_prior, d_pr_cam_scale, d_pr_pos_prior, d_pr_pos_scale;
   DevBuf<Scalars> d_sc;
@@ -1209,8 +1209,8 @@ void BA::run() {
   // ---- order the observations on the device (ba_order.cuh): shard points over ranks
   //      (p % world == rank), sort by (point, shot), put points seen by exactly the same shots next to
   //      each other (segments of the fast Schur path) ----
-  // The segmented Schur path (ba_point_blocks + ba_obs_rows + ba_schur_seg) is the default: 3.6 ms vs 5.3 ms
-  // per launch for the per-point kernel on the 2M-observation scene (profiles/README.md).
+  // The segmented Schur path (ba_point_blocks + ba_obs_rows + ba_schur_seg) is the default: points seen by the same
+  // shots share their camera-side rows, which the per-point kernel re-reads point by point.
   // OSFM_BA_SEGMENT_SCHUR=0 forces every point through ba_schur (kept for A/B runs and tests).
   static const bool use_seg = []() { const char* e = getenv("OSFM_BA_SEGMENT_SCHUR"); return !(e && e[0] == '0'); }();
   // register budget of ba_linearize<1> (A/B switch): 3, 4 or 5 resident CTAs per SM
@@ -1800,8 +1800,8 @@ void BA::run() {
         pcg_pipe.off_vec = (int)off_vec; pcg_pipe.off_cols = (int)off_cols; pcg_pipe.off_rows = (int)off_rows;
         pcg_pipe.max_rows = rows_max; pcg_pipe.max_groups = grp_max; pcg_pipe.max_cols = (int)col_max;
         pcg_pipe.off_defl = (int)off_defl; pcg_pipe.Wdef = nullptr;
-        // 128-bit barrier words (value + generation in one strong 16-byte access): measured SLOWER than flags + slots
-        // on B200 (PCG 8.69 vs 8.05 ms at C4), so it is opt-in: OSFM_BA_PCG_B128=1
+        // 128-bit barrier words (value + generation in one strong 16-byte access): measured slower than flags + slots
+        // on the previous target GPU and not re-measured on H100, so it stays opt-in: OSFM_BA_PCG_B128=1
         static const bool allow_b128 = []() { const char* e = getenv("OSFM_BA_PCG_B128"); return e && e[0] == '1'; }();
         pcg_pipe.b128 = (allow_b128 && pcg_grid <= PCG_B128_GROUP && PCG_THREADS >= 3 * PCG_B128_GROUP) ? 1 : 0;
         OSFM_CUDA(cudaFuncSetAttribute(pcg_pipelined, cudaFuncAttributeMaxDynamicSharedMemorySize, pcg_pipe_smem));

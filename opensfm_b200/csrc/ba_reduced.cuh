@@ -10,7 +10,7 @@
 //      with atomics and all-reduced — then the mirrored lower blocks,
 //   4. block-row lists (CSR over blocks, both triangles) are emitted for the PCG mat-vec.
 // For the 500-camera / 2M-observation scene this is ~16 MB instead of a 162 MB dense matrix, i.e.
-// the Schur atomics and every PCG mat-vec hit the 126 MB L2 instead of HBM.
+// the Schur atomics and every PCG mat-vec hit the 50 MB L2 of an H100 instead of HBM.
 //
 // Included by ba.cu only (shares BAView / Scalars / block_reduce_sum).
 #pragma once
@@ -438,7 +438,7 @@ __global__ void __launch_bounds__(SCHUR_THREADS)
 //   B   ba_schur_seg    : one CTA per segment: streams the contiguous rows of its points into shared
 //                         memory, accumulates in registers, flushes
 // Splitting the irregular gathers (A) from the dense accumulation (B) is what makes B short: earlier
-// single-kernel versions were latency-bound at 2 CTAs/SM (profiles/README.md).
+// single-kernel versions were latency-bound at 2 CTAs/SM.
 // Eligible: k <= 16, k * wc <= SEG_NA, wc <= 16; everything else goes through ba_schur.
 // ---------------------------------------------------------------------------
 constexpr int SEG_NA = 96;                 // max camera-side columns of a segment (k * wc)
@@ -858,7 +858,7 @@ __global__ void __launch_bounds__(SM_THREADS, 2)
   }
   // every (row < 3 np, column < ncols) entry of the operand buffers is rewritten by each chunk; only the padding
   // columns [ncols, SM_LD) the 8-wide tiles can touch have to read as zero (zeroing all 57 KB cost 5k clocks per
-  // segment, profiles/README.md)
+  // segment)
   {
     const int padc = SM_LD - ncols;
     for (int t = tid; t < 3 * SM_KC * padc; t += SM_THREADS) {
@@ -1225,8 +1225,8 @@ struct PcgState {
   double slot[2][PCG_MAX_CTAS][4];
   // wide payload of the deflated solver: 3 dot products + PCG_ND projections (double-buffered by generation parity)
   double slotx[2][PCG_MAX_CTAS][12];
-  // per-CTA arrival generation, one 128-byte line each (packed flags cost 9.3k clk per barrier,
-  // strided ones 4.4k: scripts/bench_barrier.cu)
+  // per-CTA arrival generation, one 128-byte line each (packed flags contend for one line on
+  // every arrival; one line per CTA does not)
   unsigned flags[PCG_MAX_CTAS * PCG_FLAG_STRIDE];
   // 128-bit barrier words (value, generation), double-buffered by generation parity: [parity][CTA][3 sums + pad]
   PcgWord words[2][PCG_MAX_CTAS][4];

@@ -21,8 +21,8 @@
 //     The destinations depend only on the structure, so sp_flush_tables writes them once per run(): one int per
 //     (segment, warp, tile slot, fragment element, lane) = (offset << 2 | add-U flag | double flag) or -1
 //     (20 KB per segment, 430 MB at C4).  A warp prefetches its 3.3 KB with cp.async at the start of a segment.
-//     (scripts/bench_atomics.cu: scattered fp64 RED into L2 runs at 194 G/s = 0.67 / clk / SM on this GPU, 583 G/s
-//     when a warp hits 32 consecutive elements; the 87M RED of a C4 launch need 0.45 ms at the scattered rate.)
+//     (scattered fp64 RED into L2 are several times slower than a warp's RED to 32 consecutive elements, and a C4
+//     launch issues 87M of them.)
 // Eligible: nres * (wc + 4) <= SP_ROWS plane rows per observation (2-D residuals with wc <= 9); everything else
 // keeps ba_schur_mma.  OSFM_BA_SCHUR_PIPE=0 switches back for A/B runs.
 #pragma once

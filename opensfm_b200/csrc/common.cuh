@@ -1,4 +1,4 @@
-// Shared host/device helpers for the opensfm_b200 CUDA library (sm_100a only).
+// Shared host/device helpers for the opensfm_b200 CUDA library (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 

@@ -1,4 +1,4 @@
-// Brute-force descriptor matching on B200 (sm_100a).
+// Brute-force descriptor matching on H100 (sm_90a).
 //
 // Replaces the OpenCV call under opensfm/matching.py:723-777
 // (`cv2.DescriptorMatcher.knnMatch(k=2)` + Lowe ratio test) for float32 L2
@@ -17,7 +17,7 @@
 //  bf_top2_simt<U8>   exact SIMT tile kernel (any float32 values, masks, Hamming)
 //  bf_top2_finalize   merge train chunks per query + ratio test
 //  bf_symmetric       keep (i,j) iff j's match is i (matching.py:775-777)
-// The tcgen05 tensor-core distance kernel lives in match_tc.cu.
+// The wgmma tensor-core distance kernels live in match_tc.cu.
 #include <algorithm>
 #include <cmath>
 #include <map>
@@ -313,7 +313,7 @@ constexpr int FX_MAX_DIM_T32 = 704;   // 2 * 704 * 36 * 4 B = 203 KB
 // ---------------------------------------------------------------------------
 // Merge chunks + ratio test.  grid = (ceil(max_nq/256), njobs)
 // ---------------------------------------------------------------------------
-// squared != 0: the partials hold squared distances (tcgen05 kernel; only used when float32 sqrt is
+// squared != 0: the partials hold squared distances (tensor-core L2 kernel; only used when float32 sqrt is
 // injective on them, so merging in d^2 is merging in cv2's ranking) and are sqrt'd here.
 __global__ void bf_top2_finalize(const MatchJob* __restrict__ jobs, const Top2* __restrict__ partial,
                                  int32_t* __restrict__ match_buf, double ratio, int squared) {
@@ -791,7 +791,7 @@ void Matcher::match_pairs_async(int npairs, const int* ids_a, const int* ids_b, 
     any_f32 |= !A.u8;
     max_dim_padded = std::max(max_dim_padded, A.dim_padded);
     // d^2 <= (|a| + |b|)^2 <= 2 (|a|^2 + |b|^2) must stay below 2^22 for the d^2-space ranking of the
-    // tcgen05 kernel to equal cv2's sqrt-space ranking (float32 sqrt injective on integers < 2^22)
+    // tensor-core kernel to equal cv2's sqrt-space ranking (float32 sqrt injective on integers < 2^22)
     all_tc &= (!A.u8 && A.tc_ok && B.tc_ok && 2.0f * (A.tc_max_norm + B.tc_max_norm) < 4194304.0f);
     all_h8 &= (A.u8 && A.tc_ok && B.tc_ok && A.tc_q != nullptr && B.tc_q != nullptr);
     h_out_off[p + 1] = h_out_off[p] + A.n;
@@ -856,12 +856,12 @@ void Matcher::match_pairs_async(int npairs, const int* ids_a, const int* ids_b, 
   // kernel choice
   int use = 1;
   if (kernel_choice == 2) {
-    if (!all_tc || dmask) throw ArgError("tcgen05 kernel forced but descriptors are not bf16-exact / norm-bounded, or a mask is set");
+    if (!all_tc || dmask) throw ArgError("tensor-core kernel forced but descriptors are not bf16-exact / norm-bounded, or a mask is set");
     use = 2;
   } else if (kernel_choice == 0 && all_tc && !dmask && any_f32 && tc_available()) {
     use = 2;   // (guided pairs too: the tensor-core epilogue applies the bitmask)
   } else if (kernel_choice == 0 && all_h8 && any_u8 && !dmask && !guided && npairs > 0 && tc_available()) {
-    use = 3;   // Hamming as a +-1 fp8 contraction (match_tc.cu bf_top2_tc_h8)
+    use = 3;   // Hamming as a +-1 fp8 contraction (match_tc.cu bf_top2_wg<KIND_HAMMING>)
   }
   last_kernel = use;
   last_total_results = h_out_off[npairs];

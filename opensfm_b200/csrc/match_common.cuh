@@ -1,4 +1,4 @@
-// Types shared by the SIMT and tcgen05 matching kernels.
+// Types shared by the SIMT and tensor-core (wgmma) matching kernels.
 #pragma once
 #include <cuda_bf16.h>
 
@@ -48,9 +48,9 @@ __host__ __device__ inline void top2_merge(Top2& t, const Top2& o) {
 struct MatchJob {
   const void* q;  // queries, padded rows (float32 or packed uint8 words)
   const void* t;  // trains
-  const __nv_bfloat16* q_tc;  // tcgen05 operand copies (blocked core-matrix layout), or null
+  const __nv_bfloat16* q_tc;  // tensor-core operand copies (blocked core-matrix layout), or null
   const __nv_bfloat16* t_tc;
-  const float* q_norm;        // |q_i|^2 (tcgen05 path)
+  const float* q_norm;        // |q_i|^2 (tensor-core path)
   const float* t_norm;
   int nq, nt;
   int dim, dim_padded;  // dim_padded: 4-byte elements per padded row
@@ -74,7 +74,7 @@ struct DescSet {
   void* data = nullptr;
   int n = 0, dim = 0, dim_padded = 0, row_bytes = 0;
   bool u8 = false;
-  // tcgen05 operands (float32 sets with integer values in [0,255] and dim <= 128 only)
+  // tensor-core operands (float32 sets with integer values in [0,255] and dim <= 128 only)
   void* tc_data = nullptr;  // one allocation: [A-role | B-role | norms]
   const __nv_bfloat16* tc_q = nullptr;
   const __nv_bfloat16* tc_t = nullptr;
@@ -105,7 +105,7 @@ struct Matcher {
   int device;
   cudaStream_t stream = nullptr;
   cudaEvent_t ev[4];
-  int num_sms = 148;
+  int num_sms = 132;
   int next_id = 1;
   int kernel_choice = 0;
   int last_kernel = 0;

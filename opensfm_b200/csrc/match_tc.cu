@@ -1,6 +1,7 @@
-// tcgen05 tensor-core distance kernel for brute-force L2 matching (sm_100a).
+// Tensor-core distance kernels for brute-force matching on H100 (sm_90a): warpgroup MMA (wgmma) with register
+// accumulators, operands staged by the bulk-copy (TMA) engine through an mbarrier pipeline.
 //
-// The N x M x 128 contraction of opensfm/matching.py:742-747 (cv2 knnMatch)
+// L2 ("BruteForce"): the N x M x 128 contraction of opensfm/matching.py:742-747 (cv2 knnMatch)
 // is a dense GEMM: d2(i,j) = |a_i|^2 + |b_j|^2 - 2 a_i.b_j.  For descriptors
 // whose values are integers in [0,255] (HAHOG / SIFT as OpenSfM stores them,
 // opensfm/features.py:526-534, and the synthetic scenes) every product and
@@ -14,19 +15,22 @@
 //   => accumulator(i,j) = |b_j|^2 - 2 a_i.b_j = d2(i,j) - |a_i|^2   (exact)
 //   so the epilogue needs no per-column add: ranking within a query row is
 //   the ranking of the accumulator itself.
-// Rows are stored in HBM already in the UMMA canonical K-major no-swizzle
-// ("interleave") core-matrix order: [row/8][k/8][row%8][k%8] bf16, 128 bytes
-// per core matrix, so one tile is a single contiguous range and is staged with
-// one cp.async.bulk (TMA engine) per operand tile; LBO = 128 B, SBO = 18*128 B.
+// Rows are stored in HBM already in the canonical K-major no-swizzle ("interleave") core-matrix order of wgmma:
+// [row/8][k/8][row%8][k%8] bf16, 128 bytes per core matrix, so one tile is a single contiguous range and is
+// staged with one cp.async.bulk per operand tile; LBO = 128 B (K-adjacent core matrices), SBO = 18*128 B
+// (8-row groups).
 //
-// Kernel: persistent, 1 CTA / SM, 6 warps:
-//   warp 0  bulk-copy producer (Q tile double-buffered per task, T tiles 2 stages)
-//   warp 1  TMEM alloc + single-thread tcgen05.mma issue (M=128, N=256, K=16 x 9)
-//   warps 2-5  epilogue: tcgen05.ld the 128x256 fp32 accumulator (double-buffered
-//           in TMEM, 2 x 256 columns, loads software-pipelined) and keep a running
-//           top-2 per query row in d^2 space: group-of-8 min filter (0.75 instruction /
-//           element) with exact updates only for elements that beat the row's current
-//           second best; the loop body is kept small enough for the instruction cache.
+// Kernel (bf_top2_wg, both the L2 and the Hamming kind): persistent, 1 CTA / SM, 3 warpgroups:
+//   warps 0-3, 4-7  two consumer warpgroups.  Each owns MB x 64 rows of the task's query tile and, for every
+//           128-row train tile, issues wgmma.mma_async (m64 n128, one per 64-row block) into registers, waits,
+//           hands the shared-memory stage back and keeps a running top-2 per row over its accumulator fragment:
+//           group-of-8 min filter against the row's current second best, exact updates only inside a group that
+//           beats it.  While one warpgroup runs its epilogue the other one's MMAs keep the tensor cores busy.
+//   warps 8-11  producer warpgroup: one thread issues the bulk copies (query tile buffers, train tiles in STAGES
+//           stages); the warpgroup hands most of its registers to the consumers (setmaxnreg).
+// A thread of the m64 accumulator fragment holds two rows (lane/4 and lane/4 + 8 of its warp's 16) and, of each,
+// the columns 8j + 2 (lane%4) + {0, 1}: the four threads of a quad merge their partial top-2 lists at the end of
+// a task (lexicographic (value, index), i.e. cv2's insertion order).
 #include <cuda_bf16.h>
 
 #include "common.cuh"
@@ -34,31 +38,60 @@
 
 namespace osfm {
 
-constexpr int TC_M = 256;                // query rows per task: two M = 128 MMAs share every train tile
-constexpr int TC_MH = 128;               // rows of one MMA (TMEM lanes)
-constexpr int TC_N = 128;                // train rows per tile
 constexpr int TC_KD = 128;               // descriptor dims carried
-constexpr int TC_KP = 144;               // padded K (9 x UMMA_K)
+constexpr int TC_KP = 144;               // padded K (9 x 16)
 constexpr int TC_KCH = TC_KP / 8;        // 16-byte K chunks per row
 constexpr int TC_ROW_BYTES = TC_KP * 2;  // 288
-constexpr int TC_Q_BYTES = TC_M * TC_ROW_BYTES;  // 36864
-constexpr int TC_T_BYTES = TC_N * TC_ROW_BYTES;  // 73728
-constexpr int TC_SBO = TC_KCH * 128;     // bytes between 8-row groups
 constexpr int TC_LBO = 128;              // bytes between K-adjacent core matrices
-constexpr int TC_STAGES = 2;
-constexpr int TC_EPI_WARPS = 8;            // two per TMEM lane quarter, interleaved over 16-column chunks
-constexpr int TC_THREADS = 64 + 32 * TC_EPI_WARPS;
-constexpr int TC_SMEM = 2 * TC_Q_BYTES + TC_STAGES * TC_T_BYTES;  // 221184
+constexpr int H8_ROW_BYTES = 512;
+constexpr int H8_KCH = H8_ROW_BYTES / 16;   // 16-byte K chunks per row
+constexpr int WG_N = 128;                   // train rows per tile (wgmma N)
+constexpr int WG_CONSUMERS = 2;             // consumer warpgroups per CTA
+constexpr int WG_THREADS = 128 * (WG_CONSUMERS + 1);   // + one producer warpgroup
+// Registers: the producer warpgroup releases down to 40 a thread, the consumers take 232 (64 512 of the 65 536).
+constexpr int WG_PRODUCER_REGS = 40, WG_CONSUMER_REGS = 232;
+static_assert(128 * (WG_PRODUCER_REGS + WG_CONSUMERS * WG_CONSUMER_REGS) <= 65536, "register file of an SM");
 
-int tc_tile_m() { return TC_M; }
-int tc_tile_n() { return TC_N; }
+enum { KIND_L2 = 0, KIND_HAMMING = 1 };
+template <int KIND>
+struct WgCfg;
+// L2: 256 query rows per task (128 per warpgroup, two m64 blocks = 128 accumulator registers a thread): every train
+// tile brought into shared memory feeds 256 rows, which keeps the L2 -> SM traffic at 1.1 bytes per distance.
+// Two query buffers let the next task's queries load under the current task.  2 x 72 + 2 x 36 KB = 216 KB.
+template <>
+struct WgCfg<KIND_L2> {
+  static constexpr int ROW_BYTES = TC_ROW_BYTES, MB = 2, QBUF = 2, STAGES = 2;
+};
+// Hamming: 512 fp8 per row; 128 query rows per task (64 per warpgroup), one query buffer: 64 + 2 x 64 KB = 192 KB.
+template <>
+struct WgCfg<KIND_HAMMING> {
+  static constexpr int ROW_BYTES = H8_ROW_BYTES, MB = 1, QBUF = 1, STAGES = 2;
+};
+template <int KIND>
+struct WgGeom {
+  using C = WgCfg<KIND>;
+  static constexpr int M = WG_CONSUMERS * C::MB * 64;   // query rows per task
+  static constexpr int Q_BYTES = M * C::ROW_BYTES;
+  static constexpr int T_BYTES = WG_N * C::ROW_BYTES;
+  static constexpr int SBO = C::ROW_BYTES / 16 * 128;   // bytes between 8-row groups
+  static constexpr int KSTEPS = C::ROW_BYTES / 32;      // one wgmma K step = 32 bytes of K (k16 bf16 / k32 e4m3)
+  static constexpr int SMEM = C::QBUF * Q_BYTES + C::STAGES * T_BYTES;
+};
+static_assert(WgGeom<KIND_L2>::SMEM <= 227 * 1024 - 1024, "L2 kernel exceeds the H100 shared memory of a block");
+static_assert(WgGeom<KIND_HAMMING>::SMEM <= 227 * 1024 - 1024, "Hamming kernel exceeds the H100 shared memory of a block");
+static_assert(WgGeom<KIND_L2>::M == 256, "tc_rows_padded pads sets to whole L2 query tiles");
 
+int tc_tile_m() { return WgGeom<KIND_L2>::M; }
+int tc_tile_n() { return WG_N; }
+
+// The library is built for sm_90a only, so this is the H100 class (compute capability 9.0) it can run on.
 bool tc_available() {
   int dev = 0;
   if (cudaGetDevice(&dev) != cudaSuccess) return false;
-  int major = 0;
+  int major = 0, minor = 0;
   cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev);
-  return major == 10;
+  cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, dev);
+  return major == 9 && minor == 0;
 }
 
 // ---------------------------------------------------------------------------
@@ -66,7 +99,7 @@ bool tc_available() {
 // ---------------------------------------------------------------------------
 // One warp per padded row, one pass over the uploaded float32 matrix: exactness check (integers in
 // [0,255]), |x|^2, max |x|^2, the zero-padded float32 row of the SIMT kernel (when it is not the
-// upload itself) and both bf16 operand roles in the UMMA core-matrix order.
+// upload itself) and both bf16 operand roles in the wgmma core-matrix order.
 // info[0] |= 1 if any value is not bf16-exact; info[1] = max |x|^2 as float bits.
 // SrcT = float (the reference's in-memory form, features.py:169-170) or uint8_t (the on-disk form of HAHOG / SIFT
 // descriptors, uploaded as bytes and widened here: a quarter of the host->device traffic).
@@ -168,7 +201,10 @@ void Matcher::prepare_tc(DescSet& s, const void* src, bool src_u8, float* padded
   s.tc_norm = norm;
   s.info_pending = true;
 }
-int tc_rows_padded(int n) { return (n + TC_M - 1) / TC_M * TC_M; }   // whole query tiles (and whole train tiles)
+int tc_rows_padded(int n) {   // whole query tiles (and whole train tiles) of both kernels
+  constexpr int M = WgGeom<KIND_L2>::M;
+  return (n + M - 1) / M * M;
+}
 size_t tc_operand_bytes(int rows_padded) { return 2 * (size_t)rows_padded * TC_ROW_BYTES + (size_t)rows_padded * sizeof(float); }
 bool tc_capable(int dim, bool u8, int n) { return !u8 && dim <= TC_KD && n > 0 && tc_available(); }
 
@@ -191,8 +227,7 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity, int* e
   const uint32_t addr = smem_u32(bar);
   long long t0 = 0;
   // try_wait suspends the thread for a hardware-defined time slice before it reports failure, so the loop is
-  // cheap; the clock is only consulted every 1024 failed slices (reading it on every poll cost more issue
-  // slots than the epilogue itself, profiles/r01_ncu_tc_v6.txt: 143M TRYWAIT + CS2R pairs per launch)
+  // cheap; the clock is only consulted every 1024 failed slices
   for (unsigned spins = 0;; ++spins) {
     uint32_t done;
     asm volatile(
@@ -219,69 +254,66 @@ __device__ __forceinline__ void bulk_copy_g2s(void* smem_dst, const void* gsrc, 
                "l"(gsrc), "r"(bytes), "r"(smem_u32(bar))
                : "memory");
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
+
+// wgmma shared-memory descriptor, K-major without swizzle: start >> 4 @0, LBO >> 4 @16 (K-adjacent core
+// matrices), SBO >> 4 @32 (8-row groups), base offset 0 @49, layout type 0 (interleave) @62
+template <int SBO>
+__device__ __forceinline__ uint64_t gmma_desc(uint32_t saddr) {
+  return (uint64_t)((saddr >> 4) & 0x3fff) | ((uint64_t)((TC_LBO >> 4) & 0x3fff) << 16) |
+         ((uint64_t)((SBO >> 4) & 0x3fff) << 32);
 }
-__device__ __forceinline__ void tc_mma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                            uint32_t accumulate) {
+
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// Pins the accumulator registers at this point of the program: the compiler may not move their reads above the
+// wait of the asynchronous MMA that writes them, nor their last uses below the next MMA issue.
+__device__ __forceinline__ void wg_fence_operands(float (&d)[64]) {
+#pragma unroll
+  for (int i = 0; i < 64; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+
+#define OSFM_WG_D8(d, i) \
+  "+f"(d[i]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3]), "+f"(d[i + 4]), "+f"(d[i + 5]), "+f"(d[i + 6]), "+f"(d[i + 7])
+#define OSFM_WG_D64(d)                                                                                       \
+  OSFM_WG_D8(d, 0), OSFM_WG_D8(d, 8), OSFM_WG_D8(d, 16), OSFM_WG_D8(d, 24), OSFM_WG_D8(d, 32), OSFM_WG_D8(d, 40), \
+      OSFM_WG_D8(d, 48), OSFM_WG_D8(d, 56)
+#define OSFM_WG_REGS64                                                                                   \
+  "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, " \
+  "%22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, "  \
+  "%42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, "  \
+  "%62, %63}"
+
+// D(64 x 128, fp32) (+)= A(64 x K step) * B(K step x 128); accumulate = 0 overwrites D
+template <int KIND>
+__device__ __forceinline__ void wg_mma(float (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t accumulate);
+template <>
+__device__ __forceinline__ void wg_mma<KIND_L2>(float (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
   asm volatile(
       "{\n.reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
+      "setp.ne.b32 p, %66, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 " OSFM_WG_REGS64 ", %64, %65, p, 1, 1, 0, 0;\n}\n"
+      : OSFM_WG_D64(d)
+      : "l"(adesc), "l"(bdesc), "r"(accumulate)
       : "memory");
 }
-// K-major, no swizzle (cute::UMMA::SmemDescriptor: start>>4 @0, LBO>>4 @16, SBO>>4 @32, version=1 @46)
-__device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr) {
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr >> 4) & 0x3fff);
-  d |= (uint64_t)((TC_LBO >> 4) & 0x3fff) << 16;
-  d |= (uint64_t)((TC_SBO >> 4) & 0x3fff) << 32;
-  d |= (uint64_t)1 << 46;
-  return d;
+template <>
+__device__ __forceinline__ void wg_mma<KIND_HAMMING>(float (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+  asm volatile(
+      "{\n.reg .pred p;\n"
+      "setp.ne.b32 p, %66, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n128k32.f32.e4m3.e4m3 " OSFM_WG_REGS64 ", %64, %65, p, 1, 1;\n}\n"
+      : OSFM_WG_D64(d)
+      : "l"(adesc), "l"(bdesc), "r"(accumulate)
+      : "memory");
 }
-// cute::UMMA::InstrDescriptor: c_format F32 (1) @4, a/b format BF16 (1) @7/@10, K-major both,
-// n_dim = N>>3 @17, m_dim = M>>4 @24
-constexpr uint32_t TC_IDESC = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(TC_N >> 3) << 17) |
-                              ((uint32_t)(TC_MH >> 4) << 24);
-
-#define OSFM_TMEM_LD16(taddr, v)                                                                          \
-  asm volatile(                                                                                           \
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "                                                           \
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"                                    \
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),   \
-        "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]),          \
-        "=r"(v[15])                                                                                       \
-      : "r"(taddr)                                                                                        \
-      : "memory")
-
-#define OSFM_TMEM_LD64(taddr, v)                                                                          \
-  asm volatile(                                                                                           \
-      "tcgen05.ld.sync.aligned.32x32b.x64.b32 "                                                           \
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"                                           \
-      "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,"                                  \
-      "%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,"                                  \
-      "%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, [%64];"                          \
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),   \
-        "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]),          \
-        "=r"(v[15]), "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]),        \
-        "=r"(v[22]), "=r"(v[23]), "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]),        \
-        "=r"(v[29]), "=r"(v[30]), "=r"(v[31]), "=r"(v[32]), "=r"(v[33]), "=r"(v[34]), "=r"(v[35]),        \
-        "=r"(v[36]), "=r"(v[37]), "=r"(v[38]), "=r"(v[39]), "=r"(v[40]), "=r"(v[41]), "=r"(v[42]),        \
-        "=r"(v[43]), "=r"(v[44]), "=r"(v[45]), "=r"(v[46]), "=r"(v[47]), "=r"(v[48]), "=r"(v[49]),        \
-        "=r"(v[50]), "=r"(v[51]), "=r"(v[52]), "=r"(v[53]), "=r"(v[54]), "=r"(v[55]), "=r"(v[56]),        \
-        "=r"(v[57]), "=r"(v[58]), "=r"(v[59]), "=r"(v[60]), "=r"(v[61]), "=r"(v[62]), "=r"(v[63])         \
-      : "r"(taddr)                                                                                        \
-      : "memory")
 
 struct TcTask {
   MatchJob job;
   int q0, t_begin, ntiles, chunk;
 };
 
+template <int M>
 __device__ __forceinline__ TcTask tc_decode(const MatchJob* jobs, const int* tile_prefix, int njobs, int task) {
   int lo = 0, hi = njobs - 1;
   while (lo < hi) {
@@ -293,24 +325,23 @@ __device__ __forceinline__ TcTask tc_decode(const MatchJob* jobs, const int* til
   const int local = task - tile_prefix[lo];
   const int qtile = local / t.job.nchunks;
   t.chunk = local % t.job.nchunks;
-  t.q0 = qtile * TC_M;
+  t.q0 = qtile * M;
   t.t_begin = t.chunk * t.job.chunk_len;
   const int t_end = min(t.job.nt, t.t_begin + t.job.chunk_len);
-  t.ntiles = (t_end - t.t_begin + TC_N - 1) / TC_N;
+  t.ntiles = (t_end - t.t_begin + WG_N - 1) / WG_N;
   return t;
 }
 
-// Epilogue state of one query row: the two smallest accumulator values (= d^2 - |a|^2, exact
-// integers) with their train indices.  Ranking in d^2 is the ranking cv2 uses (sqrt'd float32
-// distance, ties -> lowest index) as long as float32 sqrt is injective on the integers involved,
-// i.e. d^2 < 2^22; the host only selects this kernel for descriptor sets whose norms guarantee
-// that bound (Matcher::match_pairs_async), everything else goes to the exact SIMT kernel.
+// Epilogue state of one query row: the two smallest accumulator values (L2: d^2 - |a|^2; Hamming: 2 H - nbits;
+// exact integers either way) with their train indices.  For L2, ranking in d^2 is the ranking cv2 uses (sqrt'd
+// float32 distance, ties -> lowest index) as long as float32 sqrt is injective on the integers involved, i.e.
+// d^2 < 2^22; the host only selects this kernel for descriptor sets whose norms guarantee that bound
+// (Matcher::match_pairs_async), everything else goes to the exact SIMT kernel.
 struct RowState {
   float q1, q2;
   int i1, i2;
 };
 
-// Branch-free update (used for the first tile of a task, where most elements are records).
 __device__ __forceinline__ void row_update(RowState& st, float x, int idx) {
   const bool lt1 = x < st.q1;
   const bool lt2 = x < st.q2;
@@ -320,204 +351,189 @@ __device__ __forceinline__ void row_update(RowState& st, float x, int idx) {
   st.i1 = lt1 ? idx : st.i1;
 }
 
-// 16 accumulator columns of one row: two groups of 8, min filter against the row's current second
-// best, exact (predicated) updates only inside a group that beats it.  Deliberately small: the whole
-// epilogue loop body must stay resident in the instruction cache (an earlier fully unrolled version was
-// 89 KB of SASS and spent most of its time in instruction-fetch stalls, profiles/r01_*).
-template <int OFF, int NV, bool MASKED>
-__device__ __forceinline__ void row_consume16(RowState& st, const uint32_t (&vv)[NV], int col0, uint32_t bits16) {
-  const uint32_t* v = vv + OFF;   // OFF is a compile-time constant: the accesses below stay register-resident
-  // minima of four groups of 4 (independent chains), one test for the common case; a triggered chunk
-  // re-examines only the group(s) of 4 that beat the threshold (their updates are predicated by ptxas,
-  // 7 instructions per element, so small groups matter).  MASKED (guided matching): elements whose bit is
-  // clear read as +inf and can never enter the row's two best.
-  float x[16];
+// The 32 values of one row (H = 0: fragment row lane/4, H = 1: lane/4 + 8) in one 64 x 128 accumulator, in
+// increasing column order: col0 + 8 j + e for fragment element 4 j + 2 H + e.  Four groups of 8, one min test
+// against the row's second best each, exact (predicated) updates only inside a group that beats it.  MASKED
+// (guided matching): mw[g] holds the row's mask bits of columns 32 g .. 32 g + 31 shifted to this thread's
+// columns; a clear bit reads as +inf and can never enter the row's two best.
+template <int H, bool MASKED>
+__device__ __forceinline__ void row_consume(RowState& st, const float (&d)[64], int col0, const uint32_t (&mw)[4]) {
 #pragma unroll
-  for (int e = 0; e < 16; ++e) {
-    x[e] = __uint_as_float(v[e]);
-    if (MASKED) x[e] = ((bits16 >> e) & 1u) ? x[e] : __builtin_huge_valf();
-  }
-  if (MASKED && bits16 == 0u) return;
-  float m[4];
+  for (int g = 0; g < 4; ++g) {
+    if (MASKED && (mw[g] & 0x03030303u) == 0u) continue;
+    float x[8];
 #pragma unroll
-  for (int g = 0; g < 4; ++g) m[g] = fminf(fminf(fminf(x[g * 4], x[g * 4 + 1]), x[g * 4 + 2]), x[g * 4 + 3]);
-  if (fminf(fminf(fminf(m[0], m[1]), m[2]), m[3]) < st.q2) {
+    for (int jj = 0; jj < 4; ++jj) {
 #pragma unroll
-    for (int g = 0; g < 4; ++g) {
-      if (m[g] < st.q2) {
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {
-          if (x[g * 4 + e] < st.q2) row_update(st, x[g * 4 + e], col0 + g * 4 + e);
-        }
+      for (int e = 0; e < 2; ++e) {
+        const float v = d[4 * (4 * g + jj) + 2 * H + e];
+        x[2 * jj + e] = (!MASKED || ((mw[g] >> (8 * jj + e)) & 1u)) ? v : __builtin_huge_valf();
       }
+    }
+    const float m = fminf(fminf(fminf(x[0], x[1]), fminf(x[2], x[3])), fminf(fminf(x[4], x[5]), fminf(x[6], x[7])));
+    if (m < st.q2) {
+#pragma unroll
+      for (int k = 0; k < 8; ++k)
+        if (x[k] < st.q2) row_update(st, x[k], col0 + 32 * g + 8 * (k >> 1) + (k & 1));
     }
   }
 }
 
-template <bool MASKED>
-__global__ void __launch_bounds__(TC_THREADS, 1)
-    bf_top2_tc(const MatchJob* __restrict__ jobs, const int* __restrict__ tile_prefix, int njobs, int ntasks,
+template <int KIND, bool MASKED>
+__global__ void __launch_bounds__(WG_THREADS, 1)
+    bf_top2_wg(const MatchJob* __restrict__ jobs, const int* __restrict__ tile_prefix, int njobs, int ntasks,
                Top2* __restrict__ partial, int* __restrict__ err_flag) {
+  using C = WgCfg<KIND>;
+  using G = WgGeom<KIND>;
+  constexpr int MB = C::MB, QBUF = C::QBUF, STAGES = C::STAGES;
+  constexpr int CONSUMER_WARPS = 4 * WG_CONSUMERS;
   extern __shared__ __align__(1024) uint8_t smem[];
-  __shared__ __align__(8) uint64_t bar_qfull[2], bar_qempty[2], bar_full[TC_STAGES], bar_empty[TC_STAGES],
-      bar_accfull[2], bar_accempty[2];
-  __shared__ uint32_t tmem_base_smem;
-
-  uint8_t* q_smem[2] = {smem, smem + TC_Q_BYTES};
-  uint8_t* t_smem[TC_STAGES];
-#pragma unroll
-  for (int s = 0; s < TC_STAGES; ++s) t_smem[s] = smem + 2 * TC_Q_BYTES + s * TC_T_BYTES;
+  __shared__ __align__(8) uint64_t bar_qfull[QBUF], bar_qempty[QBUF], bar_full[STAGES], bar_empty[STAGES];
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-
   if (threadIdx.x == 0) {
-    for (int i = 0; i < 2; ++i) {
+    for (int i = 0; i < QBUF; ++i) {
       mbar_init(&bar_qfull[i], 1);
-      mbar_init(&bar_qempty[i], 1);
-      mbar_init(&bar_accfull[i], 1);
-      mbar_init(&bar_accempty[i], TC_EPI_WARPS);  // one arrival per epilogue warp
+      mbar_init(&bar_qempty[i], CONSUMER_WARPS);   // one arrival per consumer warp
     }
-    for (int i = 0; i < TC_STAGES; ++i) {
+    for (int i = 0; i < STAGES; ++i) {
       mbar_init(&bar_full[i], 1);
-      mbar_init(&bar_empty[i], 1);
+      mbar_init(&bar_empty[i], CONSUMER_WARPS);
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 512;" ::"r"(smem_u32(&tmem_base_smem))
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = tmem_base_smem;
 
-  if (warp == 0) {
+  if (warp >= CONSUMER_WARPS) {
     // ===== bulk-copy producer =====
-    if (lane == 0) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(WG_PRODUCER_REGS));
+    if (warp == CONSUMER_WARPS && lane == 0) {
       int stage = 0, ph = 0, n = 0;
       for (int task = blockIdx.x; task < ntasks; task += gridDim.x, ++n) {
-        const TcTask t = tc_decode(jobs, tile_prefix, njobs, task);
-        const int b = n & 1, qph = (n >> 1) & 1;
+        const TcTask t = tc_decode<G::M>(jobs, tile_prefix, njobs, task);
+        const int b = n % QBUF, qph = (n / QBUF) & 1;
         mbar_wait(&bar_qempty[b], qph ^ 1, err_flag);
-        // the last query tile of a job may hold <= 128 rows: only its first half is loaded and multiplied
-        const uint32_t qbytes = (t.job.nq - t.q0 > TC_MH) ? TC_Q_BYTES : TC_Q_BYTES / 2;
+        // the last query tile of a job may hold no rows for the second warpgroup: only the first half is loaded
+        const uint32_t qbytes = (t.job.nq - t.q0 > G::M / 2) ? G::Q_BYTES : G::Q_BYTES / 2;
         mbar_expect_tx(&bar_qfull[b], qbytes);
-        bulk_copy_g2s(q_smem[b], reinterpret_cast<const uint8_t*>(t.job.q_tc) + (size_t)t.q0 * TC_ROW_BYTES,
+        bulk_copy_g2s(smem + b * G::Q_BYTES, reinterpret_cast<const uint8_t*>(t.job.q_tc) + (size_t)t.q0 * C::ROW_BYTES,
                       qbytes, &bar_qfull[b]);
         for (int i = 0; i < t.ntiles; ++i) {
           mbar_wait(&bar_empty[stage], ph ^ 1, err_flag);
-          mbar_expect_tx(&bar_full[stage], TC_T_BYTES);
-          bulk_copy_g2s(t_smem[stage],
-                        reinterpret_cast<const uint8_t*>(t.job.t_tc) + (size_t)(t.t_begin + i * TC_N) * TC_ROW_BYTES,
-                        TC_T_BYTES, &bar_full[stage]);
-          if (++stage == TC_STAGES) { stage = 0; ph ^= 1; }
+          mbar_expect_tx(&bar_full[stage], G::T_BYTES);
+          bulk_copy_g2s(smem + QBUF * G::Q_BYTES + stage * G::T_BYTES,
+                        reinterpret_cast<const uint8_t*>(t.job.t_tc) + (size_t)(t.t_begin + i * WG_N) * C::ROW_BYTES,
+                        G::T_BYTES, &bar_full[stage]);
+          if (++stage == STAGES) { stage = 0; ph ^= 1; }
         }
       }
     }
-  } else if (warp == 1) {
-    // ===== MMA issuer =====
-    if (lane == 0) {
-      int stage = 0, ph = 0, n = 0, tilecount = 0;
-      for (int task = blockIdx.x; task < ntasks; task += gridDim.x, ++n) {
-        const TcTask t = tc_decode(jobs, tile_prefix, njobs, task);
-        const int b = n & 1, qph = (n >> 1) & 1;
-        mbar_wait(&bar_qfull[b], qph, err_flag);
-        const uint64_t adesc0 = make_smem_desc(smem_u32(q_smem[b]));
-        const uint64_t adesc1 = make_smem_desc(smem_u32(q_smem[b]) + (TC_MH / 8) * TC_SBO);   // query rows 128..255
-        const bool two = t.job.nq - t.q0 > TC_MH;   // a short last tile skips the second MMA (its rows do not exist)
-        for (int i = 0; i < t.ntiles; ++i, ++tilecount) {
-          const int a = tilecount & 1, aph = (tilecount >> 1) & 1;
-          mbar_wait(&bar_accempty[a], aph ^ 1, err_flag);
-          mbar_wait(&bar_full[stage], ph, err_flag);
-          tc_fence_after();
-          const uint64_t bdesc0 = make_smem_desc(smem_u32(t_smem[stage]));
-          // accumulator stage a = TMEM columns [256 a, 256 a + 256): query rows 0..127 in the first 128 columns,
-          // 128..255 in the second.  Both MMAs read the same train tile from shared memory: every byte the TMA
-          // engine brings in feeds 256 query rows (the M = 128 x N = 256 tile moved twice the bytes per output
-          // and was bound by the L2 -> SM path, profiles/README.md round 2)
-          const uint32_t d_tmem = tmem_base + (uint32_t)a * (2 * TC_N);
+    return;
+  }
+
+  // ===== consumer warpgroups =====
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(WG_CONSUMER_REGS));
+  const int wg = warp >> 2, w = warp & 3, quad = lane & 3;
+  const int wg_row0 = wg * MB * 64;   // first query row of this warpgroup in the task's tile
+  float acc[MB][64];
 #pragma unroll
-          for (int k = 0; k < TC_KP / 16; ++k) {
-            // one UMMA_K = 16 bf16 = two core matrices = 256 bytes along K
-            const uint64_t koff = (uint64_t)((k * 2 * TC_LBO) >> 4);
-            tc_mma_bf16(d_tmem, adesc0 + koff, bdesc0 + koff, TC_IDESC, k > 0 ? 1u : 0u);
-            if (two) tc_mma_bf16(d_tmem + TC_N, adesc1 + koff, bdesc0 + koff, TC_IDESC, k > 0 ? 1u : 0u);
+  for (int mb = 0; mb < MB; ++mb)
+#pragma unroll
+    for (int i = 0; i < 64; ++i) acc[mb][i] = 0.0f;
+  int stage = 0, ph = 0, n = 0;
+  for (int task = blockIdx.x; task < ntasks; task += gridDim.x, ++n) {
+    const TcTask t = tc_decode<G::M>(jobs, tile_prefix, njobs, task);
+    const int b = n % QBUF, qph = (n / QBUF) & 1;
+    const bool active = t.job.nq - t.q0 > wg_row0;
+    RowState st[2 * MB];
+#pragma unroll
+    for (int r = 0; r < 2 * MB; ++r) {
+      st[r].q1 = st[r].q2 = __builtin_huge_valf();
+      st[r].i1 = st[r].i2 = -1;
+    }
+    mbar_wait(&bar_qfull[b], qph, err_flag);
+    const uint32_t q_addr = smem_u32(smem + b * G::Q_BYTES) + (wg_row0 / 8) * G::SBO;
+    for (int i = 0; i < t.ntiles; ++i) {
+      mbar_wait(&bar_full[stage], ph, err_flag);
+      if (active) {
+        const uint32_t t_addr = smem_u32(smem + QBUF * G::Q_BYTES + stage * G::T_BYTES);
+#pragma unroll
+        for (int mb = 0; mb < MB; ++mb) wg_fence_operands(acc[mb]);
+        wg_fence();
+#pragma unroll
+        for (int k = 0; k < G::KSTEPS; ++k) {
+          // one K step = 32 bytes of K = two core matrices = 256 bytes further in both operands
+          const uint64_t koff = (uint64_t)((k * 2 * TC_LBO) >> 4);
+          const uint64_t bdesc = gmma_desc<G::SBO>(t_addr) + koff;
+#pragma unroll
+          for (int mb = 0; mb < MB; ++mb)
+            wg_mma<KIND>(acc[mb], gmma_desc<G::SBO>(q_addr + mb * 8 * G::SBO) + koff, bdesc, k > 0 ? 1u : 0u);
+        }
+        wg_commit();
+        wg_wait_all();
+#pragma unroll
+        for (int mb = 0; mb < MB; ++mb) wg_fence_operands(acc[mb]);
+      }
+      // the stage's operands have been read by this warp's MMAs: hand it back before the epilogue
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&bar_empty[stage]);
+      if (++stage == STAGES) { stage = 0; ph ^= 1; }
+      if (active) {
+        const int col_base = t.t_begin + i * WG_N;
+#pragma unroll
+        for (int mb = 0; mb < MB; ++mb) {
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            uint32_t mw[4] = {0u, 0u, 0u, 0u};
+            if (MASKED) {
+              const int gq = t.q0 + wg_row0 + mb * 64 + 16 * w + (lane >> 2) + 8 * h;
+              if (gq < t.job.nq) {
+                const uint32_t* mrow = t.job.mask_bits + (size_t)gq * t.job.mask_words;
+                const int w0 = col_base >> 5;
+#pragma unroll
+                for (int q = 0; q < 4; ++q)
+                  if (w0 + q < t.job.mask_words) mw[q] = mrow[w0 + q] >> (2 * quad);
+              }
+            }
+            if (h == 0) row_consume<0, MASKED>(st[2 * mb], acc[mb], col_base + 2 * quad, mw);
+            else row_consume<1, MASKED>(st[2 * mb + 1], acc[mb], col_base + 2 * quad, mw);
           }
-          tc_commit(&bar_empty[stage]);   // smem stage reusable when these MMAs retire
-          tc_commit(&bar_accfull[a]);     // accumulator complete
-          if (++stage == TC_STAGES) { stage = 0; ph ^= 1; }
         }
-        tc_commit(&bar_qempty[b]);  // Q buffer reusable after the task's last MMA
       }
     }
-  } else {
-    // ===== epilogue: warps 2..9; a warp may only touch TMEM lanes 32*(warp%4)..+31.  The two warps of a lane
-    // quarter take the two query halves of the task (rows 0..127 / 128..255 = the two accumulators of a stage), so
-    // each SM sub-partition always has two independent instruction streams and every thread owns one query row =====
-    const int quarter = warp & 3;
-    const int half = (warp - 2) >> 2;
-    const int row_in_tile = half * TC_MH + quarter * 32 + lane;
-    int tilecount = 0;
-    for (int task = blockIdx.x; task < ntasks; task += gridDim.x) {
-      const TcTask t = tc_decode(jobs, tile_prefix, njobs, task);
-      const int gq = t.q0 + row_in_tile;
-      const float na = gq < t.job.nq ? t.job.q_norm[gq] : 0.0f;
-      RowState st;
-      st.q1 = st.q2 = __builtin_huge_valf();
-      st.i1 = st.i2 = -1;
-      for (int i = 0; i < t.ntiles; ++i, ++tilecount) {
-        const int a = tilecount & 1, aph = (tilecount >> 1) & 1;
-        mbar_wait(&bar_accfull[a], aph, err_flag);
-        tc_fence_after();
-        const uint32_t taddr = tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)a * (2 * TC_N) + (uint32_t)half * TC_N;
-        const int col_base = t.t_begin + i * TC_N;
-        // this row's 128 columns of the tile in two 64-column loads, both in flight at once; the accumulator is
-        // handed back to the MMA issuer as soon as the values are in registers -- the TMEM stage is held for one
-        // load latency, not for the consume time (8 dependent 16-column loads per tile made the epilogue the
-        // critical path: profiles/r01_ncu_tc_v6.txt, top stall on the accumulator-full wait)
-        uint32_t va[64], vb[64];
-        uint32_t mw[4] = {0u, 0u, 0u, 0u};   // guided matching: the row's mask bits of these 128 columns
-        if (MASKED && gq < t.job.nq) {
-          const uint32_t* mrow = t.job.mask_bits + (size_t)gq * t.job.mask_words;
-          const int w0 = col_base >> 5;
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&bar_qempty[b]);
+    if (!active) continue;
 #pragma unroll
-          for (int q = 0; q < 4; ++q)
-            if (w0 + q < t.job.mask_words) mw[q] = mrow[w0 + q];
-        }
-        OSFM_TMEM_LD64(taddr, va);
-        OSFM_TMEM_LD64(taddr + 64, vb);
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&bar_accempty[a]);
-        row_consume16<0, 64, MASKED>(st, va, col_base, mw[0] & 0xffffu);
-        row_consume16<16, 64, MASKED>(st, va, col_base + 16, mw[0] >> 16);
-        row_consume16<32, 64, MASKED>(st, va, col_base + 32, mw[1] & 0xffffu);
-        row_consume16<48, 64, MASKED>(st, va, col_base + 48, mw[1] >> 16);
-        row_consume16<0, 64, MASKED>(st, vb, col_base + 64, mw[2] & 0xffffu);
-        row_consume16<16, 64, MASKED>(st, vb, col_base + 80, mw[2] >> 16);
-        row_consume16<32, 64, MASKED>(st, vb, col_base + 96, mw[3] & 0xffffu);
-        row_consume16<48, 64, MASKED>(st, vb, col_base + 112, mw[3] >> 16);
+    for (int r = 0; r < 2 * MB; ++r) {
+      Top2 a;
+      a.s1 = st[r].q1; a.i1 = st[r].i1; a.s2 = st[r].q2; a.i2 = st[r].i2;
+#pragma unroll
+      for (int off = 1; off <= 2; off <<= 1) {   // the quad's four column subsets of the row
+        Top2 o;
+        o.s1 = __shfl_xor_sync(0xffffffffu, a.s1, off);
+        o.i1 = __shfl_xor_sync(0xffffffffu, a.i1, off);
+        o.s2 = __shfl_xor_sync(0xffffffffu, a.s2, off);
+        o.i2 = __shfl_xor_sync(0xffffffffu, a.i2, off);
+        top2_merge(a, o);
       }
-      if (gq < t.job.nq) {
-        // partial results of this kernel are squared distances (exact integers in fp32)
+      const int gq = t.q0 + wg_row0 + (r >> 1) * 64 + 16 * w + (lane >> 2) + 8 * (r & 1);
+      if (quad == 0 && gq < t.job.nq) {
         Top2 out;
-        out.s1 = st.i1 >= 0 ? fmaxf(st.q1 + na, 0.0f) : __builtin_huge_valf();
-        out.i1 = st.i1;
-        out.s2 = st.i2 >= 0 ? fmaxf(st.q2 + na, 0.0f) : __builtin_huge_valf();
-        out.i2 = st.i2;
+        if (KIND == KIND_L2) {   // squared distances (exact integers in fp32)
+          const float na = t.job.q_norm[gq];
+          out.s1 = a.i1 >= 0 ? fmaxf(a.s1 + na, 0.0f) : __builtin_huge_valf();
+          out.s2 = a.i2 >= 0 ? fmaxf(a.s2 + na, 0.0f) : __builtin_huge_valf();
+        } else {                 // accumulator = 2 H - nbits  ->  the Hamming distance cv2 reports
+          const float nbits = (float)(t.job.dim * 8);
+          out.s1 = a.i1 >= 0 ? (a.s1 + nbits) * 0.5f : __builtin_huge_valf();
+          out.s2 = a.i2 >= 0 ? (a.s2 + nbits) * 0.5f : __builtin_huge_valf();
+        }
+        out.i1 = a.i1;
+        out.i2 = a.i2;
         partial[t.job.partial_off + (size_t)t.chunk * t.job.nq + gq] = out;
       }
     }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 512;" ::"r"(tmem_base) : "memory");
   }
 }
 
@@ -526,30 +542,16 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
 //
 // Bits become +-1 in fp8 (E4M3: +1 = 0x38, -1 = 0xB8, both exact): for two descriptors a, b of nbits bits
 //     sum_i a_i b_i = (#equal bits) - (#different bits) = nbits - 2 H(a, b),
-// so with the train operand negated the fp32 accumulator is 2 H - nbits, an exact integer, and its ranking inside
-// a query row is cv2's ranking by Hamming distance (ties -> lowest index through the same epilogue as the L2
-// kernel).  K = 512 fp8 per row; positions beyond nbits are 0 in real rows of both roles (they add nothing),
-// +1 in every query row and +448 in the *padding* rows of a train set, so a padding train scores
-// >= 8 * 448 - nbits > any real one and is never selected (needs >= 8 spare positions: nbytes <= 63).
-// `tcgen05.mma.kind::f8f6f4`, M = 128, N = 128, K = 32 x 16; operands in the same no-swizzle K-major core-matrix
-// order as the bf16 kernel (a core matrix row is 16 bytes = 16 fp8), 512 B per row.  1 CTA / SM, 10 warps:
-// bulk-copy producer (Q tile single-buffered: 64 KB, T tiles 2 x 64 KB), MMA issuer (2 accumulator stages of 128
-// TMEM columns), 8 epilogue warps = 4 lane quarters x 2 column halves (one 64-column TMEM load per warp and tile).
-// The popcount kernel this replaces is bound by the POPC pipe (16 / clk / SM): 2.1e11 pairs/s at 74 % of that roof.
+// so with the train operand negated the fp32 accumulator is 2 H - nbits, an exact integer (|value| <= 512, well
+// inside the precision the fp8 MMA keeps), and its ranking inside a query row is cv2's ranking by Hamming distance
+// (ties -> lowest index through the same epilogue as the L2 kernel).  K = 512 fp8 per row; positions beyond nbits
+// are 0 in real rows of both roles (they add nothing), +1 in every query row and +448 in the *padding* rows of a
+// train set, so a padding train scores >= 8 * 448 - nbits > any real one and is never selected (needs >= 8 spare
+// positions: nbytes <= 63).  wgmma m64 n128 k32 e4m3, operands in the same no-swizzle K-major core-matrix order as
+// the bf16 kernel (a core matrix row is 16 bytes = 16 fp8), 512 B per row.
 // ===========================================================================================================
-constexpr int H8_M = 128, H8_N = 128;
-constexpr int H8_ROW_BYTES = 512;
-constexpr int H8_KCH = H8_ROW_BYTES / 16;         // 16-byte K chunks per row
-constexpr int H8_SBO = H8_KCH * 128;              // bytes between 8-row groups
-constexpr int H8_Q_BYTES = H8_M * H8_ROW_BYTES;   // 65536
-constexpr int H8_T_BYTES = H8_N * H8_ROW_BYTES;   // 65536
-constexpr int H8_STAGES = 2;
-constexpr int H8_SMEM = H8_Q_BYTES + H8_STAGES * H8_T_BYTES;   // 196608
-// c_format F32 (1) @4, a/b format E4M3 (0) @7/@10, K-major, n_dim = N>>3 @17, m_dim = M>>4 @24
-constexpr uint32_t H8_IDESC = (1u << 4) | ((uint32_t)(H8_N >> 3) << 17) | ((uint32_t)(H8_M >> 4) << 24);
-
-int h8_tile_m() { return H8_M; }
-int h8_tile_n() { return H8_N; }
+int h8_tile_m() { return WgGeom<KIND_HAMMING>::M; }
+int h8_tile_n() { return WG_N; }
 size_t h8_operand_bytes(int rows_padded) { return 2 * (size_t)rows_padded * H8_ROW_BYTES; }
 bool h8_capable(int nbytes, int n) { return nbytes >= 1 && nbytes <= 63 && n > 0 && tc_available(); }
 
@@ -597,214 +599,37 @@ void Matcher::prepare_h8(DescSet& s, const uint8_t* src, int src_stride) {
   s.tc_ok = true;
 }
 
-__device__ __forceinline__ void tc_mma_f8(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n.reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f8f6f4 [%0], %1, %2, %3, p;\n}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ uint64_t h8_smem_desc(uint32_t saddr) {
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr >> 4) & 0x3fff);
-  d |= (uint64_t)((TC_LBO >> 4) & 0x3fff) << 16;
-  d |= (uint64_t)((H8_SBO >> 4) & 0x3fff) << 32;
-  d |= (uint64_t)1 << 46;
-  return d;
-}
-
-struct H8Task {
-  MatchJob job;
-  int q0, t_begin, ntiles, chunk;
-};
-__device__ __forceinline__ H8Task h8_decode(const MatchJob* jobs, const int* tile_prefix, int njobs, int task) {
-  int lo = 0, hi = njobs - 1;
-  while (lo < hi) {
-    const int mid = (lo + hi + 1) >> 1;
-    if (tile_prefix[mid] <= task) lo = mid; else hi = mid - 1;
-  }
-  H8Task t;
-  t.job = jobs[lo];
-  const int local = task - tile_prefix[lo];
-  const int qtile = local / t.job.nchunks;
-  t.chunk = local % t.job.nchunks;
-  t.q0 = qtile * H8_M;
-  t.t_begin = t.chunk * t.job.chunk_len;
-  const int t_end = min(t.job.nt, t.t_begin + t.job.chunk_len);
-  t.ntiles = (t_end - t.t_begin + H8_N - 1) / H8_N;
-  return t;
-}
-
-__global__ void __launch_bounds__(TC_THREADS, 1)
-    bf_top2_tc_h8(const MatchJob* __restrict__ jobs, const int* __restrict__ tile_prefix, int njobs, int ntasks,
-                  Top2* __restrict__ partial, int* __restrict__ err_flag) {
-  extern __shared__ __align__(1024) uint8_t smem[];
-  __shared__ __align__(8) uint64_t bar_qfull, bar_qempty, bar_full[H8_STAGES], bar_empty[H8_STAGES], bar_accfull[2],
-      bar_accempty[2];
-  __shared__ uint32_t tmem_base_smem;
-  __shared__ float4 merge_buf[H8_M];
-  uint8_t* q_smem = smem;
-  uint8_t* t_smem[H8_STAGES];
-#pragma unroll
-  for (int st = 0; st < H8_STAGES; ++st) t_smem[st] = smem + H8_Q_BYTES + st * H8_T_BYTES;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-
-  if (threadIdx.x == 0) {
-    mbar_init(&bar_qfull, 1);
-    mbar_init(&bar_qempty, 1);
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&bar_accfull[i], 1);
-      mbar_init(&bar_accempty[i], TC_EPI_WARPS);
-    }
-    for (int i = 0; i < H8_STAGES; ++i) {
-      mbar_init(&bar_full[i], 1);
-      mbar_init(&bar_empty[i], 1);
-    }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 256;" ::"r"(smem_u32(&tmem_base_smem))
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = tmem_base_smem;
-
-  if (warp == 0) {
-    if (lane == 0) {
-      int stage = 0, ph = 0, n = 0;
-      for (int task = blockIdx.x; task < ntasks; task += gridDim.x, ++n) {
-        const H8Task t = h8_decode(jobs, tile_prefix, njobs, task);
-        mbar_wait(&bar_qempty, (n & 1) ^ 1, err_flag);
-        mbar_expect_tx(&bar_qfull, H8_Q_BYTES);
-        bulk_copy_g2s(q_smem, reinterpret_cast<const uint8_t*>(t.job.q_tc) + (size_t)t.q0 * H8_ROW_BYTES, H8_Q_BYTES, &bar_qfull);
-        for (int i = 0; i < t.ntiles; ++i) {
-          mbar_wait(&bar_empty[stage], ph ^ 1, err_flag);
-          mbar_expect_tx(&bar_full[stage], H8_T_BYTES);
-          bulk_copy_g2s(t_smem[stage],
-                        reinterpret_cast<const uint8_t*>(t.job.t_tc) + (size_t)(t.t_begin + i * H8_N) * H8_ROW_BYTES,
-                        H8_T_BYTES, &bar_full[stage]);
-          if (++stage == H8_STAGES) { stage = 0; ph ^= 1; }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      int stage = 0, ph = 0, n = 0, tilecount = 0;
-      for (int task = blockIdx.x; task < ntasks; task += gridDim.x, ++n) {
-        const H8Task t = h8_decode(jobs, tile_prefix, njobs, task);
-        mbar_wait(&bar_qfull, n & 1, err_flag);
-        const uint64_t adesc0 = h8_smem_desc(smem_u32(q_smem));
-        for (int i = 0; i < t.ntiles; ++i, ++tilecount) {
-          const int a = tilecount & 1, aph = (tilecount >> 1) & 1;
-          mbar_wait(&bar_accempty[a], aph ^ 1, err_flag);
-          mbar_wait(&bar_full[stage], ph, err_flag);
-          tc_fence_after();
-          const uint64_t bdesc0 = h8_smem_desc(smem_u32(t_smem[stage]));
-          const uint32_t d_tmem = tmem_base + (uint32_t)a * H8_N;
-#pragma unroll
-          for (int k = 0; k < H8_ROW_BYTES / 32; ++k) {
-            // one UMMA_K = 32 fp8 = two core matrices = 256 bytes along K
-            const uint64_t koff = (uint64_t)((k * 2 * TC_LBO) >> 4);
-            tc_mma_f8(d_tmem, adesc0 + koff, bdesc0 + koff, H8_IDESC, k > 0 ? 1u : 0u);
-          }
-          tc_commit(&bar_empty[stage]);
-          tc_commit(&bar_accfull[a]);
-          if (++stage == H8_STAGES) { stage = 0; ph ^= 1; }
-        }
-        tc_commit(&bar_qempty);
-      }
-    }
-  } else {
-    const int quarter = warp & 3;
-    const int half = (warp - 2) >> 2;          // column half of the 128-wide tile
-    const int row_in_tile = quarter * 32 + lane;
-    int tilecount = 0;
-    for (int task = blockIdx.x; task < ntasks; task += gridDim.x) {
-      const H8Task t = h8_decode(jobs, tile_prefix, njobs, task);
-      const int gq = t.q0 + row_in_tile;
-      const float nbits = (float)(t.job.dim * 8);
-      RowState st;
-      st.q1 = st.q2 = __builtin_huge_valf();
-      st.i1 = st.i2 = -1;
-      for (int i = 0; i < t.ntiles; ++i, ++tilecount) {
-        const int a = tilecount & 1, aph = (tilecount >> 1) & 1;
-        mbar_wait(&bar_accfull[a], aph, err_flag);
-        tc_fence_after();
-        const uint32_t taddr = tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)a * H8_N + (uint32_t)half * 64;
-        const int col_base = t.t_begin + i * H8_N + half * 64;
-        uint32_t va[64];
-        OSFM_TMEM_LD64(taddr, va);
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&bar_accempty[a]);
-        row_consume16<0, 64, false>(st, va, col_base, 0u);
-        row_consume16<16, 64, false>(st, va, col_base + 16, 0u);
-        row_consume16<32, 64, false>(st, va, col_base + 32, 0u);
-        row_consume16<48, 64, false>(st, va, col_base + 48, 0u);
-      }
-      // merge the two column halves of a row (lexicographic (distance, index), like cv2's insertion order)
-      if (half == 1) merge_buf[row_in_tile] = make_float4(st.q1, __int_as_float(st.i1), st.q2, __int_as_float(st.i2));
-      asm volatile("bar.sync 1, %0;" ::"r"(32 * TC_EPI_WARPS) : "memory");
-      if (half == 0) {
-        const float4 o = merge_buf[row_in_tile];
-        Top2 a2, b2;
-        a2.s1 = st.q1; a2.i1 = st.i1; a2.s2 = st.q2; a2.i2 = st.i2;
-        b2.s1 = o.x; b2.i1 = __float_as_int(o.y); b2.s2 = o.z; b2.i2 = __float_as_int(o.w);
-        top2_merge(a2, b2);
-        if (gq < t.job.nq) {
-          Top2 out;   // accumulator = 2 H - nbits  ->  the Hamming distance cv2 reports (an integer as float)
-          out.s1 = a2.i1 >= 0 ? (a2.s1 + nbits) * 0.5f : __builtin_huge_valf();
-          out.i1 = a2.i1;
-          out.s2 = a2.i2 >= 0 ? (a2.s2 + nbits) * 0.5f : __builtin_huge_valf();
-          out.i2 = a2.i2;
-          partial[t.job.partial_off + (size_t)t.chunk * t.job.nq + gq] = out;
-        }
-      }
-      asm volatile("bar.sync 1, %0;" ::"r"(32 * TC_EPI_WARPS) : "memory");
-    }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 256;" ::"r"(tmem_base) : "memory");
-  }
+template <int KIND, bool MASKED>
+static void launch_wg(Matcher& m, int njobs, int ntasks) {
+  m.d_flags.reserve(4);
+  OSFM_CUDA(cudaMemsetAsync(m.d_flags.p + 1, 0, sizeof(int), m.stream));
+  const int grid = std::min(ntasks, m.num_sms);
+  bf_top2_wg<KIND, MASKED><<<grid, WG_THREADS, WgGeom<KIND>::SMEM, m.stream>>>(m.d_jobs.p, m.d_prefix.p, njobs, ntasks,
+                                                                             m.d_partial.p, m.d_flags.p + 1);
+  OSFM_LAUNCH_CHECK();
 }
 
 void launch_tc_h8(Matcher& m, int njobs, int ntasks) {
   if (!m.h8_attr_set) {
-    OSFM_CUDA(cudaFuncSetAttribute(bf_top2_tc_h8, cudaFuncAttributeMaxDynamicSharedMemorySize, H8_SMEM));
+    OSFM_CUDA(cudaFuncSetAttribute(bf_top2_wg<KIND_HAMMING, false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                   WgGeom<KIND_HAMMING>::SMEM));
     m.h8_attr_set = true;
   }
-  m.d_flags.reserve(4);
-  OSFM_CUDA(cudaMemsetAsync(m.d_flags.p + 1, 0, sizeof(int), m.stream));
-  const int grid = std::min(ntasks, m.num_sms);
-  bf_top2_tc_h8<<<grid, TC_THREADS, H8_SMEM, m.stream>>>(m.d_jobs.p, m.d_prefix.p, njobs, ntasks, m.d_partial.p, m.d_flags.p + 1);
-  OSFM_LAUNCH_CHECK();
+  launch_wg<KIND_HAMMING, false>(m, njobs, ntasks);
 }
 
 void launch_tc(Matcher& m, int njobs, int ntasks, bool masked) {
   if (!m.tc_attr_set) {   // per matcher (= per device)
-    OSFM_CUDA(cudaFuncSetAttribute(bf_top2_tc<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM));
-    OSFM_CUDA(cudaFuncSetAttribute(bf_top2_tc<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM));
+    OSFM_CUDA(cudaFuncSetAttribute(bf_top2_wg<KIND_L2, false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                   WgGeom<KIND_L2>::SMEM));
+    OSFM_CUDA(cudaFuncSetAttribute(bf_top2_wg<KIND_L2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                   WgGeom<KIND_L2>::SMEM));
     m.tc_attr_set = true;
   }
-  m.d_flags.reserve(4);
-  OSFM_CUDA(cudaMemsetAsync(m.d_flags.p + 1, 0, sizeof(int), m.stream));
-  const int grid = std::min(ntasks, m.num_sms);
   if (masked)
-    bf_top2_tc<true><<<grid, TC_THREADS, TC_SMEM, m.stream>>>(m.d_jobs.p, m.d_prefix.p, njobs, ntasks, m.d_partial.p,
-                                                             m.d_flags.p + 1);
+    launch_wg<KIND_L2, true>(m, njobs, ntasks);
   else
-    bf_top2_tc<false><<<grid, TC_THREADS, TC_SMEM, m.stream>>>(m.d_jobs.p, m.d_prefix.p, njobs, ntasks, m.d_partial.p,
-                                                              m.d_flags.p + 1);
-  OSFM_LAUNCH_CHECK();
+    launch_wg<KIND_L2, false>(m, njobs, ntasks);
 }
 
 }  // namespace osfm

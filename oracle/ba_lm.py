@@ -7,7 +7,7 @@ with the options the reference sets (linear solver SPARSE_SCHUR -> exact Schur
 elimination of the points + Cholesky of the reduced camera system,
 `max_num_iterations`, everything else Ceres defaults).
 
-Ceres Solver is a third-party dependency that is NOT under /root/reference
+Ceres Solver is a third-party dependency that is NOT in the OpenSfM tree
 (pinned: conda `ceres-solver=2.1`, conda.yml:10; Docker ubuntu24 libceres-dev
 2.2.0).  Its published algorithm (Ceres docs "Solving non-linear least squares"
 / trust_region_minimizer.cc / levenberg_marquardt_strategy.cc, summarised in

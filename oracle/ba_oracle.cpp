@@ -5,7 +5,7 @@
 // drives: robustified linearisation, normal-equation blocks, Schur complement
 // on the points, back-substitution, model cost change.  This is the
 // "CPU restatement of the Ceres path (not Ceres)" of BASELINE.md §3: Ceres is
-// a third-party dependency absent from /root/reference (conda ceres-solver 2.1,
+// a third-party dependency absent from the OpenSfM tree (conda ceres-solver 2.1,
 // conda.yml:10); its published algorithm is restated (SURVEY.md §8c box) and
 // anchored on the reference's call sites:
 //   opensfm/src/bundle/src/bundle_adjuster.cc:595-1121 (problem assembly),

@@ -10,7 +10,7 @@ Two checkers for the brute-force matcher:
 
 2. `knn2_numpy` / `match_brute_force_numpy`: a numpy restatement of what
    cv2.BFMatcher.knnMatch(k=2) computes (OpenCV is a third-party dependency not
-   under /root/reference; algorithm restated from its published behaviour,
+   in the OpenSfM tree; algorithm restated from its published behaviour,
    modules/core/src/batch_distance.cpp): for every query the two smallest
    `sqrt(float32 sum of squared differences)` (L2) or integer Hamming counts,
    ties resolved to the lowest train index (stable insertion with strict `<`),

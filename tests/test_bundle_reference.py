@@ -4,7 +4,7 @@ against the CUDA engine.  These are the only vectors the reference holds that pi
 (pose / scale recovery to 1e-6), so they are what ties the oracle's restated Levenberg-Marquardt and its
 secondary residual functors to the reference (SURVEY.md §8c), and the CUDA path to both.
 
-Reference test -> test here (file:line in /root/reference/opensfm/test/test_bundle.py):
+Reference test -> test here (file:line in OpenSfM's opensfm/test/test_bundle.py):
   test_unicode_strings_in_bundle :20-34, test_sigleton :46-72, test_singleton_pan_tilt_roll :75-106,
   test_pair :181-219, test_pair_with_points_priors :222-316, test_pair_non_rigid :319-352,
   test_four_cams_single_reconstruction :355-417, test_four_cams_double_reconstruction :420-500,
