@@ -16,7 +16,7 @@
 //
 // Kernels: ba_linearize (per observation), ba_colnorm_grad, ba_schur (CTA per point:
 // U, g_c, V^-1 and W V^-1 W^T scattered to S with fp64 atomics), ba_finish_system,
-// PCG kernels (block-Jacobi), ba_backsub (warp per point), ba_model_change, ba_update.
+// PCG kernels (block-Jacobi), ba_backsub (warp per point), ba_model_change_alg, ba_update.
 #include <algorithm>
 #include <dlfcn.h>
 
@@ -276,11 +276,10 @@ struct PointPriorView {
   const double* x0;
   const int* global_of;
 };
-// MODE 0: cost.  1: cost + squared column norms + gradient.  2: model cost change.  3: adds J_p^T r to the
-// right-hand side t[3][npf] of the back-substitution.  One thread per local point.
+// MODE 0: cost.  1: cost + squared column norms + gradient.  3: adds J_p^T r to the right-hand side t[3][npf] of
+// the back-substitution.  One thread per local point.
 template <int MODE>
-__global__ void ba_point_prior(PointPriorView pp, BAView v, Params p, const double* __restrict__ scale,
-                               const double* __restrict__ y, double* colnorm2, double* grad, double* t, Scalars* sc) {
+__global__ void ba_point_prior(PointPriorView pp, BAView v, Params p, double* colnorm2, double* grad, double* t, Scalars* sc) {
   const int np = blockIdx.x * blockDim.x + threadIdx.x;
   double acc = 0.0;
   if (np < v.P) {
@@ -295,14 +294,13 @@ __global__ void ba_point_prior(PointPriorView pp, BAView v, Params p, const doub
         const int col = v.nc + 3 * pf + j;
         if (MODE <= 1) acc += 0.5 * r * r;
         if (MODE == 1) { colnorm2[col] += d * d; grad[col] += d * r; }   // only this thread touches the point's columns here
-        if (MODE == 2) { const double m = -d * scale[col] * y[col]; acc += -m * (r + 0.5 * m); }
         if (MODE == 3) t[(size_t)j * v.npf + pf] += d * r;
       }
     }
   }
-  if (MODE <= 2) {
+  if (MODE <= 1) {
     const double tot = block_reduce_sum(acc);
-    if (threadIdx.x == 0 && tot != 0.0) atomicAdd(MODE == 2 ? &sc->model_change : &sc->cost, tot);
+    if (threadIdx.x == 0 && tot != 0.0) atomicAdd(&sc->cost, tot);
   }
 }
 
@@ -728,46 +726,6 @@ __global__ void __launch_bounds__(256) ba_backsub_points(BAView v, const double*
   y[nc + 3 * pf + 2] = c * t0 + e * t1 + f * t2;
 }
 
-// Ceres: model_cost_change = -sum m (r + m/2), m = Js step ; step = -y
-__global__ void __launch_bounds__(256) ba_model_change(BAView v, const double* __restrict__ scale,
-                                                       const double* __restrict__ y, Scalars* sc) {
-  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  double tot = 0.0;
-  if (i < v.N) {
-    const size_t N = (size_t)v.N;
-    const int nc = v.nc, wc = v.wc;
-    const ObsCols oc = obs_cols(v, i);
-    const int pf = v.pt_poff[v.obs_point[i]];
-    for (int q = 0; q < v.nres; ++q) {
-      double m = 0.0;
-      for (int j = 0; j < wc; ++j) {
-        const int g = oc.col(j);
-        if (g >= 0) m -= v.Jc[((size_t)q * wc + j) * N + i] * scale[g] * y[g];
-      }
-      if (pf >= 0) {
-#pragma unroll
-        for (int j = 0; j < 3; ++j) m -= v.Jp[((size_t)q * 3 + j) * N + i] * scale[nc + 3 * pf + j] * y[nc + 3 * pf + j];
-      }
-      tot += -m * (v.r[q * N + i] + 0.5 * m);
-    }
-  }
-  const double t = block_reduce_sum(tot);
-  if (threadIdx.x == 0 && t != 0.0) atomicAdd(&sc->model_change, t);
-}
-__global__ void ba_prior_model_change(PriorView pv, Params p, const double* scale, const double* y, Scalars* sc) {
-  const int row = blockIdx.x * blockDim.x + threadIdx.x;
-  double tot = 0.0;
-  if (row < pv.n_cam_rows + pv.n_pos_rows) {
-    double r, d;
-    int col;
-    prior_row(pv, p, row, &r, &col, &d);
-    const double m = -d * scale[col] * y[col];
-    tot = -m * (r + 0.5 * m);
-  }
-  const double t = block_reduce_sum(tot);
-  if (threadIdx.x == 0 && t != 0.0) atomicAdd(&sc->model_change, t);
-}
-
 // candidate = x - scale * y ; accumulates |delta|^2 and |x|^2 (free parameters only).
 // which: 0 cameras, 1 instances, 2 rig cameras, 3 points.
 __global__ void ba_update(int which, int count, const int* __restrict__ poff, const int* __restrict__ off,
@@ -819,8 +777,7 @@ __global__ void ba_grad_dot(int n, int nc, int cam_side, const double* __restric
 // from J step; the step solves (H + D) step = -g (D = LM diagonal / radius), so H step = -g - D step and
 //   model_cost_change = (y^T g_s + y^T D y) / 2,   step = -y, g_s = scale * grad   (scaled variables)
 // exactly when the linear system is solved exactly, and to the solver's 1e-8 relative residual here (every term of H
-// and g -- observations, priors, side terms -- is in the system that was solved).  Replaces ba_model_change +
-// ba_prior_model_change + side_model_change + ba_point_prior<2>: 447 MB of plane reads per LM iteration.
+// and g -- observations, priors, side terms -- is in the system that was solved).
 __global__ void ba_model_change_alg(int n, int nc, int cam_side, const double* __restrict__ grad, const double* __restrict__ scale,
                                     const double* __restrict__ diag, double inv_radius, const double* __restrict__ y, Scalars* sc) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -1072,14 +1029,18 @@ struct BA {
   void run();
 };
 
-constexpr int LIN_NB_DEFAULT = 3;
 static int grid_for(long long n, int threads) { return (int)std::max<long long>(1, (n + threads - 1) / threads); }
+// the OSFM_BA_* switches: whether environment variable `name` is set and starts with `c`
+static bool env_starts_with(const char* name, char c) {
+  const char* e = getenv(name);
+  return e && e[0] == c;
+}
 
 void BA::run() {
   OSFM_CUDA(cudaSetDevice(device));
   const auto t_start = std::chrono::high_resolution_clock::now();
   // OSFM_BA_TRACE=1: host wall-clock per phase of run() on stderr (diagnostics only)
-  static const bool trace_on = []() { const char* e = getenv("OSFM_BA_TRACE"); return e && e[0] == '1'; }();
+  static const bool trace_on = env_starts_with("OSFM_BA_TRACE", '1');
   auto t_prev = t_start;
   ar_trace = trace_on; ar_calls = 0; ar_host_ms = 0.0; ar_dev_ms = 0.0;
   auto trace = [&](const char* what) {
@@ -1212,11 +1173,9 @@ void BA::run() {
   // The segmented Schur path (ba_point_blocks + ba_obs_rows + ba_schur_seg) is the default: points seen by the same
   // shots share their camera-side rows, which the per-point kernel re-reads point by point.
   // OSFM_BA_SEGMENT_SCHUR=0 forces every point through ba_schur (kept for A/B runs and tests).
-  static const bool use_seg = []() { const char* e = getenv("OSFM_BA_SEGMENT_SCHUR"); return !(e && e[0] == '0'); }();
-  // register budget of ba_linearize<1> (A/B switch): 3, 4 or 5 resident CTAs per SM
-  static const int lin_nb = []() { const char* e = getenv("OSFM_BA_LIN_NB"); return e ? atoi(e) : LIN_NB_DEFAULT; }();
+  static const bool use_seg = !env_starts_with("OSFM_BA_SEGMENT_SCHUR", '0');
   // one projection type for all cameras and no rig-camera shots -> specialised linearisation kernels
-  static const bool lin_special = []() { const char* e = getenv("OSFM_BA_LIN_SPECIAL"); return !(e && e[0] == '0'); }();
+  static const bool lin_special = !env_starts_with("OSFM_BA_LIN_SPECIAL", '0');
   int uniform_type = -1;
   if (lin_special && K > 0) {
     uniform_type = cam_type[0];
@@ -1488,7 +1447,7 @@ void BA::run() {
       OSFM_LAUNCH_CHECK();
     }
     if (have_pp && P > 0) {
-      ba_point_prior<0><<<grid_for(P, 128), 128, 0, stream>>>(ppv, v, params_of(b), nullptr, nullptr, nullptr, nullptr, nullptr, d_sc.p);
+      ba_point_prior<0><<<grid_for(P, 128), 128, 0, stream>>>(ppv, v, params_of(b), nullptr, nullptr, nullptr, d_sc.p);
       OSFM_LAUNCH_CHECK();
     }
     allreduce_dev(&d_sc.p->cost, 1);
@@ -1504,17 +1463,13 @@ void BA::run() {
       if (uniform_type == PT_PERSPECTIVE) ba_linearize<1, 5, PT_PERSPECTIVE><<<grid_for(N, 128), 128, 0, stream>>>(v, params_of(b), d_sc.p, nullptr);
       else if (uniform_type == PT_BROWN) ba_linearize<1, 4, PT_BROWN><<<grid_for(N, 128), 128, 0, stream>>>(v, params_of(b), d_sc.p, nullptr);
       else if (uniform_type == PT_FISHEYE) ba_linearize<1, 5, PT_FISHEYE><<<grid_for(N, 128), 128, 0, stream>>>(v, params_of(b), d_sc.p, nullptr);
-      else if (lin_nb == 5) ba_linearize<1, 5><<<grid_for(N, 128), 128, 0, stream>>>(v, params_of(b), d_sc.p, nullptr);
-      else if (lin_nb == 4) ba_linearize<1, 4><<<grid_for(N, 128), 128, 0, stream>>>(v, params_of(b), d_sc.p, nullptr);
       else ba_linearize<1, 3><<<grid_for(N, 128), 128, 0, stream>>>(v, params_of(b), d_sc.p, nullptr);
       OSFM_LAUNCH_CHECK();
       tm_lin.stop(stream);
       ba_colnorm_grad_points<<<grid_for(N, 256), 256, 0, stream>>>(v, d_colnorm2.p, d_grad.p);
       OSFM_LAUNCH_CHECK();
       if (nseg > 0) {
-        // OSFM_BA_COLNORM_TMA=0: the shuffle kernel instead of the bulk-copy staged one (A/B switch)
-        static const bool use_tma = []() { const char* e = getenv("OSFM_BA_COLNORM_TMA"); return !(e && e[0] == '0'); }();
-        if (wc == 9 && nres == 2 && use_tma && have_seg_tab && sp_nchunks > 0) {
+        if (wc == 9 && nres == 2 && have_seg_tab && sp_nchunks > 0) {
           // chunk list + segment tables exist (every call but the first of a run): no dependent index loads
           if (!cc_attr) {
             OSFM_CUDA(cudaFuncSetAttribute(ba_colnorm_grad_chunks, cudaFuncAttributeMaxDynamicSharedMemorySize, CC_SMEM));
@@ -1522,7 +1477,7 @@ void BA::run() {
           }
           const int grid = std::max(1, std::min(num_sms, (sp_nchunks + CC_WARPS - 1) / CC_WARPS));
           ba_colnorm_grad_chunks<<<grid, 32 * CC_WARPS, CC_SMEM, stream>>>(v, d_sp_chunks.p, sp_nchunks, d_tab.p, d_colnorm2.p, d_grad.p);
-        } else if (wc == 9 && nres == 2 && use_tma) {
+        } else if (wc == 9 && nres == 2) {
           if (!cg_attr) {
             OSFM_CUDA(cudaFuncSetAttribute(ba_colnorm_grad_tma, cudaFuncAttributeMaxDynamicSharedMemorySize, CG_SMEM));
             cg_attr = true;
@@ -1556,7 +1511,7 @@ void BA::run() {
       }
     }
     if (have_pp && P > 0) {
-      ba_point_prior<1><<<grid_for(P, 128), 128, 0, stream>>>(ppv, v, params_of(b), nullptr, nullptr, d_colnorm2.p, d_grad.p, nullptr, d_sc.p);
+      ba_point_prior<1><<<grid_for(P, 128), 128, 0, stream>>>(ppv, v, params_of(b), d_colnorm2.p, d_grad.p, nullptr, d_sc.p);
       OSFM_LAUNCH_CHECK();
     }
     if (world > 1) {
@@ -1731,7 +1686,7 @@ void BA::run() {
       auto up16 = [](long long x) { return (x + 15) / 16 * 16; };
       const long long off_S = up16(8LL * nc), off_cols = off_S + up16(8 * ent_max), off_rows = off_cols + up16(2 * col_max);
       const long long total = off_rows + 12LL * rows_max;
-      static const bool allow_res = []() { const char* e = getenv("OSFM_BA_PCG_RESIDENT"); return !(e && e[0] == '0'); }();
+      static const bool allow_res = !env_starts_with("OSFM_BA_PCG_RESIDENT", '0');
       int max_smem = 0;
       OSFM_CUDA(cudaDeviceGetAttribute(&max_smem, cudaDevAttrMaxSharedMemoryPerBlockOptin, device));
       pcg_resident = allow_res && monotone && nc <= 65535 && total + 1024 <= max_smem;
@@ -1787,7 +1742,7 @@ void BA::run() {
       const long long total = off_defl + 2LL * PCG_ND * 8 * rows_max + 8LL * PCG_NW * G + 8LL * PCG_NW * rows_max;
       cudaFuncAttributes pipe_attr{};
       OSFM_CUDA(cudaFuncGetAttributes(&pipe_attr, pcg_pipelined));
-      static const bool allow_pipe = []() { const char* e = getenv("OSFM_BA_PCG_PIPELINED"); return !(e && e[0] == '0'); }();
+      static const bool allow_pipe = !env_starts_with("OSFM_BA_PCG_PIPELINED", '0');
       int max_smem = 0;
       OSFM_CUDA(cudaDeviceGetAttribute(&max_smem, cudaDevAttrMaxSharedMemoryPerBlockOptin, device));
       pcg_pipe_ok = allow_pipe && nc <= 65535 && rows_max <= PCG_THREADS && ent_max < (1LL << 30) &&
@@ -1800,10 +1755,6 @@ void BA::run() {
         pcg_pipe.off_vec = (int)off_vec; pcg_pipe.off_cols = (int)off_cols; pcg_pipe.off_rows = (int)off_rows;
         pcg_pipe.max_rows = rows_max; pcg_pipe.max_groups = grp_max; pcg_pipe.max_cols = (int)col_max;
         pcg_pipe.off_defl = (int)off_defl; pcg_pipe.Wdef = nullptr;
-        // 128-bit barrier words (value + generation in one strong 16-byte access): measured slower than flags + slots
-        // on the previous target GPU and not re-measured on H100, so it stays opt-in: OSFM_BA_PCG_B128=1
-        static const bool allow_b128 = []() { const char* e = getenv("OSFM_BA_PCG_B128"); return e && e[0] == '1'; }();
-        pcg_pipe.b128 = (allow_b128 && pcg_grid <= PCG_B128_GROUP && PCG_THREADS >= 3 * PCG_B128_GROUP) ? 1 : 0;
         OSFM_CUDA(cudaFuncSetAttribute(pcg_pipelined, cudaFuncAttributeMaxDynamicSharedMemorySize, pcg_pipe_smem));
       }
     }
@@ -1844,9 +1795,9 @@ void BA::run() {
     OSFM_LAUNCH_CHECK();
   }
   // deflation vectors of the reduced solve: the similarity gauge at the initial poses, in the scaled variables
-  static const bool deflate_on = []() { const char* e = getenv("OSFM_BA_PCG_DEFLATE"); return !(e && e[0] == '0'); }();
+  static const bool deflate_on = !env_starts_with("OSFM_BA_PCG_DEFLATE", '0');
   pcg_pipe.Wdef = nullptr;
-  if (deflate_on && pcg_pipe_ok && !pcg_pipe.b128 && NI > 0 && nc > 0) {
+  if (deflate_on && pcg_pipe_ok && NI > 0 && nc > 0) {
     d_Wdef.reserve((size_t)PCG_ND * nc);
     OSFM_CUDA(cudaMemsetAsync(d_Wdef.p, 0, sizeof(double) * PCG_ND * (size_t)nc, stream));
     pcg_gauge_vectors<<<grid_for(NI, 128), 128, 0, stream>>>(NI, d_inst_poff.p, params_of(cur).inst, d_scale.p, nc, d_Wdef.p);
@@ -1854,7 +1805,7 @@ void BA::run() {
     pcg_pipe.Wdef = d_Wdef.p;
   }
   // per-segment tables of the tensor-core Schur kernel (columns, block offsets, Jacobi scales): constant from here on
-  static const bool mma_on = []() { const char* e = getenv("OSFM_BA_SCHUR_MMA"); return !(e && e[0] == '0'); }();
+  static const bool mma_on = !env_starts_with("OSFM_BA_SCHUR_MMA", '0');
   // The tensor-core kernels add the same-shot blocks J^T J only in the tiles (t, t) and (t, t + 1): a shot's wc
   // columns must not span three 8-wide tiles, i.e. wc <= 9.  Wider camera sides (Brown: 9 + 6, rig cameras: + 6)
   // use the SIMT segment kernels.
@@ -1879,7 +1830,7 @@ void BA::run() {
     OSFM_LAUNCH_CHECK();
     have_seg_tab = true;
     // chunk list of the persistent Schur kernel (ba_schur_pipe.cuh)
-    static const bool pipe_on = []() { const char* e = getenv("OSFM_BA_SCHUR_PIPE"); return !(e && e[0] == '0'); }();
+    static const bool pipe_on = !env_starts_with("OSFM_BA_SCHUR_PIPE", '0');
     // (the flush table holds offset << 2: the reduced system must stay below 2^29 doubles; 20 KB of table per segment)
     use_pipe = pipe_on && v.nres * (wc + 4) <= SP_ROWS && s_upper_total + (long long)nc_pad < (1LL << 29) &&
                (long long)nseg * SP_FT_SEG * (long long)sizeof(int) <= (8LL << 30);
@@ -2110,7 +2061,7 @@ void BA::run() {
         OSFM_LAUNCH_CHECK();
       }
       if (have_pp) {
-        ba_point_prior<3><<<grid_for(P, 128), 128, 0, stream>>>(ppv, v, params_of(cur), nullptr, nullptr, nullptr, nullptr, d_bs_t.p, d_sc.p);
+        ba_point_prior<3><<<grid_for(P, 128), 128, 0, stream>>>(ppv, v, params_of(cur), nullptr, nullptr, d_bs_t.p, d_sc.p);
         OSFM_LAUNCH_CHECK();
       }
       ba_backsub_points<<<grid_for(npf, 256), 256, 0, stream>>>(v, d_scale.p, d_Vinv.p, d_bs_t.p, d_y.p);
@@ -2118,29 +2069,9 @@ void BA::run() {
       tm_back.stop(stream);
     }
     OSFM_CUDA(cudaMemsetAsync(&d_sc.p->model_change, 0, sizeof(double) * 3, stream));  // model_change, step_norm2, x_norm2
-    static const bool mc_explicit = []() { const char* e = getenv("OSFM_BA_MODEL_CHANGE_EXPLICIT"); return e && e[0] == '1'; }();
-    if (!mc_explicit) {
-      if (n > 0) {
-        ba_model_change_alg<<<grid_for(n, 256), 256, 0, stream>>>(n, nc, rank == 0, d_grad.p, d_scale.p, d_diag.p, inv_radius, d_y.p, d_sc.p);
-        OSFM_LAUNCH_CHECK();
-      }
-    } else {
-    if (N > 0) {
-      ba_model_change<<<grid_for(N, 256), 256, 0, stream>>>(v, d_scale.p, d_y.p, d_sc.p);
+    if (n > 0) {
+      ba_model_change_alg<<<grid_for(n, 256), 256, 0, stream>>>(n, nc, rank == 0, d_grad.p, d_scale.p, d_diag.p, inv_radius, d_y.p, d_sc.p);
       OSFM_LAUNCH_CHECK();
-    }
-    if (npr_local > 0) {
-      ba_prior_model_change<<<grid_for(npr_local, 128), 128, 0, stream>>>(pv, params_of(cur), d_scale.p, d_y.p, d_sc.p);
-      OSFM_LAUNCH_CHECK();
-    }
-    if (NT > 0 && add_priors) {
-      side_model_change<<<grid_for(NT, 128), 128, 0, stream>>>(sv, v, bm, params_of(cur), d_scale.p, d_y.p, d_sc.p);
-      OSFM_LAUNCH_CHECK();
-    }
-    if (have_pp && P > 0) {
-      ba_point_prior<2><<<grid_for(P, 128), 128, 0, stream>>>(ppv, v, params_of(cur), d_scale.p, d_y.p, nullptr, nullptr, nullptr, d_sc.p);
-      OSFM_LAUNCH_CHECK();
-    }
     }
     // --- candidate point ---
     const int cand = cur ^ 1;

@@ -1209,12 +1209,6 @@ __global__ void pcg_factor_groups(const double* __restrict__ Sval, BsrView h, co
 
 constexpr int PCG_MAX_CTAS = 256;
 constexpr int PCG_FLAG_STRIDE = 32;
-// Barrier word of the 128-bit variant: a partial sum and the generation it belongs to travel together, so a
-// reader that sees the generation also has the value (one L2 round trip less than flag + slot).
-struct alignas(16) PcgWord {
-  double v;
-  unsigned long long tag;
-};
 struct PcgState {
   // header: what the host reads back after a solve
   int iterations;
@@ -1228,8 +1222,6 @@ struct PcgState {
   // per-CTA arrival generation, one 128-byte line each (packed flags contend for one line on
   // every arrival; one line per CTA does not)
   unsigned flags[PCG_MAX_CTAS * PCG_FLAG_STRIDE];
-  // 128-bit barrier words (value, generation), double-buffered by generation parity: [parity][CTA][3 sums + pad]
-  PcgWord words[2][PCG_MAX_CTAS][4];
 };
 constexpr size_t PCG_STATE_HEADER = offsetof(PcgState, slot);
 
@@ -1242,29 +1234,34 @@ struct PcgResident {
 
 __device__ __forceinline__ double ldcg_d(const double* p) { return __ldcg(p); }
 
-// Grid barrier + all-reduce of two doubles for a fully resident grid (grid <= #SMs, 1 CTA / SM).
+// Grid barrier + all-reduce of NV = 2 or 3 doubles for a fully resident grid (grid <= #SMs, 1 CTA / SM).
 // Every CTA publishes its partial sums in its own slot (double-buffered by generation parity) and
 // release-stores its flag; every CTA then polls all flags (thread t polls CTA t) and sums the slots
 // in a fixed order, so all CTAs get bit-identical totals and the result does not depend on timing.
-__device__ __forceinline__ void grid_reduce2(PcgState* st, unsigned nblocks, unsigned& gen, double a, double b,
-                                             double& A, double& B, double (*red)[2]) {
+// NV = 2 ignores c and leaves C unwritten: classic PCG reduces two sums, and carrying a third costs it registers.
+template <int NV>
+__device__ __forceinline__ void grid_reduce(PcgState* st, unsigned nblocks, unsigned& gen, double a, double b, double c,
+                                            double& A, double& B, double& C, double (*red)[3]) {
+  static_assert(NV == 2 || NV == 3, "two or three sums");
   ++gen;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
 #pragma unroll
   for (int o = 16; o; o >>= 1) {
     a += __shfl_xor_sync(0xffffffffu, a, o);
     b += __shfl_xor_sync(0xffffffffu, b, o);
+    if (NV == 3) c += __shfl_xor_sync(0xffffffffu, c, o);
   }
-  if (lane == 0) { red[warp][0] = a; red[warp][1] = b; }
+  if (lane == 0) { red[warp][0] = a; red[warp][1] = b; if (NV == 3) red[warp][2] = c; }
   __syncthreads();  // also: every global write of this CTA happens-before thread 0's release below
   if (threadIdx.x == 0) {
-    double sa = 0.0, sb = 0.0;
-    for (int w = 0; w < nwarps; ++w) { sa += red[w][0]; sb += red[w][1]; }
-    __stcg(&st->slot[gen & 1][blockIdx.x][0], sa);
-    __stcg(&st->slot[gen & 1][blockIdx.x][1], sb);
+    double sa = 0.0, sb = 0.0, sc = 0.0;
+    for (int w = 0; w < nwarps; ++w) { sa += red[w][0]; sb += red[w][1]; if (NV == 3) sc += red[w][2]; }
+    double* sl = st->slot[gen & 1][blockIdx.x];
+    __stcg(reinterpret_cast<double2*>(sl), make_double2(sa, sb));
+    if (NV == 3) __stcg(sl + 2, sc);
     asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(&st->flags[blockIdx.x * PCG_FLAG_STRIDE]), "r"(gen) : "memory");
   }
-  double va = 0.0, vb = 0.0;
+  double va = 0.0, vb = 0.0, vc = 0.0;
   if (threadIdx.x < nblocks) {
     const long long t0 = clock64();
     unsigned cur;
@@ -1272,21 +1269,25 @@ __device__ __forceinline__ void grid_reduce2(PcgState* st, unsigned nblocks, uns
       asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(cur) : "l"(&st->flags[threadIdx.x * PCG_FLAG_STRIDE]) : "memory");
       if (clock64() - t0 > 8000000000LL) __trap();  // a protocol bug must not hang the GPU
     } while ((int)(cur - gen) < 0);  // monotonic: a fast CTA may already have published generation gen + 1
-    va = ldcg_d(&st->slot[gen & 1][threadIdx.x][0]);
-    vb = ldcg_d(&st->slot[gen & 1][threadIdx.x][1]);
+    const double* sl = st->slot[gen & 1][threadIdx.x];
+    const double2 ab = __ldcg(reinterpret_cast<const double2*>(sl));
+    va = ab.x; vb = ab.y;
+    if (NV == 3) vc = __ldcg(sl + 2);
   }
   __syncthreads();  // red[] is free again; the acquires above order every thread's later loads
 #pragma unroll
   for (int o = 16; o; o >>= 1) {
     va += __shfl_xor_sync(0xffffffffu, va, o);
     vb += __shfl_xor_sync(0xffffffffu, vb, o);
+    if (NV == 3) vc += __shfl_xor_sync(0xffffffffu, vc, o);
   }
-  if (lane == 0) { red[warp][0] = va; red[warp][1] = vb; }
+  if (lane == 0) { red[warp][0] = va; red[warp][1] = vb; if (NV == 3) red[warp][2] = vc; }
   __syncthreads();
-  double sa = 0.0, sb = 0.0;
+  double sa = 0.0, sb = 0.0, sc = 0.0;
   const int wmax = (int)((nblocks + 31) >> 5);
-  for (int w = 0; w < wmax; ++w) { sa += red[w][0]; sb += red[w][1]; }
+  for (int w = 0; w < wmax; ++w) { sa += red[w][0]; sb += red[w][1]; if (NV == 3) sc += red[w][2]; }
   A = sa; B = sb;
+  if (NV == 3) C = sc;
   __syncthreads();
 }
 
@@ -1315,7 +1316,7 @@ __global__ void __launch_bounds__(PCG_THREADS, 1)
                    const double* __restrict__ rhs, double* x, double* r, double* z, double* p0, double* p1, double* Ap,
                    PcgState* st, int nc, int max_iter, double tol2_rel, PcgResident R) {
   extern __shared__ __align__(16) unsigned char pcg_smem[];
-  __shared__ double red[PCG_THREADS / 32][2];
+  __shared__ double red[PCG_THREADS / 32][3];
   const int warps_per_cta = blockDim.x >> 5;
   const int warp = threadIdx.x >> 5;
   const int gw = blockIdx.x * warps_per_cta + warp;
@@ -1367,7 +1368,8 @@ __global__ void __launch_bounds__(PCG_THREADS, 1)
       pcg_apply_group(h, L, Minv, g, lane, rn, z, &a_rz, &a_rr, n, o);
       if (lane < n) p0[o] = 0.0;
     }
-    grid_reduce2(st, gridDim.x, bar_gen, a_rz, a_rr, rz_cur, bb, red);
+    double unused;
+    grid_reduce<2>(st, gridDim.x, bar_gen, a_rz, a_rr, 0.0, rz_cur, bb, unused, red);
   }
   const double tol2 = tol2_rel * bb;
   double rr = bb;
@@ -1432,7 +1434,7 @@ __global__ void __launch_bounds__(PCG_THREADS, 1)
       }
       double pAp, unused;
       const long long tk2 = clock64();
-      grid_reduce2(st, gridDim.x, bar_gen, a_pAp, 0.0, pAp, unused, red);
+      grid_reduce<2>(st, gridDim.x, bar_gen, a_pAp, 0.0, 0.0, pAp, unused, unused, red);
       const long long tk3 = clock64();
       // ---- phase B: x += alpha p ; r -= alpha Ap ; z = M^-1 r ; rz_new, rr ----
       const double alpha = rz_cur / pAp;
@@ -1451,7 +1453,7 @@ __global__ void __launch_bounds__(PCG_THREADS, 1)
       }
       double rz_new;
       const long long tk4 = clock64();
-      grid_reduce2(st, gridDim.x, bar_gen, a_rz, a_rr, rz_new, rr, red);
+      grid_reduce<2>(st, gridDim.x, bar_gen, a_rz, a_rr, 0.0, rz_new, rr, unused, red);
       if (blockIdx.x == 0 && threadIdx.x == 0) {
         const long long tk5 = clock64();
         st->prof[0] += tk1 - tk0; st->prof[1] += tk2 - tk1; st->prof[2] += tk3 - tk2; st->prof[3] += tk4 - tk3;
@@ -1487,115 +1489,7 @@ struct PcgPipe {
   const double* Wdef; // [PCG_ND][nc] deflation vectors (scaled variables), or null: plain PCG
   int max_cols;
   int max_rows, max_groups;
-  int b128;   // 1: grid_reduce3_b128 (<= 160 CTAs, >= 480 threads), 0: flags + slots
 };
-
-__device__ __forceinline__ PcgWord ld_acquire_b128(const PcgWord* p) {
-  PcgWord r;
-  unsigned long long lo, hi;
-  asm volatile("{\n.reg .b128 t;\nld.acquire.gpu.global.b128 t, [%2];\nmov.b128 {%0, %1}, t;\n}" : "=l"(lo), "=l"(hi) : "l"(p) : "memory");
-  r.v = __longlong_as_double((long long)lo);
-  r.tag = hi;
-  return r;
-}
-__device__ __forceinline__ void st_release_b128(PcgWord* p, double v, unsigned long long tag) {
-  asm volatile("{\n.reg .b128 t;\nmov.b128 t, {%1, %2};\nst.release.gpu.global.b128 [%0], t;\n}" ::"l"(p),
-               "l"((unsigned long long)__double_as_longlong(v)), "l"(tag)
-               : "memory");
-}
-// grid_reduce3 with 128-bit words (SASS LDG/STG.E.128.STRONG.GPU): threads 0..2 publish the three block sums,
-// thread t polls word t / 160 of CTA t % 160 and gets the value with the generation.  Needs <= 160 CTAs and
-// >= 480 threads; the sums are formed in a fixed order, as in grid_reduce3.
-constexpr int PCG_B128_GROUP = 160;
-__device__ __forceinline__ void grid_reduce3_b128(PcgState* st, unsigned nblocks, unsigned& gen, double a, double b, double c,
-                                                  double& A, double& B, double& C, double (*red)[3]) {
-  ++gen;
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
-#pragma unroll
-  for (int o = 16; o; o >>= 1) {
-    a += __shfl_xor_sync(0xffffffffu, a, o);
-    b += __shfl_xor_sync(0xffffffffu, b, o);
-    c += __shfl_xor_sync(0xffffffffu, c, o);
-  }
-  if (lane == 0) { red[warp][0] = a; red[warp][1] = b; red[warp][2] = c; }
-  __syncthreads();  // also: every global write of this CTA happens-before the releases below
-  if (threadIdx.x < 3) {
-    double sv = 0.0;
-    for (int w = 0; w < nwarps; ++w) sv += red[w][threadIdx.x];
-    st_release_b128(&st->words[gen & 1][blockIdx.x][threadIdx.x], sv, gen);
-  }
-  const int grp = threadIdx.x / PCG_B128_GROUP, idx = threadIdx.x - grp * PCG_B128_GROUP;
-  double val = 0.0;
-  if (grp < 3 && idx < (int)nblocks) {
-    const PcgWord* wp = &st->words[gen & 1][idx][grp];
-    const long long t0 = clock64();
-    PcgWord wv;
-    do {
-      wv = ld_acquire_b128(wp);
-      if (clock64() - t0 > 8000000000LL) __trap();  // a protocol bug must not hang the GPU
-    } while ((long long)(wv.tag - gen) < 0);
-    val = wv.v;
-  }
-  __syncthreads();  // red[] is free again; the acquires above order every thread's later loads
-#pragma unroll
-  for (int o = 16; o; o >>= 1) val += __shfl_xor_sync(0xffffffffu, val, o);
-  if (lane == 0) red[warp][0] = val;
-  __syncthreads();
-  constexpr int WPG = PCG_B128_GROUP / 32;   // warps per group
-  double sa = 0.0, sb = 0.0, sc = 0.0;
-  for (int w = 0; w < WPG; ++w) { sa += red[w][0]; sb += red[WPG + w][0]; sc += red[2 * WPG + w][0]; }
-  A = sa; B = sb; C = sc;
-  __syncthreads();
-}
-
-__device__ __forceinline__ void grid_reduce3(PcgState* st, unsigned nblocks, unsigned& gen, double a, double b, double c,
-                                             double& A, double& B, double& C, double (*red)[3]) {
-  ++gen;
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
-#pragma unroll
-  for (int o = 16; o; o >>= 1) {
-    a += __shfl_xor_sync(0xffffffffu, a, o);
-    b += __shfl_xor_sync(0xffffffffu, b, o);
-    c += __shfl_xor_sync(0xffffffffu, c, o);
-  }
-  if (lane == 0) { red[warp][0] = a; red[warp][1] = b; red[warp][2] = c; }
-  __syncthreads();  // also: every global write of this CTA happens-before thread 0's release below
-  if (threadIdx.x == 0) {
-    double sa = 0.0, sb = 0.0, sc = 0.0;
-    for (int w = 0; w < nwarps; ++w) { sa += red[w][0]; sb += red[w][1]; sc += red[w][2]; }
-    double* sl = st->slot[gen & 1][blockIdx.x];
-    __stcg(reinterpret_cast<double2*>(sl), make_double2(sa, sb));
-    __stcg(sl + 2, sc);
-    asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(&st->flags[blockIdx.x * PCG_FLAG_STRIDE]), "r"(gen) : "memory");
-  }
-  double va = 0.0, vb = 0.0, vc = 0.0;
-  if (threadIdx.x < nblocks) {
-    const long long t0 = clock64();
-    unsigned cur;
-    do {
-      asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(cur) : "l"(&st->flags[threadIdx.x * PCG_FLAG_STRIDE]) : "memory");
-      if (clock64() - t0 > 8000000000LL) __trap();  // a protocol bug must not hang the GPU
-    } while ((int)(cur - gen) < 0);  // monotonic: a fast CTA may already have published generation gen + 1
-    const double* sl = st->slot[gen & 1][threadIdx.x];
-    const double2 ab = __ldcg(reinterpret_cast<const double2*>(sl));
-    va = ab.x; vb = ab.y;
-    vc = __ldcg(sl + 2);
-  }
-  __syncthreads();
-#pragma unroll
-  for (int o = 16; o; o >>= 1) {
-    va += __shfl_xor_sync(0xffffffffu, va, o);
-    vb += __shfl_xor_sync(0xffffffffu, vb, o);
-    vc += __shfl_xor_sync(0xffffffffu, vc, o);
-  }
-  if (lane == 0) { red[warp][0] = va; red[warp][1] = vb; red[warp][2] = vc; }
-  __syncthreads();
-  double sa = 0.0, sb = 0.0, sc = 0.0;
-  const int wmax = (int)((nblocks + 31) >> 5);
-  for (int w = 0; w < wmax; ++w) { sa += red[w][0]; sb += red[w][1]; sc += red[w][2]; }
-  A = sa; B = sb; C = sc;
-  __syncthreads();
-}
 
 // Deflation vectors of the reduced system: the similarity gauge of the rig instances at the current poses.
 // Instance block = [r (camera -> world angle-axis) | t (camera origin)], x_cam = R(-r) (X - t).  Under the world map
@@ -1640,7 +1534,7 @@ __global__ void pcg_gauge_vectors(int NI, const int* __restrict__ inst_poff, con
   }
 }
 
-// The same barrier with PCG_NW doubles per CTA.  Built for latency, the only thing that matters here, and around one
+// The grid_reduce barrier with PCG_NW doubles per CTA.  Built for latency, the only thing that matters here, and around one
 // measurement: arguments and results must not live in local memory -- every poll of the barrier invalidates L1
 // (ld.acquire -> CCTL.IVALL), so a stack array written before the call and read inside it is an L2 round trip (the
 // version with in[] / out[] arrays spent 2.9k + 2.5k clocks per call on that).  Protocol: the owners of the CTA's rows
@@ -1998,8 +1892,7 @@ __global__ void __launch_bounds__(PCG_THREADS, 1)
     coarse();
   } else {
     double d0, d1, d2;
-    if (R.b128) grid_reduce3_b128(st, gridDim.x, bar_gen, 0.0, 0.0, mine ? rr_ * rr_ : 0.0, d0, d1, d2, red);
-    else grid_reduce3(st, gridDim.x, bar_gen, 0.0, 0.0, mine ? rr_ * rr_ : 0.0, d0, d1, d2, red);
+    grid_reduce<3>(st, gridDim.x, bar_gen, 0.0, 0.0, mine ? rr_ * rr_ : 0.0, d0, d1, d2, red);
     bb = d2;
   }
   const double tol2 = tol2_rel * bb;
@@ -2030,11 +1923,8 @@ __global__ void __launch_bounds__(PCG_THREADS, 1)
         grid_reduce_wide(st, gridDim.x, &bar_gen, wide_s, gather_s, inrow_s, nrows);
         gamma = wide_s[0]; delta = wide_s[1]; rr = wide_s[2];
         coarse();
-      } else if (R.b128)
-        grid_reduce3_b128(st, gridDim.x, bar_gen, mine ? rr_ * u : 0.0, mine ? w * u : 0.0, mine ? rr_ * rr_ : 0.0, gamma, delta, rr,
-                   red);
-      else
-        grid_reduce3(st, gridDim.x, bar_gen, mine ? rr_ * u : 0.0, mine ? w * u : 0.0, mine ? rr_ * rr_ : 0.0, gamma, delta, rr,
+      } else
+        grid_reduce<3>(st, gridDim.x, bar_gen, mine ? rr_ * u : 0.0, mine ? w * u : 0.0, mine ? rr_ * rr_ : 0.0, gamma, delta, rr,
                    red);
       const long long tk1 = clock64();
       if (!(rr == rr)) break;
@@ -2094,16 +1984,16 @@ __global__ void __launch_bounds__(PCG_THREADS, 1)
   if (mine) x_out[gi] = xr;
   // The residual above is the recurred one, which drifts from b - S x in pipelined CG: check the true residual of the
   // returned x with one more exchange and mat-vec, and hand the solve to the classic kernel if it is not what was claimed.
-  if (converged && bb > 0.0 && !R.b128) {
+  if (converged && bb > 0.0) {
     if (mine) mbuf[0][gi] = xr;
     double d0, d1, d2;
-    grid_reduce3(st, gridDim.x, bar_gen, 0.0, 0.0, 0.0, d0, d1, d2, red);   // x of every CTA is visible
+    grid_reduce<3>(st, gridDim.x, bar_gen, 0.0, 0.0, 0.0, d0, d1, d2, red);   // x of every CTA is visible
     stage(mbuf[0]);
     __syncthreads();
     matvec();
     __syncthreads();
     const double tr = mine ? bi - n_s[tid] : 0.0;
-    grid_reduce3(st, gridDim.x, bar_gen, 0.0, 0.0, tr * tr, d0, d1, d2, red);
+    grid_reduce<3>(st, gridDim.x, bar_gen, 0.0, 0.0, tr * tr, d0, d1, d2, red);
     rr = d2;
     if (!(rr <= 4.0 * tol2)) converged = 0;
   }

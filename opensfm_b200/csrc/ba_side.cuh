@@ -582,32 +582,6 @@ __global__ void __launch_bounds__(SIDE_THREADS)
   }
 }
 
-__global__ void side_model_change(SideView sv, BAView v, BlkMaps bm, Params p, const double* __restrict__ scale,
-                                  const double* __restrict__ y, Scalars* sc_out) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  double tot = 0.0;
-  if (i < sv.n) {
-    const SideTerm t = sv.terms[i];
-    const SideCols sc = side_cols(v, bm, sv, p, t);
-    const int NP = sc.start[t.nblocks];
-    const double* J = sv.J + sv.jofs[i];
-    const double* r = sv.r + sv.rofs[i];
-    for (int q = 0; q < t.nres; ++q) {
-      double m = 0.0;
-      for (int k = 0; k < t.nblocks; ++k) {
-        if (sc.b[k].col < 0) continue;
-        for (int a = 0; a < sc.b[k].np; ++a) {
-          const int col = sc.b[k].col + a;
-          m -= J[q * NP + sc.start[k] + a] * scale[col] * y[col];
-        }
-      }
-      tot += -m * (r[q] + 0.5 * m);
-    }
-  }
-  const double tt = block_reduce_sum(tot);
-  if (threadIdx.x == 0 && tt != 0.0) atomicAdd(&sc_out->model_change, tt);
-}
-
 // structure: every pair of free blocks of a term owns a block of the reduced system
 __global__ void side_enum_pairs(SideView sv, BAView v, BlkMaps bm, Params p, unsigned long long* tkeys, unsigned tmask,
                                 int nblk) {
