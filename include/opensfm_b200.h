@@ -280,6 +280,37 @@ int osfm_ba_eval_observation(int device, int projection_type, const double* came
                              const double* observed, double std_deviation, double* r, double* jac_camera,
                              double* jac_instance, double* jac_rig_camera, double* jac_point, int* num_residuals);
 
+/* Linear-system capture (test hook for the Schur-complement and PCG kernels).  Arms a capture of the damped
+ * reduced camera system at LM iteration `iteration` (1-based) of the next osfm_ba_run; 0 disarms.  Single-GPU
+ * only (world == 1, else OSFM_ERR_ARG).  Unarmed, run() computes exactly what it computes without the hook. */
+int osfm_ba_capture_linear_system(osfm_ba* ba, int iteration);
+enum { OSFM_SCHUR_NONE = 0, OSFM_SCHUR_PIPE = 1, OSFM_SCHUR_MMA = 2, OSFM_SCHUR_SIMT_SEGMENT = 3 };
+enum { OSFM_PCG_PIPELINED_DEFLATED = 1, OSFM_PCG_PIPELINED = 2, OSFM_PCG_CLASSIC_RESIDENT = 3,
+       OSFM_PCG_CLASSIC_STREAMED = 4 };
+typedef struct {
+  int iteration;              /* LM iteration captured */
+  int nc, n, wc, nres;        /* reduced dimension, nc + 3 * free points, camera-side width, residuals / observation */
+  double radius;              /* trust-region radius of the iteration: S holds D_c / radius on its diagonal */
+  int nseg, p_fast, p_slow;   /* segments; points in segments; points through the per-point ba_schur */
+  int schur_kernel;           /* OSFM_SCHUR_*: the segment kernel that ran (NONE when no point is in a segment) */
+  int sp_nchunks;             /* chunks of the persistent pipelined Schur kernel */
+  int pcg_kernel;             /* OSFM_PCG_*: the solver that produced y */
+  int pcg_rescued;            /* 1 = the pipelined PCG's result was rejected and the classic PCG re-solved */
+  int pcg_iterations;         /* iterations of the solver that produced y */
+  double pcg_rr;              /* |r|^2 that solver reported at exit */
+} osfm_ba_capture;
+/* What the last armed run captured.  S: dense nc x nc row-major, every stored block expanded from its own storage
+ * (upper and lower blocks separately, blocks that are not stored stay 0) after priors, side terms, damping and
+ * mirroring, i.e. the matrix the PCG receives; rhs[nc]; y[nc] the PCG solution; scale[n], diag[n] (the undamped
+ * LM diagonal) and grad[n] with the point side in the caller's order (free points by ascending index).  Any
+ * output may be NULL.  Fails when nothing was captured or nc > 8192. */
+int osfm_ba_get_captured_system(osfm_ba* ba, osfm_ba_capture* info, double* S, double* rhs, double* y, double* scale,
+                                double* diag, double* grad);
+/* The parameters at which the captured system was linearised, laid out like osfm_ba_get_cameras /
+ * _rig_instances / _rig_cameras / _points / _ext_blocks.  Any output may be NULL. */
+int osfm_ba_get_captured_parameters(osfm_ba* ba, double* cam_params, double* inst_pose6, double* rig_camera_pose6,
+                                    double* points, double* ext_values);
+
 #ifdef __cplusplus
 }
 #endif

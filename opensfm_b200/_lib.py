@@ -39,6 +39,16 @@ class BASummary(ctypes.Structure):
     ]
 
 
+class BACapture(ctypes.Structure):
+    """osfm_ba_capture (include/opensfm_b200.h)."""
+    _fields_ = [("iteration", c_int), ("nc", c_int), ("n", c_int), ("wc", c_int), ("nres", c_int), ("radius", c_double),
+                ("nseg", c_int), ("p_fast", c_int), ("p_slow", c_int), ("schur_kernel", c_int), ("sp_nchunks", c_int),
+                ("pcg_kernel", c_int), ("pcg_rescued", c_int), ("pcg_iterations", c_int), ("pcg_rr", c_double)]
+
+
+SCHUR_KERNELS = {0: "none", 1: "pipe", 2: "mma", 3: "simt_segment"}
+PCG_KERNELS = {1: "pipelined_deflated", 2: "pipelined", 3: "classic_resident", 4: "classic_streamed"}
+
 ALLREDUCE_FN = ctypes.CFUNCTYPE(c_int, c_void_p, c_int64, c_void_p, c_void_p)
 
 # name -> (restype, argtypes); every symbol include/opensfm_b200.h declares
@@ -101,6 +111,10 @@ SIGNATURES = {
     "osfm_ba_get_reprojection_errors": (c_int, [c_void_p, c_void_p]),
     "osfm_ba_eval_observation": (c_int, [c_int, c_int, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p,
                                          c_double, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, POINTER(c_int)]),
+    "osfm_ba_capture_linear_system": (c_int, [c_void_p, c_int]),
+    "osfm_ba_get_captured_system": (c_int, [c_void_p, POINTER(BACapture), c_void_p, c_void_p, c_void_p, c_void_p,
+                                            c_void_p, c_void_p]),
+    "osfm_ba_get_captured_parameters": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
 }
 
 _lib = None

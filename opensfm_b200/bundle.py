@@ -59,7 +59,8 @@ def _p(a: np.ndarray):
 
 def solve(pb: bp.BAProblem, device: int = 0, rank: int = 0, world: int = 1, allreduce=None,
           stream: Optional[int] = None, compute_reprojection_errors: bool = True,
-          out: Optional[Dict[str, np.ndarray]] = None, pinned_inputs: bool = False) -> Dict[str, Any]:
+          out: Optional[Dict[str, np.ndarray]] = None, pinned_inputs: bool = False,
+          capture_iteration: Optional[int] = None) -> Dict[str, Any]:
     """Run the GPU bundle adjustment on a BAProblem.  Returns updated parameter arrays,
     unscaled reprojection errors (bundle_adjuster.cc:1196-1208) and the run summary.
 
@@ -71,7 +72,10 @@ def solve(pb: bp.BAProblem, device: int = 0, rank: int = 0, world: int = 1, allr
     `out` may hold preallocated C-contiguous float64 arrays "points" (P, 3) and "reprojection_errors"
     (N, 3) to receive the results (page-locked buffers make the device->host copy a plain DMA).
     `pinned_inputs`: the observation arrays of `pb` are page-locked; their upload then overlaps the device-side
-    ordering (osfm_ba_set_observations_async; the arrays are kept alive here until the solve returns)."""
+    ordering (osfm_ba_set_observations_async; the arrays are kept alive here until the solve returns).
+    `capture_iteration` (single GPU, tests): result["capture"] holds the damped reduced system of that LM iteration
+    (1-based) as the PCG received it, the PCG solution, the Jacobi scale, the LM diagonal, the gradient and the
+    kernel paths that ran (osfm_ba_get_captured_system); raises if the solve ended before that iteration."""
     pb.validate(check_indices=False)
     L = _lib.load()
     h = _handle(int(device)).h
@@ -158,7 +162,16 @@ def solve(pb: bp.BAProblem, device: int = 0, rank: int = 0, world: int = 1, allr
             # the handle is reused between calls: reset whatever a previous distributed solve left
             _lib.check(L.osfm_ba_set_distributed(h, 0, 1, ctypes.cast(None, _lib.ALLREDUCE_FN), None))
         _lib.check(L.osfm_ba_set_stream(h, ctypes.c_void_p(stream) if stream is not None else None))
-        _lib.check(L.osfm_ba_run(h))
+        if capture_iteration is not None:
+            if int(capture_iteration) < 1:
+                raise ValueError("capture_iteration must be >= 1")
+            _lib.check(L.osfm_ba_capture_linear_system(h, int(capture_iteration)))
+        try:
+            _lib.check(L.osfm_ba_run(h))
+        finally:
+            if capture_iteration is not None:   # the handle is reused: later solves run unarmed
+                _lib.check(L.osfm_ba_capture_linear_system(h, 0))
+        capture = _get_capture(L, h, len(keep[1]), NI, NR, P, len(k9[1])) if capture_iteration is not None else None
         cam = np.zeros_like(keep[1])
         inst = np.zeros((NI, 6))
         rc = np.zeros((NR, 6))
@@ -188,8 +201,31 @@ def solve(pb: bp.BAProblem, device: int = 0, rank: int = 0, world: int = 1, allr
         summary = {f[0]: getattr(s, f[0]) for f in s._fields_}
         summary["message"] = s.message.decode()
         summary["termination"] = _TERMINATION[s.termination]
-        return {"cam_params": cam, "inst": inst, "rigcam": rc, "points": pts, "reprojection_errors": rep,
-                "ext_values": ext, "summary": summary}
+        res = {"cam_params": cam, "inst": inst, "rigcam": rc, "points": pts, "reprojection_errors": rep,
+               "ext_values": ext, "summary": summary}
+        if capture is not None:
+            res["capture"] = capture
+        return res
+
+
+def _get_capture(L, h, ncam: int, NI: int, NR: int, P: int, next_: int) -> Dict[str, Any]:
+    info = _lib.BACapture()
+    _lib.check(L.osfm_ba_get_captured_system(h, ctypes.byref(info), None, None, None, None, None, None))
+    nc, n = info.nc, info.n
+    cap = {f[0]: getattr(info, f[0]) for f in info._fields_}
+    cap["schur_kernel"] = _lib.SCHUR_KERNELS[info.schur_kernel]
+    cap["pcg_kernel"] = _lib.PCG_KERNELS[info.pcg_kernel]
+    arrs = {"S": np.zeros((nc, nc)), "rhs": np.zeros(nc), "y": np.zeros(nc), "scale": np.zeros(n), "diag": np.zeros(n),
+            "grad": np.zeros(n)}
+    _lib.check(L.osfm_ba_get_captured_system(h, None, *[_p(arrs[k]) for k in ("S", "rhs", "y", "scale", "diag", "grad")]))
+    # the linearisation point of the captured iteration
+    x = {"cam_params": np.zeros(ncam), "inst": np.zeros((NI, 6)), "rigcam": np.zeros((NR, 6)), "points": np.zeros((P, 3)),
+         "ext_values": np.zeros(next_)}
+    _lib.check(L.osfm_ba_get_captured_parameters(h, *[_p(x[k]) for k in ("cam_params", "inst", "rigcam", "points",
+                                                                       "ext_values")]))
+    cap.update(arrs)
+    cap["x"] = x
+    return cap
 
 
 def eval_observation(projection_type: int, camera, rig_instance, rig_camera, use_rig_camera: bool, point, observed,

@@ -908,6 +908,15 @@ struct BA {
   bool reproj_valid = false;
   osfm_ba_summary summary{};
   bool has_run = false;
+  // osfm_ba_capture_linear_system: raw copies of the reduced system at LM iteration cap_iter (0 = unarmed)
+  int cap_iter = 0;
+  bool cap_valid = false;
+  osfm_ba_capture cap_info{};
+  std::vector<double> cap_sbuf, cap_y, cap_scale, cap_diag, cap_grad;   // cap_sbuf = [rhs (nc_pad) | block values]
+  std::vector<double> cap_cam, cap_inst, cap_rc, cap_pts, cap_ext;      // the linearisation point (points engine order)
+  std::vector<int4> cap_upper;
+  std::vector<int> cap_blk_off, cap_blk_sz, cap_pt_poff, cap_global_of;
+  int cap_nc_pad = 0;
 
   // device state
   DevBuf<int> d_cam_type, d_cam_off, d_cam_np, d_cam_poff, d_inst_poff, d_rc_poff, d_pt_poff;
@@ -1053,6 +1062,8 @@ void BA::run() {
   const int S = (int)shot_inst.size(), Pfull = (int)pt_const.size();
   const long long Nfull = n_obs_full;
   if (K == 0 && Nfull > 0) throw ArgError("observations but no cameras");
+  if (cap_iter > 0 && world > 1) throw ArgError("the linear-system capture supports world == 1 only");
+  cap_valid = false;
   int64_t launches0 = g_kernel_launches.load();
 
   // ---- validation (errors mirror the reference's: missing ids -> runtime_error) ----
@@ -2049,6 +2060,46 @@ void BA::run() {
       OSFM_CUDA(cudaMemcpyAsync(d_y.p, d_px.p, sizeof(double) * nc, cudaMemcpyDeviceToDevice, stream));
       OSFM_CUDA(cudaMemcpyAsync(h_pcg.p, d_pcg.p, PCG_STATE_HEADER, cudaMemcpyDeviceToHost, stream));
       tm_pcg.stop(stream);
+      if (it == cap_iter) {
+        // test hook: raw copies only, the dense expansion is host code in osfm_ba_get_captured_system
+        const size_t nsb = (size_t)nc_pad + (size_t)s_total;
+        cap_sbuf.resize(nsb); cap_upper.resize(n_upper); cap_y.resize(nc);
+        cap_scale.resize(n); cap_diag.resize(n); cap_grad.resize(n); cap_pt_poff.resize(P); cap_global_of.resize(P);
+        OSFM_CUDA(cudaMemcpyAsync(cap_sbuf.data(), d_Sbuf.p, sizeof(double) * nsb, cudaMemcpyDeviceToHost, stream));
+        if (n_upper > 0)
+          OSFM_CUDA(cudaMemcpyAsync(cap_upper.data(), d_upper.p, sizeof(int4) * n_upper, cudaMemcpyDeviceToHost, stream));
+        OSFM_CUDA(cudaMemcpyAsync(cap_y.data(), d_px.p, sizeof(double) * nc, cudaMemcpyDeviceToHost, stream));
+        OSFM_CUDA(cudaMemcpyAsync(cap_scale.data(), d_scale.p, sizeof(double) * n, cudaMemcpyDeviceToHost, stream));
+        OSFM_CUDA(cudaMemcpyAsync(cap_diag.data(), d_diag.p, sizeof(double) * n, cudaMemcpyDeviceToHost, stream));
+        OSFM_CUDA(cudaMemcpyAsync(cap_grad.data(), d_grad.p, sizeof(double) * n, cudaMemcpyDeviceToHost, stream));
+        if (P > 0) {
+          OSFM_CUDA(cudaMemcpyAsync(cap_pt_poff.data(), d_pt_poff.p, sizeof(int) * P, cudaMemcpyDeviceToHost, stream));
+          OSFM_CUDA(cudaMemcpyAsync(cap_global_of.data(), d_global_of.p, sizeof(int) * P, cudaMemcpyDeviceToHost, stream));
+        }
+        cap_cam.resize(cam_params.size()); cap_inst.resize(inst.size()); cap_rc.resize(rc.size());
+        cap_pts.resize(3 * (size_t)P); cap_ext.resize(ext_values.size());
+        const Params xp = params_of(cur);
+        auto fetch = [&](std::vector<double>& h, const double* d) {
+          if (!h.empty()) OSFM_CUDA(cudaMemcpyAsync(h.data(), d, sizeof(double) * h.size(), cudaMemcpyDeviceToHost, stream));
+        };
+        fetch(cap_cam, xp.cam); fetch(cap_inst, xp.inst); fetch(cap_rc, xp.rc); fetch(cap_pts, xp.pts); fetch(cap_ext, xp.ext);
+        OSFM_CUDA(cudaStreamSynchronize(stream));
+        cap_blk_off = blk_off; cap_blk_sz = blk_sz; cap_nc_pad = nc_pad;
+        cap_info = osfm_ba_capture{};
+        cap_info.iteration = it; cap_info.nc = nc; cap_info.n = n; cap_info.wc = wc; cap_info.nres = nres;
+        cap_info.radius = radius;
+        cap_info.nseg = nseg; cap_info.p_fast = P_fast; cap_info.p_slow = P - P_fast;
+        cap_info.schur_kernel = nseg == 0 ? OSFM_SCHUR_NONE
+                                : !use_mma ? OSFM_SCHUR_SIMT_SEGMENT
+                                : (use_pipe && sp_nchunks > 0) ? OSFM_SCHUR_PIPE : OSFM_SCHUR_MMA;
+        cap_info.sp_nchunks = sp_nchunks;
+        cap_info.pcg_kernel = solved ? (h_pcg.p->deflated ? OSFM_PCG_PIPELINED_DEFLATED : OSFM_PCG_PIPELINED)
+                                     : (pcg_resident ? OSFM_PCG_CLASSIC_RESIDENT : OSFM_PCG_CLASSIC_STREAMED);
+        cap_info.pcg_rescued = pcg_pipe_ok && !solved;
+        cap_info.pcg_iterations = h_pcg.p->iterations;
+        cap_info.pcg_rr = h_pcg.p->rr_final;
+        cap_valid = true;
+      }
     }
     ++n_solves;
     // --- back-substitution, model cost change ---
@@ -2577,6 +2628,76 @@ int osfm_ba_eval_observation(int device, int projection_type, const double* came
   for (int i = 0; i < nres * 6; ++i) jac_rig_camera[i] = out[69 + i];
   for (int i = 0; i < nres * 3; ++i) jac_point[i] = out[87 + i];
   if (num_residuals) *num_residuals = nres;
+  OSFM_API_END
+}
+
+int osfm_ba_capture_linear_system(osfm_ba* ba, int iteration) {
+  OSFM_API_BEGIN
+  OSFM_BA_CHECK
+  if (iteration < 0) throw ArgError("capture iteration must be >= 0");
+  if (iteration > 0 && ba->impl.world != 1) throw ArgError("the linear-system capture supports world == 1 only");
+  ba->impl.cap_iter = iteration;
+  OSFM_API_END
+}
+
+int osfm_ba_get_captured_system(osfm_ba* ba, osfm_ba_capture* info, double* S, double* rhs, double* y, double* scale,
+                                double* diag, double* grad) {
+  OSFM_API_BEGIN
+  OSFM_BA_CHECK
+  const auto& b = ba->impl;
+  if (!b.cap_valid) throw std::runtime_error("no linear system was captured (not armed, or the run ended earlier)");
+  const int nc = b.cap_info.nc, n = b.cap_info.n;
+  if (nc > 8192) throw ArgError("reduced system too large for a dense copy (nc > 8192)");
+  if (info) *info = b.cap_info;
+  if (S) {
+    std::fill(S, S + (size_t)nc * nc, 0.0);
+    const double* val = b.cap_sbuf.data() + b.cap_nc_pad;
+    for (const int4& u : b.cap_upper) {
+      const int oi = b.cap_blk_off[u.x], oj = b.cap_blk_off[u.y], si = b.cap_blk_sz[u.x], sj = b.cap_blk_sz[u.y];
+      for (int r = 0; r < si; ++r)   // block (bi, bj), row-major si x sj
+        for (int c = 0; c < sj; ++c) S[(size_t)(oi + r) * nc + oj + c] = val[u.z + r * sj + c];
+      if (u.w >= 0)
+        for (int r = 0; r < sj; ++r)   // its own lower block (bj, bi), row-major sj x si
+          for (int c = 0; c < si; ++c) S[(size_t)(oj + r) * nc + oi + c] = val[u.w + r * si + c];
+    }
+  }
+  if (rhs) std::copy(b.cap_sbuf.begin(), b.cap_sbuf.begin() + nc, rhs);
+  if (y) std::copy(b.cap_y.begin(), b.cap_y.end(), y);
+  // point side: engine order -> free points by ascending caller index
+  std::vector<int> dst(std::max(n, 1));
+  for (int i = 0; i < nc; ++i) dst[i] = i;
+  {
+    std::vector<std::pair<int, int>> fp;   // (caller index, engine free index)
+    for (size_t q = 0; q < b.cap_pt_poff.size(); ++q)
+      if (b.cap_pt_poff[q] >= 0) fp.emplace_back(b.cap_global_of[q], b.cap_pt_poff[q]);
+    if (nc + 3 * (int)fp.size() != n) throw std::runtime_error("captured point layout is inconsistent");
+    std::sort(fp.begin(), fp.end());
+    for (size_t k = 0; k < fp.size(); ++k)
+      for (int j = 0; j < 3; ++j) dst[nc + 3 * fp[k].second + j] = nc + 3 * (int)k + j;
+  }
+  auto scatter = [&](const std::vector<double>& src, double* out) {
+    if (out)
+      for (int i = 0; i < n; ++i) out[dst[i]] = src[i];
+  };
+  scatter(b.cap_scale, scale);
+  scatter(b.cap_diag, diag);
+  scatter(b.cap_grad, grad);
+  OSFM_API_END
+}
+
+int osfm_ba_get_captured_parameters(osfm_ba* ba, double* cam_params, double* inst_pose6, double* rig_camera_pose6,
+                                    double* points, double* ext_values) {
+  OSFM_API_BEGIN
+  OSFM_BA_CHECK
+  const auto& b = ba->impl;
+  if (!b.cap_valid) throw std::runtime_error("no linear system was captured (not armed, or the run ended earlier)");
+  if (cam_params) std::copy(b.cap_cam.begin(), b.cap_cam.end(), cam_params);
+  if (inst_pose6) std::copy(b.cap_inst.begin(), b.cap_inst.end(), inst_pose6);
+  if (rig_camera_pose6) std::copy(b.cap_rc.begin(), b.cap_rc.end(), rig_camera_pose6);
+  if (ext_values) std::copy(b.cap_ext.begin(), b.cap_ext.end(), ext_values);
+  if (points)   // engine order -> the caller's
+    for (size_t q = 0; q < b.cap_global_of.size(); ++q)
+      for (int j = 0; j < 3; ++j) points[3 * (size_t)b.cap_global_of[q] + j] = b.cap_pts[3 * q + j];
   OSFM_API_END
 }
 

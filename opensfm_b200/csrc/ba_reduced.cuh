@@ -1214,9 +1214,11 @@ struct PcgState {
   int iterations;
   int converged;
   double rr_final;                     // |r|^2 at exit (NaN -> the step is rejected)
-  long long prof[8];                   // CTA 0 / thread 0 clock64 totals per phase (OSFM_BA_TRACE)
-  // per-CTA partial sums of the reduction riding on the barrier (double-buffered by generation parity)
-  double slot[2][PCG_MAX_CTAS][4];
+  int deflated;                        // pcg_pipelined: 1 = solved with gauge deflation (0 when W^T S W was singular)
+  long long prof[8];                  // CTA 0 / thread 0 clock64 totals per phase (OSFM_BA_TRACE)
+  // per-CTA partial sums of the reduction riding on the barrier (double-buffered by generation parity; read and
+  // written as 16-byte vectors, hence the alignment)
+  alignas(16) double slot[2][PCG_MAX_CTAS][4];
   // wide payload of the deflated solver: 3 dot products + PCG_ND projections (double-buffered by generation parity)
   double slotx[2][PCG_MAX_CTAS][12];
   // per-CTA arrival generation, one 128-byte line each (packed flags contend for one line on
@@ -1997,7 +1999,9 @@ __global__ void __launch_bounds__(PCG_THREADS, 1)
     rr = d2;
     if (!(rr <= 4.0 * tol2)) converged = 0;
   }
-  if (blockIdx.x == 0 && tid == 0) { st->iterations = it; st->rr_final = rr; st->converged = converged; }
+  if (blockIdx.x == 0 && tid == 0) {
+    st->iterations = it; st->rr_final = rr; st->converged = converged; st->deflated = defl ? 1 : 0;
+  }
 }
 
 }  // namespace osfm
