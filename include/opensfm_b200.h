@@ -311,6 +311,25 @@ int osfm_ba_get_captured_system(osfm_ba* ba, osfm_ba_capture* info, double* S, d
 int osfm_ba_get_captured_parameters(osfm_ba* ba, double* cam_params, double* inst_pose6, double* rig_camera_pose6,
                                     double* points, double* ext_values);
 
+/* Rig-instance pose covariances (bundle_adjuster.cc:1123-1194).  When enabled, run() ends with a covariance pass
+ * at the accepted parameters: (J^T J)^-1 of the robustified Jacobian over every non-constant block, bounds ignored,
+ * each rig instance's 6 x 6 diagonal block in its [rx, ry, rz, tx, ty, tz] order.  Single GPU only (run() fails
+ * with world > 1), and run() fails when the dense n_c x n_c reduced system does not fit in device memory. */
+int osfm_ba_set_compute_covariances(osfm_ba* ba, int enable);
+enum {
+  OSFM_COV_OK = 0,                     /* computed, every block finite: valid */
+  OSFM_COV_SOLVER_FAILURE = 1,         /* the solve terminated with FAILURE: not computed */
+  OSFM_COV_POINT_RANK_DEFICIENT = 2,   /* a point's 3x3 block failed the pivot test */
+  OSFM_COV_CAMERA_RANK_DEFICIENT = 3,  /* the reduced camera system failed the pivot test */
+  OSFM_COV_NON_FINITE = 4              /* a covariance entry is not finite */
+};
+/* Result of the last run(), which must have been armed.  out: NI x 36, row-major 6 x 6 per instance in the
+ * caller's order; constant instances get zeros.  Invalid (status != OSFM_COV_OK): every instance gets
+ * diag(1e-5, 1e-5, 1e-5, 1e-2, 1e-2, 1e-2).  Any output may be NULL. */
+int osfm_ba_get_covariances(osfm_ba* ba, int* valid, int* status, double* out);
+/* Device time of the last covariance pass (CUDA events): the whole pass and the Cholesky of the reduced system. */
+int osfm_ba_get_covariance_timing(osfm_ba* ba, double* pass_ms, double* cholesky_ms);
+
 #ifdef __cplusplus
 }
 #endif

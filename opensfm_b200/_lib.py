@@ -48,6 +48,8 @@ class BACapture(ctypes.Structure):
 
 SCHUR_KERNELS = {0: "none", 1: "pipe", 2: "mma", 3: "simt_segment"}
 PCG_KERNELS = {1: "pipelined_deflated", 2: "pipelined", 3: "classic_resident", 4: "classic_streamed"}
+COVARIANCE_STATUS = {0: "ok", 1: "solver_failure", 2: "point_rank_deficient", 3: "camera_rank_deficient",
+                     4: "non_finite"}
 
 ALLREDUCE_FN = ctypes.CFUNCTYPE(c_int, c_void_p, c_int64, c_void_p, c_void_p)
 
@@ -115,6 +117,9 @@ SIGNATURES = {
     "osfm_ba_get_captured_system": (c_int, [c_void_p, POINTER(BACapture), c_void_p, c_void_p, c_void_p, c_void_p,
                                             c_void_p, c_void_p]),
     "osfm_ba_get_captured_parameters": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "osfm_ba_set_compute_covariances": (c_int, [c_void_p, c_int]),
+    "osfm_ba_get_covariances": (c_int, [c_void_p, POINTER(c_int), POINTER(c_int), c_void_p]),
+    "osfm_ba_get_covariance_timing": (c_int, [c_void_p, POINTER(c_double), POINTER(c_double)]),
 }
 
 _lib = None

@@ -60,7 +60,7 @@ def _p(a: np.ndarray):
 def solve(pb: bp.BAProblem, device: int = 0, rank: int = 0, world: int = 1, allreduce=None,
           stream: Optional[int] = None, compute_reprojection_errors: bool = True,
           out: Optional[Dict[str, np.ndarray]] = None, pinned_inputs: bool = False,
-          capture_iteration: Optional[int] = None) -> Dict[str, Any]:
+          capture_iteration: Optional[int] = None, compute_covariances: bool = False) -> Dict[str, Any]:
     """Run the GPU bundle adjustment on a BAProblem.  Returns updated parameter arrays,
     unscaled reprojection errors (bundle_adjuster.cc:1196-1208) and the run summary.
 
@@ -75,7 +75,11 @@ def solve(pb: bp.BAProblem, device: int = 0, rank: int = 0, world: int = 1, allr
     ordering (osfm_ba_set_observations_async; the arrays are kept alive here until the solve returns).
     `capture_iteration` (single GPU, tests): result["capture"] holds the damped reduced system of that LM iteration
     (1-based) as the PCG received it, the PCG solution, the Jacobi scale, the LM diagonal, the gradient and the
-    kernel paths that ran (osfm_ba_get_captured_system); raises if the solve ended before that iteration."""
+    kernel paths that ran (osfm_ba_get_captured_system); raises if the solve ended before that iteration.
+    `compute_covariances` (single GPU): the result gains "covariances" (NI x 6 x 6, the rig-instance pose covariances
+    in the problem's instance order, zeros for constant instances), "covariance_valid" and "covariance_status" (one of
+    _lib.COVARIANCE_STATUS).  As in the reference, an invalid estimate leaves every instance with the default
+    diag(1e-5, 1e-5, 1e-5, 1e-2, 1e-2, 1e-2)."""
     pb.validate(check_indices=False)
     L = _lib.load()
     h = _handle(int(device)).h
@@ -162,6 +166,7 @@ def solve(pb: bp.BAProblem, device: int = 0, rank: int = 0, world: int = 1, allr
             # the handle is reused between calls: reset whatever a previous distributed solve left
             _lib.check(L.osfm_ba_set_distributed(h, 0, 1, ctypes.cast(None, _lib.ALLREDUCE_FN), None))
         _lib.check(L.osfm_ba_set_stream(h, ctypes.c_void_p(stream) if stream is not None else None))
+        _lib.check(L.osfm_ba_set_compute_covariances(h, int(bool(compute_covariances))))
         if capture_iteration is not None:
             if int(capture_iteration) < 1:
                 raise ValueError("capture_iteration must be >= 1")
@@ -205,6 +210,13 @@ def solve(pb: bp.BAProblem, device: int = 0, rank: int = 0, world: int = 1, allr
                "ext_values": ext, "summary": summary}
         if capture is not None:
             res["capture"] = capture
+        if compute_covariances:
+            cov = np.zeros((NI, 6, 6))
+            valid, status = ctypes.c_int(0), ctypes.c_int(0)
+            _lib.check(L.osfm_ba_get_covariances(h, ctypes.byref(valid), ctypes.byref(status), _p(cov)))
+            res["covariances"] = cov
+            res["covariance_valid"] = bool(valid.value)
+            res["covariance_status"] = _lib.COVARIANCE_STATUS[status.value]
         return res
 
 
@@ -328,8 +340,11 @@ class BundleAdjuster:
     (opensfm/src/bundle/python/pybind.cc:45-117, bundle_adjuster.cc:24-44, 94-412).  `run()` turns the collected
     blocks into one BAProblem (numpy index arrays, no per-observation Python work) and calls `solve()`.
 
-    Not available (raise NotImplementedError): heat maps (ceres::BiCubicInterpolator), relative depth priors and
-    covariance estimation."""
+    Covariances (set_compute_covariances, bundle_adjuster.cc:1123-1194): run() ends with the rig-instance pose
+    covariances of every shot's instance, read with get_rig_instance_covariance; get_covariance_estimation_valid()
+    says whether the estimate of the last run is valid (the default matrices otherwise).
+
+    Not available (raise NotImplementedError): heat maps (ceres::BiCubicInterpolator) and relative depth priors."""
 
     def __init__(self, device: int = 0):
         self.device = device
@@ -374,6 +389,8 @@ class BundleAdjuster:
         self._num_threads = 1
         self._linear_solver = "SPARSE_SCHUR"
         self._compute_reprojection_errors = True
+        self._compute_covariances = False
+        self._covariance_valid = False
         self._use_analytic = False
         self._summary: Optional[Dict[str, Any]] = None
 
@@ -645,11 +662,21 @@ class BundleAdjuster:
         self._compute_reprojection_errors = bool(v)
 
     def set_compute_covariances(self, v: bool) -> None:
-        if v:
-            raise NotImplementedError("covariance estimation is outside this engine's scope")
+        self._compute_covariances = bool(v)
 
     def get_covariance_estimation_valid(self) -> bool:
-        return False
+        return self._covariance_valid
+
+    def get_rig_instance_covariance(self, iid) -> np.ndarray:
+        """RigInstance::GetCovariance of the reference (bundle/data/data.h:62-66): the 6 x 6 covariance of the
+        instance's [rx, ry, rz, tx, ty, tz] from the last run with covariances on."""
+        r = self._instances.get(_key(iid))
+        if r is None:
+            raise RuntimeError("Rig instance %s doesn't exist." % _key(iid))
+        # only instances of shots get one (ComputeCovariances walks the shots)
+        if r.get("covariance") is None or not r["cameras"]:
+            raise RuntimeError("%s hasn't any covariance" % _key(iid))
+        return r["covariance"].copy()
 
     def set_adjust_absolute_position_std(self, v: bool) -> None:
         self._adjust_std = bool(v)
@@ -809,7 +836,8 @@ class BundleAdjuster:
     def run(self) -> None:
         pb = self.to_problem()
         self.apply_results(pb, solve(pb, device=self.device,
-                                     compute_reprojection_errors=self._compute_reprojection_errors))
+                                     compute_reprojection_errors=self._compute_reprojection_errors,
+                                     compute_covariances=self._compute_covariances))
 
     def apply_results(self, pb: bp.BAProblem, res: Dict[str, Any]) -> None:
         """Write the arrays of a solve of `pb` (= self.to_problem()) back into the per-id containers the getters
@@ -830,6 +858,10 @@ class BundleAdjuster:
                 self._bias[k[1]]["values"] = vals.copy()
             elif k[0] == "scale":
                 self._reconstructions[k[1]].scales[k[2]] = float(vals[0])
+        if "covariances" in res:
+            for i, iid in enumerate(inst_ids):
+                self._instances[iid]["covariance"] = np.asarray(res["covariances"][i], dtype=np.float64).copy()
+            self._covariance_valid = bool(res["covariance_valid"])
         self._pt_errors = None
         if self._compute_reprojection_errors:
             # Point::reprojection_errors: shot id -> 2-vector (3 for spherical cameras), bundle_adjuster.cc:531-566

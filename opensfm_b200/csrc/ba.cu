@@ -672,6 +672,7 @@ inline void launch_cooperative(void (*kern)(KArgs...), int grid, int block, size
 static_assert(osfm::CG_KMAX == osfm::SEG_KMAX, "colnorm tiles hold the widest segment");
 #include "ba_side.cuh"
 #include "ba_order.cuh"
+#include "ba_cov.cuh"
 namespace osfm {
 
 // ---------------------------------------------------------------------------
@@ -917,6 +918,13 @@ struct BA {
   std::vector<int4> cap_upper;
   std::vector<int> cap_blk_off, cap_blk_sz, cap_pt_poff, cap_global_of;
   int cap_nc_pad = 0;
+  // osfm_ba_set_compute_covariances: rig-instance covariances after the LM loop (ba_cov.cuh)
+  bool cov_on = false, cov_ran = false, cov_valid = false, cov_attr = false;
+  int cov_status = OSFM_COV_OK;
+  double cov_pass_ms = 0.0, cov_chol_ms = 0.0;
+  std::vector<double> cov_out;             // NI x 36, row-major
+  DevBuf<double> d_cov;                    // dense S | L22^-1 | diagonal-block inverses | original diagonal | NI x 36
+  DevBuf<int> d_cov_perm, d_cov_inst, d_cov_flags;
 
   // device state
   DevBuf<int> d_cam_type, d_cam_off, d_cam_np, d_cam_poff, d_inst_poff, d_rc_poff, d_pt_poff;
@@ -1063,7 +1071,10 @@ void BA::run() {
   const long long Nfull = n_obs_full;
   if (K == 0 && Nfull > 0) throw ArgError("observations but no cameras");
   if (cap_iter > 0 && world > 1) throw ArgError("the linear-system capture supports world == 1 only");
+  if (cov_on && world > 1) throw ArgError("covariance estimation supports world == 1 only");
   cap_valid = false;
+  cov_ran = false;
+  if (!cov_on) d_cov.release();   // the dense workspace of an earlier armed run (n_c^2 + m^2 doubles and more)
   int64_t launches0 = g_kernel_launches.load();
 
   // ---- validation (errors mirror the reference's: missing ids -> runtime_error) ----
@@ -1779,6 +1790,39 @@ void BA::run() {
   lay.colidx = d_colidx.p; lay.ngroups = ngroups; lay.grp_b1 = d_grp_b1.p; lay.grp_b2 = d_grp_b2.p;
 
   trace("structure");
+  // ---- workspace of the covariance pass, claimed before the LM loop so that a problem too large for a dense S
+  //      fails here (the pass itself runs after the loop) ----
+  std::vector<int> cov_inst, cov_bstart;   // free rig instances; starts of the Cholesky blocks (+ nc)
+  int cov_m = 0, cov_nb1 = 0;              // instance columns (last in the dense S); blocks of the leading part
+  if (cov_on) {
+    for (int i = 0; i < NI; ++i)
+      if (inst_poff[i] >= 0) cov_inst.push_back(i);
+    cov_m = 6 * (int)cov_inst.size();
+    // leading and instance columns are blocked separately: L22's diagonal blocks are blocks of the Cholesky
+    for (int k = 0; k < nc - cov_m; k += COV_NB) cov_bstart.push_back(k);
+    cov_nb1 = (int)cov_bstart.size();
+    for (int k = nc - cov_m; k < nc; k += COV_NB) cov_bstart.push_back(k);
+    const size_t nblocks = cov_bstart.size();
+    cov_bstart.push_back(nc);
+    const size_t total = (size_t)nc * nc + (size_t)cov_m * cov_m + nblocks * COV_NB * COV_NB + (size_t)nc +
+                         (size_t)NI * 36 + 1;
+    if (total > d_cov.cap) {
+      size_t free_b = 0, total_b = 0;
+      OSFM_CUDA(cudaMemGetInfo(&free_b, &total_b));
+      if (total * sizeof(double) > free_b + d_cov.cap * sizeof(double)) {
+        char msg[256];
+        snprintf(msg, sizeof(msg),
+                 "covariance estimation needs %zu bytes of device memory for the dense reduced camera system "
+                 "(n_c = %d) and its workspace; %zu bytes are free", total * sizeof(double), nc, free_b);
+        throw ArgError(msg);
+      }
+      d_cov.release();
+      OSFM_CUDA(cudaMalloc(&d_cov.p, total * sizeof(double)));
+      d_cov.cap = total;
+    }
+    d_cov_flags.reserve(COV_F_COUNT);
+  }
+
   // ---- Levenberg-Marquardt (Ceres trust_region_minimizer / levenberg_marquardt_strategy) ----
   if (world > 1) {  // all ranks enter the timed region together (their set-up times differ)
     OSFM_CUDA(cudaMemsetAsync(d_sc.p, 0, sizeof(Scalars), stream));
@@ -1880,27 +1924,17 @@ void BA::run() {
   };
   double x_norm = n > 0 ? x_norm_of(cur) : 0.0;
 
-  if (grad_max <= gtol || n == 0) {
-    termination = 0;
-    message = n == 0 ? "No free parameters." : "Gradient tolerance reached.";
-  }
-  while (termination == 1) {
-    if (it >= max_iterations) break;
-    if (radius < min_radius) { termination = 0; message = "Minimum trust region radius reached."; break; }
-    ++it;
-    if (!reuse_diagonal) {
-      ba_make_diag<<<grid_for(n, 256), 256, 0, stream>>>(d_colnorm2.p, d_scale.p, d_diag.p, n);
-      OSFM_LAUNCH_CHECK();
-    }
-    const double inv_radius = 1.0 / radius;
-    // --- reduced camera system (upper blocks accumulated with L2 atomics) ---
+  // Reduced camera system at the accepted parameters (upper blocks accumulated with L2 atomics, all-reduced, priors
+  // and side terms added, mirrored), damped with diag * inv_radius.  The LM iteration and the covariance pass
+  // (inv_radius = 0, rank_flag set: ba_cov.cuh) both build it here, through the same kernel path.
+  auto build_system = [&](double inv_radius, int* rank_flag) {
     if (nc > 0) {
       OSFM_CUDA(cudaMemsetAsync(d_Sbuf.p, 0, sizeof(double) * ((size_t)nc_pad + (size_t)s_upper_total), stream));
     }
     if (P > 0) {
       const size_t smem = (size_t)SCHUR_KC * wc * (2 * 3 * sizeof(double) + 2 * sizeof(int)) +
                           (size_t)SCHUR_KC * 8 * sizeof(int) + (size_t)SCHUR_KC * SCHUR_KC * 9 * sizeof(int);
-      tm_schur.start(stream);
+      if (!rank_flag) tm_schur.start(stream);
       if (nseg > 0) {
         if (!seg_attr) {
           OSFM_CUDA(cudaFuncSetAttribute(ba_schur_seg<9>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(SegSmem)));
@@ -1910,7 +1944,7 @@ void BA::run() {
         // default: fused fp64 tensor-core kernel; OSFM_BA_SCHUR_MMA=0 -> the older ba_obs_rows + ba_schur_seg pair
         d_Vig.reserve(3 * (size_t)std::max(npf, 1));
         ba_point_blocks<<<grid_for(P_fast, 128), 128, 0, stream>>>(v, P_fast, d_scale.p, d_diag.p, inv_radius, d_Vinv.p,
-                                                                 d_gp.p, d_Vig.p);
+                                                                 d_gp.p, d_Vig.p, rank_flag);
         OSFM_LAUNCH_CHECK();
         if (use_mma) {
           if (!mma_attr) {
@@ -1984,14 +2018,11 @@ void BA::run() {
       }
       if (P > P_fast) {
         ba_schur<<<P - P_fast, SCHUR_THREADS, smem, stream>>>(v, bm, bsr, d_scale.p, d_diag.p, inv_radius, d_S_p,
-                                                             d_rhs_p, d_Vinv.p, d_gp.p, P_fast, ppv, d_pts[cur].p);
+                                                             d_rhs_p, d_Vinv.p, d_gp.p, P_fast, ppv, d_pts[cur].p, rank_flag);
         OSFM_LAUNCH_CHECK();
       }
-      tm_schur.stop(stream);
+      if (!rank_flag) tm_schur.stop(stream);
     }
-    bool ok = true;
-    int pcg_it = 0;
-    OSFM_CUDA(cudaMemsetAsync(d_y.p, 0, sizeof(double) * nz, stream));
     if (nc > 0) {
       // the one exchange step of the LM iteration: sum of the partial reduced systems over ranks
       if (world > 1) allreduce_dev(d_Sbuf.p, (long long)nc_pad + s_upper_total);  // rhs + upper blocks, one call
@@ -2015,6 +2046,27 @@ void BA::run() {
       ba_finish_system<<<grid_for((long long)n_upper * 32, 256), 256, 0, stream>>>(d_upper.p, n_upper, bsr, d_S_p,
                                                                                  d_diag.p, inv_radius);
       OSFM_LAUNCH_CHECK();
+    }
+  };
+
+  if (grad_max <= gtol || n == 0) {
+    termination = 0;
+    message = n == 0 ? "No free parameters." : "Gradient tolerance reached.";
+  }
+  while (termination == 1) {
+    if (it >= max_iterations) break;
+    if (radius < min_radius) { termination = 0; message = "Minimum trust region radius reached."; break; }
+    ++it;
+    if (!reuse_diagonal) {
+      ba_make_diag<<<grid_for(n, 256), 256, 0, stream>>>(d_colnorm2.p, d_scale.p, d_diag.p, n);
+      OSFM_LAUNCH_CHECK();
+    }
+    const double inv_radius = 1.0 / radius;
+    build_system(inv_radius, nullptr);
+    bool ok = true;
+    int pcg_it = 0;
+    OSFM_CUDA(cudaMemsetAsync(d_y.p, 0, sizeof(double) * nz, stream));
+    if (nc > 0) {
       // --- PCG: one persistent kernel, |r| <= 1e-8 |b| ---
       tm_pcg.start(stream);
       pcg_convert<<<grid_for((long long)n_blocks_all * 32, 256), 256, 0, stream>>>(
@@ -2210,6 +2262,136 @@ void BA::run() {
   const double final_cost = eval_cost(cur);
 
   trace("lm");
+  // ---- rig-instance covariances (ba_cov.cuh): not after a FAILURE termination, as in the reference ----
+  if (cov_on) {
+    cov_out.assign((size_t)NI * 36, 0.0);
+    cov_status = OSFM_COV_SOLVER_FAILURE;
+    cov_pass_ms = cov_chol_ms = 0.0;
+    if (termination != 2) {
+      double* const A = d_cov.p;                                   // dense S -> L, column-major, ld nc
+      double* const X = A + (size_t)nc * nc;                       // L22^-1, ld m
+      double* const W = X + (size_t)cov_m * cov_m;                 // inverse of every diagonal block of L
+      double* const d0 = W + (cov_bstart.size() - 1) * COV_NB * COV_NB;   // diagonal of S before the factorisation
+      double* const out = d0 + nc;
+      int* const flags = d_cov_flags.p;
+      const int m = cov_m, n1 = nc - cov_m;
+      std::vector<int> perm(std::max(nc, 1));
+      {
+        std::vector<char> is_inst(std::max(nc, 1), 0);
+        for (size_t q = 0; q < cov_inst.size(); ++q)
+          for (int j = 0; j < 6; ++j) {
+            perm[inst_poff[cov_inst[q]] + j] = n1 + 6 * (int)q + j;
+            is_inst[inst_poff[cov_inst[q]] + j] = 1;
+          }
+        for (int g = 0, lead = 0; g < nc; ++g)
+          if (!is_inst[g]) perm[g] = lead++;
+      }
+      upload(d_cov_perm, perm, stream);
+      std::vector<int> inst_list = cov_inst;
+      if (inst_list.empty()) inst_list.push_back(0);
+      upload(d_cov_inst, inst_list, stream);
+      OSFM_CUDA(cudaMemsetAsync(flags, 0, sizeof(int) * COV_F_COUNT, stream));
+      if (!cov_attr) {
+        const int potrf_smem = 2 * COV_NB * (COV_NB + 1) * (int)sizeof(double);
+        const int gemm_smem = 2 * COV_NB * COV_LDS * (int)sizeof(double);
+        OSFM_CUDA(cudaFuncSetAttribute(cov_potrf_diag, cudaFuncAttributeMaxDynamicSharedMemorySize, potrf_smem));
+        OSFM_CUDA(cudaFuncSetAttribute(cov_gemm<COV_TRSM>, cudaFuncAttributeMaxDynamicSharedMemorySize, gemm_smem));
+        OSFM_CUDA(cudaFuncSetAttribute(cov_gemm<COV_SYRK>, cudaFuncAttributeMaxDynamicSharedMemorySize, gemm_smem));
+        OSFM_CUDA(cudaFuncSetAttribute(cov_gemm<COV_TRI_DIAG>, cudaFuncAttributeMaxDynamicSharedMemorySize, gemm_smem));
+        OSFM_CUDA(cudaFuncSetAttribute(cov_gemm<COV_TRI_UPD>, cudaFuncAttributeMaxDynamicSharedMemorySize, gemm_smem));
+        cov_attr = true;
+      }
+      cudaEvent_t ce[4];
+      for (auto& e : ce) OSFM_CUDA(cudaEventCreate(&e));
+      OSFM_CUDA(cudaEventRecord(ce[0], stream));
+      // re-linearise at the accepted parameters with the Jacobi scale of this point (the LM keeps the first one)
+      tm_lin.collect();
+      const double lin_ms = tm_lin.total_ms;
+      const long long lin_count = tm_lin.count;
+      double gm = 0.0;
+      linearize(cur, &gm);
+      tm_lin.collect();
+      tm_lin.total_ms = lin_ms; tm_lin.count = lin_count;
+      if (n > 0) {
+        ba_make_scale<<<grid_for(n, 256), 256, 0, stream>>>(d_colnorm2.p, d_scale.p, n);
+        OSFM_LAUNCH_CHECK();
+        // the diagonal only has to be finite: the system is built with inv_radius = 0
+        ba_make_diag<<<grid_for(n, 256), 256, 0, stream>>>(d_colnorm2.p, d_scale.p, d_diag.p, n);
+        OSFM_LAUNCH_CHECK();
+      }
+      if (have_seg_tab) {   // the tensor-core Schur kernels read the scale from their segment tables
+        ba_seg_tables<<<nseg, 128, 0, stream>>>(v, bm, bsr, d_seg_start.p, d_scale.p, d_tab_off.p, d_tab.p);
+        OSFM_LAUNCH_CHECK();
+      }
+      build_system(0.0, flags + COV_F_POINT_RANK);
+      OSFM_CUDA(cudaEventRecord(ce[1], stream));
+      const int gemm_smem = 2 * COV_NB * COV_LDS * (int)sizeof(double);
+      auto tiles = [](int k) { return (k + COV_NB - 1) / COV_NB; };
+      CovGemm g{A, nc, X, m, n1, nullptr, 0, 0, flags};
+      if (nc > 0) {
+        OSFM_CUDA(cudaMemsetAsync(A, 0, sizeof(double) * (size_t)nc * nc, stream));
+        OSFM_CUDA(cudaMemsetAsync(d0, 0, sizeof(double) * (size_t)nc, stream));
+        cov_densify<<<grid_for((long long)n_upper * 32, 256), 256, 0, stream>>>(d_upper.p, n_upper, bsr, d_S_p,
+                                                                               d_cov_perm.p, nc, A, d0);
+        OSFM_LAUNCH_CHECK();
+        // blocked right-looking Cholesky: diagonal block, panel below it, trailing update
+        for (size_t b = 0; b + 1 < cov_bstart.size(); ++b) {
+          const int k0 = cov_bstart[b], kb = cov_bstart[b + 1] - k0, rem = nc - k0 - kb;
+          cov_potrf_diag<<<1, COV_THREADS, 2 * COV_NB * (COV_NB + 1) * sizeof(double), stream>>>(
+              A, nc, k0, kb, d0, W + b * COV_NB * COV_NB, flags);
+          OSFM_LAUNCH_CHECK();
+          if (rem == 0) continue;
+          g.W = W + b * COV_NB * COV_NB; g.k0 = k0; g.kb = kb;
+          cov_gemm<COV_TRSM><<<dim3(tiles(rem), 1), COV_THREADS, gemm_smem, stream>>>(g);
+          OSFM_LAUNCH_CHECK();
+          cov_gemm<COV_SYRK><<<dim3(tiles(rem), tiles(rem)), COV_THREADS, gemm_smem, stream>>>(g);
+          OSFM_LAUNCH_CHECK();
+        }
+      }
+      OSFM_CUDA(cudaEventRecord(ce[2], stream));
+      if (m > 0) {
+        // X = L22^-1: X_k = W_kk X_k, then X_i -= L22_ik X_k below, block row by block row
+        cov_identity<<<grid_for((long long)m * m, 256), 256, 0, stream>>>(X, m);
+        OSFM_LAUNCH_CHECK();
+        for (size_t b = cov_nb1; b + 1 < cov_bstart.size(); ++b) {
+          const int k0 = cov_bstart[b] - n1, kb = cov_bstart[b + 1] - cov_bstart[b], rem = m - k0 - kb;
+          g.W = W + b * COV_NB * COV_NB; g.k0 = k0; g.kb = kb;
+          cov_gemm<COV_TRI_DIAG><<<dim3(1, tiles(k0 + kb)), COV_THREADS, gemm_smem, stream>>>(g);
+          OSFM_LAUNCH_CHECK();
+          if (rem == 0) continue;
+          cov_gemm<COV_TRI_UPD><<<dim3(tiles(rem), tiles(k0 + kb)), COV_THREADS, gemm_smem, stream>>>(g);
+          OSFM_LAUNCH_CHECK();
+        }
+        OSFM_CUDA(cudaMemsetAsync(out, 0, sizeof(double) * (size_t)NI * 36, stream));
+        cov_blocks<<<(int)cov_inst.size(), COV_THREADS, 0, stream>>>(X, m, d_cov_inst.p, d_inst_poff.p, d_scale.p, flags,
+                                                                     out, flags);
+        OSFM_LAUNCH_CHECK();
+      }
+      OSFM_CUDA(cudaEventRecord(ce[3], stream));
+      int hf[COV_F_COUNT];
+      OSFM_CUDA(cudaMemcpyAsync(hf, flags, sizeof(hf), cudaMemcpyDeviceToHost, stream));
+      if (m > 0) OSFM_CUDA(cudaMemcpyAsync(cov_out.data(), out, sizeof(double) * cov_out.size(), cudaMemcpyDeviceToHost, stream));
+      OSFM_CUDA(cudaStreamSynchronize(stream));
+      float ms_pass = 0.f, ms_chol = 0.f;
+      OSFM_CUDA(cudaEventElapsedTime(&ms_pass, ce[0], ce[3]));
+      OSFM_CUDA(cudaEventElapsedTime(&ms_chol, ce[1], ce[2]));
+      for (auto& e : ce) cudaEventDestroy(e);
+      cov_pass_ms = ms_pass; cov_chol_ms = ms_chol;
+      cov_status = hf[COV_F_POINT_RANK] ? OSFM_COV_POINT_RANK_DEFICIENT
+                   : hf[COV_F_CHOL]     ? OSFM_COV_CAMERA_RANK_DEFICIENT
+                   : hf[COV_F_NONFINITE] ? OSFM_COV_NON_FINITE : OSFM_COV_OK;
+      if (trace_on && hf[COV_F_CHOL])
+        fprintf(stderr, "[osfm_ba] covariances: reduced system rank deficient at dense column %d\n", hf[COV_F_CHOL_COL]);
+    }
+    cov_valid = cov_status == OSFM_COV_OK;
+    if (!cov_valid) {   // bundle_adjuster.cc:1177-1192: the default for every instance, replacing whatever was computed
+      std::fill(cov_out.begin(), cov_out.end(), 0.0);
+      for (int i = 0; i < NI; ++i)
+        for (int j = 0; j < 6; ++j) cov_out[(size_t)i * 36 + j * 7] = j < 3 ? 1e-5 : 1e-2;
+    }
+    cov_ran = true;
+    trace("covariances");
+  }
   // ---- results back to the host ----
   OSFM_CUDA(cudaMemcpyAsync(cam_params.data(), d_cam[cur].p, sizeof(double) * cam_params.size(), cudaMemcpyDeviceToHost, stream));
   OSFM_CUDA(cudaMemcpyAsync(inst.data(), d_inst[cur].p, sizeof(double) * inst.size(), cudaMemcpyDeviceToHost, stream));
@@ -2698,6 +2880,34 @@ int osfm_ba_get_captured_parameters(osfm_ba* ba, double* cam_params, double* ins
   if (points)   // engine order -> the caller's
     for (size_t q = 0; q < b.cap_global_of.size(); ++q)
       for (int j = 0; j < 3; ++j) points[3 * (size_t)b.cap_global_of[q] + j] = b.cap_pts[3 * q + j];
+  OSFM_API_END
+}
+
+int osfm_ba_set_compute_covariances(osfm_ba* ba, int enable) {
+  OSFM_API_BEGIN
+  OSFM_BA_CHECK
+  ba->impl.cov_on = enable != 0;
+  OSFM_API_END
+}
+
+int osfm_ba_get_covariances(osfm_ba* ba, int* valid, int* status, double* out) {
+  OSFM_API_BEGIN
+  OSFM_BA_CHECK
+  const auto& b = ba->impl;
+  if (!b.cov_ran) throw std::runtime_error("the last run() did not compute covariances (not armed, or it failed)");
+  if (valid) *valid = b.cov_valid ? 1 : 0;
+  if (status) *status = b.cov_status;
+  if (out) std::copy(b.cov_out.begin(), b.cov_out.end(), out);
+  OSFM_API_END
+}
+
+int osfm_ba_get_covariance_timing(osfm_ba* ba, double* pass_ms, double* cholesky_ms) {
+  OSFM_API_BEGIN
+  OSFM_BA_CHECK
+  const auto& b = ba->impl;
+  if (!b.cov_ran) throw std::runtime_error("the last run() did not compute covariances (not armed, or it failed)");
+  if (pass_ms) *pass_ms = b.cov_pass_ms;
+  if (cholesky_ms) *cholesky_ms = b.cov_chol_ms;
   OSFM_API_END
 }
 

@@ -192,10 +192,26 @@ __global__ void bsr_prior_offsets(const int* pr_blk, const int* pr_local, int n,
 constexpr int SCHUR_THREADS = 128;
 constexpr int SCHUR_KC = 16;  // observations staged per chunk
 
+// Rank rule of the covariance pass (ba_cov.cuh): J is rank deficient when a Cholesky pivot is <= COV_TAU times
+// the original diagonal entry.  Point side: the pivots of the scaled, undamped [[a b c] [b d e] [c e f]] = V
+// (the negated tests also catch NaN).  Raises flag COV_F_POINT_RANK of the pass.
+constexpr double COV_TAU = 1e-10;
+constexpr int COV_F_POINT_RANK = 0;
+__device__ __forceinline__ bool point_rank_deficient(double a, double b, double c, double d, double e, double f) {
+  if (!(a > COV_TAU * a)) return true;
+  const double p1 = d - b * b / a;
+  if (!(p1 > COV_TAU * d)) return true;
+  const double q = e - b * c / a;
+  const double p2 = f - c * c / a - q * q / p1;
+  return !(p2 > COV_TAU * f);
+}
+
+// rank_flag != null (covariance pass, inv_radius = 0): the pivot test above on every free point's V
 __global__ void __launch_bounds__(SCHUR_THREADS)
     ba_schur(BAView v, BlkMaps bm, BsrView h, const double* __restrict__ scale, const double* __restrict__ diag,
              double inv_radius, double* __restrict__ Sval, double* __restrict__ rhs, double* __restrict__ Vinv,
-             double* __restrict__ gpo, int p_off, PointPriorView pp, const double* __restrict__ pts) {
+             double* __restrict__ gpo, int p_off, PointPriorView pp, const double* __restrict__ pts,
+             int* __restrict__ rank_flag) {
   extern __shared__ double sm[];
   const int wc = v.wc, nres = v.nres, nc = v.nc;
   double* Ya = sm;                                   // [KC][wc][3]
@@ -290,6 +306,7 @@ __global__ void __launch_bounds__(SCHUR_THREADS)
       const double a = acc[0] + diag[nc + 3 * pf] * inv_radius, b = acc[1], c = acc[2];
       const double d = acc[3] + diag[nc + 3 * pf + 1] * inv_radius, e = acc[4];
       const double f = acc[5] + diag[nc + 3 * pf + 2] * inv_radius;
+      if (rank_flag && point_rank_deficient(a, b, c, d, e, f)) *rank_flag = 1;
       const double A = d * f - e * e, B = c * e - b * f, Cc = b * e - c * d;
       const double id = 1.0 / (a * A + b * B + c * Cc);
       sVi[0] = A * id; sVi[1] = B * id; sVi[2] = Cc * id;
@@ -448,10 +465,11 @@ constexpr int SEG_KMAX = 16;
 constexpr int SEG_WCMAX = 16;
 constexpr int SEG_PCHUNK = 8;              // points staged per chunk
 
-// A0: V^-1, g_p, V^-1 g_p of the points [0, p_count)
+// A0: V^-1, g_p, V^-1 g_p of the points [0, p_count); rank_flag as in ba_schur
 __global__ void __launch_bounds__(128)
     ba_point_blocks(BAView v, int p_count, const double* __restrict__ scale, const double* __restrict__ diag,
-                    double inv_radius, double* __restrict__ Vinv, double* __restrict__ gpo, double* __restrict__ Vig) {
+                    double inv_radius, double* __restrict__ Vinv, double* __restrict__ gpo, double* __restrict__ Vig,
+                    int* __restrict__ rank_flag) {
   const int p = blockIdx.x * blockDim.x + threadIdx.x;
   if (p >= p_count) return;
   const int pf = v.pt_poff[p];
@@ -474,6 +492,7 @@ __global__ void __launch_bounds__(128)
   const double a = V[0] + diag[nc + 3 * pf] * inv_radius, b = V[1], c = V[2];
   const double d = V[3] + diag[nc + 3 * pf + 1] * inv_radius, e = V[4];
   const double f = V[5] + diag[nc + 3 * pf + 2] * inv_radius;
+  if (rank_flag && point_rank_deficient(a, b, c, d, e, f)) *rank_flag = 1;
   const double A = d * f - e * e, B = c * e - b * f, Cc = b * e - c * d;
   const double id = 1.0 / (a * A + b * B + c * Cc);
   const double i00 = A * id, i01 = B * id, i02 = Cc * id, i11 = (a * f - c * c) * id, i12 = (b * c - a * e) * id,
