@@ -1920,8 +1920,8 @@ void BA::build_system(double inv_radius, int* rank_flag, bool timed) {
     if (timed) rs.tm_schur.start(stream);
     if (rs.schur != OSFM_SCHUR_NONE) {
       d_Vig.reserve(3 * (size_t)std::max(rs.npf, 1));
-      ba_point_blocks<<<grid_for(P_fast, 128), 128, 0, stream>>>(rs.v, P_fast, d_scale.p, d_diag.p, inv_radius, d_Vinv.p,
-                                                               d_gp.p, d_Vig.p, rank_flag);
+      ba_point_blocks<<<grid_for(P_fast, PB_THREADS), PB_THREADS, 0, stream>>>(rs.v, P_fast, d_scale.p, d_diag.p, inv_radius,
+                                                                             d_Vinv.p, d_gp.p, d_Vig.p, rank_flag);
       OSFM_LAUNCH_CHECK();
     }
     if (rs.schur == OSFM_SCHUR_PIPE || rs.schur == OSFM_SCHUR_MMA) {

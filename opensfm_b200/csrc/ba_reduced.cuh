@@ -465,30 +465,56 @@ constexpr int SEG_KMAX = 16;
 constexpr int SEG_WCMAX = 16;
 constexpr int SEG_PCHUNK = 8;              // points staged per chunk
 
-// A0: V^-1, g_p, V^-1 g_p of the points [0, p_count); rank_flag as in ba_schur
-__global__ void __launch_bounds__(128)
+// A0: V^-1, g_p, V^-1 g_p of the points [0, p_count); rank_flag as in ba_schur.
+// One thread per point, but the plane values are not read by it: a thread's observations are contiguous, so a
+// warp's loads would be 80 bytes apart (one 32-byte sector per lane and load, 8x the bytes the kernel needs).  The
+// CTA's points own one contiguous observation range; it is staged through shared memory in tiles of PB_TILE
+// observations with coalesced loads, and every thread sums its own observations out of the tile in the same order.
+constexpr int PB_THREADS = 128;
+constexpr int PB_TILE = 256;
+__global__ void __launch_bounds__(PB_THREADS)
     ba_point_blocks(BAView v, int p_count, const double* __restrict__ scale, const double* __restrict__ diag,
                     double inv_radius, double* __restrict__ Vinv, double* __restrict__ gpo, double* __restrict__ Vig,
                     int* __restrict__ rank_flag) {
-  const int p = blockIdx.x * blockDim.x + threadIdx.x;
-  if (p >= p_count) return;
-  const int pf = v.pt_poff[p];
-  if (pf < 0) return;
+  __shared__ double tile[12][PB_TILE];   // r (nres) + Jp (3 nres) rows, nres <= 3
+  const int p0 = blockIdx.x * PB_THREADS;
+  const int p = p0 + threadIdx.x;
+  const int p_end = min(p0 + PB_THREADS, p_count);
+  const int pf = p < p_count ? v.pt_poff[p] : -1;
   const size_t N = (size_t)v.N;
-  const int nc = v.nc;
-  const double sp0 = scale[nc + 3 * pf], sp1 = scale[nc + 3 * pf + 1], sp2 = scale[nc + 3 * pf + 2];
+  const int nc = v.nc, nres = v.nres, nrows = 4 * nres;
+  double sp0 = 0.0, sp1 = 0.0, sp2 = 0.0;
+  long long my_lo = 0, my_hi = 0;
+  if (pf >= 0) {
+    sp0 = scale[nc + 3 * pf]; sp1 = scale[nc + 3 * pf + 1]; sp2 = scale[nc + 3 * pf + 2];
+    my_lo = v.pt_start[p]; my_hi = v.pt_start[p + 1];
+  }
   double V[9];
 #pragma unroll
   for (int j = 0; j < 9; ++j) V[j] = 0.0;
-  for (long long i = v.pt_start[p]; i < v.pt_start[p + 1]; ++i)
-    for (int q = 0; q < v.nres; ++q) {
-      const double x = v.Jp[((size_t)q * 3 + 0) * N + i] * sp0;
-      const double y = v.Jp[((size_t)q * 3 + 1) * N + i] * sp1;
-      const double z = v.Jp[((size_t)q * 3 + 2) * N + i] * sp2;
-      const double rq = v.r[q * N + i];
-      V[0] += x * x; V[1] += x * y; V[2] += x * z; V[3] += y * y; V[4] += y * z; V[5] += z * z;
-      V[6] += x * rq; V[7] += y * rq; V[8] += z * rq;
+  const long long o_lo = v.pt_start[p0], o_hi = v.pt_start[p_end];
+  for (long long t0 = o_lo; t0 < o_hi; t0 += PB_TILE) {
+    const int len = (int)min((long long)PB_TILE, o_hi - t0);
+    __syncthreads();   // the previous tile is consumed
+    for (int idx = threadIdx.x; idx < nrows * PB_TILE; idx += PB_THREADS) {
+      const int row = idx / PB_TILE, el = idx - row * PB_TILE;
+      if (el < len) tile[row][el] = row < nres ? v.r[(size_t)row * N + t0 + el] : v.Jp[(size_t)(row - nres) * N + t0 + el];
     }
+    __syncthreads();
+    const long long i0 = max(my_lo, t0), i1 = min(my_hi, t0 + len);
+    for (long long i = i0; i < i1; ++i) {
+      const int el = (int)(i - t0);
+      for (int q = 0; q < nres; ++q) {
+        const double x = tile[nres + q * 3 + 0][el] * sp0;
+        const double y = tile[nres + q * 3 + 1][el] * sp1;
+        const double z = tile[nres + q * 3 + 2][el] * sp2;
+        const double rq = tile[q][el];
+        V[0] += x * x; V[1] += x * y; V[2] += x * z; V[3] += y * y; V[4] += y * z; V[5] += z * z;
+        V[6] += x * rq; V[7] += y * rq; V[8] += z * rq;
+      }
+    }
+  }
+  if (pf < 0) return;
   const double a = V[0] + diag[nc + 3 * pf] * inv_radius, b = V[1], c = V[2];
   const double d = V[3] + diag[nc + 3 * pf + 1] * inv_radius, e = V[4];
   const double f = V[5] + diag[nc + 3 * pf + 2] * inv_radius;
