@@ -1044,6 +1044,7 @@ struct BA {
   PinnedBuf<PcgState> h_pcg;
   DevBuf<int> d_pcg_rowlo;
   DevBuf<int> d_pcg_grplo;
+  DevBuf<char> d_grp_shared;               // per preconditioner group: its two block rows share one column list
   DevBuf<unsigned long long> d_prof;
   DevBuf<long long> d_tab_off, d_tab_sizes;
   DevBuf<int> d_sp_nch, d_sp_chunk0;       // chunks per segment / first chunk of every segment (ba_schur_pipe)
@@ -1657,6 +1658,9 @@ void BA::plan_pcg() {
       const long long total = off_rows + 12LL * rows_max;
       rs.pcg_resident = switches().pcg_resident && monotone && nc <= 65535 && total + 1024 <= max_smem;
       rs.pcg_smem = rs.pcg_resident ? (int)total : 0;
+      if (switches().trace)
+        fprintf(stderr, "[osfm_ba] pcg plan: classic resident %s, %lld B of shared memory per CTA, %d B available\n",
+                rs.pcg_resident ? "on" : "off", total, max_smem - 1024);
       if (rs.pcg_resident) {
         upload(d_pcg_rowlo, row_lo, stream);
         PcgResident& pr = rs.pcg_res;
@@ -1665,51 +1669,32 @@ void BA::plan_pcg() {
         OSFM_CUDA(cudaFuncSetAttribute(pcg_persistent<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, rs.pcg_smem));
       }
     }
-    // pipelined PCG: whole preconditioner groups per CTA, balanced by stored entries
+    // pipelined PCG: whole preconditioner groups per CTA (ba_pcg_plan.h)
     {
-      std::vector<long long> wsum(ngroups + 1, 0);
-      auto gw_of = [&](int g, long long* cols, int* rows) {
-        long long w = 0;
-        for (int k = 0; k < 2; ++k) {
-          const int b = k ? rs.grp_b2[g] : rs.grp_b1[g];
-          if (b < 0) continue;
-          w += (long long)rs.blk_sz[b] * row_M[b];
-          if (cols) *cols += row_M[b];
-          if (rows) *rows += rs.blk_sz[b];
-        }
-        return w;
-      };
-      for (int g = 0; g < ngroups; ++g) wsum[g + 1] = wsum[g] + gw_of(g, nullptr, nullptr);
-      const std::vector<int> grp_lo = balanced_cut(wsum, G);
-      long long ent_max = 0, col_max = 0;
-      int rows_max = 0, grp_max = 0;
-      for (int c = 0; c < G; ++c) {
-        long long cols = 0;
-        int rows = 0;
-        for (int g = grp_lo[c]; g < grp_lo[c + 1]; ++g) gw_of(g, &cols, &rows);
-        ent_max = std::max(ent_max, wsum[grp_lo[c + 1]] - wsum[grp_lo[c]]);
-        col_max = std::max(col_max, cols);
-        rows_max = std::max(rows_max, rows);
-        grp_max = std::max(grp_max, grp_lo[c + 1] - grp_lo[c]);
-      }
-      const long long off_S = up16(8 * col_max), off_Minv = off_S + up16(8 * ent_max);
-      const long long off_vec = off_Minv + 8LL * grp_max * MAXB * MAXB, off_cols = off_vec + up16(24LL * rows_max);
-      const long long off_rows = off_cols + up16(2 * col_max);
-      const long long off_defl = up16(off_rows + 36LL * rows_max + 4LL * (grp_max + 1));
-      // own rows of the deflation vectors W and of S W, then the gather buffer of the wide barrier
-      const long long total = off_defl + 2LL * PCG_ND * 8 * rows_max + 8LL * PCG_NW * G + 8LL * PCG_NW * rows_max;
+      std::vector<int> row_ptr, row_col;
+      download(row_ptr, d_row_ptr.p, nblk + 1, stream);
+      download(row_col, d_row_col.p, rs.n_blocks_all, stream);
+      OSFM_CUDA(cudaStreamSynchronize(stream));
+      std::vector<char> shared(ngroups, 0);
+      for (int g = 0; g < ngroups; ++g) shared[g] = pcg_rows_share_columns(row_ptr, row_col, rs.grp_b1[g], rs.grp_b2[g]);
       cudaFuncAttributes pipe_attr{};
       OSFM_CUDA(cudaFuncGetAttributes(&pipe_attr, pcg_pipelined));
-      rs.pcg_pipe_ok = switches().pcg_pipelined && nc <= 65535 && rows_max <= PCG_THREADS && ent_max < (1LL << 30) &&
-                       total + (long long)pipe_attr.sharedSizeBytes + 1024 <= max_smem;
-      rs.pcg_pipe_smem = rs.pcg_pipe_ok ? (int)total : 0;
+      const PcgPipePlan plan = plan_pcg_pipelined(rs.grp_b1, rs.grp_b2, rs.blk_sz, row_M, shared, G,
+                                                  (long long)max_smem - (long long)pipe_attr.sharedSizeBytes - 1024);
+      rs.pcg_pipe_ok = switches().pcg_pipelined && nc <= 65535 && plan.fits;
+      rs.pcg_pipe_smem = rs.pcg_pipe_ok ? (int)plan.total : 0;
+      if (switches().trace)
+        fprintf(stderr, "[osfm_ba] pcg plan: pipelined %s, %lld B of shared memory per CTA, %lld B available (%d CTAs, "
+                "worst CTA: %lld entries, %lld columns, %d rows, %d groups)\n", rs.pcg_pipe_ok ? "on" : "off", plan.total,
+                plan.available, G, plan.max.ent, plan.max.cols, plan.max.rows, plan.max.groups);
       if (rs.pcg_pipe_ok) {
-        upload(d_pcg_grplo, grp_lo, stream);
+        upload(d_pcg_grplo, plan.grp_lo, stream);
+        upload(d_grp_shared, shared, stream);
         PcgPipe& pp = rs.pcg_pipe;
-        pp.grp_lo = d_pcg_grplo.p; pp.off_S = (int)off_S; pp.off_Minv = (int)off_Minv;
-        pp.off_vec = (int)off_vec; pp.off_cols = (int)off_cols; pp.off_rows = (int)off_rows;
-        pp.max_rows = rows_max; pp.max_groups = grp_max; pp.max_cols = (int)col_max;
-        pp.off_defl = (int)off_defl; pp.Wdef = nullptr;
+        pp.grp_lo = d_pcg_grplo.p; pp.grp_shared = d_grp_shared.p; pp.off_S = (int)plan.off_S;
+        pp.off_Minv = (int)plan.off_Minv; pp.off_vec = (int)plan.off_vec; pp.off_cols = (int)plan.off_cols;
+        pp.off_rows = (int)plan.off_rows; pp.max_rows = plan.max.rows; pp.max_groups = plan.max.groups;
+        pp.max_cols = (int)plan.max.cols; pp.off_defl = (int)plan.off_defl; pp.Wdef = nullptr;
         OSFM_CUDA(cudaFuncSetAttribute(pcg_pipelined, cudaFuncAttributeMaxDynamicSharedMemorySize, rs.pcg_pipe_smem));
       }
     }
@@ -2361,8 +2346,9 @@ void BA::run() {
     const double inv_radius = 1.0 / radius;
     build_system(inv_radius, nullptr, true);
     OSFM_CUDA(cudaMemsetAsync(d_y.p, 0, sizeof(double) * rs.nz, stream));
+    int pcg_path = 0;
     if (nc > 0) {
-      const int pcg_path = solve_reduced();
+      pcg_path = solve_reduced();
       if (it == cap_iter) capture_linear_system(it, radius, pcg_path);
     }
     ++n_solves;
@@ -2382,7 +2368,7 @@ void BA::run() {
       const PcgState& h = *h_pcg.p;
       const int pcg_it = h.iterations, its = std::max(pcg_it, 1);
       rs.pcg_total += pcg_it;
-      if (switches().trace)
+      if (switches().trace && (pcg_path == OSFM_PCG_CLASSIC_RESIDENT || pcg_path == OSFM_PCG_CLASSIC_STREAMED))  // classic
         fprintf(stderr, "[osfm_ba] pcg %d its, CTA0 clocks/it: stage %lld matvec %lld reduce1 %lld phaseB %lld reduce2 %lld (resident %d)\n",
                 pcg_it, h.prof[0] / its, h.prof[1] / its, h.prof[2] / its, h.prof[3] / its, h.prof[4] / its, (int)rs.pcg_resident);
       if (!(h.rr_final == h.rr_final)) ok = false;

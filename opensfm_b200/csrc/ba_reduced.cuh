@@ -16,6 +16,8 @@
 #pragma once
 #include <cub/cub.cuh>
 
+#include "ba_pcg_plan.h"
+
 namespace osfm {
 
 constexpr unsigned long long BSR_EMPTY = ~0ull;
@@ -1141,7 +1143,6 @@ __global__ void __launch_bounds__(256)
 // streams one scalar row with fully coalesced loads.
 // ---------------------------------------------------------------------------
 constexpr int MAXB = 16;
-constexpr int PCG_THREADS = 512;
 
 struct PcgLayout {
   const int* row_of;     // [nc] block row of every scalar row
@@ -1522,15 +1523,16 @@ __global__ void __launch_bounds__(PCG_THREADS, 1)
 // preconditioner groups: their rows of S, the groups' inverse blocks and all eight recurrence
 // vectors of those rows stay in shared memory / registers for the whole solve; the only vector that
 // moves through L2 is m = M^-1 w (nc doubles, double-buffered by iteration parity): after the barrier a
-// CTA gathers, per owned block row, the entries of m its columns need into a packed copy (mp), so the
-// rows then stream S and mp from shared memory without bank conflicts.
+// CTA gathers, per column list of its block rows, the entries of m those columns need into a packed copy
+// (mp), so the rows then stream S and mp from shared memory without bank conflicts.  The two block rows
+// of a group usually store the same block columns (a camera and the rig instance of its only shot); they
+// then share one column list and one packed copy.
 // The recurrences drift from the true residual earlier than classic CG; the kernel reports
 // converged = 0 on stagnation / breakdown and the host re-solves with pcg_persistent.
 // ---------------------------------------------------------------------------
-constexpr int PCG_ND = 7;   // deflation vectors: the similarity gauge of the rig instances (3 translations, 3 rotations, scale)
-constexpr int PCG_NW = 10;  // doubles per CTA on the wide barrier: gamma, delta, |r|^2, PCG_ND projections
-struct PcgPipe {
-  const int* grp_lo;  // [grid + 1] group range of every CTA (balanced by stored entries)
+struct PcgPipe {   // the layout of plan_pcg_pipelined (ba_pcg_plan.h)
+  const int* grp_lo;  // [grid + 1] group range of every CTA
+  const char* grp_shared;  // [ngroups] 1 = the two block rows of the group have one column list
   int off_S, off_Minv, off_vec, off_cols, off_rows;  // byte offsets into dynamic shared memory; mp at 0
   int off_defl;       // [2][PCG_ND][max_rows] doubles: own rows of W and of S W
   const double* Wdef; // [PCG_ND][nc] deflation vectors (scaled variables), or null: plain PCG
@@ -1659,8 +1661,9 @@ __global__ void __launch_bounds__(PCG_THREADS, 1)
   int* row_len = row_coff + R.max_rows;
   int* row_gidx = row_len + R.max_rows;
   int* grp_row0 = row_gidx + R.max_rows;  // [max_groups + 1]
-  // mat-vec units: up to three consecutive rows of one block row (they share the packed m of that block row)
-  int* unit_soff = grp_row0 + R.max_groups + 1;  // [max_rows] each
+  int* grp_moff = grp_row0 + R.max_groups + 1;  // [max_groups + 1] offset of the group's n x n inverse in Minv_s
+  // mat-vec units: up to three consecutive rows with one column list (they share its packed m)
+  int* unit_soff = grp_moff + R.max_groups + 1;  // [max_rows] each
   int* unit_coff = unit_soff + R.max_rows;
   int* unit_len = unit_coff + R.max_rows;
   int* unit_lr0 = unit_len + R.max_rows;
@@ -1682,13 +1685,16 @@ __global__ void __launch_bounds__(PCG_THREADS, 1)
 
   const int g_lo = R.grp_lo[blockIdx.x], g_hi = R.grp_lo[blockIdx.x + 1], ng = g_hi - g_lo;
   if (tid == 0) {
-    int lr = 0, s_off = 0, c_off = 0;
+    int lr = 0, s_off = 0, c_off = 0, m_off = 0;
     for (int g = g_lo; g < g_hi; ++g) {
       grp_row0[g - g_lo] = lr;
+      grp_moff[g - g_lo] = m_off;
+      const int lr0 = lr;
       for (int k = 0; k < 2; ++k) {
         const int b = k ? L.grp_b2[g] : L.grp_b1[g];
         if (b < 0) continue;
         const int n = h.blk_sz[b], M = L.row_M[b];
+        if (k && R.grp_shared[g]) c_off -= M;   // the second block row reads the first one's column list
         for (int r = 0; r < n; ++r, ++lr) {
           row_soff[lr] = s_off + r * M;
           row_coff[lr] = c_off;
@@ -1698,13 +1704,15 @@ __global__ void __launch_bounds__(PCG_THREADS, 1)
         s_off += n * M;
         c_off += M;
       }
+      m_off += (lr - lr0) * (lr - lr0);
     }
     grp_row0[ng] = lr;
+    grp_moff[ng] = m_off;
     s_nrows = lr;
     s_ncols = c_off;
     int nu = 0;
     for (int r0 = 0; r0 < lr;) {
-      int nr = 1;  // rows r0 .. r0 + nr - 1 belong to the same block row iff they share the column list
+      int nr = 1;  // rows r0 .. r0 + nr - 1 with one column list, consecutive in S_s (across the block rows of a group)
       while (nr < 3 && r0 + nr < lr && row_coff[r0 + nr] == row_coff[r0] && row_soff[r0 + nr] == row_soff[r0] + nr * row_len[r0]) ++nr;
       unit_soff[nu] = row_soff[r0]; unit_coff[nu] = row_coff[r0]; unit_len[nu] = row_len[r0]; unit_lr0[nu] = r0; unit_nr[nu] = nr;
       ++nu;
@@ -1718,21 +1726,26 @@ __global__ void __launch_bounds__(PCG_THREADS, 1)
     const int i = row_gidx[lr], b = L.row_of[i], M = row_len[lr];
     const double* src = Spcg + L.rowbase[b] + (long long)(i - h.blk_off[b]) * M;
     for (int q = lane; q < M; q += 32) S_s[row_soff[lr] + q] = __ldcs(src + q);
-    if (i == h.blk_off[b]) {
+    // the first row of a block row that owns its column list (not the second block row of a shared group)
+    if (i == h.blk_off[b] && (lr == 0 || row_coff[lr] != row_coff[lr - 1])) {
       const int* csrc = L.colidx + L.cbase[b];
       for (int q = lane; q < M; q += 32) cols_s[row_coff[lr] + q] = (unsigned short)csrc[q];
     }
   }
-  for (int t = tid; t < ng * MAXB * MAXB; t += blockDim.x) Minv_s[t] = Minv[(size_t)g_lo * MAXB * MAXB + t];
+  for (int gl = warp; gl < ng; gl += nwarps) {   // the group inverses, packed at n x n
+    const int n = grp_row0[gl + 1] - grp_row0[gl];
+    const double* src = Minv + (size_t)(g_lo + gl) * MAXB * MAXB;
+    for (int t = lane; t < n * n; t += 32) Minv_s[grp_moff[gl] + t] = src[(t / n) * MAXB + t % n];
+  }
 
   // group solve: n_s[rows of g] = Minv_g * w_s[rows of g]; optionally published to a global vector
   auto group_solve = [&](double* publish) {
     for (int gl = warp; gl < ng; gl += nwarps) {
       const int r0 = grp_row0[gl], n = grp_row0[gl + 1] - r0;
-      const double* M = Minv_s + gl * MAXB * MAXB;
+      const double* M = Minv_s + grp_moff[gl];
       double sv = 0.0;
       if (lane < n)
-        for (int j = 0; j < n; ++j) sv += M[lane * MAXB + j] * w_s[r0 + j];
+        for (int j = 0; j < n; ++j) sv += M[lane * n + j] * w_s[r0 + j];
       if (lane < n) {
         g_s[r0 + lane] = sv;
         publish[row_gidx[r0 + lane]] = sv;

@@ -51,6 +51,7 @@ def worker(tree, problem_path):
             "linearize_launches": s["linearize_launches"], "time_pcg_ms": s["time_pcg_ms"],
             "time_backsub_ms": s["time_backsub_ms"], "time_device_ms": s["time_device_ms"],
             "iterations": s["iterations"], "kernel_launches": s["kernel_launches"],
+            "pcg_iterations": s["pcg_iterations"], "linear_solves": s["linear_solves"],
             "value": pb.num_observations * s["iterations"] / (s["time_device_ms"] * 1e-3),
             "final_cost": s["final_cost"], "termination": s["termination"]}), flush=True)
 
@@ -102,8 +103,9 @@ def main():
                 for t, p in zip(names, procs):
                     row = ask(p)
                     report["runs"].setdefault(t, []).append(row)
-                    print("run %d %-40s schur %.3f ms/launch  device %.1f ms  value %.4e  its %d" % (
-                        r, t, row["schur_ms_per_launch"], row["time_device_ms"], row["value"], row["iterations"]), flush=True)
+                    print("run %d %-40s schur %.3f ms/launch  pcg %.2f ms (%d its / %d solves)  device %.1f ms  value %.4e  its %d" % (
+                        r, t, row["schur_ms_per_launch"], row["time_pcg_ms"], row["pcg_iterations"], row["linear_solves"],
+                        row["time_device_ms"], row["value"], row["iterations"]), flush=True)
         finally:
             for p in procs:
                 p.stdin.close()
@@ -114,7 +116,8 @@ def main():
             rows = report["runs"][t]
             summary[t] = {k: {"median": statistics.median(x[k] for x in rows), "min": min(x[k] for x in rows),
                               "max": max(x[k] for x in rows)}
-                          for k in ("schur_ms_per_launch", "time_device_ms", "value", "time_linearize_ms", "time_pcg_ms")}
+                          for k in ("schur_ms_per_launch", "time_device_ms", "value", "time_linearize_ms", "time_pcg_ms",
+                                    "pcg_iterations", "linear_solves", "iterations")}
         report["summary"] = summary
         if a.trace:
             report["trace"] = {}
@@ -127,7 +130,8 @@ def main():
                     p.wait()
                 with open(log) as ef:
                     lines = ef.read().splitlines()
-                report["trace"][names[i]] = [ln for ln in lines if "schur" in ln or "consumer group" in ln][-8:]
+                report["trace"][names[i]] = ([ln for ln in lines if "schur" in ln or "consumer group" in ln][-8:] +
+                                             [ln for ln in lines if "pcg" in ln])
     print(json.dumps({"card": report["card"], "library_mb": report["library_mb"], "summary": report["summary"], "trace": report.get("trace")}, indent=1))
     if a.out:
         with open(a.out, "w") as f:
