@@ -90,6 +90,11 @@ int osfm_matcher_match_pairs_async(osfm_matcher* m, int npairs, const int* ids_a
 int osfm_matcher_set_bearings(osfm_matcher* m, int id, const float* bearings_n_by_3);
 int osfm_matcher_match_pairs_guided_async(osfm_matcher* m, int npairs, const int* ids_a, const int* ids_b,
                                           const double* pose12, double threshold, double lowes_ratio, int symmetric);
+/* Test hook: the epipolar bitmask the last guided submission built for its pair `pair`, in both layouts the
+ * matcher uses -- F: n1 rows of ceil(n2 / 32) words (bit j % 32 of word j / 32 = feature j of image b passes for
+ * feature i of image a), T: n2 rows of ceil(n1 / 32) words, the transpose.  Fails if the last submission was not
+ * guided or `pair` is out of range. */
+int osfm_matcher_get_epipolar_masks(osfm_matcher* m, int pair, uint32_t* F, uint32_t* T);
 int osfm_matcher_sync(osfm_matcher* m);
 /* Copy the last batch's results to the host: concatenated per pair, n(ids_a[p]) entries each. */
 int osfm_matcher_fetch(osfm_matcher* m, int32_t* out_match, int64_t capacity);

@@ -74,6 +74,7 @@ SIGNATURES = {
     "osfm_matcher_set_bearings": (c_int, [c_void_p, c_int, c_void_p]),
     "osfm_matcher_match_pairs_guided_async": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_double, c_double,
                                                        c_int]),
+    "osfm_matcher_get_epipolar_masks": (c_int, [c_void_p, c_int, c_void_p, c_void_p]),
     "osfm_matcher_sync": (c_int, [c_void_p]),
     "osfm_matcher_fetch": (c_int, [c_void_p, c_void_p, c_int64]),
     "osfm_matcher_fetch_pairs": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, POINTER(c_int64)]),

@@ -470,14 +470,23 @@ struct EpiPair {
 __global__ void epi_vectors(const EpiPair* __restrict__ pairs) {
   const EpiPair& p = pairs[blockIdx.y];
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  const double tx = p.pose[9], ty = p.pose[10], tz = p.pose[11];
-  const double tn = sqrt(tx * tx + ty * ty + tz * tz);
-  const double t[3] = {tx / tn, ty / tn, tz / tn};
+  // Eigen's normalized() (Dot.h): a vector whose squared norm is 0 comes back unchanged.  So t = 0 gives zero
+  // epipolar vectors (symmetric_epi = 0: every element passes a positive threshold) and a bearing parallel to t
+  // a zero e, never a division by zero.
+  auto normalize = [](double v[3]) {
+    const double z = v[0] * v[0] + v[1] * v[1] + v[2] * v[2];
+    if (z > 0.0) {
+      const double n = sqrt(z);
+      v[0] /= n; v[1] /= n; v[2] /= n;
+    }
+  };
+  double t[3] = {p.pose[9], p.pose[10], p.pose[11]};
+  normalize(t);
   auto emit = [&](double* out, const double b[3]) {
     double e[3] = {t[1] * b[2] - t[2] * b[1], t[2] * b[0] - t[0] * b[2], t[0] * b[1] - t[1] * b[0]};
-    const double en = sqrt(e[0] * e[0] + e[1] * e[1] + e[2] * e[2]);
+    normalize(e);
     out[0] = b[0]; out[1] = b[1]; out[2] = b[2];
-    out[3] = e[0] / en; out[4] = e[1] / en; out[5] = e[2] / en;
+    out[3] = e[0]; out[4] = e[1]; out[5] = e[2];
   };
   if (i < p.n1) {
     const double b[3] = {(double)p.b1[3 * i], (double)p.b1[3 * i + 1], (double)p.b1[3 * i + 2]};
@@ -508,7 +517,10 @@ __global__ void __launch_bounds__(256) epi_mask_bits(const EpiPair* __restrict__
   const float NaNf = __int_as_float(0x7fc00000);
   float cj[6] = {NaNf, NaNf, NaNf, NaNf, NaNf, NaNf};
   if (j < p.n2) for (int e = 0; e < 6; ++e) cj[e] = (float)p.v2[6 * (size_t)j + e];
-  const float s_thr = (float)sin(threshold);
+  // The reference tests asin(sym) = pi/2 - acos(sym) < threshold; asin lies in [-pi/2, pi/2], where sin is
+  // increasing, so the clamped threshold decides the same.  Past pi/2 the test is sym < 1: the band around 1 goes
+  // to fp64, where sym > 1 gives acos = NaN and fails, as in the reference.
+  const float s_thr = (float)sin(fmin(fmax(threshold, -M_PI / 2.0), M_PI / 2.0));
   const float lo = s_thr - 2e-6f, hi = s_thr + 2e-6f;
   for (int ibl = 0; ibl < 8; ++ibl) {
     const int ib = ib0 + ibl;
@@ -675,8 +687,8 @@ int Matcher::add_async(const void* host, int n, int dim, bool u8, bool u8_as_l2)
   const int row_bytes = (int)(((size_t)dim * esz + 63) / 64 * 64);
   s.dim_padded = row_bytes / 4;  // in 4-byte elements
   s.row_bytes = row_bytes;
-  const bool tc = tc_capable(dim, u8, n);
-  const bool h8 = u8 && h8_capable(dim, n);     // Hamming on the tensor cores: +-1 fp8 operands
+  const bool tc = tc_capable(dim, u8);
+  const bool h8 = u8 && h8_capable(dim);     // Hamming on the tensor cores: +-1 fp8 operands
   const size_t data_bytes = ((size_t)std::max(n, 1) * row_bytes + 255) / 256 * 256;
   s.rows_padded = (tc || h8) ? tc_rows_padded(n) : 0;
   const size_t tc_bytes = tc ? tc_operand_bytes(s.rows_padded) : h8 ? h8_operand_bytes(s.rows_padded) : 0;
@@ -721,6 +733,10 @@ int Matcher::add_async(const void* host, int n, int dim, bool u8, bool u8_as_l2)
       OSFM_LAUNCH_CHECK();
     }
     if (h8) prepare_h8(s, static_cast<const uint8_t*>(s.data), row_bytes);
+  } else {
+    // a set without rows is trivially exact: its jobs have no query tiles or no train tiles, so it must not move
+    // the rest of a submission off the tensor cores
+    s.tc_ok = tc || h8;
   }
   const int id = next_id++;
   sets[id] = s;
@@ -774,6 +790,7 @@ void Matcher::match_pairs_async(int npairs, const int* ids_a, const int* ids_b, 
   if (npairs > 30000) throw ArgError("at most 30000 pairs per submission");
   const int ndir = symmetric ? 2 : 1;
   const int njobs = npairs * ndir;
+  last_masks.clear();
   h_jobs.assign(njobs, MatchJob());
   h_prefix.assign(njobs + 1, 0);
   h_out_off.assign(npairs + 1, 0);
@@ -793,7 +810,7 @@ void Matcher::match_pairs_async(int npairs, const int* ids_a, const int* ids_b, 
     // d^2 <= (|a| + |b|)^2 <= 2 (|a|^2 + |b|^2) must stay below 2^22 for the d^2-space ranking of the
     // tensor-core kernel to equal cv2's sqrt-space ranking (float32 sqrt injective on integers < 2^22)
     all_tc &= (!A.u8 && A.tc_ok && B.tc_ok && 2.0f * (A.tc_max_norm + B.tc_max_norm) < 4194304.0f);
-    all_h8 &= (A.u8 && A.tc_ok && B.tc_ok && A.tc_q != nullptr && B.tc_q != nullptr);
+    all_h8 &= (A.u8 && A.tc_ok && B.tc_ok);
     h_out_off[p + 1] = h_out_off[p] + A.n;
     for (int d = 0; d < ndir; ++d) {
       MatchJob& j = h_jobs[p * ndir + d];
@@ -851,6 +868,7 @@ void Matcher::match_pairs_async(int npairs, const int* ids_a, const int* ids_b, 
         j.mask_bits = d == 0 ? e.F : e.T;
         j.mask_words = d == 0 ? e.w2 : e.w1;
       }
+      last_masks.push_back(EpiMasks{e.F, e.T, e.n1, e.n2, e.w1, e.w2});
     }
   }
   // kernel choice
@@ -984,6 +1002,18 @@ void Matcher::match_pairs_async(int npairs, const int* ids_a, const int* ids_b, 
   }
   results_in_match_buf = !symmetric;
   OSFM_CUDA(cudaEventRecord(ev[3], stream));
+}
+
+void Matcher::get_epipolar_masks(int pair, uint32_t* F, uint32_t* T) {
+  if (last_masks.empty()) throw ArgError("the last submission was not guided");
+  if (pair < 0 || pair >= (int)last_masks.size()) throw ArgError("pair index out of range");
+  if (!F || !T) throw ArgError("null output");
+  OSFM_CUDA(cudaSetDevice(device));
+  const EpiMasks& e = last_masks[pair];
+  const size_t fw = (size_t)e.n1 * e.w2, tw = (size_t)e.n2 * e.w1;
+  if (fw) OSFM_CUDA(cudaMemcpyAsync(F, e.F, sizeof(uint32_t) * fw, cudaMemcpyDeviceToHost, stream));
+  if (tw) OSFM_CUDA(cudaMemcpyAsync(T, e.T, sizeof(uint32_t) * tw, cudaMemcpyDeviceToHost, stream));
+  OSFM_CUDA(cudaStreamSynchronize(stream));
 }
 
 void Matcher::sync() {
@@ -1203,8 +1233,16 @@ int osfm_matcher_match_pairs_guided_async(osfm_matcher* m, int npairs, const int
   OSFM_API_BEGIN
   OSFM_M_LOCK
   if (npairs > 0 && (!ids_a || !ids_b || !pose12)) throw osfm::ArgError("null pair list / poses");
-  if (!(threshold > 0.0)) throw osfm::ArgError("guided matching threshold must be positive");
+  // any threshold is the reference's comparison `angle < threshold`: at or below 0 nothing passes
+  if (std::isnan(threshold)) throw osfm::ArgError("guided matching threshold is NaN");
   m->impl.match_pairs_async(npairs, ids_a, ids_b, lowes_ratio, symmetric != 0, nullptr, pose12, threshold);
+  OSFM_API_END
+}
+
+int osfm_matcher_get_epipolar_masks(osfm_matcher* m, int pair, uint32_t* F, uint32_t* T) {
+  OSFM_API_BEGIN
+  OSFM_M_LOCK
+  m->impl.get_epipolar_masks(pair, F, T);
   OSFM_API_END
 }
 

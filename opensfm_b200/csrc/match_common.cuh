@@ -92,6 +92,12 @@ struct DescSet {
   int bear_slab = -1;
 };
 
+// The two layouts of one pair's epipolar bitmask in the last guided submission (the test hook reads them back).
+struct EpiMasks {
+  const uint32_t *F, *T;   // F: n1 rows of w2 words (over n2), T: n2 rows of w1 words (over n1)
+  int n1, n2, w1, w2;
+};
+
 struct Slab {
   char* base = nullptr;
   size_t cap = 0, used = 0;   // bump pointer
@@ -129,6 +135,7 @@ struct Matcher {
   DevBuf<long long> d_pair_off;
   DevBuf<int32_t> d_pairs;
   DevBuf<double> d_epi_vec, d_epi_pose;
+  std::vector<EpiMasks> last_masks;   // empty unless the last submission was guided
   PinnedBuf<double> p_epi_pose;
   PinnedBuf<MatchJob> p_jobs;
   PinnedBuf<int> p_prefix;
@@ -159,6 +166,7 @@ struct Matcher {
   void match_pairs_async(int npairs, const int* ids_a, const int* ids_b, double ratio, bool symmetric,
                          const uint8_t* dmask, const double* pose12 = nullptr, double epi_threshold = 0.0);
   void set_bearings(int id, const float* host_n_by_3);
+  void get_epipolar_masks(int pair, uint32_t* F, uint32_t* T);
   void sync();
   void fetch(int32_t* out, int64_t capacity);
   long long fetch_pairs(long long* offsets_out, int32_t* pairs_out, long long capacity_rows);
@@ -177,12 +185,12 @@ int tc_tile_n();
 void launch_tc(Matcher& m, int njobs, int ntiles, bool masked);
 int tc_rows_padded(int n);
 size_t tc_operand_bytes(int rows_padded);
-bool tc_capable(int dim, bool u8, int n);
+bool tc_capable(int dim, bool u8);
 // tensor-core Hamming (match_tc.cu)
 int h8_tile_m();
 int h8_tile_n();
 size_t h8_operand_bytes(int rows_padded);
-bool h8_capable(int nbytes, int n);
+bool h8_capable(int nbytes);
 void launch_tc_h8(Matcher& m, int njobs, int ntiles);
 
 }  // namespace osfm

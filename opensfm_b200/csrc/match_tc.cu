@@ -206,7 +206,7 @@ int tc_rows_padded(int n) {   // whole query tiles (and whole train tiles) of bo
   return (n + M - 1) / M * M;
 }
 size_t tc_operand_bytes(int rows_padded) { return 2 * (size_t)rows_padded * TC_ROW_BYTES + (size_t)rows_padded * sizeof(float); }
-bool tc_capable(int dim, bool u8, int n) { return !u8 && dim <= TC_KD && n > 0 && tc_available(); }
+bool tc_capable(int dim, bool u8) { return !u8 && dim <= TC_KD && tc_available(); }
 
 // ---------------------------------------------------------------------------
 // PTX wrappers
@@ -517,6 +517,10 @@ __global__ void __launch_bounds__(WG_THREADS, 1)
         o.i2 = __shfl_xor_sync(0xffffffffu, a.i2, off);
         top2_merge(a, o);
       }
+      // padding trains (index >= nt) lose to every real one but still enter the list of a query with fewer than
+      // two real candidates (Hamming scores them finite): a train set of one row must give no match, as in cv2
+      if (a.i2 >= t.job.nt) a.i2 = -1;
+      if (a.i1 >= t.job.nt) a.i1 = -1;
       const int gq = t.q0 + wg_row0 + (r >> 1) * 64 + 16 * w + (lane >> 2) + 8 * (r & 1);
       if (quad == 0 && gq < t.job.nq) {
         Top2 out;
@@ -546,14 +550,14 @@ __global__ void __launch_bounds__(WG_THREADS, 1)
 // inside the precision the fp8 MMA keeps), and its ranking inside a query row is cv2's ranking by Hamming distance
 // (ties -> lowest index through the same epilogue as the L2 kernel).  K = 512 fp8 per row; positions beyond nbits
 // are 0 in real rows of both roles (they add nothing), +1 in every query row and +448 in the *padding* rows of a
-// train set, so a padding train scores >= 8 * 448 - nbits > any real one and is never selected (needs >= 8 spare
-// positions: nbytes <= 63).  wgmma m64 n128 k32 e4m3, operands in the same no-swizzle K-major core-matrix order as
+// train set, so a padding train scores >= 8 * 448 - nbits > any real one and never ranks above it (needs >= 8 spare
+// positions: nbytes <= 63); the epilogue drops the padding trains a query with fewer than two real ones keeps.  wgmma m64 n128 k32 e4m3, operands in the same no-swizzle K-major core-matrix order as
 // the bf16 kernel (a core matrix row is 16 bytes = 16 fp8), 512 B per row.
 // ===========================================================================================================
 int h8_tile_m() { return WgGeom<KIND_HAMMING>::M; }
 int h8_tile_n() { return WG_N; }
 size_t h8_operand_bytes(int rows_padded) { return 2 * (size_t)rows_padded * H8_ROW_BYTES; }
-bool h8_capable(int nbytes, int n) { return nbytes >= 1 && nbytes <= 63 && n > 0 && tc_available(); }
+bool h8_capable(int nbytes) { return nbytes >= 1 && nbytes <= 63 && tc_available(); }
 
 // one thread per (row, 16-byte K chunk): 16 bits of the source row -> 16 fp8 values in both roles
 __global__ void __launch_bounds__(256)

@@ -232,6 +232,27 @@ class PairMatcher:
             start = end
         return out
 
+    def last_epipolar_masks(self, i: int) -> Tuple[np.ndarray, np.ndarray]:
+        """Test hook: the epipolar masks the last guided submission built on the device for its pair i, as boolean
+        arrays (n1 x n2 for the a -> b pass, n2 x n1 for the b -> a pass).  `match_pairs_guided` submits in rounds of
+        `mask_budget_bytes`; this reads the last round, whose pairs are numbered from 0.  Raises ValueError if the
+        last submission was not guided or i is out of range."""
+        n1 = n2 = 0
+        if 0 <= i < len(self._pairs):
+            a, b = self._pairs[i]
+            n1, n2 = self._n[a], self._n[b]
+        F = np.zeros((n1, (n2 + 31) // 32), dtype=np.uint32)
+        T = np.zeros((n2, (n1 + 31) // 32), dtype=np.uint32)
+        _lib.check(self._m.L.osfm_matcher_get_epipolar_masks(self._m.h, int(i), F.ctypes.data_as(ctypes.c_void_p),
+                                                             T.ctypes.data_as(ctypes.c_void_p)))
+
+        def bits(words: np.ndarray, ncols: int) -> np.ndarray:
+            # word w, bit k = column 32 w + k: little-endian bytes, least significant bit first
+            u8 = words.astype("<u4").view(np.uint8).reshape(words.shape[0], -1)
+            return np.unpackbits(u8, axis=1, bitorder="little")[:, :ncols].astype(bool)
+
+        return bits(F, n2), bits(T, n1)
+
     def sync(self) -> None:
         _lib.check(self._m.L.osfm_matcher_sync(self._m.h))
 

@@ -128,24 +128,42 @@ def match_brute_force_symmetric_numpy(fi, fj, config, maskij=None) -> List[Tuple
     return list(mij & mji)
 
 
+def _eigen_normalized(v: np.ndarray) -> np.ndarray:
+    """Eigen's `normalized()` row by row (Eigen/src/Core/Dot.h since 3.3): v / sqrt(squaredNorm) when the squared
+    norm is positive, the vector unchanged (no division by zero) when it is 0."""
+    z = np.einsum("...i,...i->...", v, v)[..., None]
+    return np.where(z > 0.0, v / np.sqrt(np.where(z > 0.0, z, 1.0)), v)
+
+
+def epipolar_sym(b1: np.ndarray, b2: np.ndarray, R: np.ndarray, t: np.ndarray) -> np.ndarray:
+    """The n1 x n2 fp64 `symmetric_epi` of geometry::EpipolarAngleTwoBearingsMany
+    (opensfm/src/geometry/src/triangulation.cc:195-219) on float32 bearings (matching.py:860-861):
+    (|e1_i . R b2_j| + |b1_i . e2_j|) / 2 with e1_i = normalized(t^ x b1_i), e2_j = normalized(t^ x R b2_j),
+    t^ = normalized(t).  A zero t or a bearing parallel to t gives zero vectors, as in Eigen."""
+    b1 = np.asarray(b1).astype(np.float32).astype(np.float64)
+    b2 = np.asarray(b2).astype(np.float32).astype(np.float64)
+    R = np.asarray(R, dtype=np.float64).reshape(3, 3)
+    tn = _eigen_normalized(np.asarray(t, dtype=np.float64).reshape(3))
+    b2w = b2 @ R.T
+    e1 = _eigen_normalized(np.cross(tn, b1))
+    e2 = _eigen_normalized(np.cross(tn, b2w))
+    return (np.abs(e1 @ b2w.T) + np.abs(b1 @ e2.T)) / 2.0
+
+
+def epipolar_angles(b1: np.ndarray, b2: np.ndarray, R: np.ndarray, t: np.ndarray) -> np.ndarray:
+    """EpipolarAngleTwoBearingsMany: pi/2 - acos(symmetric_epi), NaN where the fp64 value exceeds 1."""
+    with np.errstate(invalid="ignore"):
+        return np.pi / 2.0 - np.arccos(epipolar_sym(b1, b2, R, t))
+
+
 def epipolar_mask(b1: np.ndarray, b2: np.ndarray, R: np.ndarray, t: np.ndarray, threshold: float) -> np.ndarray:
     """matching.compute_inliers_bearing_epipolar (opensfm/matching.py:847-868) around
     geometry::EpipolarAngleTwoBearingsMany (opensfm/src/geometry/src/triangulation.cc:195-219), restated in numpy
     fp64: bearings are cast to float32 first (matching.py:860-861), R = pose.get_R_cam_to_world(),
-    t = pose.get_origin() of image 2 relative to image 1.  Returns the boolean n1 x n2 mask."""
-    b1 = np.asarray(b1).astype(np.float32).astype(np.float64)
-    b2 = np.asarray(b2).astype(np.float32).astype(np.float64)
-    R = np.asarray(R, dtype=np.float64).reshape(3, 3)
-    t = np.asarray(t, dtype=np.float64).reshape(3)
-    tn = t / np.linalg.norm(t)
-    b2w = b2 @ R.T
-    with np.errstate(invalid="ignore", divide="ignore"):
-        e1 = np.cross(tn, b1)
-        e1 = e1 / np.linalg.norm(e1, axis=1, keepdims=True)
-        e2 = np.cross(tn, b2w)
-        e2 = e2 / np.linalg.norm(e2, axis=1, keepdims=True)
-        sym = (np.abs(e1 @ b2w.T) + np.abs(b1 @ e2.T)) / 2.0
-        return (np.pi / 2.0 - np.arccos(sym)) < threshold
+    t = pose.get_origin() of image 2 relative to image 1.  Returns the boolean n1 x n2 mask `angle < threshold`
+    (false where the angle is NaN)."""
+    with np.errstate(invalid="ignore"):
+        return epipolar_angles(b1, b2, R, t) < threshold
 
 
 def match_using_words(f1: np.ndarray, words1: np.ndarray, f2: np.ndarray, words2_first: np.ndarray, lowes_ratio: float,
