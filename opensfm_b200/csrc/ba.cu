@@ -344,10 +344,10 @@ __device__ __forceinline__ void seg_scan_by_point(int pt, double (&val)[NV]) {
   }
 }
 
-// Point-side columns: one thread per observation (coalesced plane reads), run totals by shuffles,
-// one atomic per (run, column) -- a run is cut only at warp boundaries.
-__global__ void __launch_bounds__(256) ba_colnorm_grad_points(BAView v, double* colnorm2, double* grad) {
-  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+// Point-side columns of the observations i >= i0: one thread per observation (coalesced plane reads), run totals
+// by shuffles, one atomic per (run, column) -- a run is cut only at warp boundaries.
+__global__ void __launch_bounds__(256) ba_colnorm_grad_points(BAView v, long long i0, double* colnorm2, double* grad) {
+  const long long i = i0 + (long long)blockIdx.x * blockDim.x + threadIdx.x;
   const size_t N = (size_t)v.N;
   const bool in = i < v.N;
   const int pt = in ? v.obs_point[i] : -1;
@@ -940,6 +940,7 @@ struct RunState {
   int schur = OSFM_SCHUR_NONE;    // OSFM_SCHUR_*: the segment kernel of build_system
   bool seg_tab = false;           // ba_seg_tables has run (gcol of every segment column)
   int sp_nchunks = 0;             // chunk list of ba_schur_pipe (0 = none)
+  bool lin_fused = false;         // ba_linearize_fused: the linearisation also forms the sums of ba_point_blocks_sums
   bool pcg_resident = false, pcg_pipe_ok = false;   // the classic PCG keeps S in shared memory; pipelined PCG fits
   int pcg_smem = 0, pcg_pipe_smem = 0;
   PcgResident pcg_res{};
@@ -1051,6 +1052,7 @@ struct BA {
   DevBuf<SchurChunk> d_sp_chunks;
   DevBuf<int> d_sp_ftab;                   // flush destinations per segment (sp_flush_tables)
   DevBuf<int> d_tab;
+  DevBuf<double> d_ptsum;                  // [9][npf] unscaled Jp^T Jp (upper) and Jp^T r per point (ba_linearize_fused)
   std::vector<const void*> smem_opted;     // kernels opted into their dynamic shared memory (per handle = per device)
   int num_sms = 132;
   DevBuf<int> d_pr_cam_param, d_pr_cam_col, d_pr_cam_log, d_pr_pos_inst, d_pr_pos_axis, d_pr_pos_col;
@@ -1163,7 +1165,7 @@ struct BA {
 
   void run();
   void plan_layout(), order_observations(), plan_prior_rows(), upload_problem(), discover_structure(), plan_pcg(),
-      reserve_covariance(), build_segment_tables();
+      reserve_covariance(), build_segment_tables(), segment_table_scales();
   double eval_cost(int b), linearize(int b, bool timed, double* grad_max);
   void build_system(double inv_radius, int* rank_flag, bool timed), back_substitute();
   int solve_reduced();
@@ -1737,8 +1739,9 @@ void BA::reserve_covariance() {
   d_cov_flags.reserve(COV_F_COUNT);
 }
 
-// Per-segment tables of the tensor-core Schur kernels (columns, block offsets, Jacobi scales) and the chunk list of
-// the persistent one; decides the Schur path of the run.  The scale is constant from here on.
+// Per-segment tables of the tensor-core Schur kernels (columns, block offsets) and the chunk list of the persistent
+// one; decides the Schur path of the run and whether the linearisation runs over the chunk list (ba_linearize_fused).
+// Structure only, before the first linearisation: the Jacobi scales of the tables follow in segment_table_scales().
 void BA::build_segment_tables() {
   const int nseg = rs.nseg, wc = rs.wc;
   // The tensor-core kernels add the same-shot blocks J^T J only in the tiles (t, t) and (t, t + 1): a shot's wc
@@ -1759,7 +1762,7 @@ void BA::build_segment_tables() {
     OSFM_CUDA(cudaMemcpyAsync(&total_ints, d_tab_off.p + nseg, sizeof(long long), cudaMemcpyDeviceToHost, stream));
     OSFM_CUDA(cudaStreamSynchronize(stream));
     d_tab.reserve((size_t)total_ints + 2);
-    ba_seg_tables<<<nseg, 128, 0, stream>>>(rs.v, rs.bm, rs.bsr, d_seg_start.p, d_scale.p, d_tab_off.p, d_tab.p);
+    ba_seg_tables<<<nseg, 128, 0, stream>>>(rs.v, rs.bm, rs.bsr, d_seg_start.p, nullptr, d_tab_off.p, d_tab.p);
     OSFM_LAUNCH_CHECK();
     rs.seg_tab = true;
     // chunk list of the persistent Schur kernel (ba_schur_pipe.cuh)
@@ -1789,6 +1792,14 @@ void BA::build_segment_tables() {
   rs.schur = nseg == 0 ? OSFM_SCHUR_NONE
              : !use_mma ? OSFM_SCHUR_SIMT_SEGMENT
              : (use_pipe && rs.sp_nchunks > 0) ? OSFM_SCHUR_PIPE : OSFM_SCHUR_MMA;
+  rs.lin_fused = rs.sp_nchunks > 0 && wc == 9 && rs.nres == 2 && rs.uniform_type == PT_PERSPECTIVE;
+}
+
+// The Jacobi scale of every segment column into the tables, whenever d_scale has been (re)computed.
+void BA::segment_table_scales() {
+  if (!rs.seg_tab) return;
+  ba_seg_scales<<<rs.nseg, 128, 0, stream>>>(rs.v, d_seg_start.p, d_scale.p, d_tab_off.p, d_tab.p);
+  OSFM_LAUNCH_CHECK();
 }
 
 // cost at parameter set b (sum over ranks)
@@ -1820,15 +1831,31 @@ double BA::linearize(int b, bool timed, double* grad_max) {
   OSFM_CUDA(cudaMemsetAsync(d_sc.p, 0, sizeof(Scalars), stream));
   OSFM_CUDA(cudaMemsetAsync(d_colnorm2.p, 0, sizeof(double) * rs.nz, stream));
   OSFM_CUDA(cudaMemsetAsync(d_grad.p, 0, sizeof(double) * rs.nz, stream));
-  if (N > 0) {
+  if (N > 0 && rs.lin_fused) {
+    // planes, cost and the segment observations' column norms / gradient / point sums in one pass; the observations
+    // outside the segments get their sums from the plane-reading kernels
+    d_ptsum.reserve(9 * (size_t)std::max(rs.npf, 1));
+    const int grid = (int)((n_fast_obs + FL_WIN - 1) / FL_WIN + (N - n_fast_obs + FL_THREADS - 1) / FL_THREADS);
+    if (timed) rs.tm_lin.start(stream);
+    ba_linearize_fused<PT_PERSPECTIVE><<<grid, FL_THREADS, 0, stream>>>(rs.v, params_of(b), d_sc.p, d_sp_chunks.p, rs.sp_nchunks,
+                                                                        n_fast_obs, d_tab.p, d_colnorm2.p, d_grad.p, d_ptsum.p);
+    OSFM_LAUNCH_CHECK();
+    if (timed) rs.tm_lin.stop(stream);
+    if (N > n_fast_obs) {
+      ba_colnorm_grad_points<<<grid_for(N - n_fast_obs, 256), 256, 0, stream>>>(rs.v, n_fast_obs, d_colnorm2.p, d_grad.p);
+      OSFM_LAUNCH_CHECK();
+      ba_colnorm_grad<<<grid_for(N - n_fast_obs, 256), 256, 0, stream>>>(rs.v, n_fast_obs, d_colnorm2.p, d_grad.p);
+      OSFM_LAUNCH_CHECK();
+    }
+  } else if (N > 0) {
     if (timed) rs.tm_lin.start(stream);
     launch_linearize<1>(b);
     if (timed) rs.tm_lin.stop(stream);
-    ba_colnorm_grad_points<<<grid_for(N, 256), 256, 0, stream>>>(rs.v, d_colnorm2.p, d_grad.p);
+    ba_colnorm_grad_points<<<grid_for(N, 256), 256, 0, stream>>>(rs.v, 0, d_colnorm2.p, d_grad.p);
     OSFM_LAUNCH_CHECK();
     if (nseg > 0) {
       if (wc == 9 && rs.nres == 2 && rs.sp_nchunks > 0) {
-        // the chunk list exists (every call but the first of a run): no dependent index loads
+        // the chunk list exists: no dependent index loads
         opt_in_smem(ba_colnorm_grad_chunks, CC_SMEM);
         const int grid = std::max(1, std::min(num_sms, (rs.sp_nchunks + CC_WARPS - 1) / CC_WARPS));
         ba_colnorm_grad_chunks<<<grid, 32 * CC_WARPS, CC_SMEM, stream>>>(rs.v, d_sp_chunks.p, rs.sp_nchunks, d_tab.p,
@@ -1905,8 +1932,12 @@ void BA::build_system(double inv_radius, int* rank_flag, bool timed) {
     if (timed) rs.tm_schur.start(stream);
     if (rs.schur != OSFM_SCHUR_NONE) {
       d_Vig.reserve(3 * (size_t)std::max(rs.npf, 1));
-      ba_point_blocks<<<grid_for(P_fast, PB_THREADS), PB_THREADS, 0, stream>>>(rs.v, P_fast, d_scale.p, d_diag.p, inv_radius,
-                                                                             d_Vinv.p, d_gp.p, d_Vig.p, rank_flag);
+      if (rs.lin_fused)   // the point sums of the linearisation
+        ba_point_blocks_sums<<<grid_for(P_fast, PB_THREADS), PB_THREADS, 0, stream>>>(
+            rs.v, P_fast, d_ptsum.p, d_scale.p, d_diag.p, inv_radius, d_Vinv.p, d_gp.p, d_Vig.p, rank_flag);
+      else
+        ba_point_blocks<<<grid_for(P_fast, PB_THREADS), PB_THREADS, 0, stream>>>(rs.v, P_fast, d_scale.p, d_diag.p, inv_radius,
+                                                                               d_Vinv.p, d_gp.p, d_Vig.p, rank_flag);
       OSFM_LAUNCH_CHECK();
     }
     if (rs.schur == OSFM_SCHUR_PIPE || rs.schur == OSFM_SCHUR_MMA) {
@@ -2092,7 +2123,7 @@ void BA::capture_linear_system(int it, double radius, int pcg_path) {
 
 // Rig-instance covariances (ba_cov.cuh) at the accepted parameters: not after a FAILURE termination, as in the reference
 void BA::covariance_pass(int termination) {
-  const int nc = rs.nc, n = rs.n, NI = rs.NI, nseg = rs.nseg;
+  const int nc = rs.nc, n = rs.n, NI = rs.NI;
   cov_out.assign((size_t)NI * 36, 0.0);
   cov_status = OSFM_COV_SOLVER_FAILURE;
   cov_pass_ms = cov_chol_ms = 0.0;
@@ -2139,10 +2170,7 @@ void BA::covariance_pass(int termination) {
       ba_make_diag<<<grid_for(n, 256), 256, 0, stream>>>(d_colnorm2.p, d_scale.p, d_diag.p, n);
       OSFM_LAUNCH_CHECK();
     }
-    if (rs.seg_tab) {   // the tensor-core Schur kernels read the scale from their segment tables
-      ba_seg_tables<<<nseg, 128, 0, stream>>>(rs.v, rs.bm, rs.bsr, d_seg_start.p, d_scale.p, d_tab_off.p, d_tab.p);
-      OSFM_LAUNCH_CHECK();
-    }
+    segment_table_scales();   // the tensor-core Schur kernels read the scale from their segment tables
     build_system(0.0, flags + COV_F_POINT_RANK, false);
     OSFM_CUDA(cudaEventRecord(ce[1], stream));
     auto tiles = [](int k) { return (k + COV_NB - 1) / COV_NB; };
@@ -2313,6 +2341,7 @@ void BA::run() {
   int termination = 1;
   std::string message = "Maximum number of iterations reached.";
 
+  build_segment_tables();
   double grad_max = 0.0;
   double cost = linearize(cur, true, &grad_max);
   const double initial_cost = cost;
@@ -2320,6 +2349,7 @@ void BA::run() {
     ba_make_scale<<<grid_for(n, 256), 256, 0, stream>>>(d_colnorm2.p, d_scale.p, n);
     OSFM_LAUNCH_CHECK();
   }
+  segment_table_scales();   // the scale is constant from here on
   // deflation vectors of the reduced solve: the similarity gauge at the initial poses, in the scaled variables
   if (switches().pcg_deflate && rs.pcg_pipe_ok && rs.NI > 0 && nc > 0) {
     d_Wdef.reserve((size_t)PCG_ND * nc);
@@ -2328,7 +2358,6 @@ void BA::run() {
     OSFM_LAUNCH_CHECK();
     rs.pcg_pipe.Wdef = d_Wdef.p;
   }
-  build_segment_tables();
   double x_norm = n > 0 ? x_norm_of(cur) : 0.0;
 
   if (grad_max <= gtol || n == 0) {

@@ -474,6 +474,28 @@ constexpr int SEG_PCHUNK = 8;              // points staged per chunk
 // observations with coalesced loads, and every thread sums its own observations out of the tile in the same order.
 constexpr int PB_THREADS = 128;
 constexpr int PB_TILE = 256;
+// Damps the scaled V (upper triangle xx xy xz yy yz zz) and g_p (V[6..8]) of free point pf, tests its rank, stores
+// V^-1, g_p and V^-1 g_p.
+__device__ __forceinline__ void point_block_finish(const BAView& v, int pf, const double (&V)[9], const double* __restrict__ diag,
+                                                   double inv_radius, double* __restrict__ Vinv, double* __restrict__ gpo,
+                                                   double* __restrict__ Vig, int* __restrict__ rank_flag) {
+  const int nc = v.nc;
+  const double a = V[0] + diag[nc + 3 * pf] * inv_radius, b = V[1], c = V[2];
+  const double d = V[3] + diag[nc + 3 * pf + 1] * inv_radius, e = V[4];
+  const double f = V[5] + diag[nc + 3 * pf + 2] * inv_radius;
+  if (rank_flag && point_rank_deficient(a, b, c, d, e, f)) *rank_flag = 1;
+  const double A = d * f - e * e, B = c * e - b * f, Cc = b * e - c * d;
+  const double id = 1.0 / (a * A + b * B + c * Cc);
+  const double i00 = A * id, i01 = B * id, i02 = Cc * id, i11 = (a * f - c * c) * id, i12 = (b * c - a * e) * id,
+               i22 = (a * d - b * b) * id;
+  const size_t NP = (size_t)v.npf;
+  Vinv[0 * NP + pf] = i00; Vinv[1 * NP + pf] = i01; Vinv[2 * NP + pf] = i02;
+  Vinv[3 * NP + pf] = i11; Vinv[4 * NP + pf] = i12; Vinv[5 * NP + pf] = i22;
+  gpo[0 * NP + pf] = V[6]; gpo[1 * NP + pf] = V[7]; gpo[2 * NP + pf] = V[8];
+  Vig[0 * NP + pf] = i00 * V[6] + i01 * V[7] + i02 * V[8];
+  Vig[1 * NP + pf] = i01 * V[6] + i11 * V[7] + i12 * V[8];
+  Vig[2 * NP + pf] = i02 * V[6] + i12 * V[7] + i22 * V[8];
+}
 __global__ void __launch_bounds__(PB_THREADS)
     ba_point_blocks(BAView v, int p_count, const double* __restrict__ scale, const double* __restrict__ diag,
                     double inv_radius, double* __restrict__ Vinv, double* __restrict__ gpo, double* __restrict__ Vig,
@@ -517,21 +539,7 @@ __global__ void __launch_bounds__(PB_THREADS)
     }
   }
   if (pf < 0) return;
-  const double a = V[0] + diag[nc + 3 * pf] * inv_radius, b = V[1], c = V[2];
-  const double d = V[3] + diag[nc + 3 * pf + 1] * inv_radius, e = V[4];
-  const double f = V[5] + diag[nc + 3 * pf + 2] * inv_radius;
-  if (rank_flag && point_rank_deficient(a, b, c, d, e, f)) *rank_flag = 1;
-  const double A = d * f - e * e, B = c * e - b * f, Cc = b * e - c * d;
-  const double id = 1.0 / (a * A + b * B + c * Cc);
-  const double i00 = A * id, i01 = B * id, i02 = Cc * id, i11 = (a * f - c * c) * id, i12 = (b * c - a * e) * id,
-               i22 = (a * d - b * b) * id;
-  const size_t NP = (size_t)v.npf;
-  Vinv[0 * NP + pf] = i00; Vinv[1 * NP + pf] = i01; Vinv[2 * NP + pf] = i02;
-  Vinv[3 * NP + pf] = i11; Vinv[4 * NP + pf] = i12; Vinv[5 * NP + pf] = i22;
-  gpo[0 * NP + pf] = V[6]; gpo[1 * NP + pf] = V[7]; gpo[2 * NP + pf] = V[8];
-  Vig[0 * NP + pf] = i00 * V[6] + i01 * V[7] + i02 * V[8];
-  Vig[1 * NP + pf] = i01 * V[6] + i11 * V[7] + i12 * V[8];
-  Vig[2 * NP + pf] = i02 * V[6] + i12 * V[7] + i22 * V[8];
+  point_block_finish(v, pf, V, diag, inv_radius, Vinv, gpo, Vig, rank_flag);
 }
 
 // A1: rows of every (observation i < n_obs, local column c2) in plane layout rows[(c2*3 + j) * n_obs + i]
@@ -786,7 +794,8 @@ struct SegMmaSmem {
   int offt[SEG_KMAX * SEG_KMAX * 9];
 };
 
-// Per-segment tables (constant over the LM iterations of a run, built once by ba_seg_tables):
+// Per-segment tables (constant over the LM iterations of a run, built once by ba_seg_tables before the first
+// linearisation; scol by ba_seg_scales once the Jacobi scale is known, or by ba_seg_tables when it is given one):
 //   [ gcol (ncols) | meta (ncols) | offt (k (k + 1) / 2 shot pairs a <= b, 9 slot pairs each) ] ints, then
 //   scol (ncols doubles, 8-byte aligned).  tab_off[s] = offset of segment s in ints.
 __host__ __device__ inline int seg_pair_index(int a, int b, int k) { return a * k - a * (a - 1) / 2 + (b - a); }
@@ -836,7 +845,7 @@ __global__ void __launch_bounds__(128)
     }
     gcol[t] = g;
     meta[t] = m;
-    scol[t] = g >= 0 ? scale[g] : 0.0;
+    if (scale) scol[t] = g >= 0 ? scale[g] : 0.0;
   }
   __syncthreads();
   for (int idx = threadIdx.x; idx < k * k * 9; idx += blockDim.x) {
@@ -846,6 +855,21 @@ __global__ void __launch_bounds__(128)
     const int B1 = oblk[a][ss / 3], B2 = oblk[bb][ss % 3];
     offt[seg_pair_index(a, bb, k) * 9 + ss] = (B1 < 0 || B2 < 0) ? -1 : bsr_lookup(h, min(B1, B2), max(B1, B2));
   }
+}
+
+// The Jacobi scale of every segment column (scol of the tables above), from gcol: once the scale is known, and again
+// when it changes (the covariance pass).  One CTA per segment.
+__global__ void __launch_bounds__(128)
+    ba_seg_scales(BAView v, const int* __restrict__ seg_start, const double* __restrict__ scale,
+                  const long long* __restrict__ tab_off, int* __restrict__ tab) {
+  const int p0 = seg_start[blockIdx.x];
+  const int k = (int)(v.pt_start[p0 + 1] - v.pt_start[p0]);
+  const int ncols = k * v.wc;
+  const int* gcol = tab + tab_off[blockIdx.x];
+  long long nints = 2LL * ncols + 9LL * (k * (k + 1) / 2);
+  nints += nints & 1;
+  double* scol = reinterpret_cast<double*>(tab + tab_off[blockIdx.x] + nints);
+  for (int t = threadIdx.x; t < ncols; t += blockDim.x) scol[t] = gcol[t] >= 0 ? scale[gcol[t]] : 0.0;
 }
 
 __device__ __forceinline__ void dmma884(double& c0, double& c1, double a, double b) {

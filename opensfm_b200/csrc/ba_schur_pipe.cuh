@@ -318,6 +318,268 @@ __global__ void __launch_bounds__(32 * CC_WARPS, 1)
   }
 }
 
+// ---------------------------------------------------------------------------------------------------------
+// Linearisation over the chunk list, with the reductions that otherwise re-read the planes it writes (every camera
+// perspective, no rig cameras: wc == 9, nres == 2).  Every thread evaluates one observation as ba_linearize<1, NB, TYPE> does and writes the
+// same planes; it also puts the 27 products its observation adds to the sums into shared memory:
+//   camera side  Jc_j^2 and Jc_j r (9 columns each, summed over the two residual rows),
+//   point side   the upper triangle of Jp^T Jp (6) and Jp^T r (3).
+// CTA b owns the chunks that start in the observation window [b W, (b + 1) W) of the segment observations: whole
+// chunks, so whole points, fewer than W + SP_OBS observations, handled in passes of FL_THREADS.  After a pass
+//   * the first thread of every point (of its part in the pass) sums the point's products in observation order and,
+//     once the point is complete, stores its column norms and gradient into colnorm2 / grad and the nine sums into
+//     ptsum[9][npf] (ba_point_blocks_sums) with plain stores: no other CTA sees the point;
+//   * thread (segment piece, shot slot c, column j) sums the piece's products of that column, and issues one fp64
+//     atomic per column into colnorm2 / grad when the piece ends (destinations from the per-segment table, -1 for
+//     constant blocks).
+// A point or a piece that crosses the pass boundary carries its partial sums in shared memory.  CTAs past the last
+// window linearise the observations outside the segments ([n_fast, N)) without reductions.
+// ---------------------------------------------------------------------------------------------------------
+constexpr int FL_THREADS = 128;             // observations per pass
+constexpr int FL_WIN = 128;                 // observation window of a CTA's chunk starts
+constexpr int FL_MAXCH = FL_WIN;            // chunk starts in one window (a chunk has at least one observation)
+constexpr int FL_NV = 27;                   // products per observation: 9 + 9 camera side, 6 + 3 point side
+static_assert(FL_WIN + SP_OBS <= 2 * FL_THREADS, "a CTA's observations take at most two passes");
+
+struct FlSmem {
+  double st[FL_NV][FL_THREADS];             // products of the pass's observations
+  double cost[FL_THREADS];                  // per thread, over the passes
+  double pcarry[9];                         // the point that crosses the pass boundary
+  double ccarry[2][SEG_KMAX * 9];           // the segment piece that crosses it
+  long long pc_tab[FL_MAXCH];               // per piece: its segment's table (offset into tab)
+  int ch_lo[FL_MAXCH + 1];                  // per chunk: first observation, relative to the CTA's first; [nch] = end
+  int ch_k[FL_MAXCH], ch_pf[FL_MAXCH], ch_seg[FL_MAXCH];
+  int pc_lo[FL_MAXCH + 1], pc_k[FL_MAXCH], pc_item0[FL_MAXCH + 1];   // pieces (runs of one segment's chunks)
+  int nch, npc;
+  long long base;
+};
+
+// last index q in [lo, hi) with a[q] <= x (a ascending, a[lo] <= x)
+__device__ __forceinline__ int fl_find(const int* a, int lo, int hi, int x) {
+  while (hi - lo > 1) {
+    const int mid = (lo + hi) >> 1;
+    if (a[mid] <= x) lo = mid; else hi = mid;
+  }
+  return lo;
+}
+
+// One observation, as the uniform-type branch of ba_linearize<1>: writes r, Jc, Jp and returns the cost.  With PROD
+// also its FL_NV products, st[q * FL_THREADS] (formed column by column, so that the weighted values need not stay
+// live together).
+template <int TYPE, bool PROD>
+__device__ __forceinline__ double fl_eval(const BAView& v, const Params& p, long long i, double* st) {
+  const int shot = v.obs_shot[i];
+  const int cam = v.shot_cam[shot];
+  constexpr int C = 3;
+  const int pt = v.obs_point[i];
+  double camp[MAX_CAM_PARAMS], ri[6], rc[6], X[3];
+#pragma unroll
+  for (int j = 0; j < C; ++j) camp[j] = p.cam[v.cam_off[cam] + j];
+#pragma unroll
+  for (int j = 0; j < 6; ++j) ri[j] = p.inst[6 * (size_t)v.shot_inst[shot] + j];
+#pragma unroll
+  for (int j = 0; j < 3; ++j) X[j] = p.pts[3 * (size_t)pt + j];
+  double r[3], jc[3 * MAX_CAM_PARAMS], jri[18], jrc[18], jp[9];
+  observation_eval(TYPE, camp, ri, rc, false, X, v.obs_x[i], v.obs_y[i], v.obs_isig[i], r, jc, jri, jrc, jp);
+  const double s = r[0] * r[0] + r[1] * r[1];
+  double w;
+  double cost = 0.5 * robust_loss(v.loss, v.loss_a, s, &w);
+  const bool pfree = v.pt_poff[pt] >= 0;
+  if (!pfree && v.cam_poff[cam] < 0 && v.inst_poff[v.shot_inst[shot]] < 0) cost = 0.0;   // see ba_linearize
+  const size_t N = (size_t)v.N;
+  const double r0 = w * r[0], r1 = w * r[1];
+  v.r[i] = r0;
+  v.r[N + i] = r1;
+#pragma unroll
+  for (int j = 0; j < 9; ++j) {
+    const double a0 = w * (j < C ? jc[j] : jri[j - C]), a1 = w * (j < C ? jc[C + j] : jri[6 + j - C]);
+    v.Jc[(size_t)j * N + i] = a0;
+    v.Jc[(size_t)(9 + j) * N + i] = a1;
+    if (PROD) {
+      st[j * FL_THREADS] = a0 * a0 + a1 * a1;
+      st[(9 + j) * FL_THREADS] = a0 * r0 + a1 * r1;
+    }
+  }
+  double x[2][3];
+#pragma unroll
+  for (int k = 0; k < 2; ++k)
+#pragma unroll
+    for (int j = 0; j < 3; ++j) {
+      x[k][j] = pfree ? w * jp[k * 3 + j] : 0.0;
+      v.Jp[((size_t)k * 3 + j) * N + i] = x[k][j];
+    }
+  if (PROD) {
+    st[18 * FL_THREADS] = x[0][0] * x[0][0] + x[1][0] * x[1][0];
+    st[19 * FL_THREADS] = x[0][0] * x[0][1] + x[1][0] * x[1][1];
+    st[20 * FL_THREADS] = x[0][0] * x[0][2] + x[1][0] * x[1][2];
+    st[21 * FL_THREADS] = x[0][1] * x[0][1] + x[1][1] * x[1][1];
+    st[22 * FL_THREADS] = x[0][1] * x[0][2] + x[1][1] * x[1][2];
+    st[23 * FL_THREADS] = x[0][2] * x[0][2] + x[1][2] * x[1][2];
+    st[24 * FL_THREADS] = x[0][0] * r0 + x[1][0] * r1;
+    st[25 * FL_THREADS] = x[0][1] * r0 + x[1][1] * r1;
+    st[26 * FL_THREADS] = x[0][2] * r0 + x[1][2] * r1;
+  }
+  return cost;
+}
+
+template <int TYPE>
+__global__ void __launch_bounds__(FL_THREADS, 5)
+    ba_linearize_fused(BAView v, Params p, Scalars* sc, const SchurChunk* __restrict__ chunks, int nchunks,
+                       long long n_fast, const int* __restrict__ tab, double* __restrict__ colnorm2,
+                       double* __restrict__ grad, double* __restrict__ ptsum) {
+  static_assert(TYPE == PT_PERSPECTIVE, "3 camera parameters + 6 pose parameters = 9 columns; the fisheye model does "
+                                       "not fit the 5-CTA register bound without spills");
+  __shared__ FlSmem sm;
+  const int t = threadIdx.x;
+  const long long nwin = (n_fast + FL_WIN - 1) / FL_WIN;
+  double cost = 0.0;
+  if (blockIdx.x >= nwin) {   // observations outside the segments: planes and cost only
+    const long long i = n_fast + (blockIdx.x - nwin) * (long long)FL_THREADS + t;
+    if (i < v.N) cost = fl_eval<TYPE, false>(v, p, i, nullptr);
+  } else {
+    // ---- chunks of the window, and their runs by segment ("pieces") ----
+    if (t == 0) {
+      const long long w0 = (long long)blockIdx.x * FL_WIN, w1 = min(w0 + FL_WIN, n_fast);
+      auto first_at = [&](long long x) {   // first chunk with ibase >= x
+        int lo = 0, hi = nchunks;
+        while (lo < hi) {
+          const int mid = (lo + hi) >> 1;
+          if (__ldg(&chunks[mid].ibase) < x) lo = mid + 1; else hi = mid;
+        }
+        return lo;
+      };
+      const int c_lo = first_at(w0), c_hi = first_at(w1);
+      sm.nch = c_hi - c_lo;
+      sm.ch_seg[0] = c_lo;   // passed on to the loaders below
+      sm.base = c_lo < nchunks ? __ldg(&chunks[c_lo].ibase) : n_fast;
+      sm.ch_lo[sm.nch] = (int)((c_hi < nchunks ? __ldg(&chunks[c_hi].ibase) : n_fast) - sm.base);
+    }
+    __syncthreads();
+    const int nch = sm.nch, c_lo = sm.ch_seg[0];
+    const long long base = sm.base;
+    __syncthreads();   // ch_seg[0] is overwritten below
+    if (nch > 0) {   // (uniform over the CTA)
+      for (int q = t; q < nch; q += FL_THREADS) {
+        const SchurChunk e = sp_load_chunk(chunks, c_lo + q);
+        sm.ch_lo[q] = (int)(e.ibase - base);
+        sm.ch_k[q] = e.k;
+        sm.ch_pf[q] = e.pf0;
+        sm.ch_seg[q] = e.seg;
+        if (q == 0 || e.seg_chunk0 == c_lo + q) sm.pc_tab[q] = e.tab_off;   // a piece starts here
+      }
+      __syncthreads();
+      if (t == 0) {
+        int npc = 0, item = 0;
+        for (int q = 0; q < nch; ++q) {
+          if (q == 0 || sm.ch_seg[q] != sm.ch_seg[q - 1]) {
+            sm.pc_lo[npc] = sm.ch_lo[q];
+            sm.pc_k[npc] = sm.ch_k[q];
+            sm.pc_tab[npc] = sm.pc_tab[q];   // npc <= q: written before it is read again
+            sm.pc_item0[npc] = item;
+            item += 9 * sm.ch_k[q];
+            ++npc;
+          }
+        }
+        sm.pc_lo[npc] = sm.ch_lo[nch];
+        sm.pc_item0[npc] = item;
+        sm.npc = npc;
+      }
+      sm.cost[t] = 0.0;
+      __syncthreads();
+      // the loop state is re-read from shared memory after every barrier: nothing but p0 and the cost stays live
+      // across the evaluation, which needs every register the 5-CTA bound leaves
+      for (int p0 = 0; p0 < sm.ch_lo[sm.nch]; p0 += FL_THREADS) {
+        if (p0 + t < sm.ch_lo[sm.nch]) sm.cost[t] += fl_eval<TYPE, true>(v, p, sm.base + p0 + t, &sm.st[0][t]);
+        __syncthreads();
+        const int nch = sm.nch, npc = sm.npc;
+        const int p1 = min(sm.ch_lo[nch], p0 + FL_THREADS);
+        const int e = p0 + t;
+        int ch = 0, k = 1, c = 0, pi = 0;   // chunk of observation e, point in the chunk, shot slot
+        if (e < p1) {
+          ch = fl_find(sm.ch_lo, 0, nch, e);
+          k = sm.ch_k[ch];
+          const int rel = e - sm.ch_lo[ch];
+          pi = rel / k;
+          c = rel - pi * k;
+        }
+        // point side: the first thread of every point's part in this pass
+        if (e < p1 && (c == 0 || e == p0)) {
+          const int run = min(k - c, p1 - e);
+          double s[9];
+#pragma unroll
+          for (int q = 0; q < 9; ++q) s[q] = c != 0 ? sm.pcarry[q] : 0.0;
+          for (int u = 0; u < run; ++u) {
+#pragma unroll
+            for (int q = 0; q < 9; ++q) s[q] += sm.st[18 + q][t + u];
+          }
+          if (c + run == k) {
+            const int pf0 = sm.ch_pf[ch];
+            if (pf0 >= 0) {
+              const int pf = pf0 + pi;
+              const size_t NP = (size_t)v.npf;
+              const size_t col = (size_t)v.nc + 3 * (size_t)pf;
+              colnorm2[col] = s[0]; colnorm2[col + 1] = s[3]; colnorm2[col + 2] = s[5];
+              grad[col] = s[6]; grad[col + 1] = s[7]; grad[col + 2] = s[8];
+#pragma unroll
+              for (int q = 0; q < 9; ++q) ptsum[q * NP + pf] = s[q];
+            }
+          } else {   // continues in the next pass (read there by its thread 0, after two barriers)
+#pragma unroll
+            for (int q = 0; q < 9; ++q) sm.pcarry[q] = s[q];
+          }
+        }
+        // camera side: items (piece, c, j) of the pieces that overlap this pass
+        const int qa = fl_find(sm.pc_lo, 0, npc, p0), qb = fl_find(sm.pc_lo, 0, npc, p1 - 1) + 1;
+        const int i0 = sm.pc_item0[qa], i1 = sm.pc_item0[qb];
+        for (int it = i0 + t; it < i1; it += FL_THREADS) {
+          const int q = fl_find(sm.pc_item0, qa, qb, it);
+          const int a = it - sm.pc_item0[q];
+          const int kq = sm.pc_k[q], cq = a / 9, j = a - cq * 9;
+          const int lo = sm.pc_lo[q], hi = sm.pc_lo[q + 1];
+          int e0 = lo + cq;   // first observation of slot cq at or after p0
+          if (e0 < p0) e0 += (p0 - e0 + kq - 1) / kq * kq;
+          double n2 = 0.0, gr = 0.0;
+          if (lo < p0) { n2 = sm.ccarry[0][a]; gr = sm.ccarry[1][a]; }
+          for (int ee = e0; ee < min(hi, p1); ee += kq) {
+            n2 += sm.st[j][ee - p0];
+            gr += sm.st[9 + j][ee - p0];
+          }
+          if (hi > p1) {
+            sm.ccarry[0][a] = n2; sm.ccarry[1][a] = gr;
+          } else {
+            const int col = __ldg(tab + sm.pc_tab[q] + a);
+            if (col >= 0) { atomicAdd(&colnorm2[col], n2); atomicAdd(&grad[col], gr); }
+          }
+        }
+        __syncthreads();   // the products of the next pass overwrite st
+      }
+      cost = sm.cost[t];
+    }
+  }
+  const double tot = block_reduce_sum(cost);
+  if (threadIdx.x == 0 && tot != 0.0) atomicAdd(&sc->cost, tot);
+}
+
+// V^-1, g_p, V^-1 g_p of the points [0, p_count) from the unscaled sums of ba_linearize_fused (ptsum[9][npf]:
+// Jp^T Jp upper triangle xx xy xz yy yz zz, then Jp^T r): V_s = s_i s_j V_ij, g_s = s_i g_i; then as ba_point_blocks.
+__global__ void __launch_bounds__(PB_THREADS)
+    ba_point_blocks_sums(BAView v, int p_count, const double* __restrict__ ptsum, const double* __restrict__ scale,
+                         const double* __restrict__ diag, double inv_radius, double* __restrict__ Vinv,
+                         double* __restrict__ gpo, double* __restrict__ Vig, int* __restrict__ rank_flag) {
+  const int p = blockIdx.x * PB_THREADS + threadIdx.x;
+  if (p >= p_count) return;
+  const int pf = v.pt_poff[p];
+  if (pf < 0) return;
+  const size_t NP = (size_t)v.npf;
+  const int nc = v.nc;
+  const double s0 = scale[nc + 3 * pf], s1 = scale[nc + 3 * pf + 1], s2 = scale[nc + 3 * pf + 2];
+  double V[9];
+  V[0] = ptsum[0 * NP + pf] * s0 * s0; V[1] = ptsum[1 * NP + pf] * s0 * s1; V[2] = ptsum[2 * NP + pf] * s0 * s2;
+  V[3] = ptsum[3 * NP + pf] * s1 * s1; V[4] = ptsum[4 * NP + pf] * s1 * s2; V[5] = ptsum[5 * NP + pf] * s2 * s2;
+  V[6] = ptsum[6 * NP + pf] * s0; V[7] = ptsum[7 * NP + pf] * s1; V[8] = ptsum[8 * NP + pf] * s2;
+  point_block_finish(v, pf, V, diag, inv_radius, Vinv, gpo, Vig, rank_flag);
+}
+
 template <int WC, bool PROF>
 __global__ void __launch_bounds__(SP_THREADS, 1)
     ba_schur_pipe(BAView v, const SchurChunk* __restrict__ chunks, int nchunks, const int* __restrict__ tab,

@@ -6,9 +6,11 @@ worker process per tree; the workers then take turns, one full bundle() each, fo
 the Schur time per launch (CUDA events around ba_point_blocks + the Schur kernel inside run()), time_device_ms, the
 headline value (observations x LM iterations / time_device_ms, as bench.py computes it), the iteration count; per tree, the
 device memory the library holds after its first run.  With --trace each tree also does one run under OSFM_BA_TRACE=1 and its in-kernel
-clock lines are printed.  The card's name and power limit are read in the same process.  Fails without a GPU.
+clock lines are printed.  With --profile each tree also does one run of its own under torch.profiler (CUDA activities), after
+the timed runs and in a fresh process, and the device time of every kernel of that one bundle() is printed, summed by
+kernel name, with its launch count.  The card's name and power limit are read in the same process.  Fails without a GPU.
 
-    python tools/measure_schur.py --trees OLD_TREE . --runs 5 [--trace] [--out FILE]"""
+    python tools/measure_schur.py --trees OLD_TREE . --runs 5 [--trace] [--profile] [--out FILE]"""
 import argparse
 import json
 import os
@@ -28,7 +30,7 @@ def card():
 
 
 def worker(tree, problem_path):
-    """Loads the library of `tree`, then answers one JSON line per 'run' read from stdin."""
+    """Loads the library of `tree`, then answers one JSON line per 'run' or 'profile' read from stdin."""
     sys.path.insert(0, os.path.abspath(tree))
     import torch
     from opensfm_b200 import bundle
@@ -42,6 +44,9 @@ def worker(tree, problem_path):
     free1, _ = torch.cuda.mem_get_info()
     print(json.dumps({"ready": True, "library_mb": (free0 - free1) / 2 ** 20}), flush=True)
     for line in sys.stdin:
+        if line.strip() == "profile":
+            print(json.dumps(profile_one(bundle, pb)), flush=True)
+            continue
         if line.strip() != "run":
             break
         s = bundle.solve(pb)["summary"]
@@ -54,6 +59,27 @@ def worker(tree, problem_path):
             "pcg_iterations": s["pcg_iterations"], "linear_solves": s["linear_solves"],
             "value": pb.num_observations * s["iterations"] / (s["time_device_ms"] * 1e-3),
             "final_cost": s["final_cost"], "termination": s["termination"]}), flush=True)
+
+
+def profile_one(bundle, pb):
+    """One bundle() under torch.profiler: {kernel name: [device ms, launches]}, the summary's phase timers."""
+    import torch
+    from torch.profiler import ProfilerActivity, profile
+
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        s = bundle.solve(pb)["summary"]
+        torch.cuda.synchronize()
+    kernels = {}
+    for ev in prof.events():   # device-side events: one per kernel launch, memset and copy
+        if ev.device_type != torch.autograd.DeviceType.CUDA:
+            continue
+        name = ev.name.split("(")[0].replace("void ", "").replace("osfm::", "")
+        k = kernels.setdefault(name, [0.0, 0])
+        k[0] += ev.device_time_total / 1e3
+        k[1] += 1
+    return {"kernels": kernels, "time_device_ms": s["time_device_ms"], "time_linearize_ms": s["time_linearize_ms"],
+            "time_schur_ms": s["time_schur_ms"], "iterations": s["iterations"],
+            "linearize_launches": s["linearize_launches"], "schur_launches": s["schur_launches"]}
 
 
 def spawn(tree, problem_path, env=None, stderr=None):
@@ -76,6 +102,7 @@ def main():
     ap.add_argument("--trees", nargs="+", default=[ROOT])
     ap.add_argument("--runs", type=int, default=5)
     ap.add_argument("--trace", action="store_true")
+    ap.add_argument("--profile", action="store_true")
     ap.add_argument("--out", default=None)
     ap.add_argument("--worker", default=None, help=argparse.SUPPRESS)
     ap.add_argument("--problem", default=None, help=argparse.SUPPRESS)
@@ -132,6 +159,21 @@ def main():
                     lines = ef.read().splitlines()
                 report["trace"][names[i]] = ([ln for ln in lines if "schur" in ln or "consumer group" in ln][-8:] +
                                              [ln for ln in lines if "pcg" in ln])
+        if a.profile:
+            report["profile"] = {}
+            for i, t in enumerate(a.trees):
+                p = spawn(t, problem_path)
+                p.stdin.write("profile\n")
+                p.stdin.flush()
+                prof = json.loads(p.stdout.readline())
+                p.stdin.close()
+                p.wait()
+                report["profile"][names[i]] = prof
+                print("profile %s (one bundle, %d LM iterations, %d linearisations, %d Schur builds; device %.2f ms without the profiler: %.2f)" % (
+                    names[i], prof["iterations"], prof["linearize_launches"], prof["schur_launches"], prof["time_device_ms"],
+                    summary[names[i]]["time_device_ms"]["median"]))
+                for kname, (ms, cnt) in sorted(prof["kernels"].items(), key=lambda kv: -kv[1][0]):
+                    print("  %9.3f ms %5d x  %s" % (ms, cnt, kname))
     print(json.dumps({"card": report["card"], "library_mb": report["library_mb"], "summary": report["summary"], "trace": report.get("trace")}, indent=1))
     if a.out:
         with open(a.out, "w") as f:
