@@ -121,8 +121,30 @@ int osfm_match_words(osfm_matcher* m, const float* f1, int n1, const int32_t* wo
                      const float* f2, int n2, const int32_t* words2, int dim, float lowes_ratio, int max_checks,
                      int32_t* out_match);
 /* features::compute_vlad_distances (matching.cc:122-145): Euclidean distance of VLAD descriptor `query` to each of
- * the n descriptors (n x dim float32, row-major); out_n[query] = 0. */
+ * the n descriptors (n x dim float32, row-major), sqrt(sum (double(a) - double(b))^2); out_n[query] = 0. */
 int osfm_vlad_distances(osfm_matcher* m, const float* vlad, int n, int dim, int query, double* out_n);
+
+/* VLAD pair selection (pairs_selection.match_candidates_with_vlad, opensfm/pairs_selection.py:351-431, 471-490,
+ * 764-795; vlad.py).  osfm_matcher_vlad_compute: the VLAD descriptor of each listed resident set against
+ * `centers` (ncenters x dim float32, row-major) -- features::compute_vlad_descriptor (matching.cc:90-119), bit for
+ * bit, then vlad.signed_square_root_normalize -- kept on the device with the set.  out_valid[i] = 0 for Hamming
+ * sets and sets of another dimension (they get no descriptor, as unnormalized_vlad returns None).  float32 and
+ * uint8-stored L2 sets are read as float32.  Fails (OSFM_ERR_ARG) on non-finite centres or descriptors. */
+int osfm_matcher_vlad_compute(osfm_matcher* m, int count, const int* set_ids, const float* centers, int ncenters, int dim,
+                              int* out_valid);
+/* Copy one set's VLAD descriptor (ncenters * dim floats): unnormalised if `unnormalized`, else normalised. */
+int osfm_matcher_vlad_get(osfm_matcher* m, int set_id, int unnormalized, float* out);
+/* For every reference set r, the k nearest candidate sets by (distance, candidate index) -- a stable argsort of the
+ * distances over the candidates in the given order, NaN last -- among the candidates j with bit j % 32 of
+ * cand_mask_bits[r * ceil(ncand / 32) + j / 32] set (NULL: all) other than r's own set.  camera_labels: NULL, or
+ * nref + ncand ints (the references' labels, then the candidates'): then the k nearest of r's camera and the k
+ * nearest of other cameras (pairs_from_neighbors).  Distances as osfm_vlad_distances, computed block by block on
+ * the device.  Output: the selected (column, distance) of reference r in rows out_offsets[r] .. out_offsets[r + 1]
+ * of out_cols / out_dist, columns ascending; out_offsets has nref + 1 entries, the outputs room for
+ * nref * min(k, ncand) rows (twice that with camera labels). */
+int osfm_matcher_vlad_select(osfm_matcher* m, int nref, const int* ref_ids, int ncand, const int* cand_ids,
+                             const uint32_t* cand_mask_bits, const int* camera_labels, int k, int64_t* out_offsets,
+                             int32_t* out_cols, double* out_dist);
 
 /* ------------------------------------------------------------------------
  * BA

@@ -85,6 +85,10 @@ SIGNATURES = {
     "osfm_match_words": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_float,
                                   c_int, c_void_p]),
     "osfm_vlad_distances": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
+    "osfm_matcher_vlad_compute": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_int, c_int, c_void_p]),
+    "osfm_matcher_vlad_get": (c_int, [c_void_p, c_int, c_int, c_void_p]),
+    "osfm_matcher_vlad_select": (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int, c_void_p,
+                                         c_void_p, c_void_p]),
     "osfm_ba_create": (c_int, [c_int, POINTER(c_void_p)]),
     "osfm_ba_destroy": (c_int, [c_void_p]),
     "osfm_camera_num_params": (c_int, [c_int]),

@@ -653,6 +653,7 @@ void Matcher::refresh_info() {
 void Matcher::free_set(DescSet& s) {
   slab_release(s.slab, s.data, s.slab_bytes);
   if (s.bearings) { slab_release(s.bear_slab, s.bearings, s.bear_bytes); s.bearings = nullptr; s.bear_slab = -1; }
+  if (s.vlad) { slab_release(s.vlad_slab, s.vlad, s.vlad_bytes); s.vlad = nullptr; s.vlad_slab = -1; }
   if (s.slot >= 0) {
     cudaMemsetAsync(d_info.p + 2 * s.slot, 0, 2 * sizeof(int), stream);
     free_slots.push_back(s.slot);

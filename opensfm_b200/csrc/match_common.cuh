@@ -90,6 +90,10 @@ struct DescSet {
   // unit bearing vectors of the features (n x 3 float32), for guided matching; null until set
   float* bearings = nullptr;
   int bear_slab = -1;
+  // VLAD descriptor of the set (vlad.cu): [unnormalised | normalised], vlad_len floats each; null until computed
+  float* vlad = nullptr;
+  int vlad_len = 0, vlad_slab = -1;
+  size_t vlad_bytes = 0;
 };
 
 // The two layouts of one pair's epipolar bitmask in the last guided submission (the test hook reads them back).
@@ -140,6 +144,11 @@ struct Matcher {
   PinnedBuf<MatchJob> p_jobs;
   PinnedBuf<int> p_prefix;
   PinnedBuf<long long> p_out_off;
+  // VLAD workspaces (vlad.cu): centres, per-feature nearest centre, error flags, distance block, job / selection tables
+  DevBuf<float> d_vlad_centers;
+  DevBuf<int> d_vlad_assign, d_vlad_flags;
+  DevBuf<double> d_vlad_dist;
+  DevBuf<uint8_t> d_vlad_tab;
 
   explicit Matcher(int dev);
   ~Matcher();

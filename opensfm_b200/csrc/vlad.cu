@@ -1,0 +1,559 @@
+// VLAD pair selection on the device (SURVEY.md §8f.3): descriptors of resident descriptor sets, all-pairs
+// distances and the per-image neighbour selection of pairs_selection.match_candidates_with_vlad.
+//
+// Replaces features::compute_vlad_descriptor and features::compute_vlad_distances
+// (opensfm/src/features/src/matching.cc:90-145), vlad.signed_square_root_normalize (opensfm/vlad.py) and
+// construct_pairs / pairs_from_neighbors (opensfm/pairs_selection.py:471-490, 764-795).
+//
+// compute_vlad_descriptor: every feature goes to the first centre of smallest squared distance below FLT_MAX, the
+// distance summed in dimension order with separate float32 subtract, multiply and add (Eigen reduces the strided
+// row of a column-major MatXf sequentially; no FMA contraction, like the reference's x86-64 baseline build), and its
+// residual f - c is added to the centre's segment, feature after feature.  Both steps here do the same float32
+// operations in the same order, so the unnormalised vector is bit for bit the reference's.
+#include <cfloat>
+#include <cmath>
+#include <mutex>
+#include <vector>
+
+#include <cub/cub.cuh>
+
+#include "common.cuh"
+#include "match_common.cuh"
+
+namespace osfm {
+
+namespace {
+
+constexpr int VA_THREADS = 128;          // word assignment: one thread per feature
+constexpr int VA_CH = 32;                // centres whose distance chains one thread interleaves
+constexpr int VN_THREADS_MAX = 256;      // accumulation + normalisation: one CTA per set
+constexpr int VD_TM = 32, VD_TN = 64, VD_TK = 32;   // distance tile: reference rows x candidate rows x elements
+constexpr int VS_THREADS = 256;          // selection: one CTA per reference row
+constexpr size_t VLAD_SMEM_MAX = 200 * 1024;
+
+struct VladJob {
+  const float* f;    // float32 rows, stride ld (the set's zero-padded copy)
+  float* v;          // [unnormalised | normalised], 2 x L floats
+  long long aoff;    // first entry of the set in the assignment buffer
+  int n, ld;
+};
+
+// Nearest centre of every feature.  ct: the centres transposed, [dim][ncp] with ncp = ncenters rounded up to VA_CH
+// and the padding centres at +inf (their distance is +inf, never below FLT_MAX).  flags |= 1 for a non-finite
+// descriptor element, |= 2 for a feature with no centre below FLT_MAX (the reference indexes segment(-D) there).
+__global__ void __launch_bounds__(VA_THREADS)
+    vlad_assign_kernel(const VladJob* __restrict__ jobs, const float* __restrict__ ct, int ncp, int dim,
+                       int* __restrict__ assign, int* __restrict__ flags) {
+  extern __shared__ float4 smem4[];
+  float* sc = reinterpret_cast<float*>(smem4);
+  for (int e = threadIdx.x; e < dim * ncp; e += blockDim.x) sc[e] = ct[e];
+  __syncthreads();
+  const VladJob job = jobs[blockIdx.y];
+  const int i = blockIdx.x * VA_THREADS + threadIdx.x;
+  if (i >= job.n) return;
+  const float* f = job.f + (size_t)i * job.ld;
+  float best = FLT_MAX;
+  int best_c = -1;
+  bool finite = true;
+  for (int c0 = 0; c0 < ncp; c0 += VA_CH) {
+    float s[VA_CH];
+#pragma unroll
+    for (int j = 0; j < VA_CH; ++j) s[j] = 0.0f;   // 0 + (f0 - c0)^2 == (f0 - c0)^2 exactly
+    for (int k4 = 0; k4 < dim; k4 += 4) {
+      const float4 x4 = __ldg(reinterpret_cast<const float4*>(f + k4));   // rows are 64-byte aligned, zero-padded
+      const float xs[4] = {x4.x, x4.y, x4.z, x4.w};
+#pragma unroll
+      for (int u = 0; u < 4; ++u) {
+        const int k = k4 + u;
+        if (k >= dim) break;
+        const float x = xs[u];
+        if (c0 == 0) finite &= isfinite(x);
+        const float4* cr = reinterpret_cast<const float4*>(sc + (size_t)k * ncp + c0);
+#pragma unroll
+        for (int q = 0; q < VA_CH / 4; ++q) {
+          const float4 c = cr[q];
+          float t;
+          t = __fsub_rn(x, c.x); s[4 * q + 0] = __fadd_rn(s[4 * q + 0], __fmul_rn(t, t));
+          t = __fsub_rn(x, c.y); s[4 * q + 1] = __fadd_rn(s[4 * q + 1], __fmul_rn(t, t));
+          t = __fsub_rn(x, c.z); s[4 * q + 2] = __fadd_rn(s[4 * q + 2], __fmul_rn(t, t));
+          t = __fsub_rn(x, c.w); s[4 * q + 3] = __fadd_rn(s[4 * q + 3], __fmul_rn(t, t));
+        }
+      }
+    }
+#pragma unroll
+    for (int j = 0; j < VA_CH; ++j)
+      if (s[j] < best) { best = s[j]; best_c = c0 + j; }
+  }
+  if (!finite) atomicOr(flags, 1);
+  else if (best_c < 0) atomicOr(flags, 2);
+  assign[job.aoff + i] = best_c;
+}
+
+// numpy's sign(v) * sqrt(|v|) in float32
+__device__ __forceinline__ float signed_sqrt(float v) {
+  return v > 0.0f ? __fsqrt_rn(v) : v < 0.0f ? -__fsqrt_rn(-v) : (v == 0.0f ? 0.0f : v);
+}
+
+// One CTA per set: v[c][k] += f[k] - c[k] feature after feature (thread k owns column k of every segment, so each
+// element's sum runs in feature order), then the unnormalised vector, its signed square root and the division by
+// the norm (sum of squares in fp64, rounded to float32, float32 square root; a zero vector becomes 0/0 = NaN).
+// Every feature without a centre (assignment -1) has raised a flag in vlad_assign_kernel, earlier on this stream;
+// then the call fails and nothing is accumulated, so no assignment below is negative.
+__global__ void __launch_bounds__(VN_THREADS_MAX)
+    vlad_accumulate_kernel(const VladJob* __restrict__ jobs, const float* __restrict__ centers, int nc, int dim,
+                           const int* __restrict__ assign, const int* __restrict__ flags) {
+  if (*flags) return;
+  extern __shared__ float4 smem4[];
+  float* v = reinterpret_cast<float*>(smem4);
+  __shared__ double warp_sum[VN_THREADS_MAX / 32];
+  __shared__ float s_norm;
+  const VladJob job = jobs[blockIdx.x];
+  const int L = nc * dim;
+  for (int e = threadIdx.x; e < L; e += blockDim.x) v[e] = 0.0f;
+  __syncthreads();
+  const int* a = assign + job.aoff;
+  for (int k = threadIdx.x; k < dim; k += blockDim.x) {
+    constexpr int B = 8;   // loads of the next B features are issued before their ordered updates
+    int i = 0;
+    for (; i + B <= job.n; i += B) {
+      int c[B];
+      float r[B];
+#pragma unroll
+      for (int u = 0; u < B; ++u) c[u] = __ldg(a + i + u);
+#pragma unroll
+      for (int u = 0; u < B; ++u)
+        r[u] = __fsub_rn(__ldg(job.f + (size_t)(i + u) * job.ld + k), __ldg(centers + (size_t)c[u] * dim + k));
+#pragma unroll
+      for (int u = 0; u < B; ++u) v[c[u] * dim + k] = __fadd_rn(v[c[u] * dim + k], r[u]);
+    }
+    for (; i < job.n; ++i) {
+      const int c = __ldg(a + i);
+      v[c * dim + k] = __fadd_rn(v[c * dim + k], __fsub_rn(__ldg(job.f + (size_t)i * job.ld + k), __ldg(centers + (size_t)c * dim + k)));
+    }
+  }
+  __syncthreads();
+  double part = 0.0;
+  for (int e = threadIdx.x; e < L; e += blockDim.x) {
+    const float x = v[e];
+    job.v[e] = x;
+    const float w = signed_sqrt(x);
+    v[e] = w;
+    part += (double)w * (double)w;
+  }
+  for (int o = 16; o; o >>= 1) part += __shfl_xor_sync(0xffffffffu, part, o);
+  if ((threadIdx.x & 31) == 0) warp_sum[threadIdx.x >> 5] = part;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double t = 0.0;
+    for (int w = 0; w < (int)(blockDim.x >> 5); ++w) t += warp_sum[w];
+    s_norm = __fsqrt_rn(__double2float_rn(t));
+  }
+  __syncthreads();
+  const float nrm = s_norm;
+  for (int e = threadIdx.x; e < L; e += blockDim.x) job.v[L + e] = __fdiv_rn(v[e], nrm);
+}
+
+// out[i * ldo + j] = sqrt(sum_e (double(a_i[e]) - double(b_j[e]))^2), e ascending in one chain per output, so
+// d(a, b) == d(b, a) bit for bit.  Direct differences, not |a|^2 + |b|^2 - 2ab, which cancels for near-duplicates.
+// Register tile: each thread 2 reference rows x 4 candidate rows; operands staged through shared memory as fp64.
+__global__ void __launch_bounds__(256)
+    vlad_distance_kernel(const float* const* __restrict__ arows, int na, const float* const* __restrict__ brows, int nb,
+                         int L, double* __restrict__ out, long long ldo) {
+  __shared__ double As[VD_TK][VD_TM + 1];
+  __shared__ double Bs[VD_TK][VD_TN + 1];
+  const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
+  const int a0 = blockIdx.y * VD_TM, b0 = blockIdx.x * VD_TN;
+  const int kk = threadIdx.x & (VD_TK - 1), r0 = threadIdx.x / VD_TK;   // staging: element kk of rows r0 + 8 r
+  const float* ap[VD_TM / 8];
+  const float* bp[VD_TN / 8];
+#pragma unroll
+  for (int r = 0; r < VD_TM / 8; ++r) ap[r] = a0 + r0 + 8 * r < na ? arows[a0 + r0 + 8 * r] : nullptr;
+#pragma unroll
+  for (int r = 0; r < VD_TN / 8; ++r) bp[r] = b0 + r0 + 8 * r < nb ? brows[b0 + r0 + 8 * r] : nullptr;
+  double acc[2][4];
+#pragma unroll
+  for (int i = 0; i < 2; ++i)
+#pragma unroll
+    for (int j = 0; j < 4; ++j) acc[i][j] = 0.0;
+  for (int k0 = 0; k0 < L; k0 += VD_TK) {
+    const int k = k0 + kk;
+#pragma unroll
+    for (int r = 0; r < VD_TM / 8; ++r) As[kk][r0 + 8 * r] = (ap[r] && k < L) ? (double)__ldg(ap[r] + k) : 0.0;
+#pragma unroll
+    for (int r = 0; r < VD_TN / 8; ++r) Bs[kk][r0 + 8 * r] = (bp[r] && k < L) ? (double)__ldg(bp[r] + k) : 0.0;
+    __syncthreads();
+#pragma unroll 4
+    for (int e = 0; e < VD_TK; ++e) {
+      double x[2], y[4];
+#pragma unroll
+      for (int i = 0; i < 2; ++i) x[i] = As[e][ty + 16 * i];
+#pragma unroll
+      for (int j = 0; j < 4; ++j) y[j] = Bs[e][tx + 16 * j];
+#pragma unroll
+      for (int i = 0; i < 2; ++i)
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          const double t = x[i] - y[j];
+          acc[i][j] = fma(t, t, acc[i][j]);   // zero padding adds fma(0, 0, s) = s
+        }
+    }
+    __syncthreads();
+  }
+#pragma unroll
+  for (int i = 0; i < 2; ++i)
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const int ia = a0 + ty + 16 * i, jb = b0 + tx + 16 * j;
+      if (ia < na && jb < nb) out[(size_t)ia * ldo + jb] = sqrt(acc[i][j]);
+    }
+}
+
+// Order-preserving key of a distance: ascending for numbers, every NaN after them (np.argsort's order).
+__device__ __forceinline__ unsigned long long dist_key(double d) {
+  if (isnan(d)) return ~0ull;
+  const unsigned long long b = (unsigned long long)__double_as_longlong(d);
+  return (b >> 63) ? ~b : (b | (1ull << 63));
+}
+
+// One CTA per reference row of the block: the k smallest eligible candidates by (distance, column) -- the order a
+// stable argsort over the reference's sorted candidate list gives -- per camera group.  With camera labels there are
+// two groups, the candidates of the reference's camera and the others (pairs_from_neighbors), otherwise one.
+// Selection: radix select of the k-th key over eight 8-bit digits, then one pass in column order that keeps every
+// key below it and the first `need` keys equal to it.  Output: the selected columns in ascending order.
+__global__ void __launch_bounds__(VS_THREADS)
+    vlad_select_kernel(const double* __restrict__ dist, int ncand, int row0, int nref, const int* __restrict__ ref_ids,
+                       const int* __restrict__ cand_ids, const uint32_t* __restrict__ mask, int mask_words,
+                       const int* __restrict__ labels, int k, int stride, int* __restrict__ out_count,
+                       int* __restrict__ out_cols, double* __restrict__ out_dist) {
+  using Scan = cub::BlockScan<int, VS_THREADS>;
+  __shared__ typename Scan::TempStorage scan_tmp;
+  __shared__ int hist[256];
+  __shared__ unsigned long long s_prefix;
+  __shared__ int s_need;
+  const int row = row0 + blockIdx.x;
+  const double* d = dist + (size_t)blockIdx.x * ncand;
+  const int self = ref_ids[row];
+  const int ngroups = labels ? 2 : 1;
+  const size_t base = (size_t)row * stride;
+  int written = 0;
+  for (int g = 0; g < ngroups; ++g) {
+    auto eligible = [&](int j) {
+      if (cand_ids[j] == self) return false;
+      if (mask && !((mask[(size_t)row * mask_words + (j >> 5)] >> (j & 31)) & 1u)) return false;
+      if (labels && ((labels[nref + j] == labels[row]) != (g == 0))) return false;
+      return true;
+    };
+    int cnt = 0;
+    for (int j = threadIdx.x; j < ncand; j += VS_THREADS) cnt += eligible(j);
+    int total_elig;
+    Scan(scan_tmp).ExclusiveSum(cnt, cnt, total_elig);
+    __syncthreads();
+    const bool take_all = total_elig <= k;
+    unsigned long long thr = ~0ull;
+    int need = 0;
+    if (!take_all) {
+      if (threadIdx.x == 0) { s_prefix = 0ull; s_need = k; }
+      for (int shift = 56; shift >= 0; shift -= 8) {
+        for (int b = threadIdx.x; b < 256; b += VS_THREADS) hist[b] = 0;
+        __syncthreads();
+        const unsigned long long prefix = s_prefix;
+        const unsigned long long hi = shift == 56 ? 0ull : (~0ull << (shift + 8));
+        for (int j = threadIdx.x; j < ncand; j += VS_THREADS) {
+          if (!eligible(j)) continue;
+          const unsigned long long key = dist_key(d[j]);
+          if ((key & hi) == (prefix & hi)) atomicAdd(&hist[(key >> shift) & 255], 1);
+        }
+        __syncthreads();
+        if (threadIdx.x == 0) {
+          int cum = 0, want = s_need, b = 0;
+          for (; b < 255 && cum + hist[b] < want; ++b) cum += hist[b];
+          s_need = want - cum;
+          s_prefix = prefix | ((unsigned long long)b << shift);
+        }
+        __syncthreads();
+      }
+      thr = s_prefix;
+      need = s_need;   // keys equal to thr to keep, lowest columns first
+    }
+    int eq_before = 0;
+    for (int j0 = 0; j0 < ncand; j0 += VS_THREADS) {
+      const int j = j0 + threadIdx.x;
+      bool lt = false, eq = false;
+      double dj = 0.0;
+      if (j < ncand && eligible(j)) {
+        dj = d[j];
+        if (take_all) lt = true;
+        else {
+          const unsigned long long key = dist_key(dj);
+          lt = key < thr;
+          eq = key == thr;
+        }
+      }
+      int eq_rank, eq_total;
+      Scan(scan_tmp).ExclusiveSum((int)eq, eq_rank, eq_total);
+      __syncthreads();
+      const bool take = lt || (eq && eq_before + eq_rank < need);
+      int pos, ntake;
+      Scan(scan_tmp).ExclusiveSum((int)take, pos, ntake);
+      __syncthreads();
+      if (take) {
+        out_cols[base + written + pos] = j;
+        out_dist[base + written + pos] = dj;
+      }
+      written += ntake;
+      eq_before += eq_total;
+    }
+  }
+  if (threadIdx.x == 0) out_count[row] = written;
+}
+
+}  // namespace
+
+// Launch the distance kernel for na reference rows x nb candidate rows into out (na rows of ldo doubles).
+static void launch_vlad_distances(cudaStream_t stream, const float* const* arows, int na, const float* const* brows,
+                                  int nb, int L, double* out, long long ldo) {
+  dim3 grid((unsigned)((nb + VD_TN - 1) / VD_TN), (unsigned)((na + VD_TM - 1) / VD_TM));
+  vlad_distance_kernel<<<grid, 256, 0, stream>>>(arows, na, brows, nb, L, out, ldo);
+  OSFM_LAUNCH_CHECK();
+}
+
+}  // namespace osfm
+
+struct osfm_matcher;   // defined in match.cu: { Matcher impl; std::mutex mu; }
+namespace osfm {
+Matcher& matcher_impl(osfm_matcher* m);
+std::mutex& matcher_mutex(osfm_matcher* m);
+
+static void release_vlad(Matcher& M, DescSet& s) {   // the caller has synchronised the stream
+  if (s.vlad) M.slab_release(s.vlad_slab, s.vlad, s.vlad_bytes);
+  s.vlad = nullptr;
+  s.vlad_slab = -1;
+  s.vlad_len = 0;
+  s.vlad_bytes = 0;
+}
+
+static const DescSet& vlad_set(Matcher& M, int id, int L) {
+  auto it = M.sets.find(id);
+  if (it == M.sets.end()) throw ArgError("unknown descriptor set id");
+  if (!it->second.vlad) throw ArgError("descriptor set has no VLAD descriptor (osfm_matcher_vlad_compute)");
+  if (L >= 0 && it->second.vlad_len != L) throw ArgError("VLAD descriptors of different lengths");
+  return it->second;
+}
+}  // namespace osfm
+
+extern "C" {
+
+int osfm_matcher_vlad_compute(osfm_matcher* m, int count, const int* set_ids, const float* centers, int ncenters, int dim,
+                              int* out_valid) {
+  OSFM_API_BEGIN
+  using namespace osfm;
+  if (!m) throw ArgError("null matcher");
+  if (count < 0 || ncenters <= 0 || dim <= 0) throw ArgError("bad VLAD sizes");
+  if ((count > 0 && (!set_ids || !out_valid)) || !centers) throw ArgError("null arrays");
+  const int ncp = (ncenters + VA_CH - 1) / VA_CH * VA_CH;
+  const size_t L = (size_t)ncenters * dim;
+  if ((size_t)dim * ncp * sizeof(float) > VLAD_SMEM_MAX || L * sizeof(float) > VLAD_SMEM_MAX)
+    throw ArgError("VLAD vocabulary too large: ncenters x dim float32 must fit in 200 KB of shared memory");
+  for (size_t e = 0; e < L; ++e)
+    if (!std::isfinite(centers[e])) throw ArgError("non-finite VLAD centre");
+  std::lock_guard<std::mutex> lock(matcher_mutex(m));
+  Matcher& M = matcher_impl(m);
+  OSFM_CUDA(cudaSetDevice(M.device));
+  for (int i = 0; i < count; ++i)
+    if (!M.sets.count(set_ids[i])) throw ArgError("unknown descriptor set id");
+  OSFM_CUDA(cudaStreamSynchronize(M.stream));   // earlier work may still read VLADs released below
+  // one descriptor per set; Hamming sets and sets of another dimension have none (unnormalized_vlad -> None)
+  std::vector<VladJob> jobs;
+  std::vector<int> job_set;
+  long long nfeat = 0;
+  int max_n = 0;
+  for (int i = 0; i < count; ++i) {
+    DescSet& s = M.sets[set_ids[i]];
+    const bool valid = !s.u8 && s.dim == dim;
+    out_valid[i] = valid;
+    if (s.vlad && (!valid || (size_t)s.vlad_len != L)) release_vlad(M, s);
+    if (!valid) continue;
+    if (!s.vlad) {
+      s.vlad_bytes = 2 * L * sizeof(float);
+      s.vlad = static_cast<float*>(M.slab_alloc(s.vlad_bytes, &s.vlad_slab));
+      s.vlad_len = (int)L;
+    }
+    VladJob j;
+    j.f = static_cast<const float*>(s.data);   // float32 zero-padded rows for every non-Hamming set (match.cu add_async)
+    j.v = s.vlad;
+    j.aoff = nfeat;
+    j.n = s.n;
+    j.ld = s.dim_padded;
+    jobs.push_back(j);
+    job_set.push_back(set_ids[i]);
+    nfeat += s.n;
+    max_n = std::max(max_n, s.n);
+  }
+  if (jobs.empty()) return OSFM_OK;
+  // centres: row-major for the residuals, transposed and padded with +inf for the assignment
+  std::vector<float> hc(L + (size_t)dim * ncp, __builtin_huge_valf());
+  std::copy(centers, centers + L, hc.begin());
+  for (int c = 0; c < ncenters; ++c)
+    for (int k = 0; k < dim; ++k) hc[L + (size_t)k * ncp + c] = centers[(size_t)c * dim + k];
+  M.d_vlad_centers.reserve(hc.size());
+  M.d_vlad_assign.reserve((size_t)std::max<long long>(nfeat, 1));
+  M.d_vlad_flags.reserve(1);
+  M.d_vlad_tab.reserve(sizeof(VladJob) * jobs.size());
+  OSFM_CUDA(cudaMemcpyAsync(M.d_vlad_centers.p, hc.data(), sizeof(float) * hc.size(), cudaMemcpyHostToDevice, M.stream));
+  OSFM_CUDA(cudaMemcpyAsync(M.d_vlad_tab.p, jobs.data(), sizeof(VladJob) * jobs.size(), cudaMemcpyHostToDevice, M.stream));
+  OSFM_CUDA(cudaMemsetAsync(M.d_vlad_flags.p, 0, sizeof(int), M.stream));
+  const VladJob* d_jobs = reinterpret_cast<const VladJob*>(M.d_vlad_tab.p);
+  const size_t smem_a = (size_t)dim * ncp * sizeof(float), smem_n = L * sizeof(float);
+  OSFM_CUDA(cudaFuncSetAttribute(vlad_assign_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_a));
+  OSFM_CUDA(cudaFuncSetAttribute(vlad_accumulate_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_n));
+  const int nthreads = std::min(VN_THREADS_MAX, std::max(32, (dim + 31) / 32 * 32));
+  for (size_t j0 = 0; j0 < jobs.size(); j0 += 32768) {   // gridDim.y <= 65535
+    const int nj = (int)std::min<size_t>(32768, jobs.size() - j0);
+    if (max_n > 0) {
+      dim3 grid((unsigned)((max_n + VA_THREADS - 1) / VA_THREADS), (unsigned)nj);
+      vlad_assign_kernel<<<grid, VA_THREADS, smem_a, M.stream>>>(d_jobs + j0, M.d_vlad_centers.p + L, ncp, dim,
+                                                                 M.d_vlad_assign.p, M.d_vlad_flags.p);
+      OSFM_LAUNCH_CHECK();
+    }
+    vlad_accumulate_kernel<<<nj, nthreads, smem_n, M.stream>>>(d_jobs + j0, M.d_vlad_centers.p, ncenters, dim,
+                                                              M.d_vlad_assign.p, M.d_vlad_flags.p);
+    OSFM_LAUNCH_CHECK();
+  }
+  int flags = 0;
+  OSFM_CUDA(cudaMemcpyAsync(&flags, M.d_vlad_flags.p, sizeof(int), cudaMemcpyDeviceToHost, M.stream));
+  OSFM_CUDA(cudaStreamSynchronize(M.stream));
+  if (flags) {
+    for (int id : job_set) release_vlad(M, M.sets[id]);
+    throw ArgError(flags & 1 ? "non-finite descriptor element in a VLAD input set"
+                             : "a feature's squared distance to every VLAD centre overflows float32");
+  }
+  OSFM_API_END
+}
+
+int osfm_matcher_vlad_get(osfm_matcher* m, int set_id, int unnormalized, float* out) {
+  OSFM_API_BEGIN
+  using namespace osfm;
+  if (!m || !out) throw ArgError("null arguments");
+  std::lock_guard<std::mutex> lock(matcher_mutex(m));
+  Matcher& M = matcher_impl(m);
+  OSFM_CUDA(cudaSetDevice(M.device));
+  const DescSet& s = vlad_set(M, set_id, -1);
+  const float* src = s.vlad + (unnormalized ? 0 : s.vlad_len);
+  OSFM_CUDA(cudaMemcpyAsync(out, src, sizeof(float) * (size_t)s.vlad_len, cudaMemcpyDeviceToHost, M.stream));
+  OSFM_CUDA(cudaStreamSynchronize(M.stream));
+  OSFM_API_END
+}
+
+int osfm_matcher_vlad_select(osfm_matcher* m, int nref, const int* ref_ids, int ncand, const int* cand_ids,
+                             const uint32_t* cand_mask_bits, const int* camera_labels, int k, int64_t* out_offsets,
+                             int32_t* out_cols, double* out_dist) {
+  OSFM_API_BEGIN
+  using namespace osfm;
+  if (!m) throw ArgError("null matcher");
+  if (nref < 0 || ncand < 0 || k < 0) throw ArgError("bad VLAD selection sizes");
+  if ((nref > 0 && (!ref_ids || !out_offsets)) || (ncand > 0 && !cand_ids)) throw ArgError("null arrays");
+  std::lock_guard<std::mutex> lock(matcher_mutex(m));
+  Matcher& M = matcher_impl(m);
+  OSFM_CUDA(cudaSetDevice(M.device));
+  if (nref == 0) return OSFM_OK;
+  out_offsets[0] = 0;
+  const int ngroups = camera_labels ? 2 : 1;
+  const int stride = ngroups * std::min(k, ncand);
+  if (ncand == 0 || stride == 0) {
+    for (int r = 0; r < nref; ++r) out_offsets[r + 1] = 0;
+    return OSFM_OK;
+  }
+  if (!out_cols || !out_dist) throw ArgError("null output arrays");
+  int L = -1;
+  std::vector<const float*> rows((size_t)nref + ncand);
+  for (int r = 0; r < nref; ++r) {
+    const DescSet& s = vlad_set(M, ref_ids[r], L);
+    L = s.vlad_len;
+    rows[r] = s.vlad + L;
+  }
+  for (int j = 0; j < ncand; ++j) rows[(size_t)nref + j] = vlad_set(M, cand_ids[j], L).vlad + L;
+  const int mask_words = (ncand + 31) / 32;
+  // device tables: row pointers | ids | labels | mask | counts | columns | distances
+  auto up256 = [](size_t x) { return (x + 255) / 256 * 256; };
+  const size_t o_ids = up256(sizeof(float*) * rows.size());
+  const size_t o_lab = o_ids + up256(sizeof(int) * rows.size());
+  const size_t o_mask = o_lab + up256(camera_labels ? sizeof(int) * rows.size() : 0);
+  const size_t o_cnt = o_mask + up256(cand_mask_bits ? sizeof(uint32_t) * (size_t)nref * mask_words : 0);
+  const size_t o_cols = o_cnt + up256(sizeof(int) * (size_t)nref);
+  const size_t o_dist = o_cols + up256(sizeof(int) * (size_t)nref * stride);
+  const size_t total = o_dist + sizeof(double) * (size_t)nref * stride;
+  M.d_vlad_tab.reserve(total);
+  uint8_t* base = M.d_vlad_tab.p;
+  std::vector<int> ids((size_t)nref + ncand);
+  std::copy(ref_ids, ref_ids + nref, ids.begin());
+  std::copy(cand_ids, cand_ids + ncand, ids.begin() + nref);
+  OSFM_CUDA(cudaMemcpyAsync(base, rows.data(), sizeof(float*) * rows.size(), cudaMemcpyHostToDevice, M.stream));
+  OSFM_CUDA(cudaMemcpyAsync(base + o_ids, ids.data(), sizeof(int) * ids.size(), cudaMemcpyHostToDevice, M.stream));
+  if (camera_labels)
+    OSFM_CUDA(cudaMemcpyAsync(base + o_lab, camera_labels, sizeof(int) * rows.size(), cudaMemcpyHostToDevice, M.stream));
+  if (cand_mask_bits)
+    OSFM_CUDA(cudaMemcpyAsync(base + o_mask, cand_mask_bits, sizeof(uint32_t) * (size_t)nref * mask_words,
+                              cudaMemcpyHostToDevice, M.stream));
+  const float* const* d_rows = reinterpret_cast<const float* const*>(base);
+  const int* d_ids = reinterpret_cast<const int*>(base + o_ids);
+  int* d_cnt = reinterpret_cast<int*>(base + o_cnt);
+  int* d_cols = reinterpret_cast<int*>(base + o_cols);
+  double* d_dist = reinterpret_cast<double*>(base + o_dist);
+  // reference rows in blocks: the distance block stays under 256 MB (a multiple of the tile height)
+  // and the distance grid's y dimension (block / VD_TM tiles) within 65535
+  const long long budget = (256ll << 20) / (long long)(sizeof(double) * ncand);
+  const long long cap = std::min<long long>(budget / VD_TM * VD_TM, 65535ll * VD_TM);
+  const int block = (int)std::max<long long>(VD_TM, std::min<long long>(nref, cap));
+  M.d_vlad_dist.reserve((size_t)block * ncand);
+  for (int r0 = 0; r0 < nref; r0 += block) {
+    const int nb = std::min(block, nref - r0);
+    launch_vlad_distances(M.stream, d_rows + r0, nb, d_rows + nref, ncand, L, M.d_vlad_dist.p, ncand);
+    vlad_select_kernel<<<nb, VS_THREADS, 0, M.stream>>>(
+        M.d_vlad_dist.p, ncand, r0, nref, d_ids, d_ids + nref,
+        cand_mask_bits ? reinterpret_cast<const uint32_t*>(base + o_mask) : nullptr, mask_words,
+        camera_labels ? reinterpret_cast<const int*>(base + o_lab) : nullptr, k, stride, d_cnt, d_cols, d_dist);
+    OSFM_LAUNCH_CHECK();
+  }
+  std::vector<int> cnt(nref);
+  std::vector<int> cols((size_t)nref * stride);
+  std::vector<double> dist((size_t)nref * stride);
+  OSFM_CUDA(cudaMemcpyAsync(cnt.data(), d_cnt, sizeof(int) * nref, cudaMemcpyDeviceToHost, M.stream));
+  OSFM_CUDA(cudaMemcpyAsync(cols.data(), d_cols, sizeof(int) * cols.size(), cudaMemcpyDeviceToHost, M.stream));
+  OSFM_CUDA(cudaMemcpyAsync(dist.data(), d_dist, sizeof(double) * dist.size(), cudaMemcpyDeviceToHost, M.stream));
+  OSFM_CUDA(cudaStreamSynchronize(M.stream));
+  int64_t o = 0;
+  for (int r = 0; r < nref; ++r) {
+    std::copy(cols.begin() + (size_t)r * stride, cols.begin() + (size_t)r * stride + cnt[r], out_cols + o);
+    std::copy(dist.begin() + (size_t)r * stride, dist.begin() + (size_t)r * stride + cnt[r], out_dist + o);
+    o += cnt[r];
+    out_offsets[r + 1] = o;
+  }
+  OSFM_API_END
+}
+
+int osfm_vlad_distances(osfm_matcher* m, const float* vlad, int n, int dim, int query, double* out_n) {
+  OSFM_API_BEGIN
+  using namespace osfm;
+  if (!m) throw ArgError("null matcher");
+  if (n <= 0 || dim <= 0 || query < 0 || query >= n || !vlad || !out_n) throw ArgError("bad VLAD arguments");
+  std::lock_guard<std::mutex> lock(matcher_mutex(m));
+  Matcher& M = matcher_impl(m);
+  OSFM_CUDA(cudaSetDevice(M.device));
+  // the 1 x n block of the selection's distance kernel over the uploaded rows
+  const size_t b_v = (sizeof(float) * (size_t)n * dim + 255) / 256 * 256;
+  const size_t b_p = (sizeof(float*) * (size_t)n + 255) / 256 * 256;
+  M.staging.reserve(b_v + b_p + sizeof(double) * (size_t)n);
+  float* d_v = reinterpret_cast<float*>(M.staging.p);
+  const float** d_p = reinterpret_cast<const float**>(M.staging.p + b_v);
+  double* d_out = reinterpret_cast<double*>(M.staging.p + b_v + b_p);
+  std::vector<const float*> rows(n);
+  for (int i = 0; i < n; ++i) rows[i] = d_v + (size_t)i * dim;
+  OSFM_CUDA(cudaMemcpyAsync(d_v, vlad, sizeof(float) * (size_t)n * dim, cudaMemcpyHostToDevice, M.stream));
+  OSFM_CUDA(cudaMemcpyAsync(d_p, rows.data(), sizeof(float*) * (size_t)n, cudaMemcpyHostToDevice, M.stream));
+  launch_vlad_distances(M.stream, d_p + query, 1, d_p, n, dim, d_out, n);
+  OSFM_CUDA(cudaMemcpyAsync(out_n, d_out, sizeof(double) * (size_t)n, cudaMemcpyDeviceToHost, M.stream));
+  OSFM_CUDA(cudaStreamSynchronize(M.stream));
+  OSFM_API_END
+}
+
+}  // extern "C"

@@ -132,6 +132,7 @@ class PairMatcher:
         self._keep: Dict[Any, np.ndarray] = {}
         self._rows: Optional[np.ndarray] = None
         self._pairs: List[Tuple[Any, Any]] = []
+        self._vlad: Dict[Any, int] = {}   # image -> length of its resident VLAD descriptor (0: it has none)
         if kernel:
             _lib.check(self._m.L.osfm_matcher_set_kernel(self._m.h, int(kernel)))
 
@@ -150,6 +151,7 @@ class PairMatcher:
             _lib.check(self._m.L.osfm_matcher_remove(self._m.h, self._ids[key]))
         self._ids[key] = out.value
         self._n[key] = d.shape[0]
+        self._vlad.pop(key, None)
 
     def add_many(self, items: Sequence[Tuple[Any, np.ndarray]], uint8_is_l2: bool = False) -> None:
         """Upload many images' descriptors with a single host synchronisation (same dtype and
@@ -177,12 +179,85 @@ class PairMatcher:
                 _lib.check(self._m.L.osfm_matcher_remove(self._m.h, self._ids[k]))
             self._ids[k] = int(i)
             self._n[k] = d.shape[0]
+            self._vlad.pop(k, None)
 
     def clear(self) -> None:
         """Drop every resident descriptor set (device memory stays with the matcher for reuse)."""
         _lib.check(self._m.L.osfm_matcher_clear(self._m.h))
         self._ids.clear()
         self._n.clear()
+        self._vlad.clear()
+
+    # -- VLAD (opensfm/vlad.py, pairs_selection.vlad_histograms) ---------------------------------------------------
+    def compute_vlad(self, keys: Iterable[Any], centers: np.ndarray) -> List[Any]:
+        """Compute the VLAD descriptor of every resident image in `keys` against the visual words `centers`
+        (ncenters x dim) and keep it on the device.  Returns the keys that have one: Hamming images and images of
+        another descriptor length have none, as `vlad.unnormalized_vlad` returns None for them."""
+        keys = list(dict.fromkeys(keys))
+        c = np.ascontiguousarray(centers, dtype=np.float32)
+        if c.ndim != 2:
+            raise ValueError("centers must be ncenters x dim")
+        ids = np.array([self._ids[k] for k in keys], dtype=np.int32)
+        valid = np.zeros(len(keys), dtype=np.int32)
+        for k in keys:
+            self._vlad.pop(k, None)
+        _lib.check(self._m.L.osfm_matcher_vlad_compute(self._m.h, len(keys), ids.ctypes.data_as(ctypes.c_void_p),
+                                                       c.ctypes.data_as(ctypes.c_void_p), c.shape[0], c.shape[1],
+                                                       valid.ctypes.data_as(ctypes.c_void_p)))
+        for k, v in zip(keys, valid):
+            self._vlad[k] = c.size if v else 0
+        return [k for k, v in zip(keys, valid) if v]
+
+    def vlad_descriptor(self, key: Any, normalized: bool = True) -> np.ndarray:
+        """The resident VLAD descriptor of one image (float32, ncenters * dim): signed-square-root normalised, or the
+        unnormalised sum of residuals.  Raises KeyError if the image has none."""
+        if not self._vlad.get(key):
+            raise KeyError("no VLAD descriptor for image %r" % (key,))
+        out = np.empty(self._vlad[key], dtype=np.float32)
+        _lib.check(self._m.L.osfm_matcher_vlad_get(self._m.h, self._ids[key], int(not normalized),
+                                                   out.ctypes.data_as(ctypes.c_void_p)))
+        return out
+
+    def has_vlad(self, key: Any) -> Optional[bool]:
+        """None if `compute_vlad` never ran on the image, else whether it has a VLAD descriptor."""
+        return None if key not in self._vlad else bool(self._vlad[key])
+
+    def vlad_histograms(self, keys: Iterable[Any], centers: np.ndarray) -> Dict[Any, np.ndarray]:
+        """pairs_selection.vlad_histograms (pairs_selection.py:732-745) for resident images: {key: normalised
+        float32 VLAD vector}, images without a descriptor left out.  The descriptors stay on the device for
+        `pairs_selection.match_candidates_with_vlad`."""
+        return {k: self.vlad_descriptor(k) for k in self.compute_vlad(keys, centers)}
+
+    def vlad_select(self, refs: Sequence[Any], cands: Sequence[Any], k: int, cand_mask: Optional[np.ndarray] = None,
+                    labels: Optional[np.ndarray] = None) -> List[Tuple[np.ndarray, np.ndarray]]:
+        """Per reference image, the columns of `cands` (and their distances) that osfm_matcher_vlad_select keeps:
+        the k nearest by (distance, column), per camera group when `labels` (len(refs) + len(cands) ints) is given.
+        cand_mask: None or a len(refs) x len(cands) boolean array of allowed candidates."""
+        nref, ncand = len(refs), len(cands)
+        ri = np.array([self._ids[r] for r in refs], dtype=np.int32)
+        ci = np.array([self._ids[c] for c in cands], dtype=np.int32)
+        bits = None
+        if cand_mask is not None:
+            m = np.asarray(cand_mask, dtype=bool).reshape(nref, ncand)
+            packed = np.packbits(m, axis=1, bitorder="little")
+            words = (ncand + 31) // 32
+            padded = np.zeros((nref, 4 * words), dtype=np.uint8)
+            padded[:, :packed.shape[1]] = packed
+            bits = np.ascontiguousarray(padded).view("<u4")
+        lab = None if labels is None else np.ascontiguousarray(labels, dtype=np.int32)
+        if lab is not None and lab.shape != (nref + ncand,):
+            raise ValueError("labels must hold len(refs) + len(cands) ints")
+        cap = max(nref * min(k, ncand) * (2 if lab is not None else 1), 1)
+        offs = np.zeros(nref + 1, dtype=np.int64)
+        cols = np.empty(cap, dtype=np.int32)
+        dist = np.empty(cap, dtype=np.float64)
+
+        def ptr(a):
+            return None if a is None else a.ctypes.data_as(ctypes.c_void_p)
+
+        _lib.check(self._m.L.osfm_matcher_vlad_select(self._m.h, nref, ptr(ri), ncand, ptr(ci), ptr(bits), ptr(lab),
+                                                      int(k), ptr(offs), ptr(cols), ptr(dist)))
+        return [(cols[offs[r]:offs[r + 1]], dist[offs[r]:offs[r + 1]]) for r in range(nref)]
 
     def submit(self, pairs: Sequence[Tuple[Any, Any]], lowes_ratio: float, symmetric: bool = True) -> None:
         ia = np.array([self._ids[a] for a, _ in pairs], dtype=np.int32)

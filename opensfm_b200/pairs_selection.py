@@ -1,0 +1,96 @@
+"""VLAD pair selection on the GPU: the `opensfm.vlad` / `opensfm.pairs_selection` names this engine replaces.
+
+    unnormalized_vlad(features, centers)                       opensfm/vlad.py
+    PairMatcher.vlad_histograms(keys, centers)                 pairs_selection.py:732-745 (vlad_histograms)
+    match_candidates_with_vlad(matcher, images_ref, ...)       pairs_selection.py:351-392, 471-490, 764-795
+
+The VLAD descriptors are computed from the descriptor sets a `PairMatcher` already holds on the device and stay
+there; the all-pairs distances and the neighbour selection run on the device too, so only the selected pairs come
+back.  The selected pairs go straight into `PairMatcher.match_pairs` on the same matcher.  GPS preemption
+(`preempt_candidates`) needs the dataset's topocentric reference and stays with the caller.
+"""
+from __future__ import annotations
+
+import ctypes
+from typing import Any, Dict, Optional, Sequence, Tuple
+
+import numpy as np
+
+from . import _lib
+from .matching import PairMatcher, _thread_matcher
+
+
+def unnormalized_vlad(features: np.ndarray, centers: np.ndarray, device: int = 0) -> Optional[np.ndarray]:
+    """vlad.unnormalized_vlad: the sum of residuals to the nearest centre (float32, len(centers) * dim), bit for bit
+    features::compute_vlad_descriptor; None when the descriptor length or dtype differs from the centres'."""
+    if centers.shape[1] != features.shape[1] or centers.dtype != features.dtype:
+        return None
+    f = np.ascontiguousarray(features, dtype=np.float32)
+    c = np.ascontiguousarray(centers, dtype=np.float32)
+    m = _thread_matcher(device)
+    sid = ctypes.c_int()
+    _lib.check(m.L.osfm_matcher_add_f32(m.h, f.ctypes.data_as(ctypes.c_void_p), f.shape[0], f.shape[1], ctypes.byref(sid)))
+    try:
+        ids = np.array([sid.value], dtype=np.int32)
+        valid = np.zeros(1, dtype=np.int32)
+        _lib.check(m.L.osfm_matcher_vlad_compute(m.h, 1, ids.ctypes.data_as(ctypes.c_void_p), c.ctypes.data_as(ctypes.c_void_p),
+                                                 c.shape[0], c.shape[1], valid.ctypes.data_as(ctypes.c_void_p)))
+        out = np.empty(c.size, dtype=np.float32)
+        _lib.check(m.L.osfm_matcher_vlad_get(m.h, sid.value, 1, out.ctypes.data_as(ctypes.c_void_p)))
+    finally:
+        _lib.check(m.L.osfm_matcher_remove(m.h, sid.value))
+    return out
+
+
+def sorted_pair(im1: Any, im2: Any) -> Tuple[Any, Any]:
+    """pairs_selection.sorted_pair."""
+    return (im1, im2) if im1 < im2 else (im2, im1)
+
+
+def match_candidates_with_vlad(matcher: PairMatcher, images_ref: Sequence[Any], images_cand: Sequence[Any],
+                               exifs: Dict[Any, Any], max_neighbors: int, enforce_other_cameras: bool,
+                               candidates: Optional[Dict[Any, Sequence[Any]]] = None) -> Dict[Tuple[Any, Any], float]:
+    """pairs_selection.match_candidates_with_vlad: {sorted pair: VLAD distance} of every reference image with its
+    `max_neighbors` nearest candidates (and as many of other cameras when `enforce_other_cameras`; cameras are
+    `exifs[image]["camera"]`).
+
+    `matcher` holds the images' descriptors and their VLAD descriptors (`PairMatcher.vlad_histograms` /
+    `compute_vlad`); images whose VLAD could not be computed are skipped, as the reference drops them.
+    `candidates`: {reference image: candidate images}, the first value `preempt_candidates` returns; None or empty
+    means every reference image against every candidate image, the reference's fallback.
+
+    Distances are fp64, sqrt(sum (double(a) - double(b))^2), where the reference takes a float32 norm; ties go to
+    the candidate that comes first in sorted order, which is the order compute_vlad_distances lists them in."""
+    if max_neighbors <= 0:
+        return {}
+
+    def has(im):
+        state = matcher.has_vlad(im)
+        if state is None:
+            raise ValueError("image %r has no VLAD state: run PairMatcher.vlad_histograms on it first" % (im,))
+        return state
+
+    mask = None
+    if not candidates:
+        refs = [im for im in dict.fromkeys(images_ref) if has(im)]
+        cands = sorted({c for c in images_cand if has(c)})
+    else:
+        refs = [im for im in candidates if has(im)]
+        per_ref = [{c for c in candidates[im] if has(c)} for im in refs]
+        cands = sorted(set().union(*per_ref)) if per_ref else []
+        col = {c: j for j, c in enumerate(cands)}
+        if any(len(s) != len(cands) for s in per_ref):
+            mask = np.zeros((len(refs), len(cands)), dtype=bool)
+            for r, s in enumerate(per_ref):
+                mask[r, [col[c] for c in s]] = True
+    if not refs or not cands:
+        return {}
+    labels = None
+    if enforce_other_cameras:
+        names: Dict[Any, int] = {}
+        labels = np.array([names.setdefault(exifs[im]["camera"], len(names)) for im in list(refs) + cands], dtype=np.int32)
+    pairs: Dict[Tuple[Any, Any], float] = {}
+    for im, (cols, dist) in zip(refs, matcher.vlad_select(refs, cands, max_neighbors, mask, labels)):
+        for j, d in zip(cols.tolist(), dist.tolist()):
+            pairs[sorted_pair(im, cands[j])] = d
+    return pairs
