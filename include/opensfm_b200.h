@@ -320,7 +320,7 @@ typedef struct {
   double radius;              /* trust-region radius of the iteration: S holds D_c / radius on its diagonal */
   int nseg, p_fast, p_slow;   /* segments; points in segments; points through the per-point ba_schur */
   int schur_kernel;           /* OSFM_SCHUR_*: the segment kernel that ran (NONE when no point is in a segment) */
-  int sp_nchunks;             /* chunks of the persistent pipelined Schur kernel */
+  int sp_nchunks;             /* chunks of the segment chunk list (0 = none: no segments, or wc != 9 or nres != 2) */
   int pcg_kernel;             /* OSFM_PCG_*: the solver that produced y */
   int pcg_rescued;            /* 1 = the pipelined PCG's result was rejected and the classic PCG re-solved */
   int pcg_iterations;         /* iterations of the solver that produced y */

@@ -14,9 +14,12 @@
 //   S[nc*nc], rhs[nc]                     reduced camera system (dense, symmetric)
 //   Vinv[6][npf], vectors[nc + 3 npf]     per-point inverse blocks, LM vectors
 //
-// Kernels: ba_linearize (per observation), ba_colnorm_grad, ba_schur (CTA per point:
-// U, g_c, V^-1 and W V^-1 W^T scattered to S with fp64 atomics), ba_finish_system,
-// PCG kernels (block-Jacobi), ba_backsub (warp per point), ba_model_change_alg, ba_update.
+// Kernels: ba_linearize (per observation); column norms and gradient over the segment chunk list when the camera
+// side is 9 wide with 2 residual rows (ba_linearize_fused, ba_colnorm_grad_chunks: ba_schur_pipe.cuh), else a warp
+// per segment (ba_colnorm_grad_seg), ba_colnorm_grad for the other observations; the segment Schur kernels
+// (ba_reduced.cuh, ba_schur_pipe.cuh) and ba_schur (CTA per point: U, g_c, V^-1 and W V^-1 W^T scattered to S with
+// fp64 atomics), ba_finish_system, PCG kernels (block-Jacobi), ba_backsub (warp per point), ba_model_change_alg,
+// ba_update.
 #include <algorithm>
 #include <dlfcn.h>
 
@@ -441,163 +444,6 @@ __global__ void __launch_bounds__(256, WCT ? 3 : 2) ba_colnorm_grad_seg(BAView v
   }
 }
 
-// ---------------------------------------------------------------------------------------------------------
-// The same camera-side sums with the observation tiles staged by the TMA engine (cp.async.bulk + mbarrier).
-// The residual / Jacobian planes of a chunk of a segment (<= 8 points seen by the same k shots) are, per plane,
-// one contiguous run of 8 * np * k bytes: a warp stages the 2 + 2 * 9 runs of a chunk into its shared-memory
-// tile with one bulk copy each (lane 0 issues them, all complete on one mbarrier), double-buffered so that the
-// copy of the next chunk is in flight while the current one is reduced.  Lane l owns the accumulators
-// (shot c, column j) = l, l + 32, l + 64 and walks the points of the chunk in shared memory: no shuffles, no
-// atomics until the segment's k * 9 sums are flushed.  wc == 9, nres == 2 (one 3-parameter camera + pose per
-// shot: BASELINE configs[1..3]); chunks whose runs are not 16-byte aligned are staged with plain loads.
-// ---------------------------------------------------------------------------------------------------------
-constexpr int CG_WARPS = 4;
-constexpr int CG_ROWS = 20;                         // r[2] + Jc[2 * 9]
-constexpr int CG_PCHUNK = 8, CG_KMAX = 16;          // points per chunk, shots per segment (= SEG_KMAX, ba_reduced.cuh)
-constexpr int CG_OBS = CG_PCHUNK * CG_KMAX;         // observations per chunk
-constexpr int CG_STAGE_DOUBLES = CG_ROWS * CG_OBS;
-constexpr int CG_SMEM = CG_WARPS * 2 * CG_STAGE_DOUBLES * (int)sizeof(double);   // 163,840 bytes
-
-__device__ __forceinline__ uint32_t cg_smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void cg_mbar_wait(uint64_t* bar, uint32_t parity) {
-  const uint32_t addr = cg_smem_u32(bar);
-  for (;;) {
-    uint32_t done;
-    asm volatile(
-        "{\n.reg .pred p;\n"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n"
-        "selp.u32 %0, 1, 0, p;\n}\n"
-        : "=r"(done)
-        : "r"(addr), "r"(parity)
-        : "memory");
-    if (done) return;
-  }
-}
-
-__global__ void __launch_bounds__(32 * CG_WARPS, 1)
-    ba_colnorm_grad_tma(BAView v, const int* __restrict__ seg_start, int nseg, const long long* __restrict__ tab_off,
-                        const int* __restrict__ tab, double* colnorm2, double* grad) {
-  extern __shared__ __align__(128) double cg_tiles[];
-  __shared__ __align__(8) uint64_t bars[CG_WARPS][2];
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (threadIdx.x == 0) {
-    for (int w = 0; w < CG_WARPS; ++w)
-      for (int st = 0; st < 2; ++st)
-        asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(cg_smem_u32(&bars[w][st])), "r"(1));
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  __syncthreads();
-  double* tile[2] = {cg_tiles + (size_t)(warp * 2) * CG_STAGE_DOUBLES, cg_tiles + (size_t)(warp * 2 + 1) * CG_STAGE_DOUBLES};
-  const size_t N = (size_t)v.N;
-  const int gw = blockIdx.x * CG_WARPS + warp, nw = gridDim.x * CG_WARPS;
-  uint32_t phase[2] = {0u, 0u};
-
-  // stage chunk [pc0, pc0 + np) of a segment with k shots into tile[st]; returns whether the TMA path was used
-  auto stage = [&](int st, int pc0, int np, int k) -> bool {
-    const long long ibase = v.pt_start[pc0];
-    const int run = np * k;
-    const bool aligned = ((ibase | (long long)run | (long long)N) & 1LL) == 0;   // 16-byte aligned runs in every plane
-    if (aligned) {
-      if (lane == 0) {
-        const uint32_t bytes = (uint32_t)run * 8u;
-        asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(cg_smem_u32(&bars[warp][st])),
-                     "r"(bytes * CG_ROWS)
-                     : "memory");
-        for (int row = 0; row < CG_ROWS; ++row) {
-          const double* src = (row < 2 ? v.r + (size_t)row * N : v.Jc + (size_t)(row - 2) * N) + ibase;
-          asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
-                           cg_smem_u32(tile[st] + row * CG_OBS)),
-                       "l"(src), "r"(bytes), "r"(cg_smem_u32(&bars[warp][st]))
-                       : "memory");
-        }
-      }
-    } else {
-      for (int idx = lane; idx < CG_ROWS * run; idx += 32) {
-        const int row = idx / run, e = idx - row * run;
-        tile[st][row * CG_OBS + e] = (row < 2 ? v.r + (size_t)row * N : v.Jc + (size_t)(row - 2) * N)[ibase + e];
-      }
-    }
-    return aligned;
-  };
-
-  // (segment, chunk) walk of this warp, one step ahead for the prefetch
-  int s = gw, pc = 0, p_end = 0, k = 0;
-  auto open_segment = [&]() {
-    while (s < nseg) {
-      pc = seg_start[s]; p_end = seg_start[s + 1];
-      if (pc < p_end) { k = (int)(v.pt_start[pc + 1] - v.pt_start[pc]); return true; }
-      s += nw;
-    }
-    return false;
-  };
-  if (!open_segment()) return;
-  int st = 0;
-  bool cur_tma = stage(0, pc, min(CG_PCHUNK, p_end - pc), k);
-  double n2[3] = {0.0, 0.0, 0.0}, gr[3] = {0.0, 0.0, 0.0};
-  while (true) {
-    const int np = min(CG_PCHUNK, p_end - pc);
-    const int cur_k = k, cur_pc = pc;
-    const bool last_chunk = pc + np >= p_end;
-    // next (segment, chunk)
-    int ns = s, npc = pc + np, np_end = p_end, nk = k;
-    bool have_next = true;
-    if (last_chunk) {
-      ns = s + nw;
-      have_next = false;
-      while (ns < nseg) {
-        npc = seg_start[ns]; np_end = seg_start[ns + 1];
-        if (npc < np_end) { nk = (int)(v.pt_start[npc + 1] - v.pt_start[npc]); have_next = true; break; }
-        ns += nw;
-      }
-    }
-    bool next_tma = false;
-    if (have_next) next_tma = stage(st ^ 1, npc, min(CG_PCHUNK, np_end - npc), nk);
-    if (cur_tma) { cg_mbar_wait(&bars[warp][st], phase[st]); phase[st] ^= 1u; }
-    else __syncwarp();
-    // reduce the chunk: accumulator a = c * 9 + j
-    const double* T = tile[st];
-    const int nacc = cur_k * 9;
-#pragma unroll
-    for (int u = 0; u < 3; ++u) {
-      const int a = lane + 32 * u;
-      if (a < nacc) {
-        const int c = a / 9, j = a - c * 9;
-        for (int pi = 0; pi < np; ++pi) {
-          const int e = pi * cur_k + c;
-          const double j0 = T[(2 + j) * CG_OBS + e], j1 = T[(2 + 9 + j) * CG_OBS + e];
-          n2[u] += j0 * j0 + j1 * j1;
-          gr[u] += j0 * T[e] + j1 * T[CG_OBS + e];
-        }
-      }
-    }
-    __syncwarp();   // the tile may be overwritten by the copy issued two steps from now
-    if (last_chunk) {
-      const long long base = v.pt_start[seg_start[s]];
-#pragma unroll
-      for (int u = 0; u < 3; ++u) {
-        const int a = lane + 32 * u;
-        if (a < nacc) {
-          int col;
-          if (tab) {   // per-segment column table (ba_seg_tables): one load instead of the shot -> camera -> offset chain
-            col = tab[tab_off[s] + a];
-          } else {
-            const int c = a / 9, j = a - c * 9;
-            const ObsCols oc = obs_cols(v, base + c);
-            col = oc.col(j);
-          }
-          if (col >= 0) { atomicAdd(&colnorm2[col], n2[u]); atomicAdd(&grad[col], gr[u]); }
-        }
-        n2[u] = 0.0; gr[u] = 0.0;
-      }
-    }
-    (void)cur_pc;
-    if (!have_next) break;
-    s = ns; pc = npc; p_end = np_end; k = nk;
-    cur_tma = next_tma;
-    st ^= 1;
-  }
-}
-
 __global__ void ba_prior_colnorm_grad(PriorView pv, Params p, double* colnorm2, double* grad) {
   const int row = blockIdx.x * blockDim.x + threadIdx.x;
   if (row >= pv.n_cam_rows + pv.n_pos_rows) return;
@@ -669,7 +515,6 @@ inline void launch_cooperative(void (*kern)(KArgs...), int grid, int block, size
   launch_cooperative_impl(kern, grid, block, smem, st, a, std::index_sequence_for<KArgs...>{});
 }
 }  // namespace osfm
-static_assert(osfm::CG_KMAX == osfm::SEG_KMAX, "colnorm tiles hold the widest segment");
 #include "ba_side.cuh"
 #include "ba_order.cuh"
 #include "ba_cov.cuh"
@@ -910,6 +755,14 @@ static const BaSwitches& switches() {
   return s;
 }
 
+// How linearize() forms the camera-side column norms and gradient of the segment observations (RunState::lin)
+enum LinPath {
+  LIN_NONE,       // no segments
+  LIN_FUSED,      // ba_linearize_fused: with the planes, over the chunk list (also the sums of ba_point_blocks_sums)
+  LIN_CHUNKS,     // ba_colnorm_grad_chunks over the chunk list
+  LIN_SEGMENTS,   // ba_colnorm_grad_seg, a warp per segment (no chunk list: wc != 9 or nres != 2)
+};
+
 // What one run() derives from the problem, rebuilt by every run(): sizes, host tables, device views, kernel paths.
 struct RunState {
   std::chrono::high_resolution_clock::time_point t_start, t_prev;   // run() start, last trace line
@@ -938,9 +791,9 @@ struct RunState {
   int cov_m = 0, cov_nb1 = 0;              // instance columns (last in the dense S); blocks of the leading part
   // kernel paths
   int schur = OSFM_SCHUR_NONE;    // OSFM_SCHUR_*: the segment kernel of build_system
+  LinPath lin = LIN_NONE;         // the segment column norms of linearize
   bool seg_tab = false;           // ba_seg_tables has run (gcol of every segment column)
-  int sp_nchunks = 0;             // chunk list of ba_schur_pipe (0 = none)
-  bool lin_fused = false;         // ba_linearize_fused: the linearisation also forms the sums of ba_point_blocks_sums
+  int sp_nchunks = 0;             // segment chunk list (0 = none)
   bool pcg_resident = false, pcg_pipe_ok = false;   // the classic PCG keeps S in shared memory; pipelined PCG fits
   int pcg_smem = 0, pcg_pipe_smem = 0;
   PcgResident pcg_res{};
@@ -1739,17 +1592,15 @@ void BA::reserve_covariance() {
   d_cov_flags.reserve(COV_F_COUNT);
 }
 
-// Per-segment tables of the tensor-core Schur kernels (columns, block offsets) and the chunk list of the persistent
-// one; decides the Schur path of the run and whether the linearisation runs over the chunk list (ba_linearize_fused).
-// Structure only, before the first linearisation: the Jacobi scales of the tables follow in segment_table_scales().
+// Structure of the segments, before the first linearisation (the Jacobi scales of the tables follow in
+// segment_table_scales()): the per-segment tables (columns, block offsets), the segment chunk list and the flush table
+// of the persistent Schur kernel.  Decides the Schur path and the linearisation path of the run.
 void BA::build_segment_tables() {
   const int nseg = rs.nseg, wc = rs.wc;
   // The tensor-core kernels add the same-shot blocks J^T J only in the tiles (t, t) and (t, t + 1): a shot's wc
   // columns must not span three 8-wide tiles, i.e. wc <= 9.  Wider camera sides (Brown: 9 + 6, rig cameras: + 6)
   // use the SIMT segment kernels.
-  const bool use_mma = switches().schur_mma && wc <= 9;
-  bool use_pipe = false;
-  if (nseg > 0 && use_mma && rs.nblk > 0) {
+  if (nseg > 0 && rs.nblk > 0 && wc <= 9) {
     d_tab_off.reserve((size_t)nseg + 1); d_tab_sizes.reserve((size_t)nseg + 1);
     ba_seg_table_sizes<<<grid_for(nseg + 1, 256), 256, 0, stream>>>(rs.v, d_seg_start.p, nseg, d_tab_sizes.p);
     OSFM_LAUNCH_CHECK();
@@ -1765,34 +1616,42 @@ void BA::build_segment_tables() {
     ba_seg_tables<<<nseg, 128, 0, stream>>>(rs.v, rs.bm, rs.bsr, d_seg_start.p, nullptr, d_tab_off.p, d_tab.p);
     OSFM_LAUNCH_CHECK();
     rs.seg_tab = true;
-    // chunk list of the persistent Schur kernel (ba_schur_pipe.cuh)
-    // (the flush table holds offset << 2: the reduced system must stay below 2^29 doubles; 20 KB of table per segment)
-    use_pipe = switches().schur_pipe && rs.nres * (wc + 4) <= SP_ROWS && rs.s_upper_total + (long long)rs.nc_pad < (1LL << 29) &&
-               (long long)nseg * SP_FT_SEG * (long long)sizeof(int) <= (8LL << 30);
-    if (use_pipe) {
-      d_sp_nch.reserve((size_t)nseg + 1); d_sp_chunk0.reserve((size_t)nseg + 1);
-      sp_chunk_counts<<<grid_for(nseg + 1, 256), 256, 0, stream>>>(rs.v, d_seg_start.p, nseg, d_sp_nch.p);
-      OSFM_LAUNCH_CHECK();
-      size_t tb2 = 0;
-      cub::DeviceScan::ExclusiveSum(nullptr, tb2, d_sp_nch.p, d_sp_chunk0.p, nseg + 1, stream);
-      d_cub.reserve(tb2 + 256);
-      tb2 = d_cub.cap;
-      OSFM_CUDA(cub::DeviceScan::ExclusiveSum(d_cub.p, tb2, d_sp_nch.p, d_sp_chunk0.p, nseg + 1, stream));
-      OSFM_CUDA(cudaMemcpyAsync(&rs.sp_nchunks, d_sp_chunk0.p + nseg, sizeof(int), cudaMemcpyDeviceToHost, stream));
-      OSFM_CUDA(cudaStreamSynchronize(stream));
-      d_sp_chunks.reserve((size_t)rs.sp_nchunks + 1);
-      sp_fill_chunks<<<grid_for((long long)nseg * 32, 256), 256, 0, stream>>>(rs.v, d_seg_start.p, nseg, d_sp_chunk0.p,
-                                                                            d_tab_off.p, d_sp_chunks.p);
-      OSFM_LAUNCH_CHECK();
-      d_sp_ftab.reserve((size_t)nseg * SP_FT_SEG);
-      sp_flush_tables<<<nseg, SP_CONS_THREADS, 0, stream>>>(rs.v, d_seg_start.p, d_tab_off.p, d_tab.p, d_sp_ftab.p);
-      OSFM_LAUNCH_CHECK();
-    }
+  }
+  // The chunk list (ba_schur_pipe.cuh) of the camera side every chunk-list kernel is written for: a 3-parameter camera
+  // and a pose per shot, 2-D residuals
+  if (rs.seg_tab && wc == 9 && rs.nres == 2) {
+    d_sp_nch.reserve((size_t)nseg + 1); d_sp_chunk0.reserve((size_t)nseg + 1);
+    sp_chunk_counts<<<grid_for(nseg + 1, 256), 256, 0, stream>>>(rs.v, d_seg_start.p, nseg, d_sp_nch.p);
+    OSFM_LAUNCH_CHECK();
+    size_t tb = 0;
+    cub::DeviceScan::ExclusiveSum(nullptr, tb, d_sp_nch.p, d_sp_chunk0.p, nseg + 1, stream);
+    d_cub.reserve(tb + 256);
+    tb = d_cub.cap;
+    OSFM_CUDA(cub::DeviceScan::ExclusiveSum(d_cub.p, tb, d_sp_nch.p, d_sp_chunk0.p, nseg + 1, stream));
+    OSFM_CUDA(cudaMemcpyAsync(&rs.sp_nchunks, d_sp_chunk0.p + nseg, sizeof(int), cudaMemcpyDeviceToHost, stream));
+    OSFM_CUDA(cudaStreamSynchronize(stream));
+    d_sp_chunks.reserve((size_t)rs.sp_nchunks + 1);
+    sp_fill_chunks<<<grid_for((long long)nseg * 32, 256), 256, 0, stream>>>(rs.v, d_seg_start.p, nseg, d_sp_chunk0.p,
+                                                                          d_tab_off.p, d_sp_chunks.p);
+    OSFM_LAUNCH_CHECK();
+  }
+  // the persistent Schur kernel runs over the chunk list; its flush table holds offset << 2 (the reduced system must
+  // stay below 2^29 doubles) and takes 20 KB per segment
+  const bool use_mma = switches().schur_mma && wc <= 9;
+  const bool use_pipe = use_mma && switches().schur_pipe && rs.sp_nchunks > 0 &&
+                        rs.s_upper_total + (long long)rs.nc_pad < (1LL << 29) &&
+                        (long long)nseg * SP_FT_SEG * (long long)sizeof(int) <= (8LL << 30);
+  if (use_pipe) {
+    d_sp_ftab.reserve((size_t)nseg * SP_FT_SEG);
+    sp_flush_tables<<<nseg, SP_CONS_THREADS, 0, stream>>>(rs.v, d_seg_start.p, d_tab_off.p, d_tab.p, d_sp_ftab.p);
+    OSFM_LAUNCH_CHECK();
   }
   rs.schur = nseg == 0 ? OSFM_SCHUR_NONE
              : !use_mma ? OSFM_SCHUR_SIMT_SEGMENT
-             : (use_pipe && rs.sp_nchunks > 0) ? OSFM_SCHUR_PIPE : OSFM_SCHUR_MMA;
-  rs.lin_fused = rs.sp_nchunks > 0 && wc == 9 && rs.nres == 2 && rs.uniform_type == PT_PERSPECTIVE;
+             : use_pipe ? OSFM_SCHUR_PIPE : OSFM_SCHUR_MMA;
+  rs.lin = nseg == 0 ? LIN_NONE
+           : rs.sp_nchunks == 0 ? LIN_SEGMENTS
+           : rs.uniform_type == PT_PERSPECTIVE ? LIN_FUSED : LIN_CHUNKS;
 }
 
 // The Jacobi scale of every segment column into the tables, whenever d_scale has been (re)computed.
@@ -1831,7 +1690,7 @@ double BA::linearize(int b, bool timed, double* grad_max) {
   OSFM_CUDA(cudaMemsetAsync(d_sc.p, 0, sizeof(Scalars), stream));
   OSFM_CUDA(cudaMemsetAsync(d_colnorm2.p, 0, sizeof(double) * rs.nz, stream));
   OSFM_CUDA(cudaMemsetAsync(d_grad.p, 0, sizeof(double) * rs.nz, stream));
-  if (N > 0 && rs.lin_fused) {
+  if (N > 0 && rs.lin == LIN_FUSED) {
     // planes, cost and the segment observations' column norms / gradient / point sums in one pass; the observations
     // outside the segments get their sums from the plane-reading kernels
     d_ptsum.reserve(9 * (size_t)std::max(rs.npf, 1));
@@ -1853,22 +1712,15 @@ double BA::linearize(int b, bool timed, double* grad_max) {
     if (timed) rs.tm_lin.stop(stream);
     ba_colnorm_grad_points<<<grid_for(N, 256), 256, 0, stream>>>(rs.v, 0, d_colnorm2.p, d_grad.p);
     OSFM_LAUNCH_CHECK();
-    if (nseg > 0) {
-      if (wc == 9 && rs.nres == 2 && rs.sp_nchunks > 0) {
-        // the chunk list exists: no dependent index loads
-        opt_in_smem(ba_colnorm_grad_chunks, CC_SMEM);
-        const int grid = std::max(1, std::min(num_sms, (rs.sp_nchunks + CC_WARPS - 1) / CC_WARPS));
-        ba_colnorm_grad_chunks<<<grid, 32 * CC_WARPS, CC_SMEM, stream>>>(rs.v, d_sp_chunks.p, rs.sp_nchunks, d_tab.p,
-                                                                          d_colnorm2.p, d_grad.p);
-      } else if (wc == 9 && rs.nres == 2) {
-        opt_in_smem(ba_colnorm_grad_tma, CG_SMEM);
-        const int grid = std::max(1, std::min(num_sms, (nseg + CG_WARPS - 1) / CG_WARPS));
-        ba_colnorm_grad_tma<<<grid, 32 * CG_WARPS, CG_SMEM, stream>>>(rs.v, d_seg_start.p, nseg, rs.seg_tab ? d_tab_off.p : nullptr,
-                                                                      rs.seg_tab ? d_tab.p : nullptr, d_colnorm2.p, d_grad.p);
-      } else {
-        auto kern = wc == 9 ? ba_colnorm_grad_seg<9> : ba_colnorm_grad_seg<0>;
-        kern<<<grid_for((long long)nseg * 32, 256), 256, 0, stream>>>(rs.v, d_seg_start.p, nseg, d_colnorm2.p, d_grad.p);
-      }
+    if (rs.lin == LIN_CHUNKS) {   // no dependent index loads
+      opt_in_smem(ba_colnorm_grad_chunks, CC_SMEM);
+      const int grid = std::max(1, std::min(num_sms, (rs.sp_nchunks + CC_WARPS - 1) / CC_WARPS));
+      ba_colnorm_grad_chunks<<<grid, 32 * CC_WARPS, CC_SMEM, stream>>>(rs.v, d_sp_chunks.p, rs.sp_nchunks, d_tab.p,
+                                                                        d_colnorm2.p, d_grad.p);
+      OSFM_LAUNCH_CHECK();
+    } else if (rs.lin == LIN_SEGMENTS) {
+      auto kern = wc == 9 ? ba_colnorm_grad_seg<9> : ba_colnorm_grad_seg<0>;
+      kern<<<grid_for((long long)nseg * 32, 256), 256, 0, stream>>>(rs.v, d_seg_start.p, nseg, d_colnorm2.p, d_grad.p);
       OSFM_LAUNCH_CHECK();
     }
     if (N > n_fast_obs) {
@@ -1932,7 +1784,7 @@ void BA::build_system(double inv_radius, int* rank_flag, bool timed) {
     if (timed) rs.tm_schur.start(stream);
     if (rs.schur != OSFM_SCHUR_NONE) {
       d_Vig.reserve(3 * (size_t)std::max(rs.npf, 1));
-      if (rs.lin_fused)   // the point sums of the linearisation
+      if (rs.lin == LIN_FUSED)   // the point sums of the linearisation
         ba_point_blocks_sums<<<grid_for(P_fast, PB_THREADS), PB_THREADS, 0, stream>>>(
             rs.v, P_fast, d_ptsum.p, d_scale.p, d_diag.p, inv_radius, d_Vinv.p, d_gp.p, d_Vig.p, rank_flag);
       else
@@ -1948,8 +1800,7 @@ void BA::build_system(double inv_radius, int* rank_flag, bool timed) {
         prof = d_prof.p;
       }
       if (rs.schur == OSFM_SCHUR_PIPE) {
-        auto kern = wc == 9 ? (prof ? ba_schur_pipe<9, true> : ba_schur_pipe<9, false>)
-                            : (prof ? ba_schur_pipe<0, true> : ba_schur_pipe<0, false>);
+        auto kern = prof ? ba_schur_pipe<true> : ba_schur_pipe<false>;
         opt_in_smem(kern, (int)sizeof(SpSmem));
         const int grid = std::max(1, std::min(num_sms, rs.sp_nchunks));
         kern<<<grid, SP_THREADS, sizeof(SpSmem), stream>>>(rs.v, d_sp_chunks.p, rs.sp_nchunks, d_tab.p, d_scale.p, d_Vinv.p,

@@ -23,9 +23,11 @@
 //     (20 KB per segment, 430 MB at C4).  A warp prefetches its 3.3 KB with cp.async at the start of a segment.
 //     (scattered fp64 RED into L2 are several times slower than a warp's RED to 32 consecutive elements, and a C4
 //     launch issues 87M of them.)
-// Eligible: nres * (wc + 4) <= SP_ROWS plane rows per observation (2-D residuals with wc <= 9); everything else
-// keeps ba_schur_mma.  OSFM_BA_SCHUR_PIPE=0 switches back for A/B runs.
+// Eligible: wc == 9, nres == 2 (a 3-parameter camera and a pose per shot), the camera side of the chunk list;
+// everything else keeps ba_schur_mma.  OSFM_BA_SCHUR_PIPE=0 switches back for A/B runs.
 #pragma once
+
+#include "async_copy.cuh"
 
 namespace osfm {
 
@@ -35,12 +37,12 @@ constexpr int SP_PROD_THREADS = 32 * SP_PROD_WARPS;
 constexpr int SP_CONS_THREADS = 32 * SP_CONS_WARPS;
 constexpr int SP_THREADS = SP_PROD_THREADS + 2 * SP_CONS_THREADS;   // 640
 constexpr int SP_ROWS = 26;                         // staged plane rows: r (nres) + Jp (3 nres) + Jc (wc nres)
+static_assert(SP_ROWS == 2 * (1 + 3 + 9), "the plane rows of an observation with wc == 9, nres == 2");
 constexpr int SP_OBS = SM_PCH * SEG_KMAX;           // 128 observations per chunk at most
 constexpr int SP_SLOTS = SM_NT + 1;                 // tiles of a row pair (p, nt - 1 - p): nt + 1
 constexpr int SP_NPAIR9 = 9 * (SEG_KMAX * (SEG_KMAX + 1) / 2);
 static_assert(2 * SP_OBS == SP_PROD_THREADS, "two producer threads per observation of a chunk");
 static_assert(2 * SP_CONS_WARPS >= SM_NT, "a consumer warp per pair of tile rows");
-static_assert((SP_ROWS / 2) - 4 <= 9, "same-shot blocks are only accumulated in the tiles (t, t) and (t, t + 1): wc <= 9");
 
 struct SchurChunk {      // 48 bytes, read with three 16-byte loads
   long long ibase;       // first observation of the chunk (sorted order)
@@ -104,45 +106,18 @@ struct SpSmem {
   // full[group][buffer]: a group waits only for the chunks it owns, so it has to see every phase of the barrier it
   // waits on (mbarrier parity waits cannot tell phase u + 1 from phase u - 1) -> one "full" barrier per (group, buffer);
   // empty[buffer] is waited on by the producers alone, once per use.
-  unsigned long long full[2][2], empty[2];
+  uint64_t full[2][2], empty[2];
 };
 
-__device__ __forceinline__ uint32_t sp_saddr(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void sp_cp8(void* dst, const void* src) {
-  asm volatile("cp.async.ca.shared.global [%0], [%1], 8;" ::"r"(sp_saddr(dst)), "l"(src) : "memory");
+  asm volatile("cp.async.ca.shared.global [%0], [%1], 8;" ::"r"(smem_u32(dst)), "l"(src) : "memory");
 }
 __device__ __forceinline__ void sp_cp4(void* dst, const void* src) {
-  asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(sp_saddr(dst)), "l"(src) : "memory");
+  asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(smem_u32(dst)), "l"(src) : "memory");
 }
 __device__ __forceinline__ void sp_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
 __device__ __forceinline__ void sp_wait_all() { asm volatile("cp.async.wait_group 0;" ::: "memory"); }
 __device__ __forceinline__ void sp_bar(int id, int count) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory"); }
-__device__ __forceinline__ void sp_mbar_init(unsigned long long* b, int count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(sp_saddr(b)), "r"(count) : "memory");
-}
-__device__ __forceinline__ void sp_mbar_arrive(unsigned long long* b) {
-  asm volatile("{\n.reg .b64 st;\nmbarrier.arrive.shared::cta.b64 st, [%0];\n}" ::"r"(sp_saddr(b)) : "memory");
-}
-__device__ __forceinline__ void sp_mbar_wait(unsigned long long* b, int parity) {
-  const uint32_t a = sp_saddr(b);
-  uint32_t done = 0;
-  long long t0 = 0;
-  int spins = 0;
-  while (true) {
-    asm volatile(
-        "{\n.reg .pred p;\n"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n"
-        "selp.u32 %0, 1, 0, p;\n}"
-        : "=r"(done)
-        : "r"(a), "r"(parity)
-        : "memory");
-    if (done) break;
-    if ((++spins & 1023) == 0) {   // a protocol bug must not hang the GPU
-      if (t0 == 0) t0 = clock64();
-      else if (clock64() - t0 > 8000000000LL) __trap();
-    }
-  }
-}
 __device__ __forceinline__ SchurChunk sp_load_chunk(const SchurChunk* chunks, int n) {
   const int4* p = reinterpret_cast<const int4*>(chunks + n);
   union { int4 q[3]; SchurChunk e; } u;
@@ -203,11 +178,11 @@ __global__ void __launch_bounds__(SP_CONS_THREADS)
 }
 
 // ---------------------------------------------------------------------------------------------------------
-// Camera-side gradient and squared column norms over the chunk list (wc == 9, nres == 2): ba_colnorm_grad_tma
-// (ba.cu) walks seg_start / pt_start with three dependent loads per chunk before it can issue the next copy; here a
-// warp owns a contiguous range of chunks (cut at segment starts), reads one 48-byte entry per chunk (the entry of
-// chunk n + 1 is in registers while chunk n is reduced) and takes the global columns from the per-segment table.
-// Staging as there: one bulk copy (TMA engine) per plane row and chunk, two stages per warp, one mbarrier each.
+// Camera-side gradient and squared column norms over the chunk list (wc == 9, nres == 2): a warp owns a contiguous
+// range of chunks (cut at segment starts), reads one 48-byte entry per chunk (the entry of chunk n + 1 is in registers
+// while chunk n is reduced; walking seg_start / pt_start instead costs three dependent loads per chunk before the next
+// copy can be issued) and takes the global columns from the per-segment table.  Staging: one bulk copy (TMA engine)
+// per plane row and chunk, two stages per warp, one mbarrier each.
 // ---------------------------------------------------------------------------------------------------------
 constexpr int CC_WARPS = 5;
 constexpr int CC_ROWS = 20;                       // r[2] + Jc[2 * 9]
@@ -218,11 +193,11 @@ __global__ void __launch_bounds__(32 * CC_WARPS, 1)
     ba_colnorm_grad_chunks(BAView v, const SchurChunk* __restrict__ chunks, int nchunks, const int* __restrict__ tab,
                            double* colnorm2, double* grad) {
   extern __shared__ __align__(128) double cc_tiles[];
-  __shared__ __align__(8) unsigned long long bars[CC_WARPS][2];
+  __shared__ __align__(8) uint64_t bars[CC_WARPS][2];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (threadIdx.x == 0) {
     for (int w = 0; w < CC_WARPS; ++w)
-      for (int st = 0; st < 2; ++st) sp_mbar_init(&bars[w][st], 1);
+      for (int st = 0; st < 2; ++st) mbar_init(&bars[w][st], 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
@@ -246,14 +221,10 @@ __global__ void __launch_bounds__(32 * CC_WARPS, 1)
     if (aligned) {
       if (lane == 0) {
         const uint32_t bytes = (uint32_t)run * 8u;
-        const uint32_t bar = sp_saddr(&bars[warp][st]);
-        asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes * CC_ROWS) : "memory");
+        mbar_expect_tx(&bars[warp][st], bytes * CC_ROWS);
         for (int row = 0; row < CC_ROWS; ++row) {
           const double* src = (row < 2 ? v.r + (size_t)row * N : v.Jc + (size_t)(row - 2) * N) + e.ibase;
-          asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
-                           sp_saddr(tile[st] + row * SP_OBS)),
-                       "l"(src), "r"(bytes), "r"(bar)
-                       : "memory");
+          bulk_copy_g2s(tile[st] + row * SP_OBS, src, bytes, &bars[warp][st]);
         }
       }
     } else {
@@ -288,7 +259,7 @@ __global__ void __launch_bounds__(32 * CC_WARPS, 1)
       }
     }
     if (cur_tma) {
-      sp_mbar_wait(&bars[warp][st], st ? phase1 : phase0);
+      mbar_wait(&bars[warp][st], st ? phase1 : phase0);
       if (st) phase1 ^= 1u; else phase0 ^= 1u;
     } else {
       __syncwarp();
@@ -580,7 +551,7 @@ __global__ void __launch_bounds__(PB_THREADS)
   point_block_finish(v, pf, V, diag, inv_radius, Vinv, gpo, Vig, rank_flag);
 }
 
-template <int WC, bool PROF>
+template <bool PROF>
 __global__ void __launch_bounds__(SP_THREADS, 1)
     ba_schur_pipe(BAView v, const SchurChunk* __restrict__ chunks, int nchunks, const int* __restrict__ tab,
                   const double* __restrict__ scale, const double* __restrict__ Vinv, const double* __restrict__ Vig,
@@ -590,7 +561,7 @@ __global__ void __launch_bounds__(SP_THREADS, 1)
   //   [4..8] consumer group 0 / [9..13] group 1: (unused), wait for operands, mma, flush, segments
   extern __shared__ __align__(16) unsigned char sp_raw[];
   SpSmem& sm = *reinterpret_cast<SpSmem*>(sp_raw);
-  const int wc = WC ? WC : v.wc;
+  constexpr int wc = 9;
   const int nres = v.nres;
   const int tid = threadIdx.x;
 
@@ -606,9 +577,9 @@ __global__ void __launch_bounds__(SP_THREADS, 1)
 
   if (tid == 0) {
     for (int i = 0; i < 2; ++i) {
-      sp_mbar_init(&sm.full[0][i], SP_PROD_THREADS);
-      sp_mbar_init(&sm.full[1][i], SP_PROD_THREADS);
-      sp_mbar_init(&sm.empty[i], SP_CONS_WARPS);
+      mbar_init(&sm.full[0][i], SP_PROD_THREADS);
+      mbar_init(&sm.full[1][i], SP_PROD_THREADS);
+      mbar_init(&sm.empty[i], SP_CONS_WARPS);
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
@@ -636,7 +607,7 @@ __global__ void __launch_bounds__(SP_THREADS, 1)
             for (int j = 0; j < 3; ++j) sp_cp8(&S.pl[nres + q * 3 + j][t], &v.Jp[((size_t)q * 3 + j) * N + i]);
           }
 #pragma unroll
-          for (int c2 = 0; c2 < (WC ? WC : SEG_WCMAX); ++c2)
+          for (int c2 = 0; c2 < wc; ++c2)
             if (c2 >= c2_lo && c2 < c2_hi) sp_cp8(&S.pl[nres * 4 + q * wc + c2][t], &v.Jc[((size_t)q * wc + c2) * N + i]);
         }
       }
@@ -672,7 +643,7 @@ __global__ void __launch_bounds__(SP_THREADS, 1)
       SpOperand& O = sm.op[buf];
       const int np = e.np, k = e.k, run = np * k, ncols = k * wc;
       const bool pfree = e.pf0 >= 0;
-      sp_mbar_wait(&sm.empty[buf], (use & 1) ^ 1);   // the consumers released this operand buffer
+      mbar_wait(&sm.empty[buf], (use & 1) ^ 1);   // the consumers released this operand buffer
       pmark(1);
       // rows [3 np, 4 ksteps) and the padding columns [ncols, 8 nt) must read as zero
       {
@@ -707,7 +678,7 @@ __global__ void __launch_bounds__(SP_THREADS, 1)
           for (int e3 = 0; e3 < 3; ++e3) vg[e3] = pd[6 + e3];
         }
 #pragma unroll
-        for (int cc = 0; cc < ((WC ? WC : SEG_WCMAX) + 1) / 2; ++cc) {
+        for (int cc = 0; cc < (wc + 1) / 2; ++cc) {
           const int c2 = c2_lo + cc;
           if (c2 >= c2_hi) break;
           const int col = bb * wc + c2;
@@ -730,7 +701,7 @@ __global__ void __launch_bounds__(SP_THREADS, 1)
           O.G[lp][col] = gr;
         }
       }
-      sp_mbar_arrive(&sm.full[e.seg & 1][buf]);
+      mbar_arrive(&sm.full[e.seg & 1][buf]);
       pmark(2);
     }
     if (PROF && tid == 0) {
@@ -790,7 +761,7 @@ __global__ void __launch_bounds__(SP_THREADS, 1)
         sp_commit();
       }
     }
-    sp_mbar_wait(&sm.full[g][buf], (buf ? uses1++ : uses0++) & 1);
+    mbar_wait(&sm.full[g][buf], (buf ? uses1++ : uses0++) & 1);
     cmark(1);
     {
       const SpOperand& O = sm.op[buf];
@@ -820,7 +791,7 @@ __global__ void __launch_bounds__(SP_THREADS, 1)
         for (int lp = 0; lp < np; ++lp) racc += O.G[lp][gt];
     }
     __syncwarp();
-    if (lane == 0) sp_mbar_arrive(&sm.empty[buf]);
+    if (lane == 0) mbar_arrive(&sm.empty[buf]);
     cmark(2);
     if (n == e.seg_chunk0 + e.seg_nch - 1) {
       // ---- flush the segment: destinations from the table, values straight from the fragments ----

@@ -33,6 +33,7 @@
 // a task (lexicographic (value, index), i.e. cv2's insertion order).
 #include <cuda_bf16.h>
 
+#include "async_copy.cuh"
 #include "common.cuh"
 #include "match_common.cuh"
 
@@ -209,52 +210,8 @@ size_t tc_operand_bytes(int rows_padded) { return 2 * (size_t)rows_padded * TC_R
 bool tc_capable(int dim, bool u8) { return !u8 && dim <= TC_KD && tc_available(); }
 
 // ---------------------------------------------------------------------------
-// PTX wrappers
+// wgmma PTX wrappers (mbarrier and bulk copy: async_copy.cuh)
 // ---------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
-__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-// Bounded wait: a protocol bug must surface as a trapped kernel, never as a hung GPU.
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity, int* err_flag) {
-  const uint32_t addr = smem_u32(bar);
-  long long t0 = 0;
-  // try_wait suspends the thread for a hardware-defined time slice before it reports failure, so the loop is
-  // cheap; the clock is only consulted every 1024 failed slices
-  for (unsigned spins = 0;; ++spins) {
-    uint32_t done;
-    asm volatile(
-        "{\n.reg .pred p;\n"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n"
-        "selp.u32 %0, 1, 0, p;\n}\n"
-        : "=r"(done)
-        : "r"(addr), "r"(parity)
-        : "memory");
-    if (done) return;
-    if ((spins & 1023u) == 1023u) {
-      const long long now = clock64();
-      if (t0 == 0) t0 = now;
-      else if (now - t0 > 4000000000LL) {
-        atomicExch(err_flag, 1);
-        __trap();
-      }
-    }
-  }
-}
-__device__ __forceinline__ void bulk_copy_g2s(void* smem_dst, const void* gsrc, uint32_t bytes, uint64_t* bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
-                   smem_u32(smem_dst)),
-               "l"(gsrc), "r"(bytes), "r"(smem_u32(bar))
-               : "memory");
-}
-
 // wgmma shared-memory descriptor, K-major without swizzle: start >> 4 @0, LBO >> 4 @16 (K-adjacent core
 // matrices), SBO >> 4 @32 (8-row groups), base offset 0 @49, layout type 0 (interleave) @62
 template <int SBO>

@@ -12,10 +12,12 @@ Every scene captures LM iteration 1 (osfm_ba_capture_linear_system) and checks
 The same scenes run under the OSFM_BA_* switches (in subprocesses: the switches are read once per process), each
 compared against the oracle.
 
-No input reaches ba_schur_pipe<0, *>: wc < 9 needs a camera with fewer than 3 parameters, i.e. SPHERICAL (wc = 7),
-whose 3 residuals need nres * (wc + 4) = 33 > SP_ROWS = 26 staged rows, so such problems run ba_schur_mma<0>.  Scenes
-with FISHEYE624 or BROWN plus rig cameras (wc > 16) have no segment-eligible point at all and run the per-point
+The segment chunk list, and with it ba_schur_pipe, ba_linearize_fused and ba_colnorm_grad_chunks, exists for camera
+sides 9 wide with 2 residual rows only (whichever Schur kernel runs): wc < 9 needs a camera with fewer than 3
+parameters, i.e. SPHERICAL (wc = 7, 3 residuals), so such problems run ba_schur_mma<0> and ba_colnorm_grad_seg<0>.
+Scenes with FISHEYE624 or BROWN plus rig cameras (wc > 16) have no segment-eligible point at all and run the per-point
 ba_schur only."""
+import functools
 import json
 import os
 import subprocess
@@ -216,7 +218,8 @@ def test_reduced_system_matches_oracle(name):
 
 
 def test_iteration_two_uses_the_chunked_linearisation():
-    """Iteration 2 (after an accepted step) computes column norms and gradient with ba_colnorm_grad_chunks.  The oracle
+    """Iteration 2 (after an accepted step) computes column norms and gradient over the segment chunk list
+    (ba_linearize_fused: the scene is all perspective).  The oracle
     is linearised at the parameters the engine linearised at (captured with the system), so the comparison is as
     exact as at iteration 1."""
     pb = scenes.SCENES["pipe_many_chunks"]()
@@ -272,6 +275,13 @@ VARIANTS = {
 }
 
 
+@functools.lru_cache(maxsize=None)
+def _default_chunks(name):
+    pb = scenes.SCENES[name]()
+    pb.max_iterations = 1
+    return bundle.solve(pb, capture_iteration=1)["capture"]["sp_nchunks"]
+
+
 def _variant_main(out_path, variant):
     ms = [measure(s, variant) for s in sorted(scenes.SCENES)]
     with open(out_path, "w") as f:
@@ -292,4 +302,10 @@ def test_kernel_variant_matches_oracle(variant, tmp_path):
     for m in ms:
         for k, v in _variant_path(variant, m["name"]).items():
             assert m[k] == v, (variant, m["name"], k, m)
+        if variant in ("cta_per_segment_schur", "simt_segment_schur"):
+            # the Schur switches replace the Schur kernel only: the chunk list (so the linearisation) is the default's,
+            # and the 1e-12 checks of check() cover the chunk-list column norms under the switch
+            want = _default_chunks(m["name"])
+            assert (want > 0) == (m["wc"] == 9 and m["nres"] == 2 and m["nseg"] > 0), (m["name"], want, m)
+            assert m["sp_nchunks"] == want, (variant, m["name"], want, m)
         check(m)
