@@ -275,19 +275,22 @@ typedef struct {
   double initial_cost, final_cost;
   double time_run_s;          /* wall time of run() (ba_helpers.cc:749-753) */
   double time_device_ms;      /* CUDA-event time of the LM loop */
-  double time_linearize_ms;   /* summed CUDA-event time of the linearise+accumulate kernel */
+  /* phase times: summed device-clock (%globaltimer) spans of the linearise+accumulate kernel, the Schur-complement
+     kernels, the PCG solves and the back-substitution inside the LM loop */
+  double time_linearize_ms;
   int64_t linearize_launches;
-  double time_schur_ms;       /* summed CUDA-event time of the Schur-complement kernel */
+  double time_schur_ms;
   int64_t schur_launches;
-  double time_pcg_ms;         /* summed CUDA-event time of the PCG solves */
+  double time_pcg_ms;
   double time_backsub_ms;
   int64_t num_observations_local; /* observations held by this rank */
   int reduced_dim;            /* dimension of the reduced camera system */
   int reduced_blocks;         /* stored blocks of the block-sparse reduced system (both triangles) */
   int64_t reduced_nnz;        /* stored doubles of the reduced system */
   int jac_planes;             /* doubles stored per observation: nres * (wc + 3 + 1) */
-  int64_t kernel_launches;
+  int64_t kernel_launches;     /* kernels executed by run() (the device-driven loop's graph counted per execution) */
   char message[128];
+  int device_loop;             /* 1: the LM loop ran as one CUDA graph with device-side step control */
 } osfm_ba_summary;
 int osfm_ba_get_summary(osfm_ba* ba, osfm_ba_summary* out);
 

@@ -36,6 +36,7 @@ class BASummary(ctypes.Structure):
         ("time_schur_ms", c_double), ("schur_launches", c_int64), ("time_pcg_ms", c_double),
         ("time_backsub_ms", c_double), ("num_observations_local", c_int64), ("reduced_dim", c_int),
         ("reduced_blocks", c_int), ("reduced_nnz", c_int64), ("jac_planes", c_int), ("kernel_launches", c_int64), ("message", ctypes.c_char * 128),
+        ("device_loop", c_int),
     ]
 
 

@@ -72,6 +72,28 @@ struct Scalars {
   double gdot;           // gradient . step (projected line search of bounded problems)
 };
 
+// Levenberg-Marquardt state of run(), owned by the device: the step control kernels (ba_lm_*) read and write it, the
+// loop's other kernels and conditional nodes follow its branch word, the host reads it when the loop is done (and
+// after every decision when the host drives the loop).
+enum LmBranch { LM_EVAL = 1, LM_ACCEPT = 2, LM_PCG_CLASSIC = 4 };   // bits of LmState::branch
+enum LmMessage { LM_MSG_MAX_ITERATIONS, LM_MSG_NO_FREE, LM_MSG_GTOL, LM_MSG_MIN_RADIUS, LM_MSG_INVALID, LM_MSG_PTOL,
+                 LM_MSG_FTOL };
+enum LmPhase { LM_PH_LIN, LM_PH_SCHUR, LM_PH_PCG, LM_PH_BACK, LM_PH_COUNT };   // the summary's phase timers
+struct LmState {
+  double radius, decrease_factor, cost, initial_cost, x_norm;
+  int reuse_diagonal;
+  int it, n_invalid, n_success, n_solves, n_eval, n_classic, pcg_total;   // n_eval: valid steps, n_classic: PCG fallbacks
+  int termination, message;   // osfm_ba_summary::termination (1 while running), LmMessage
+  int running;                // ba_lm_next: another iteration follows
+  int branch;                 // LmBranch bits of the current iteration
+  int pcg_path;               // OSFM_PCG_* that solved the last system (when the pipelined PCG ran first)
+  unsigned long long phase_t0[LM_PH_COUNT], phase_ns[LM_PH_COUNT];   // %globaltimer stamps
+  int phase_count[LM_PH_COUNT];
+};
+// Ceres' defaults (trust_region_minimizer / levenberg_marquardt_strategy)
+constexpr double LM_RADIUS0 = 1e4, LM_MAX_RADIUS = 1e16, LM_MIN_RADIUS = 1e-32, LM_MIN_REL_DECREASE = 1e-3;
+constexpr double LM_FTOL = 1e-6, LM_GTOL = 1e-10, LM_PTOL = 1e-8;
+
 __device__ __forceinline__ double block_reduce_sum(double v) {
   __shared__ double sh[32];
   const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
@@ -459,10 +481,20 @@ __global__ void ba_make_scale(const double* colnorm2, double* scale, int n) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n) scale[i] = 1.0 / (1.0 + sqrt(colnorm2[i]));
 }
-// diag2 = clamp(colnorm2 * scale^2, 1e-6, 1e32) / radius ; also gradient max-norm
-__global__ void ba_make_diag(const double* colnorm2, const double* scale, double* diag, int n) {
+// diag = clamp(colnorm2 * scale^2, 1e-6, 1e32), kept when the LM state reuses the diagonal; with diag_r, also the
+// damping of this iteration diag_r = diag / radius
+__global__ void ba_make_diag(const double* colnorm2, const double* scale, double* diag, int n, const LmState* st = nullptr,
+                             double* diag_r = nullptr) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) diag[i] = fmin(fmax(colnorm2[i] * scale[i] * scale[i], 1e-6), 1e32);
+  if (i >= n) return;
+  double d;
+  if (st && st->reuse_diagonal) {
+    d = diag[i];
+  } else {
+    d = fmin(fmax(colnorm2[i] * scale[i] * scale[i], 1e-6), 1e32);
+    diag[i] = d;
+  }
+  if (diag_r) diag_r[i] = d * (1.0 / st->radius);
 }
 // Multi-GPU: everything rank-summed after a linearisation travels in ONE buffer
 //   pack = [ colnorm2 (nc) | grad (nc) | cost | per-rank max |point gradient| (world) ]
@@ -484,12 +516,19 @@ __global__ void ba_unpack_lin(const double* __restrict__ pack, int nc, int world
   for (int o = 16; o; o >>= 1) v = fmax(v, __shfl_xor_sync(0xffffffffu, v, o));
   if ((threadIdx.x & 31) == 0 && v > 0.0) atomic_max_nonneg(&sc->grad_max_bits, v);
 }
-__global__ void ba_grad_max(const double* grad, int n, Scalars* sc) {
+// one atomic per CTA: a C4 gradient has 600k entries, and per-warp atomics on one address serialise in L2
+__global__ void __launch_bounds__(256) ba_grad_max(const double* grad, int n, Scalars* sc) {
+  __shared__ double wmax[8];
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   double v = i < n ? fabs(grad[i]) : 0.0;
 #pragma unroll
   for (int o = 16; o; o >>= 1) v = fmax(v, __shfl_xor_sync(0xffffffffu, v, o));
-  if ((threadIdx.x & 31) == 0 && v > 0.0) atomic_max_nonneg(&sc->grad_max_bits, v);
+  if ((threadIdx.x & 31) == 0) wmax[threadIdx.x >> 5] = v;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    for (int w = 1; w < (int)(blockDim.x >> 5); ++w) v = fmax(v, wmax[w]);
+    if (v > 0.0) atomic_max_nonneg(&sc->grad_max_bits, v);
+  }
 }
 
 }  // namespace osfm
@@ -572,7 +611,7 @@ __global__ void __launch_bounds__(256) ba_backsub_points(BAView v, const double*
   y[nc + 3 * pf + 2] = c * t0 + e * t1 + f * t2;
 }
 
-// candidate = x - scale * y ; accumulates |delta|^2 and |x|^2 (free parameters only).
+// candidate = x - scale * y ; accumulates |delta|^2 and |candidate|^2 (free parameters only).
 // which: 0 cameras, 1 instances, 2 rig cameras, 3 points.
 __global__ void ba_update(int which, int count, const int* __restrict__ poff, const int* __restrict__ off,
                           const int* __restrict__ np, int stride, int base, const double* __restrict__ src,
@@ -591,9 +630,9 @@ __global__ void ba_update(int which, int count, const int* __restrict__ poff, co
         const int gi = which == 3 ? base + 3 * g + j : g + j;
         double d = -alpha * scale[gi] * y[gi];
         if (lower && val + d < lower[o + j]) d = lower[o + j] - val;   // projection onto the bound (ceres bounded LM)
-        xn += val * val;
         sn += d * d;
         val += d;
+        xn += val * val;
       }
       dst[o + j] = val;
     }
@@ -633,6 +672,117 @@ __global__ void ba_model_change_alg(int n, int nc, int cam_side, const double* _
   if (threadIdx.x == 0 && t != 0.0) atomicAdd(&sc->model_change, t);
 }
 
+// ---------------------------------------------------------------------------
+// Levenberg-Marquardt step control (one thread each).  Ceres' trust_region_minimizer with the
+// levenberg_marquardt_strategy: the same tests in the same order.  `cond`: when `set_cond`, the conditional node
+// handle of the device-driven loop's graph that the kernel's decision drives.
+// ---------------------------------------------------------------------------
+// after the first linearisation and the |x| pass (Scalars: cost, max |g|, |x|^2)
+__global__ void ba_lm_init(LmState* st, const Scalars* sc, int n) {
+  st->radius = LM_RADIUS0;
+  st->decrease_factor = 2.0;
+  st->cost = st->initial_cost = sc->cost;
+  st->x_norm = n > 0 ? sqrt(sc->x_norm2) : 0.0;
+  st->termination = 1;
+  st->message = LM_MSG_MAX_ITERATIONS;
+  if (n == 0) { st->termination = 0; st->message = LM_MSG_NO_FREE; }
+  else if (sc->grad_max_bits <= LM_GTOL) { st->termination = 0; st->message = LM_MSG_GTOL; }
+}
+// head of the loop: whether another iteration runs (the WHILE condition)
+__global__ void ba_lm_next(LmState* st, int max_iterations, cudaGraphConditionalHandle cond, int set_cond) {
+  int run = 0;
+  if (st->termination == 1 && st->it < max_iterations) {
+    if (st->radius < LM_MIN_RADIUS) { st->termination = 0; st->message = LM_MSG_MIN_RADIUS; }
+    else { ++st->it; run = 1; }
+  }
+  st->running = run;
+  st->branch = 0;
+  if (set_cond) cudaGraphSetConditional(cond, run);
+}
+// after the pipelined PCG: the classic PCG from scratch when its recurrences stagnated or broke down
+__global__ void ba_lm_pcg_check(LmState* st, const PcgState* pcg, int classic_path, cudaGraphConditionalHandle cond,
+                                int set_cond) {
+  const int fallback = pcg->converged ? 0 : 1;
+  if (fallback) {
+    st->pcg_total += pcg->iterations;
+    st->pcg_path = classic_path;
+    st->branch |= LM_PCG_CLASSIC;
+    ++st->n_classic;
+  } else {
+    st->pcg_path = pcg->deflated ? OSFM_PCG_PIPELINED_DEFLATED : OSFM_PCG_PIPELINED;
+  }
+  if (set_cond) cudaGraphSetConditional(cond, fallback);
+}
+// after the candidate update: an invalid step (solver NaN, no model decrease, non-finite step) halves the radius
+__global__ void ba_lm_check(LmState* st, const Scalars* sc, const PcgState* pcg, int nc, cudaGraphConditionalHandle cond,
+                            int set_cond) {
+  ++st->n_solves;
+  bool ok = true;
+  if (nc > 0) {
+    st->pcg_total += pcg->iterations;
+    if (!(pcg->rr_final == pcg->rr_final)) ok = false;
+  }
+  const double step_norm = sqrt(sc->step_norm2);
+  int eval = 0;
+  if (!ok || !(sc->model_change > 0.0) || !isfinite(step_norm)) {
+    if (++st->n_invalid >= 5) {
+      st->termination = 2;
+      st->message = LM_MSG_INVALID;
+    } else {
+      st->radius *= 0.5;
+      st->reuse_diagonal = 1;
+    }
+  } else {
+    st->n_invalid = 0;
+    ++st->n_eval;
+    st->branch |= LM_EVAL;
+    eval = 1;
+  }
+  if (set_cond) cudaGraphSetConditional(cond, eval);
+}
+// after the candidate cost (Scalars: candidate cost, |delta|^2, |candidate|^2): tolerances, then the ratio test
+__global__ void ba_lm_step(LmState* st, const Scalars* sc, cudaGraphConditionalHandle cond, int set_cond) {
+  int accept = 0;
+  if (st->branch & LM_EVAL) {
+    const double step_norm = sqrt(sc->step_norm2), cost_change = st->cost - sc->cost;
+    if (step_norm <= LM_PTOL * (st->x_norm + LM_PTOL)) {
+      st->termination = 0;
+      st->message = LM_MSG_PTOL;
+    } else if (fabs(cost_change) <= LM_FTOL * st->cost) {
+      st->termination = 0;
+      st->message = LM_MSG_FTOL;
+    } else {
+      const double rel = cost_change / sc->model_change;
+      if (rel > LM_MIN_REL_DECREASE) {
+        st->x_norm = sqrt(sc->x_norm2);
+        st->radius = fmin(LM_MAX_RADIUS, st->radius / fmax(1.0 / 3.0, 1.0 - pow(2.0 * rel - 1.0, 3.0)));
+        st->decrease_factor = 2.0;
+        st->reuse_diagonal = 0;
+        ++st->n_success;
+        st->branch |= LM_ACCEPT;
+        accept = 1;
+      } else {
+        st->radius /= st->decrease_factor;
+        st->decrease_factor *= 2.0;
+        st->reuse_diagonal = 1;
+      }
+    }
+  }
+  if (set_cond) cudaGraphSetConditional(cond, accept);
+}
+// after the relinearisation at an accepted step (Scalars: cost, max |g|)
+__global__ void ba_lm_accepted(LmState* st, const Scalars* sc) {
+  st->cost = sc->cost;
+  if (sc->grad_max_bits <= LM_GTOL) { st->termination = 0; st->message = LM_MSG_GTOL; }
+}
+// phase timers: ends phase `stop` and starts phase `start` (-1: none) at the device's nanosecond clock
+__global__ void ba_lm_phase(LmState* st, int stop, int start) {
+  unsigned long long t;
+  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+  if (stop >= 0) { st->phase_ns[stop] += t - st->phase_t0[stop]; ++st->phase_count[stop]; }
+  if (start >= 0) st->phase_t0[start] = t;
+}
+
 // single-observation device evaluation (test hook)
 __global__ void ba_eval_one(int type, const double* in, int use_rc, double* out, int* nres_out) {
   // in: cam[16] ri[6] rc[6] X[3] obs[2] isig[1]
@@ -651,25 +801,6 @@ __global__ void ba_eval_one(int type, const double* in, int use_rc, double* out,
 // ---------------------------------------------------------------------------
 // Host side
 // ---------------------------------------------------------------------------
-// CUDA-event stopwatch on the launching stream; collect() after a stream synchronize.
-struct EventTimer {
-  cudaEvent_t a = nullptr, b = nullptr;
-  double total_ms = 0.0;
-  long long count = 0;
-  bool pending = false;
-  void init() { OSFM_CUDA(cudaEventCreate(&a)); OSFM_CUDA(cudaEventCreate(&b)); }
-  void destroy() { if (a) cudaEventDestroy(a); if (b) cudaEventDestroy(b); a = b = nullptr; }
-  void start(cudaStream_t st) { collect(); OSFM_CUDA(cudaEventRecord(a, st)); }
-  void stop(cudaStream_t st) { OSFM_CUDA(cudaEventRecord(b, st)); pending = true; }
-  void collect() {
-    if (!pending) return;
-    OSFM_CUDA(cudaEventSynchronize(b));
-    float ms = 0.f;
-    OSFM_CUDA(cudaEventElapsedTime(&ms, a, b));
-    total_ms += ms; ++count; pending = false;
-  }
-};
-
 template <class T>
 static void upload(DevBuf<T>& d, const std::vector<T>& h, cudaStream_t st) {
   d.reserve(std::max<size_t>(h.size(), 1));
@@ -749,6 +880,7 @@ struct BaSwitches {
   bool pcg_resident = !env_starts_with("OSFM_BA_PCG_RESIDENT", '0');   // else the classic PCG streams S from memory
   bool pcg_pipelined = !env_starts_with("OSFM_BA_PCG_PIPELINED", '0');   // else the classic PCG only
   bool pcg_deflate = !env_starts_with("OSFM_BA_PCG_DEFLATE", '0');   // else the pipelined PCG without gauge deflation
+  bool host_loop = env_starts_with("OSFM_BA_HOST_LOOP", '1');   // the host drives the LM loop even where a graph could
 };
 static const BaSwitches& switches() {
   static const BaSwitches s;
@@ -777,8 +909,6 @@ struct RunState {
   int uniform_type = -1;          // the projection type of every camera when no shot uses a rig camera, else -1
   bool constrained = false;       // a free ext parameter with a finite lower bound (ceres: Problem::IsConstrained)
   bool have_pp = false, add_priors = false;
-  int cur = 0;                    // index of the accepted parameter set
-  int pcg_total = 0;
   // host tables (-1 = constant)
   std::vector<int> cam_off, cam_np, cam_poff, inst_poff, rc_poff, ext_off, ext_poff, blk_off, blk_sz;
   std::vector<int> cam_blk, inst_blk, rc_blk, ext_blk, side_jofs, side_rofs, grp_b1, grp_b2;
@@ -802,7 +932,14 @@ struct RunState {
   BAView v{}; PriorView pv{}; SideView sv{}; PointPriorView ppv{}; BlkMaps bm{}; BsrView bsr{}; PcgLayout lay{};
   double *d_rhs_p = nullptr, *d_S_p = nullptr;
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;   // around the LM loop
-  EventTimer tm_lin, tm_schur, tm_pcg, tm_back;
+  // Device-driven LM loop: the graph under capture (null: the host drives the loop and launches directly), the
+  // nodes the next captured work depends on, the conditional handles of the iteration body, and the kernels captured
+  // into each part of the body (unconditional part, PCG fallback, candidate cost, acceptance)
+  cudaGraph_t cap_graph = nullptr;
+  std::vector<cudaGraphNode_t> cap_deps;
+  cudaGraphConditionalHandle h_pcg = 0, h_eval = 0, h_accept = 0;
+  int64_t k_body = 0, k_pcg = 0, k_eval = 0, k_accept = 0;
+  bool device_loop = false;
 };
 
 struct BA {
@@ -912,6 +1049,9 @@ struct BA {
   DevBuf<double> d_pr_cam_prior, d_pr_cam_scale, d_pr_pos_prior, d_pr_pos_scale;
   DevBuf<Scalars> d_sc;
   PinnedBuf<Scalars> h_sc;
+  DevBuf<LmState> d_lm;
+  PinnedBuf<LmState> h_lm;
+  DevBuf<double> d_diag_r;                 // diag / radius of the current LM iteration
   DevBuf<int> d_pr_pos_kind, d_ext_off, d_ext_np, d_ext_poff, d_ext_blk, d_side_jofs, d_side_rofs;
   DevBuf<double> d_ext[2], d_ext_lower, d_side_consts, d_side_J, d_side_r, d_pp_d, d_pp_x0;
   DevBuf<SideTerm> d_side_terms;
@@ -924,6 +1064,8 @@ struct BA {
     OSFM_CUDA(cudaEventCreateWithFlags(&ev_obs, cudaEventDisableTiming));
     h_sc.reserve(1);
     h_pcg.reserve(1);
+    d_lm.reserve(1);
+    h_lm.reserve(1);
     OSFM_CUDA(cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, device));
   }
   ~BA() {
@@ -938,6 +1080,67 @@ struct BA {
     OSFM_CUDA(cudaMemcpyAsync(h_sc.p, d_sc.p, sizeof(Scalars), cudaMemcpyDeviceToHost, stream));
     OSFM_CUDA(cudaStreamSynchronize(stream));
     return *h_sc.p;
+  }
+  const LmState& read_lm() {
+    OSFM_CUDA(cudaMemcpyAsync(h_lm.p, d_lm.p, sizeof(LmState), cudaMemcpyDeviceToHost, stream));
+    OSFM_CUDA(cudaStreamSynchronize(stream));
+    return *h_lm.p;
+  }
+  // LM phase timer stamps (ba_lm_phase) around the work of the iteration
+  void lm_phase(int stop, int start) {
+    ba_lm_phase<<<1, 1, 0, stream>>>(d_lm.p, stop, start);
+    OSFM_LAUNCH_CHECK();
+  }
+  // Device-driven loop: stream work from here on is captured into g, after the nodes rs.cap_deps
+  void capture_begin(cudaGraph_t g) {
+    rs.cap_graph = g;
+    OSFM_CUDA(cudaStreamBeginCaptureToGraph(stream, g, rs.cap_deps.data(), nullptr, rs.cap_deps.size(),
+                                            cudaStreamCaptureModeRelaxed));
+  }
+  // ... up to here; the nodes the capture ended with become rs.cap_deps
+  void capture_end() {
+    cudaStreamCaptureStatus status;
+    const cudaGraphNode_t* deps = nullptr;
+    size_t ndeps = 0;
+    OSFM_CUDA(cudaStreamGetCaptureInfo(stream, &status, nullptr, nullptr, &deps, &ndeps));
+    rs.cap_deps.assign(deps, deps + ndeps);
+    cudaGraph_t g = nullptr;
+    OSFM_CUDA(cudaStreamEndCapture(stream, &g));
+  }
+  // A conditional node of `type` on `handle` after the captured work; returns its body graph, the node becomes the
+  // dependency of what follows
+  cudaGraph_t add_conditional(cudaGraph_t g, cudaGraphConditionalHandle handle, cudaGraphConditionalNodeType type) {
+    cudaGraphNodeParams p{};
+    p.type = cudaGraphNodeTypeConditional;
+    p.conditional.handle = handle;
+    p.conditional.type = type;
+    p.conditional.size = 1;
+    cudaGraphNode_t node;
+    OSFM_CUDA(cudaGraphAddNode(&node, g, rs.cap_deps.data(), rs.cap_deps.size(), &p));
+    rs.cap_deps.assign(1, node);
+    return p.conditional.phGraph_out[0];
+  }
+  // The work of `fn` when the LM state's branch word has `bit` set: read back by the host-driven loop; in the
+  // device-driven loop, the body of an IF node on `handle` (set by the kernel before it).  Returns the kernels `fn`
+  // launched.
+  template <class F>
+  int64_t lm_if(cudaGraphConditionalHandle handle, int bit, F fn) {
+    const int64_t k0 = g_kernel_launches.load();
+    if (!rs.cap_graph) {
+      if (read_lm().branch & bit) fn();
+      return 0;
+    }
+    cudaGraph_t outer = rs.cap_graph;
+    capture_end();
+    cudaGraph_t body = add_conditional(outer, handle, cudaGraphCondTypeIf);
+    std::vector<cudaGraphNode_t> after = rs.cap_deps;
+    rs.cap_deps.clear();
+    capture_begin(body);
+    fn();
+    capture_end();
+    rs.cap_deps = after;
+    capture_begin(outer);
+    return g_kernel_launches.load() - k0;
   }
   // OSFM_BA_TRACE: number of all-reduces and the host time spent issuing them (+ device time when traced)
   int ar_calls = 0;
@@ -1005,24 +1208,24 @@ struct BA {
     if (P) { ba_update<<<grid_for(P, 128), 128, 0, stream>>>(3, P, d_pt_poff.p, nullptr, nullptr, 3, rs.nc, a.pts, b.pts, d_scale.p, d_y.p, d_sc.p, 1, nullptr, alpha); OSFM_LAUNCH_CHECK(); }
     if (NE) { ba_update<<<grid_for(NE, 128), 128, 0, stream>>>(0, NE, d_ext_poff.p, d_ext_off.p, d_ext_np.p, 0, 0, a.ext, b.ext, d_scale.p, d_y.p, d_sc.p, rank == 0, lower, alpha); OSFM_LAUNCH_CHECK(); }
   }
-  // |x| of the free parameters of set b
-  double x_norm_of(int b) {
+  // |x|^2 of the free parameters of set b into Scalars::x_norm2
+  void x_norm_pass(int b) {
     OSFM_CUDA(cudaMemsetAsync(&d_sc.p->x_norm2, 0, sizeof(double), stream));
     OSFM_CUDA(cudaMemsetAsync(d_y.p, 0, sizeof(double) * rs.nz, stream));
     update_params(b, b, 1.0, nullptr);
     allreduce_dev(&d_sc.p->x_norm2, 1);
-    return std::sqrt(read_scalars().x_norm2);
   }
+  // Parameter set 0 holds the accepted parameters, set 1 the candidate
   Params params_of(int b) { return Params{d_cam[b].p, d_inst[b].p, d_rc[b].p, d_pts[b].p, d_ext[b].p}; }
   RunState rs;
 
   void run();
   void plan_layout(), order_observations(), plan_prior_rows(), upload_problem(), discover_structure(), plan_pcg(),
       reserve_covariance(), build_segment_tables(), segment_table_scales();
-  double eval_cost(int b), linearize(int b, bool timed, double* grad_max);
-  void build_system(double inv_radius, int* rank_flag, bool timed), back_substitute();
-  int solve_reduced();
-  void capture_linear_system(int it, double radius, int pcg_path), covariance_pass(int termination);
+  void eval_cost(int b), linearize(int b, bool timed);
+  void build_system(const double* diag, double inv_radius, int* rank_flag, bool timed), back_substitute();
+  void solve_reduced(), lm_iteration(), line_search(), accept_candidate(), run_lm_graph();
+  void capture_linear_system(int it, double radius), covariance_pass(int termination);
   void write_results(osfm_ba_summary sum);
 };
 
@@ -1325,8 +1528,9 @@ void BA::upload_problem() {
   const size_t Nz = (size_t)std::max<long long>(rs.N, 1);
   d_r.reserve(nres * Nz); d_Jc.reserve((size_t)nres * wc * Nz); d_Jp.reserve((size_t)nres * 3 * Nz);
   d_Vinv.reserve(6 * (size_t)std::max(npf, 1)); d_gp.reserve(3 * (size_t)std::max(npf, 1));
+  d_Vig.reserve(3 * (size_t)std::max(npf, 1)); d_bs_t.reserve(3 * (size_t)std::max(npf, 1));
   const size_t nz = rs.nz;
-  d_scale.reserve(nz); d_colnorm2.reserve(nz); d_grad.reserve(nz); d_diag.reserve(nz); d_y.reserve(nz);
+  d_scale.reserve(nz); d_colnorm2.reserve(nz); d_grad.reserve(nz); d_diag.reserve(nz); d_diag_r.reserve(nz); d_y.reserve(nz);
   d_px.reserve(std::max(nc, 1)); d_pr.reserve(std::max(nc, 1)); d_pz.reserve(std::max(nc, 1));
   d_pp.reserve(std::max(nc, 1)); d_pAp.reserve(std::max(nc, 1));
   d_pcg.reserve(1);
@@ -1649,6 +1853,10 @@ void BA::build_segment_tables() {
   rs.schur = nseg == 0 ? OSFM_SCHUR_NONE
              : !use_mma ? OSFM_SCHUR_SIMT_SEGMENT
              : use_pipe ? OSFM_SCHUR_PIPE : OSFM_SCHUR_MMA;
+  if (rs.schur == OSFM_SCHUR_SIMT_SEGMENT) {
+    const size_t rows = (size_t)rs.n_fast_obs * wc * 3 + 8;
+    d_rowsJ.reserve(rows); d_rowsW.reserve(rows); d_rowsY.reserve(rows);
+  }
   rs.lin = nseg == 0 ? LIN_NONE
            : rs.sp_nchunks == 0 ? LIN_SEGMENTS
            : rs.uniform_type == PT_PERSPECTIVE ? LIN_FUSED : LIN_CHUNKS;
@@ -1661,8 +1869,8 @@ void BA::segment_table_scales() {
   OSFM_LAUNCH_CHECK();
 }
 
-// cost at parameter set b (sum over ranks)
-double BA::eval_cost(int b) {
+// cost at parameter set b (sum over ranks) into Scalars::cost
+void BA::eval_cost(int b) {
   OSFM_CUDA(cudaMemsetAsync(&d_sc.p->cost, 0, sizeof(double), stream));
   if (rs.N > 0) launch_linearize<0>(b);
   const int npr_local = rs.pv.n_cam_rows + rs.pv.n_pos_rows;
@@ -1679,12 +1887,12 @@ double BA::eval_cost(int b) {
     OSFM_LAUNCH_CHECK();
   }
   allreduce_dev(&d_sc.p->cost, 1);
-  return read_scalars().cost;
 }
 
 
-// residual + Jacobian planes, column norms, gradient at parameter set b; returns the cost.  `timed`: into tm_lin.
-double BA::linearize(int b, bool timed, double* grad_max) {
+// residual + Jacobian planes, column norms, gradient at parameter set b; the cost and max |g| into Scalars.  `timed`:
+// into the linearisation phase timer.
+void BA::linearize(int b, bool timed) {
   const long long N = rs.N, n_fast_obs = rs.n_fast_obs;
   const int nc = rs.nc, n = rs.n, nseg = rs.nseg, wc = rs.wc, NT = rs.NT;
   OSFM_CUDA(cudaMemsetAsync(d_sc.p, 0, sizeof(Scalars), stream));
@@ -1695,11 +1903,11 @@ double BA::linearize(int b, bool timed, double* grad_max) {
     // outside the segments get their sums from the plane-reading kernels
     d_ptsum.reserve(9 * (size_t)std::max(rs.npf, 1));
     const int grid = (int)((n_fast_obs + FL_WIN - 1) / FL_WIN + (N - n_fast_obs + FL_THREADS - 1) / FL_THREADS);
-    if (timed) rs.tm_lin.start(stream);
+    if (timed) lm_phase(-1, LM_PH_LIN);
     ba_linearize_fused<PT_PERSPECTIVE><<<grid, FL_THREADS, 0, stream>>>(rs.v, params_of(b), d_sc.p, d_sp_chunks.p, rs.sp_nchunks,
                                                                         n_fast_obs, d_tab.p, d_colnorm2.p, d_grad.p, d_ptsum.p);
     OSFM_LAUNCH_CHECK();
-    if (timed) rs.tm_lin.stop(stream);
+    if (timed) lm_phase(LM_PH_LIN, -1);
     if (N > n_fast_obs) {
       ba_colnorm_grad_points<<<grid_for(N - n_fast_obs, 256), 256, 0, stream>>>(rs.v, n_fast_obs, d_colnorm2.p, d_grad.p);
       OSFM_LAUNCH_CHECK();
@@ -1707,9 +1915,9 @@ double BA::linearize(int b, bool timed, double* grad_max) {
       OSFM_LAUNCH_CHECK();
     }
   } else if (N > 0) {
-    if (timed) rs.tm_lin.start(stream);
+    if (timed) lm_phase(-1, LM_PH_LIN);
     launch_linearize<1>(b);
-    if (timed) rs.tm_lin.stop(stream);
+    if (timed) lm_phase(LM_PH_LIN, -1);
     ba_colnorm_grad_points<<<grid_for(N, 256), 256, 0, stream>>>(rs.v, 0, d_colnorm2.p, d_grad.p);
     OSFM_LAUNCH_CHECK();
     if (rs.lin == LIN_CHUNKS) {   // no dependent index loads
@@ -1765,15 +1973,13 @@ double BA::linearize(int b, bool timed, double* grad_max) {
     ba_grad_max<<<grid_for(n, 256), 256, 0, stream>>>(d_grad.p, n, d_sc.p);
     OSFM_LAUNCH_CHECK();
   }
-  const Scalars s = read_scalars();
-  *grad_max = s.grad_max_bits;
-  return s.cost;
 }
 
 // Reduced camera system at the accepted parameters (upper blocks accumulated with L2 atomics, all-reduced, priors
-// and side terms added, mirrored), damped with diag * inv_radius.  The LM iteration and the covariance pass
-// (inv_radius = 0, rank_flag set: ba_cov.cuh) both build it here, through the same kernel path.  `timed`: into tm_schur.
-void BA::build_system(double inv_radius, int* rank_flag, bool timed) {
+// and side terms added, mirrored), damped with diag * inv_radius.  The LM iteration (diag / radius of its state, 1)
+// and the covariance pass (inv_radius = 0, rank_flag set: ba_cov.cuh) both build it here, through the same kernel
+// path.  `timed`: into the Schur phase timer.
+void BA::build_system(const double* diag, double inv_radius, int* rank_flag, bool timed) {
   const int nc = rs.nc, P = rs.P, P_fast = rs.P_fast, nseg = rs.nseg, wc = rs.wc;
   const bool trace_on = switches().trace;
   double *const d_rhs_p = rs.d_rhs_p, *const d_S_p = rs.d_S_p;
@@ -1781,14 +1987,13 @@ void BA::build_system(double inv_radius, int* rank_flag, bool timed) {
   if (P > 0) {
     const size_t smem = (size_t)SCHUR_KC * wc * (2 * 3 * sizeof(double) + 2 * sizeof(int)) +
                         (size_t)SCHUR_KC * 8 * sizeof(int) + (size_t)SCHUR_KC * SCHUR_KC * 9 * sizeof(int);
-    if (timed) rs.tm_schur.start(stream);
+    if (timed) lm_phase(-1, LM_PH_SCHUR);
     if (rs.schur != OSFM_SCHUR_NONE) {
-      d_Vig.reserve(3 * (size_t)std::max(rs.npf, 1));
       if (rs.lin == LIN_FUSED)   // the point sums of the linearisation
         ba_point_blocks_sums<<<grid_for(P_fast, PB_THREADS), PB_THREADS, 0, stream>>>(
-            rs.v, P_fast, d_ptsum.p, d_scale.p, d_diag.p, inv_radius, d_Vinv.p, d_gp.p, d_Vig.p, rank_flag);
+            rs.v, P_fast, d_ptsum.p, d_scale.p, diag, inv_radius, d_Vinv.p, d_gp.p, d_Vig.p, rank_flag);
       else
-        ba_point_blocks<<<grid_for(P_fast, PB_THREADS), PB_THREADS, 0, stream>>>(rs.v, P_fast, d_scale.p, d_diag.p, inv_radius,
+        ba_point_blocks<<<grid_for(P_fast, PB_THREADS), PB_THREADS, 0, stream>>>(rs.v, P_fast, d_scale.p, diag, inv_radius,
                                                                                d_Vinv.p, d_gp.p, d_Vig.p, rank_flag);
       OSFM_LAUNCH_CHECK();
     }
@@ -1835,8 +2040,6 @@ void BA::build_system(double inv_radius, int* rank_flag, bool timed) {
       }
     } else if (rs.schur == OSFM_SCHUR_SIMT_SEGMENT) {
       const long long n_fast = rs.n_fast_obs;
-      d_rowsJ.reserve((size_t)n_fast * wc * 3 + 8); d_rowsW.reserve((size_t)n_fast * wc * 3 + 8);
-      d_rowsY.reserve((size_t)n_fast * wc * 3 + 8);
       ba_obs_rows<<<grid_for(n_fast * wc, 256), 256, 0, stream>>>(rs.v, rs.bm, rs.bsr, n_fast, d_scale.p, d_Vinv.p, d_Vig.p,
                                                                 d_rowsJ.p, d_rowsW.p, d_rowsY.p, d_rhs_p);
       OSFM_LAUNCH_CHECK();
@@ -1847,11 +2050,11 @@ void BA::build_system(double inv_radius, int* rank_flag, bool timed) {
       OSFM_LAUNCH_CHECK();
     }
     if (P > P_fast) {
-      ba_schur<<<P - P_fast, SCHUR_THREADS, smem, stream>>>(rs.v, rs.bm, rs.bsr, d_scale.p, d_diag.p, inv_radius, d_S_p,
-                                                           d_rhs_p, d_Vinv.p, d_gp.p, P_fast, rs.ppv, d_pts[rs.cur].p, rank_flag);
+      ba_schur<<<P - P_fast, SCHUR_THREADS, smem, stream>>>(rs.v, rs.bm, rs.bsr, d_scale.p, diag, inv_radius, d_S_p,
+                                                           d_rhs_p, d_Vinv.p, d_gp.p, P_fast, rs.ppv, d_pts[0].p, rank_flag);
       OSFM_LAUNCH_CHECK();
     }
-    if (timed) rs.tm_schur.stop(stream);
+    if (timed) lm_phase(LM_PH_SCHUR, -1);
   }
   if (nc > 0) {
     // the one exchange step of the LM iteration: sum of the partial reduced systems over ranks
@@ -1863,97 +2066,106 @@ void BA::build_system(double inv_radius, int* rank_flag, bool timed) {
     pall.n_pos_rows = (int)rs.pr_pos_inst.size();
     const int nall = pall.n_cam_rows + pall.n_pos_rows;
     if (nall > 0) {
-      ba_prior_system<<<grid_for(nall, 128), 128, 0, stream>>>(pall, params_of(rs.cur), d_scale.p, d_prior_diag_off.p,
+      ba_prior_system<<<grid_for(nall, 128), 128, 0, stream>>>(pall, params_of(0), d_scale.p, d_prior_diag_off.p,
                                                               d_S_p, d_rhs_p);
       OSFM_LAUNCH_CHECK();
     }
     if (rs.NT > 0) {
-      side_system<<<rs.NT, SIDE_THREADS, 0, stream>>>(rs.sv, rs.v, rs.bm, params_of(rs.cur), rs.bsr, d_scale.p, d_S_p, d_rhs_p);
+      side_system<<<rs.NT, SIDE_THREADS, 0, stream>>>(rs.sv, rs.v, rs.bm, params_of(0), rs.bsr, d_scale.p, d_S_p, d_rhs_p);
       OSFM_LAUNCH_CHECK();
     }
     ba_finish_system<<<grid_for((long long)rs.n_upper * 32, 256), 256, 0, stream>>>(d_upper.p, rs.n_upper, rs.bsr, d_S_p,
-                                                                                  d_diag.p, inv_radius);
+                                                                                  diag, inv_radius);
     OSFM_LAUNCH_CHECK();
   }
 }
 
 // PCG on the damped reduced system, |r| <= 1e-8 |b|, into y: the pipelined kernel, and the classic one from scratch
-// when its recurrences stagnate or break down.  Returns the OSFM_PCG_* path that produced y.
-int BA::solve_reduced() {
+// when its recurrences stagnate or break down (ba_lm_pcg_check decides on the device).
+void BA::solve_reduced() {
   const int nc = rs.nc;
-  rs.tm_pcg.start(stream);
+  lm_phase(-1, LM_PH_PCG);
   pcg_convert<<<grid_for((long long)rs.n_blocks_all * 32, 256), 256, 0, stream>>>(
       rs.d_S_p, d_row_col.p, d_row_off.p, d_qoff.p, d_blk_row.p, rs.n_blocks_all, rs.bsr, d_row_M.p, d_rowbase.p, d_Spcg.p);
   OSFM_LAUNCH_CHECK();
-  pcg_factor_groups<<<grid_for(rs.ngroups, 64), 64, 0, stream>>>(rs.d_S_p, rs.bsr, d_diag_off.p, d_grp_b1.p, d_grp_b2.p,
+  pcg_factor_groups<<<grid_for((long long)rs.ngroups * 32, 32 * PFG_WARPS), 32 * PFG_WARPS, 0, stream>>>(rs.d_S_p, rs.bsr, d_diag_off.p, d_grp_b1.p, d_grp_b2.p,
                                                                 rs.ngroups, d_Minv.p);
   OSFM_LAUNCH_CHECK();
   OSFM_CUDA(cudaMemsetAsync(d_pcg.p, 0, sizeof(PcgState), stream));
   const int max_pcg = std::min(2 * nc + 100, 5000);
-  int path = 0;
-  if (rs.pcg_pipe_ok) {
-    launch_cooperative(pcg_pipelined, rs.pcg_grid, PCG_THREADS, rs.pcg_pipe_smem, stream, d_Spcg.p, rs.lay, rs.bsr, d_Minv.p,
-                       rs.d_rhs_p, d_px.p, d_pz.p, d_pp.p, d_pcg.p, nc, max_pcg, 1e-16, rs.pcg_pipe);
-    OSFM_LAUNCH_CHECK();
-    OSFM_CUDA(cudaMemcpyAsync(h_pcg.p, d_pcg.p, PCG_STATE_HEADER, cudaMemcpyDeviceToHost, stream));
-    OSFM_CUDA(cudaStreamSynchronize(stream));
-    const PcgState& h = *h_pcg.p;
-    const int its = std::max(h.iterations, 1);
-    if (switches().trace)
-      fprintf(stderr, "[osfm_ba] pipelined pcg %d its converged %d, CTA0 clocks/it: stage %lld matvec %lld reduce %lld update %lld"
-              " | wide barrier (all calls / its): own sums %lld release %lld collect %lld column sums %lld\n",
-              h.iterations, h.converged, h.prof[0] / its, h.prof[1] / its, h.prof[2] / its, h.prof[3] / its, h.prof[4] / its,
-              h.prof[5] / its, h.prof[6] / its, h.prof[7] / its);
-    if (h.converged) {
-      path = h.deflated ? OSFM_PCG_PIPELINED_DEFLATED : OSFM_PCG_PIPELINED;
-    } else {  // stagnation / breakdown of the pipelined recurrences: classic PCG from scratch
-      rs.pcg_total += h.iterations;
-      OSFM_CUDA(cudaMemsetAsync(d_pcg.p, 0, sizeof(PcgState), stream));
-    }
-  }
-  if (!path) {
-    path = rs.pcg_resident ? OSFM_PCG_CLASSIC_RESIDENT : OSFM_PCG_CLASSIC_STREAMED;
+  const int classic_path = rs.pcg_resident ? OSFM_PCG_CLASSIC_RESIDENT : OSFM_PCG_CLASSIC_STREAMED;
+  auto classic = [&]() {
     launch_cooperative(rs.pcg_resident ? pcg_persistent<true> : pcg_persistent<false>, rs.pcg_grid, PCG_THREADS, rs.pcg_smem,
                        stream, d_Spcg.p, rs.lay, rs.bsr, d_Minv.p, rs.d_rhs_p, d_px.p, d_pr.p, d_pz.p, d_pp.p, d_pAp.p, d_Ap.p,
                        d_pcg.p, nc, max_pcg, 1e-16, rs.pcg_res);
     OSFM_LAUNCH_CHECK();
+    if (switches().trace) {
+      OSFM_CUDA(cudaMemcpyAsync(h_pcg.p, d_pcg.p, PCG_STATE_HEADER, cudaMemcpyDeviceToHost, stream));
+      OSFM_CUDA(cudaStreamSynchronize(stream));
+      const PcgState& h = *h_pcg.p;
+      const int its = std::max(h.iterations, 1);
+      fprintf(stderr, "[osfm_ba] pcg %d its, CTA0 clocks/it: stage %lld matvec %lld reduce1 %lld phaseB %lld reduce2 %lld (resident %d)\n",
+              h.iterations, h.prof[0] / its, h.prof[1] / its, h.prof[2] / its, h.prof[3] / its, h.prof[4] / its, (int)rs.pcg_resident);
+    }
+  };
+  if (rs.pcg_pipe_ok) {
+    launch_cooperative(pcg_pipelined, rs.pcg_grid, PCG_THREADS, rs.pcg_pipe_smem, stream, d_Spcg.p, rs.lay, rs.bsr, d_Minv.p,
+                       rs.d_rhs_p, d_px.p, d_pz.p, d_pp.p, d_pcg.p, nc, max_pcg, 1e-16, rs.pcg_pipe);
+    OSFM_LAUNCH_CHECK();
+    if (switches().trace) {
+      OSFM_CUDA(cudaMemcpyAsync(h_pcg.p, d_pcg.p, PCG_STATE_HEADER, cudaMemcpyDeviceToHost, stream));
+      OSFM_CUDA(cudaStreamSynchronize(stream));
+      const PcgState& h = *h_pcg.p;
+      const int its = std::max(h.iterations, 1);
+      fprintf(stderr, "[osfm_ba] pipelined pcg %d its converged %d, CTA0 clocks/it: stage %lld matvec %lld reduce %lld update %lld"
+              " | wide barrier (all calls / its): own sums %lld release %lld collect %lld column sums %lld\n",
+              h.iterations, h.converged, h.prof[0] / its, h.prof[1] / its, h.prof[2] / its, h.prof[3] / its, h.prof[4] / its,
+              h.prof[5] / its, h.prof[6] / its, h.prof[7] / its);
+    }
+    ba_lm_pcg_check<<<1, 1, 0, stream>>>(d_lm.p, d_pcg.p, classic_path, rs.h_pcg, rs.cap_graph != nullptr);
+    OSFM_LAUNCH_CHECK();
+    rs.k_pcg = lm_if(rs.h_pcg, LM_PCG_CLASSIC, [&]() {
+      OSFM_CUDA(cudaMemsetAsync(d_pcg.p, 0, sizeof(PcgState), stream));
+      classic();
+    });
+  } else {
+    classic();
   }
   OSFM_CUDA(cudaMemcpyAsync(d_y.p, d_px.p, sizeof(double) * nc, cudaMemcpyDeviceToDevice, stream));
-  OSFM_CUDA(cudaMemcpyAsync(h_pcg.p, d_pcg.p, PCG_STATE_HEADER, cudaMemcpyDeviceToHost, stream));
-  rs.tm_pcg.stop(stream);
-  return path;
+  lm_phase(LM_PH_PCG, -1);
 }
 
 // back-substitution: the point part of y from its camera part
 void BA::back_substitute() {
   const int P = rs.P, npf = rs.npf;
   if (P == 0 || npf == 0) return;
-  rs.tm_back.start(stream);
-  d_bs_t.reserve(3 * (size_t)npf);
+  lm_phase(-1, LM_PH_BACK);
   OSFM_CUDA(cudaMemsetAsync(d_bs_t.p, 0, sizeof(double) * 3 * (size_t)npf, stream));
   if (rs.N > 0) {
     ba_backsub_rows<<<grid_for(rs.N, 256), 256, 0, stream>>>(rs.v, d_scale.p, d_y.p, d_bs_t.p);
     OSFM_LAUNCH_CHECK();
   }
   if (rs.have_pp) {
-    ba_point_prior<3><<<grid_for(P, 128), 128, 0, stream>>>(rs.ppv, rs.v, params_of(rs.cur), nullptr, nullptr, d_bs_t.p, d_sc.p);
+    ba_point_prior<3><<<grid_for(P, 128), 128, 0, stream>>>(rs.ppv, rs.v, params_of(0), nullptr, nullptr, d_bs_t.p, d_sc.p);
     OSFM_LAUNCH_CHECK();
   }
   ba_backsub_points<<<grid_for(npf, 256), 256, 0, stream>>>(rs.v, d_scale.p, d_Vinv.p, d_bs_t.p, d_y.p);
   OSFM_LAUNCH_CHECK();
-  rs.tm_back.stop(stream);
+  lm_phase(LM_PH_BACK, -1);
 }
 
 // osfm_ba_capture_linear_system: raw copies of the system the PCG solved, the dense expansion is host code in
 // osfm_ba_get_captured_system
-void BA::capture_linear_system(int it, double radius, int pcg_path) {
+void BA::capture_linear_system(int it, double radius) {
   const int nc = rs.nc, n = rs.n, P = rs.P;
+  const int pcg_path = rs.pcg_pipe_ok ? read_lm().pcg_path : rs.pcg_resident ? OSFM_PCG_CLASSIC_RESIDENT : OSFM_PCG_CLASSIC_STREAMED;
+  OSFM_CUDA(cudaMemcpyAsync(h_pcg.p, d_pcg.p, PCG_STATE_HEADER, cudaMemcpyDeviceToHost, stream));
   download(cap_sbuf, d_Sbuf.p, (size_t)rs.nc_pad + (size_t)rs.s_total, stream);
   download(cap_upper, d_upper.p, rs.n_upper, stream);
   download(cap_y, d_px.p, nc, stream);
   download(cap_scale, d_scale.p, n, stream); download(cap_diag, d_diag.p, n, stream); download(cap_grad, d_grad.p, n, stream);
   download(cap_pt_poff, d_pt_poff.p, P, stream); download(cap_global_of, d_global_of.p, P, stream);
-  const Params xp = params_of(rs.cur);
+  const Params xp = params_of(0);
   download(cap_cam, xp.cam, cam_params.size(), stream); download(cap_inst, xp.inst, inst.size(), stream);
   download(cap_rc, xp.rc, rc.size(), stream); download(cap_pts, xp.pts, 3 * (size_t)P, stream);
   download(cap_ext, xp.ext, ext_values.size(), stream);
@@ -2012,8 +2224,7 @@ void BA::covariance_pass(int termination) {
     for (auto& e : ce) OSFM_CUDA(cudaEventCreate(&e));
     OSFM_CUDA(cudaEventRecord(ce[0], stream));
     // re-linearise at the accepted parameters with the Jacobi scale of this point (the LM keeps the first one)
-    double gm = 0.0;
-    linearize(rs.cur, false, &gm);
+    linearize(0, false);
     if (n > 0) {
       ba_make_scale<<<grid_for(n, 256), 256, 0, stream>>>(d_colnorm2.p, d_scale.p, n);
       OSFM_LAUNCH_CHECK();
@@ -2022,7 +2233,7 @@ void BA::covariance_pass(int termination) {
       OSFM_LAUNCH_CHECK();
     }
     segment_table_scales();   // the tensor-core Schur kernels read the scale from their segment tables
-    build_system(0.0, flags + COV_F_POINT_RANK, false);
+    build_system(d_diag.p, 0.0, flags + COV_F_POINT_RANK, false);
     OSFM_CUDA(cudaEventRecord(ce[1], stream));
     auto tiles = [](int k) { return (k + COV_NB - 1) / COV_NB; };
     CovGemm g{A, nc, X, m, n1, nullptr, 0, 0, flags};
@@ -2094,7 +2305,7 @@ void BA::covariance_pass(int termination) {
 // Accepted parameters, points and reprojection errors back to the caller; the summary of the run (`sum` holds the
 // LM loop's counts and costs)
 void BA::write_results(osfm_ba_summary sum) {
-  const int cur = rs.cur, P = rs.P, Pfull = rs.Pfull;
+  const int cur = 0, P = rs.P, Pfull = rs.Pfull;
   const long long Nfull = rs.Nfull;
   download(cam_params, d_cam[cur].p, cam_params.size(), stream); download(inst, d_inst[cur].p, inst.size(), stream);
   download(rc, d_rc[cur].p, rc.size(), stream); download(ext_values, d_ext[cur].p, ext_values.size(), stream);
@@ -2126,24 +2337,138 @@ void BA::write_results(osfm_ba_summary sum) {
   float dev_ms = 0.f;
   OSFM_CUDA(cudaEventElapsedTime(&dev_ms, rs.ev0, rs.ev1));
   cudaEventDestroy(rs.ev0); cudaEventDestroy(rs.ev1);
-  rs.tm_lin.collect(); rs.tm_schur.collect(); rs.tm_pcg.collect(); rs.tm_back.collect();
+  const LmState& lm = read_lm();
   sum.time_device_ms = dev_ms;
-  sum.time_linearize_ms = rs.tm_lin.total_ms;
-  sum.linearize_launches = rs.tm_lin.count;
-  sum.time_schur_ms = rs.tm_schur.total_ms;
-  sum.schur_launches = rs.tm_schur.count;
-  sum.time_pcg_ms = rs.tm_pcg.total_ms;
-  sum.time_backsub_ms = rs.tm_back.total_ms;
+  sum.time_linearize_ms = lm.phase_ns[LM_PH_LIN] * 1e-6;
+  sum.linearize_launches = lm.phase_count[LM_PH_LIN];
+  sum.time_schur_ms = lm.phase_ns[LM_PH_SCHUR] * 1e-6;
+  sum.schur_launches = lm.phase_count[LM_PH_SCHUR];
+  sum.time_pcg_ms = lm.phase_ns[LM_PH_PCG] * 1e-6;
+  sum.time_backsub_ms = lm.phase_ns[LM_PH_BACK] * 1e-6;
   sum.num_observations_local = rs.N;
   sum.reduced_dim = rs.nc;
   sum.reduced_blocks = rs.n_blocks_all;
   sum.reduced_nnz = rs.s_total;
   sum.jac_planes = rs.nres * (rs.wc + 3 + 1);
-  rs.tm_lin.destroy(); rs.tm_schur.destroy(); rs.tm_pcg.destroy(); rs.tm_back.destroy();
+  // kernels executed: the device-driven loop's graph ran the kernels captured into its body once per iteration and
+  // those of its conditional bodies once per time taken
   sum.kernel_launches = g_kernel_launches.load() - rs.launches0;
+  if (rs.device_loop)
+    sum.kernel_launches += (int64_t)(lm.it - 1) * rs.k_body + (int64_t)(lm.n_classic - 1) * rs.k_pcg +
+                           (int64_t)(lm.n_eval - 1) * rs.k_eval + (int64_t)(lm.n_success - 1) * rs.k_accept;
+  sum.device_loop = rs.device_loop ? 1 : 0;
   sum.time_run_s = std::chrono::duration<double>(std::chrono::high_resolution_clock::now() - rs.t_start).count();
   summary = sum;
   has_run = true;
+}
+
+// One LM iteration after ba_lm_next started it: the damped reduced system, its solve, the candidate and its model
+// cost change, the candidate cost, and at an accepted step the relinearisation.  Only enqueues work: the host-driven
+// loop reads the LM state at each decision, the device-driven loop captures this once into its graph.
+void BA::lm_iteration() {
+  const int n = rs.n, nc = rs.nc;
+  const int graph = rs.cap_graph != nullptr;
+  ba_make_diag<<<grid_for(n, 256), 256, 0, stream>>>(d_colnorm2.p, d_scale.p, d_diag.p, n, d_lm.p, d_diag_r.p);
+  OSFM_LAUNCH_CHECK();
+  build_system(d_diag_r.p, 1.0, nullptr, true);
+  OSFM_CUDA(cudaMemsetAsync(d_y.p, 0, sizeof(double) * rs.nz, stream));
+  if (nc > 0) {
+    solve_reduced();
+    if (cap_iter > 0 && read_lm().it == cap_iter) capture_linear_system(cap_iter, h_lm.p->radius);
+  }
+  back_substitute();
+  OSFM_CUDA(cudaMemsetAsync(&d_sc.p->model_change, 0, sizeof(double) * 3, stream));  // model_change, step_norm2, x_norm2
+  if (n > 0) {
+    ba_model_change_alg<<<grid_for(n, 256), 256, 0, stream>>>(n, nc, rank == 0, d_grad.p, d_scale.p, d_diag_r.p, 1.0, d_y.p, d_sc.p);
+    OSFM_LAUNCH_CHECK();
+  }
+  update_params(0, 1, 1.0, d_ext_lower.p);
+  if (world > 1) allreduce_dev(&d_sc.p->model_change, 3);
+  ba_lm_check<<<1, 1, 0, stream>>>(d_lm.p, d_sc.p, d_pcg.p, nc, rs.h_eval, graph);
+  OSFM_LAUNCH_CHECK();
+  rs.k_eval = lm_if(rs.h_eval, LM_EVAL, [&]() {
+    eval_cost(1);
+    if (rs.constrained) line_search();
+  });
+  ba_lm_step<<<1, 1, 0, stream>>>(d_lm.p, d_sc.p, rs.h_accept, graph);
+  OSFM_LAUNCH_CHECK();
+  rs.k_accept = lm_if(rs.h_accept, LM_ACCEPT, [&]() { accept_candidate(); });
+}
+
+// Ceres: a problem with parameter bounds is "constrained": TrustRegionMinimizer::DoLineSearch runs a projected Armijo
+// search along the step (sufficient decrease 1e-4, at most 20 contractions; bisection here, Ceres' default
+// interpolates a cubic) and the candidate is the point it accepts.  The model cost change stays that of the full
+// step, as in Ceres.  Host code (host-driven loop): leaves the accepted candidate, its cost and norms in Scalars.
+void BA::line_search() {
+  const int n = rs.n, nc = rs.nc;
+  const double cost = read_lm().cost;
+  double cand_cost = read_scalars().cost;
+  auto step_to = [&](double alpha) {   // candidate = Project(x - alpha * scale * y) and its cost
+    OSFM_CUDA(cudaMemsetAsync(&d_sc.p->step_norm2, 0, sizeof(double) * 2, stream));
+    update_params(0, 1, alpha, d_ext_lower.p);
+    if (world > 1) allreduce_dev(&d_sc.p->step_norm2, 2);
+    eval_cost(1);
+  };
+  OSFM_CUDA(cudaMemsetAsync(&d_sc.p->gdot, 0, sizeof(double), stream));
+  ba_grad_dot<<<grid_for(n, 256), 256, 0, stream>>>(n, nc, rank == 0, d_grad.p, d_scale.p, d_y.p, d_sc.p);
+  OSFM_LAUNCH_CHECK();
+  if (world > 1) allreduce_dev(&d_sc.p->gdot, 1);
+  const double g0 = read_scalars().gdot;
+  double alpha = 1.0;
+  for (int ls = 0; ls < 20; ++ls) {
+    if (ls > 0) { step_to(alpha); cand_cost = read_scalars().cost; }
+    if (std::isfinite(cand_cost) && cand_cost <= cost + 1e-4 * g0 * alpha) return;
+    alpha *= 0.5;
+  }
+  step_to(1.0);
+}
+
+// The candidate (parameter set 1) becomes the accepted set 0, relinearised there
+void BA::accept_candidate() {
+  const Params a = params_of(0), c = params_of(1);
+  auto copy = [&](double* dst, const double* src, size_t count) {
+    if (count) OSFM_CUDA(cudaMemcpyAsync(dst, src, sizeof(double) * count, cudaMemcpyDeviceToDevice, stream));
+  };
+  copy(a.cam, c.cam, cam_params.size());
+  copy(a.inst, c.inst, inst.size());
+  copy(a.rc, c.rc, rc.size());
+  copy(a.pts, c.pts, 3 * (size_t)rs.P);
+  copy(a.ext, c.ext, ext_values.size());
+  linearize(0, true);
+  ba_lm_accepted<<<1, 1, 0, stream>>>(d_lm.p, d_sc.p);
+  OSFM_LAUNCH_CHECK();
+}
+
+// The device-driven loop: ba_lm_next, then WHILE (running) { lm_iteration(); ba_lm_next }, captured into one graph
+// and launched once.  The counts of kernels captured into each part turn the graph's run into kernels executed.
+void BA::run_lm_graph() {
+  cudaGraph_t g = nullptr;
+  OSFM_CUDA(cudaGraphCreate(&g, 0));
+  cudaGraphConditionalHandle h_while;
+  OSFM_CUDA(cudaGraphConditionalHandleCreate(&h_while, g, 0, 0));
+  rs.cap_deps.clear();
+  capture_begin(g);
+  ba_lm_next<<<1, 1, 0, stream>>>(d_lm.p, max_iterations, h_while, 1);
+  OSFM_LAUNCH_CHECK();
+  capture_end();
+  cudaGraph_t body = add_conditional(g, h_while, cudaGraphCondTypeWhile);
+  OSFM_CUDA(cudaGraphConditionalHandleCreate(&rs.h_pcg, body, 0, 0));
+  OSFM_CUDA(cudaGraphConditionalHandleCreate(&rs.h_eval, body, 0, 0));
+  OSFM_CUDA(cudaGraphConditionalHandleCreate(&rs.h_accept, body, 0, 0));
+  rs.cap_deps.clear();
+  const int64_t k0 = g_kernel_launches.load();
+  capture_begin(body);
+  lm_iteration();
+  ba_lm_next<<<1, 1, 0, stream>>>(d_lm.p, max_iterations, h_while, 1);
+  OSFM_LAUNCH_CHECK();
+  capture_end();
+  rs.cap_graph = nullptr;
+  rs.k_body = g_kernel_launches.load() - k0 - rs.k_pcg - rs.k_eval - rs.k_accept;
+  cudaGraphExec_t exec = nullptr;
+  OSFM_CUDA(cudaGraphInstantiate(&exec, g, 0));
+  OSFM_CUDA(cudaGraphLaunch(exec, stream));
+  OSFM_CUDA(cudaGraphExecDestroy(exec));   // released when the launch completes
+  OSFM_CUDA(cudaGraphDestroy(g));
 }
 
 void BA::run() {
@@ -2167,7 +2492,6 @@ void BA::run() {
   upload_problem();
   OSFM_CUDA(cudaEventCreate(&rs.ev0)); OSFM_CUDA(cudaEventCreate(&rs.ev1));
   trace("upload");
-  rs.tm_lin.init(); rs.tm_schur.init(); rs.tm_pcg.init(); rs.tm_back.init();
   trace("pre-struct");
   discover_structure();
   plan_pcg();
@@ -2175,27 +2499,23 @@ void BA::run() {
   if (cov_on) reserve_covariance();
 
   // ---- Levenberg-Marquardt (Ceres trust_region_minimizer / levenberg_marquardt_strategy) ----
+  // The step control is device code (ba_lm_*).  One process, no bounds, no capture and no trace: the loop is one CUDA
+  // graph launch (a WHILE node around the iteration body).  Otherwise the host drives the same body and reads the
+  // LM state after each decision: the all-reduce callback and the projected line search are host code.
   const int n = rs.n, nc = rs.nc;
-  int& cur = rs.cur;
+  // The graph is built for the pipelined PCG with the classic one as its conditional fallback; a problem whose
+  // pipelined plan does not fit runs the host-driven loop.
+  rs.device_loop = world == 1 && !rs.constrained && cap_iter == 0 && !switches().trace && !switches().host_loop &&
+                   rs.pcg_pipe_ok && stream != cudaStreamLegacy;
   if (world > 1) {  // all ranks enter the timed region together (their set-up times differ)
     OSFM_CUDA(cudaMemsetAsync(d_sc.p, 0, sizeof(Scalars), stream));
     allreduce_dev(&d_sc.p->cost, 1);
     OSFM_CUDA(cudaStreamSynchronize(stream));
   }
+  OSFM_CUDA(cudaMemsetAsync(d_lm.p, 0, sizeof(LmState), stream));
   OSFM_CUDA(cudaEventRecord(rs.ev0, stream));
-  double radius = 1e4;
-  const double max_radius = 1e16, min_radius = 1e-32, min_rel_decrease = 1e-3;
-  const double ftol = 1e-6, gtol = 1e-10, ptol = 1e-8;
-  double decrease_factor = 2.0;
-  bool reuse_diagonal = false;
-  int n_invalid = 0, it = 0, n_success = 0, n_solves = 0;
-  int termination = 1;
-  std::string message = "Maximum number of iterations reached.";
-
   build_segment_tables();
-  double grad_max = 0.0;
-  double cost = linearize(cur, true, &grad_max);
-  const double initial_cost = cost;
+  linearize(0, true);
   if (n > 0) {
     ba_make_scale<<<grid_for(n, 256), 256, 0, stream>>>(d_colnorm2.p, d_scale.p, n);
     OSFM_LAUNCH_CHECK();
@@ -2205,118 +2525,40 @@ void BA::run() {
   if (switches().pcg_deflate && rs.pcg_pipe_ok && rs.NI > 0 && nc > 0) {
     d_Wdef.reserve((size_t)PCG_ND * nc);
     OSFM_CUDA(cudaMemsetAsync(d_Wdef.p, 0, sizeof(double) * PCG_ND * (size_t)nc, stream));
-    pcg_gauge_vectors<<<grid_for(rs.NI, 128), 128, 0, stream>>>(rs.NI, d_inst_poff.p, params_of(cur).inst, d_scale.p, nc, d_Wdef.p);
+    pcg_gauge_vectors<<<grid_for(rs.NI, 128), 128, 0, stream>>>(rs.NI, d_inst_poff.p, params_of(0).inst, d_scale.p, nc, d_Wdef.p);
     OSFM_LAUNCH_CHECK();
     rs.pcg_pipe.Wdef = d_Wdef.p;
   }
-  double x_norm = n > 0 ? x_norm_of(cur) : 0.0;
-
-  if (grad_max <= gtol || n == 0) {
-    termination = 0;
-    message = n == 0 ? "No free parameters." : "Gradient tolerance reached.";
-  }
-  while (termination == 1) {
-    if (it >= max_iterations) break;
-    if (radius < min_radius) { termination = 0; message = "Minimum trust region radius reached."; break; }
-    ++it;
-    if (!reuse_diagonal) {
-      ba_make_diag<<<grid_for(n, 256), 256, 0, stream>>>(d_colnorm2.p, d_scale.p, d_diag.p, n);
+  if (n > 0) x_norm_pass(0);
+  ba_lm_init<<<1, 1, 0, stream>>>(d_lm.p, d_sc.p, n);
+  OSFM_LAUNCH_CHECK();
+  if (rs.device_loop) {
+    run_lm_graph();
+  } else {
+    for (;;) {
+      ba_lm_next<<<1, 1, 0, stream>>>(d_lm.p, max_iterations, 0, 0);
       OSFM_LAUNCH_CHECK();
-    }
-    const double inv_radius = 1.0 / radius;
-    build_system(inv_radius, nullptr, true);
-    OSFM_CUDA(cudaMemsetAsync(d_y.p, 0, sizeof(double) * rs.nz, stream));
-    int pcg_path = 0;
-    if (nc > 0) {
-      pcg_path = solve_reduced();
-      if (it == cap_iter) capture_linear_system(it, radius, pcg_path);
-    }
-    ++n_solves;
-    back_substitute();
-    OSFM_CUDA(cudaMemsetAsync(&d_sc.p->model_change, 0, sizeof(double) * 3, stream));  // model_change, step_norm2, x_norm2
-    if (n > 0) {
-      ba_model_change_alg<<<grid_for(n, 256), 256, 0, stream>>>(n, nc, rank == 0, d_grad.p, d_scale.p, d_diag.p, inv_radius, d_y.p, d_sc.p);
-      OSFM_LAUNCH_CHECK();
-    }
-    // --- candidate point ---
-    const int cand = cur ^ 1;
-    update_params(cur, cand, 1.0, d_ext_lower.p);
-    if (world > 1) allreduce_dev(&d_sc.p->model_change, 3);
-    const Scalars sm = read_scalars();
-    bool ok = true;
-    if (nc > 0) {
-      const PcgState& h = *h_pcg.p;
-      const int pcg_it = h.iterations, its = std::max(pcg_it, 1);
-      rs.pcg_total += pcg_it;
-      if (switches().trace && (pcg_path == OSFM_PCG_CLASSIC_RESIDENT || pcg_path == OSFM_PCG_CLASSIC_STREAMED))  // classic
-        fprintf(stderr, "[osfm_ba] pcg %d its, CTA0 clocks/it: stage %lld matvec %lld reduce1 %lld phaseB %lld reduce2 %lld (resident %d)\n",
-                pcg_it, h.prof[0] / its, h.prof[1] / its, h.prof[2] / its, h.prof[3] / its, h.prof[4] / its, (int)rs.pcg_resident);
-      if (!(h.rr_final == h.rr_final)) ok = false;
-    }
-    const double model_change = sm.model_change;
-    double step_norm = std::sqrt(sm.step_norm2);
-    if (!ok || !(model_change > 0.0) || !std::isfinite(step_norm)) {
-      if (++n_invalid >= 5) { termination = 2; message = "Too many consecutive invalid steps."; break; }
-      radius *= 0.5;
-      reuse_diagonal = true;
-      continue;
-    }
-    n_invalid = 0;
-    double cand_cost = eval_cost(cand);
-    if (rs.constrained) {
-      // Ceres: a problem with parameter bounds is "constrained": TrustRegionMinimizer::DoLineSearch runs a projected
-      // Armijo search along the step (sufficient decrease 1e-4, at most 20 contractions; bisection here, Ceres'
-      // default interpolates a cubic) and the candidate is the point it accepts.  The model cost change stays
-      // that of the full step, as in Ceres.
-      auto step_to = [&](double alpha) {   // candidate = Project(x - alpha * scale * y); |delta|
-        OSFM_CUDA(cudaMemsetAsync(&d_sc.p->step_norm2, 0, sizeof(double) * 2, stream));
-        update_params(cur, cand, alpha, d_ext_lower.p);
-        if (world > 1) allreduce_dev(&d_sc.p->step_norm2, 2);
-        return std::sqrt(read_scalars().step_norm2);
-      };
-      OSFM_CUDA(cudaMemsetAsync(&d_sc.p->gdot, 0, sizeof(double), stream));
-      ba_grad_dot<<<grid_for(n, 256), 256, 0, stream>>>(n, nc, rank == 0, d_grad.p, d_scale.p, d_y.p, d_sc.p);
-      OSFM_LAUNCH_CHECK();
-      if (world > 1) allreduce_dev(&d_sc.p->gdot, 1);
-      const double g0 = read_scalars().gdot;
-      double alpha = 1.0;
-      bool ok_ls = false;
-      for (int ls = 0; ls < 20; ++ls) {
-        if (ls > 0) { step_norm = step_to(alpha); cand_cost = eval_cost(cand); }
-        if (std::isfinite(cand_cost) && cand_cost <= cost + 1e-4 * g0 * alpha) { ok_ls = true; break; }
-        alpha *= 0.5;
-      }
-      if (!ok_ls) { step_norm = step_to(1.0); cand_cost = eval_cost(cand); }
-    }
-    if (step_norm <= ptol * (x_norm + ptol)) { termination = 0; message = "Parameter tolerance reached."; break; }
-    const double cost_change = cost - cand_cost;
-    if (std::fabs(cost_change) <= ftol * cost) { termination = 0; message = "Function tolerance reached."; break; }
-    const double rel = cost_change / model_change;
-    if (rel > min_rel_decrease) {
-      cur = cand;
-      cost = linearize(cur, true, &grad_max);
-      x_norm = x_norm_of(cur);
-      radius = std::min(max_radius, radius / std::max(1.0 / 3.0, 1.0 - std::pow(2.0 * rel - 1.0, 3)));
-      decrease_factor = 2.0;
-      reuse_diagonal = false;
-      ++n_success;
-      if (grad_max <= gtol) { termination = 0; message = "Gradient tolerance reached."; break; }
-    } else {
-      radius /= decrease_factor;
-      decrease_factor *= 2.0;
-      reuse_diagonal = true;
+      if (!read_lm().running) break;
+      lm_iteration();
     }
   }
   OSFM_CUDA(cudaEventRecord(rs.ev1, stream));
+  static const char* const messages[] = {"Maximum number of iterations reached.", "No free parameters.",
+                                         "Gradient tolerance reached.", "Minimum trust region radius reached.",
+                                         "Too many consecutive invalid steps.", "Parameter tolerance reached.",
+                                         "Function tolerance reached."};
+  const LmState lm = read_lm();
+  const int termination = lm.termination;
   osfm_ba_summary sum{};
-  sum.iterations = it;
-  sum.successful_steps = n_success;
-  sum.linear_solves = n_solves;
-  sum.pcg_iterations = rs.pcg_total;
+  sum.iterations = lm.it;
+  sum.successful_steps = lm.n_success;
+  sum.linear_solves = lm.n_solves;
+  sum.pcg_iterations = lm.pcg_total;
   sum.termination = termination;
-  sum.initial_cost = initial_cost;
-  sum.final_cost = eval_cost(cur);
-  snprintf(sum.message, sizeof(sum.message), "%s", message.c_str());
+  sum.initial_cost = lm.initial_cost;
+  eval_cost(0);
+  sum.final_cost = read_scalars().cost;
+  snprintf(sum.message, sizeof(sum.message), "%s", messages[lm.message]);
   trace("lm");
 
   if (cov_on) covariance_pass(termination);

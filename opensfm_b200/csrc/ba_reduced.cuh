@@ -1223,58 +1223,73 @@ __global__ void __launch_bounds__(256)
   }
 }
 
-// Cholesky-inverts the diagonal matrix of every preconditioner group into Minv[g][MAXB*MAXB].
-__global__ void pcg_factor_groups(const double* __restrict__ Sval, BsrView h, const int* __restrict__ diag_off,
-                                  const int* __restrict__ grp_b1, const int* __restrict__ grp_b2, int ngroups,
-                                  double* __restrict__ Minv) {
-  const int g = blockIdx.x * blockDim.x + threadIdx.x;
-  if (g >= ngroups) return;
+// Cholesky-inverts the diagonal matrix of every preconditioner group into Minv[g][MAXB*MAXB].  One warp per group,
+// the factor in shared memory: lane 0 takes the pivot of column j, lanes j + 1 .. n - 1 its rows below, then lane c
+// solves for column c of the inverse (every value is computed by one lane in the order of the serial algorithm).
+constexpr int PFG_WARPS = 4;
+__global__ void __launch_bounds__(32 * PFG_WARPS)
+    pcg_factor_groups(const double* __restrict__ Sval, BsrView h, const int* __restrict__ diag_off,
+                      const int* __restrict__ grp_b1, const int* __restrict__ grp_b2, int ngroups,
+                      double* __restrict__ Minv) {
+  __shared__ double Ls[PFG_WARPS][MAXB * MAXB];
+  const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int g = blockIdx.x * PFG_WARPS + w;
+  if (g >= ngroups) return;   // warp-uniform
+  double* L = Ls[w];
   const int b1 = grp_b1[g], b2 = grp_b2[g];
   const int n1 = h.blk_sz[b1], n2 = b2 >= 0 ? h.blk_sz[b2] : 0;
   const int n = n1 + n2;
-  double L[MAXB * MAXB];
   const double* D1 = Sval + diag_off[b1];
-  for (int i = 0; i < n1; ++i)
-    for (int j = 0; j <= i; ++j) L[i * MAXB + j] = D1[i * n1 + j];
+  for (int t = lane; t < n1 * n1; t += 32) {
+    const int i = t / n1, j = t - i * n1;
+    if (j <= i) L[i * MAXB + j] = D1[t];
+  }
   if (b2 >= 0) {
     const double* D2 = Sval + diag_off[b2];
-    for (int i = 0; i < n2; ++i)
-      for (int j = 0; j <= i; ++j) L[(n1 + i) * MAXB + n1 + j] = D2[i * n2 + j];
+    for (int t = lane; t < n2 * n2; t += 32) {
+      const int i = t / n2, j = t - i * n2;
+      if (j <= i) L[(n1 + i) * MAXB + n1 + j] = D2[t];
+    }
     const int o12 = bsr_lookup(h, min(b1, b2), max(b1, b2));
-    for (int i = 0; i < n2; ++i)
-      for (int j = 0; j < n1; ++j) {
-        // lower-left part = block (b2 rows, b1 cols); the stored upper block is (min, max)
-        double v = 0.0;
-        if (o12 >= 0) v = b1 < b2 ? Sval[o12 + j * n2 + i] : Sval[o12 + i * n1 + j];
-        L[(n1 + i) * MAXB + j] = v;
-      }
+    for (int t = lane; t < n2 * n1; t += 32) {
+      const int i = t / n1, j = t - i * n1;
+      // lower-left part = block (b2 rows, b1 cols); the stored upper block is (min, max)
+      double v = 0.0;
+      if (o12 >= 0) v = b1 < b2 ? Sval[o12 + j * n2 + i] : Sval[o12 + i * n1 + j];
+      L[(n1 + i) * MAXB + j] = v;
+    }
   }
+  __syncwarp();
   for (int j = 0; j < n; ++j) {
-    double d = L[j * MAXB + j];
-    for (int k = 0; k < j; ++k) d -= L[j * MAXB + k] * L[j * MAXB + k];
-    d = sqrt(fmax(d, 1e-300));
-    L[j * MAXB + j] = d;
-    for (int i = j + 1; i < n; ++i) {
+    if (lane == 0) {
+      double d = L[j * MAXB + j];
+      for (int k = 0; k < j; ++k) d -= L[j * MAXB + k] * L[j * MAXB + k];
+      L[j * MAXB + j] = sqrt(fmax(d, 1e-300));
+    }
+    __syncwarp();
+    const int i = j + 1 + lane;
+    if (i < n) {
       double s = L[i * MAXB + j];
       for (int k = 0; k < j; ++k) s -= L[i * MAXB + k] * L[j * MAXB + k];
-      L[i * MAXB + j] = s / d;
+      L[i * MAXB + j] = s / L[j * MAXB + j];
     }
+    __syncwarp();
   }
+  if (lane >= n) return;
+  const int c = lane;
   double* out = Minv + (size_t)g * MAXB * MAXB;
-  for (int c = 0; c < n; ++c) {
-    double y[MAXB];
-    for (int i = 0; i < n; ++i) {
-      double s = (i == c) ? 1.0 : 0.0;
-      for (int k = 0; k < i; ++k) s -= L[i * MAXB + k] * y[k];
-      y[i] = s / L[i * MAXB + i];
-    }
-    for (int i = n - 1; i >= 0; --i) {
-      double s = y[i];
-      for (int k = i + 1; k < n; ++k) s -= L[k * MAXB + i] * y[k];
-      y[i] = s / L[i * MAXB + i];
-    }
-    for (int i = 0; i < n; ++i) out[i * MAXB + c] = y[i];
+  double y[MAXB];
+  for (int i = 0; i < n; ++i) {
+    double s = (i == c) ? 1.0 : 0.0;
+    for (int k = 0; k < i; ++k) s -= L[i * MAXB + k] * y[k];
+    y[i] = s / L[i * MAXB + i];
   }
+  for (int i = n - 1; i >= 0; --i) {
+    double s = y[i];
+    for (int k = i + 1; k < n; ++k) s -= L[k * MAXB + i] * y[k];
+    y[i] = s / L[i * MAXB + i];
+  }
+  for (int i = 0; i < n; ++i) out[i * MAXB + c] = y[i];
 }
 
 constexpr int PCG_MAX_CTAS = 256;
