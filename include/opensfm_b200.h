@@ -146,6 +146,40 @@ int osfm_matcher_vlad_select(osfm_matcher* m, int nref, const int* ref_ids, int 
                              const uint32_t* cand_mask_bits, const int* camera_labels, int k, int64_t* out_offsets,
                              int32_t* out_cols, double* out_dist);
 
+/* BoW pair selection (pairs_selection.match_candidates_with_bow, opensfm/pairs_selection.py:281-348, 690-727;
+ * bow.py).  osfm_matcher_bow_words: the k nearest of the nwords vocabulary words (nwords x dim float32, row-major)
+ * of every row of each listed resident set, as cv2 BruteForce knnMatch(desc, vocab, k) returns them (bow.py
+ * map_to_words): ranked by the float32 square root of the squared distance summed in cv2's order, ties to the lower
+ * word.  1 <= k <= 64; min(k, nwords) words per row.  The rows of set i are rows out_offsets[i] .. out_offsets[i + 1]
+ * of out_words (out_offsets: count + 1 entries; out_words: NULL, or room for all rows of the valid sets); the first
+ * word of every row stays on the device with the set.  out_valid[i] = 0 for Hamming sets and sets of another
+ * dimension (no rows).  float32 and uint8-stored L2 sets are read as float32.  Fails (OSFM_ERR_ARG) on non-finite
+ * vocabulary or descriptor elements. */
+int osfm_matcher_bow_words(osfm_matcher* m, int count, const int* set_ids, const float* vocab, int nwords, int dim,
+                           int k, int64_t* out_offsets, int32_t* out_words, int* out_valid);
+/* One-shot osfm_matcher_bow_words of n x dim float32 descriptors from host memory: out = n x min(k, nwords). */
+int osfm_bow_map_to_words(osfm_matcher* m, const float* desc, int n, int dim, const float* vocab, int nwords, int k,
+                          int32_t* out);
+/* BagOfWords.histogram of each listed set's resident first words: h = bincount(words, nwords) * weights, h / h.sum(),
+ * float64 in numpy's order (bit for bit), kept on the device with the set.  out_valid[i] = 0 for sets without
+ * words of an nwords-word vocabulary (osfm_matcher_bow_words) and sets of 8 or fewer rows (load_histograms). */
+int osfm_matcher_bow_histograms(osfm_matcher* m, int count, const int* set_ids, const double* weights, int nwords,
+                                int* out_valid);
+/* Copy one set's BoW histogram (nwords doubles). */
+int osfm_matcher_bow_get(osfm_matcher* m, int set_id, double* out);
+/* One-shot BagOfWords.histogram of n word indices from host memory (no minimum count): out = nwords doubles. */
+int osfm_bow_histogram(osfm_matcher* m, const int32_t* words, int n, const double* weights, int nwords, double* out);
+/* osfm_matcher_vlad_select over the BoW histograms, with the distance np.fabs(h - h2).sum() (numpy's pairwise
+ * order, bit for bit).  cand_order: NULL (every candidate, ties to the lower column), or nref x ncand ints, the
+ * position of candidate j in reference r's own candidate list or -1 if it is not in it: then only listed candidates
+ * are eligible and ties go to the earlier position (bow_distances walks each list in the given order). */
+int osfm_matcher_bow_select(osfm_matcher* m, int nref, const int* ref_ids, int ncand, const int* cand_ids,
+                            const int32_t* cand_order, const int* camera_labels, int k, int64_t* out_offsets,
+                            int32_t* out_cols, double* out_dist);
+/* np.fabs(h - h2).sum() of histogram `query` and each of the n histograms (n x len float64, row-major), in numpy's
+ * pairwise order; out_n[query] = 0. */
+int osfm_bow_distances(osfm_matcher* m, const double* hist, int n, int len, int query, double* out_n);
+
 /* ------------------------------------------------------------------------
  * BA
  * ---------------------------------------------------------------------- */

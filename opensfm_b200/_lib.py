@@ -90,6 +90,15 @@ SIGNATURES = {
     "osfm_matcher_vlad_get": (c_int, [c_void_p, c_int, c_int, c_void_p]),
     "osfm_matcher_vlad_select": (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int, c_void_p,
                                          c_void_p, c_void_p]),
+    "osfm_matcher_bow_words": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p,
+                                       c_void_p]),
+    "osfm_bow_map_to_words": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_int, c_int, c_void_p]),
+    "osfm_matcher_bow_histograms": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_int, c_void_p]),
+    "osfm_matcher_bow_get": (c_int, [c_void_p, c_int, c_void_p]),
+    "osfm_bow_histogram": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p]),
+    "osfm_matcher_bow_select": (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int, c_void_p,
+                                        c_void_p, c_void_p]),
+    "osfm_bow_distances": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
     "osfm_ba_create": (c_int, [c_int, POINTER(c_void_p)]),
     "osfm_ba_destroy": (c_int, [c_void_p]),
     "osfm_camera_num_params": (c_int, [c_int]),

@@ -146,18 +146,7 @@ __global__ void __launch_bounds__(256) bf_top2_simt(const MatchJob* __restrict__
 }
 
 // ---------------------------------------------------------------------------
-// General float32 descriptors, bit-exact with cv2's summation order.
-//
-// cv2::batchDistance -> normL2Sqr_(const float*, const float*, int) (OpenCV core, the x86-64 baseline
-// build of the opencv-python wheels: 4-lane universal intrinsics, no FMA) accumulates
-//     acc[a][l] += t*t   for element e = 16*blk + 4*a + l   (four 4-lane accumulators, mul then add),
-// combines  v[l] = ((acc[0][l] + acc[1][l]) + acc[2][l]) + acc[3][l],
-// reduces   d = (v[0] + v[2]) + (v[1] + v[3]),
-// and adds the dim % 16 tail sequentially, d += t*t.  (Probed against live cv2 4.13 in
-// tests/test_match_oracle.py::test_cv2_float_sum_order; integer-valued descriptors are exact in any order.)
-// Every accumulator receives one term per 16-element block, so the kernel walks the 16 (a, l) slots in
-// the outer loop and the blocks in the inner loop: one live accumulator per pair instead of sixteen.
-// Both operand tiles hold whole rows in shared memory ([element][row], 128-bit conflict-free reads).
+// General float32 descriptors, bit-exact with cv2's summation order (cv_tile_d2, match_common.cuh).
 // MT = micro-tile edge per thread (4 -> 64x64 CTA tile, 2 -> 32x32 for long descriptors).
 // ---------------------------------------------------------------------------
 template <int MT>
@@ -191,20 +180,7 @@ __global__ void __launch_bounds__(256) bf_top2_f32_cv(const MatchJob* __restrict
 
   const int tid = threadIdx.x;
   const int ty = tid >> 4, tx = tid & 15;
-  const int nvec = D >> 2;
-
-  auto load_tile = [&](float* dst, const float* __restrict__ src, int r0, int rend) {
-    for (int idx = tid; idx < TS * nvec; idx += 256) {
-      const int row = idx % TS, v = idx / TS;
-      float4 x = make_float4(0.f, 0.f, 0.f, 0.f);
-      if (r0 + row < rend) x = *reinterpret_cast<const float4*>(src + (size_t)(r0 + row) * D + v * 4);
-      dst[(v * 4 + 0) * LD + row] = x.x;
-      dst[(v * 4 + 1) * LD + row] = x.y;
-      dst[(v * 4 + 2) * LD + row] = x.z;
-      dst[(v * 4 + 3) * LD + row] = x.w;
-    }
-  };
-  load_tile(As, Q, q0, job.nq);
+  cv_load_tile<TS, LD>(As, Q, q0, job.nq, D);
 
   Top2 best[MT];
 #pragma unroll
@@ -212,77 +188,10 @@ __global__ void __launch_bounds__(256) bf_top2_f32_cv(const MatchJob* __restrict
 
   for (int t0 = t_begin; t0 < t_end; t0 += TS) {
     __syncthreads();  // previous tile's readers are done (and As is complete on the first pass)
-    load_tile(Bs, T, t0, t_end);
+    cv_load_tile<TS, LD>(Bs, T, t0, t_end, D);
     __syncthreads();
-    float u[MT][MT], w[MT][MT];
-#pragma unroll
-    for (int li = 0; li < 4; ++li) {
-      const int l = (li == 0) ? 0 : (li == 1) ? 2 : (li == 2) ? 1 : 3;  // lanes 0, 2 feed u; 1, 3 feed w
-      float s[MT][MT];
-#pragma unroll
-      for (int a = 0; a < 4; ++a) {
-        float acc[MT][MT];
-#pragma unroll
-        for (int i = 0; i < MT; ++i)
-#pragma unroll
-          for (int j = 0; j < MT; ++j) acc[i][j] = 0.f;
-        const float* pa = As + (size_t)(4 * a + l) * LD + ty * MT;
-        const float* pb = Bs + (size_t)(4 * a + l) * LD + tx * MT;
-        for (int blk = 0; blk < nblk; ++blk) {
-          float av[MT], bv[MT];
-          if constexpr (MT == 4) {
-            const float4 a4 = *reinterpret_cast<const float4*>(pa);
-            const float4 b4 = *reinterpret_cast<const float4*>(pb);
-            av[0] = a4.x; av[1] = a4.y; av[2] = a4.z; av[3] = a4.w;
-            bv[0] = b4.x; bv[1] = b4.y; bv[2] = b4.z; bv[3] = b4.w;
-          } else {
-            const float2 a2 = *reinterpret_cast<const float2*>(pa);
-            const float2 b2 = *reinterpret_cast<const float2*>(pb);
-            av[0] = a2.x; av[1] = a2.y; bv[0] = b2.x; bv[1] = b2.y;
-          }
-#pragma unroll
-          for (int i = 0; i < MT; ++i)
-#pragma unroll
-            for (int j = 0; j < MT; ++j) {
-              const float t = __fsub_rn(av[i], bv[j]);
-              acc[i][j] = __fadd_rn(acc[i][j], __fmul_rn(t, t));   // mul, then add: no FMA contraction
-            }
-          pa += 16 * LD;
-          pb += 16 * LD;
-        }
-#pragma unroll
-        for (int i = 0; i < MT; ++i)
-#pragma unroll
-          for (int j = 0; j < MT; ++j) s[i][j] = a == 0 ? acc[i][j] : __fadd_rn(s[i][j], acc[i][j]);
-      }
-#pragma unroll
-      for (int i = 0; i < MT; ++i)
-#pragma unroll
-        for (int j = 0; j < MT; ++j) {
-          if (li == 0) u[i][j] = s[i][j];
-          else if (li == 1) u[i][j] = __fadd_rn(u[i][j], s[i][j]);
-          else if (li == 2) w[i][j] = s[i][j];
-          else w[i][j] = __fadd_rn(w[i][j], s[i][j]);
-        }
-    }
     float d2[MT][MT];
-#pragma unroll
-    for (int i = 0; i < MT; ++i)
-#pragma unroll
-      for (int j = 0; j < MT; ++j) d2[i][j] = __fadd_rn(u[i][j], w[i][j]);
-    // scalar tail of the true dimension (zero padding beyond it adds +0)
-    for (int e = nblk * 16; e < D; ++e) {
-      float av[MT], bv[MT];
-#pragma unroll
-      for (int i = 0; i < MT; ++i) { av[i] = As[(size_t)e * LD + ty * MT + i]; bv[i] = Bs[(size_t)e * LD + tx * MT + i]; }
-#pragma unroll
-      for (int i = 0; i < MT; ++i)
-#pragma unroll
-        for (int j = 0; j < MT; ++j) {
-          const float t = __fsub_rn(av[i], bv[j]);
-          d2[i][j] = __fadd_rn(d2[i][j], __fmul_rn(t, t));
-        }
-    }
+    cv_tile_d2<MT, LD>(As, Bs, D, nblk, ty, tx, d2);
 #pragma unroll
     for (int i = 0; i < MT; ++i) {
       const int gq = q0 + ty * MT + i;
@@ -654,6 +563,8 @@ void Matcher::free_set(DescSet& s) {
   slab_release(s.slab, s.data, s.slab_bytes);
   if (s.bearings) { slab_release(s.bear_slab, s.bearings, s.bear_bytes); s.bearings = nullptr; s.bear_slab = -1; }
   if (s.vlad) { slab_release(s.vlad_slab, s.vlad, s.vlad_bytes); s.vlad = nullptr; s.vlad_slab = -1; }
+  if (s.bow_words) { slab_release(s.bow_words_slab, s.bow_words, s.bow_words_bytes); s.bow_words = nullptr; s.bow_words_slab = -1; }
+  if (s.bow_hist) { slab_release(s.bow_hist_slab, s.bow_hist, s.bow_hist_bytes); s.bow_hist = nullptr; s.bow_hist_slab = -1; }
   if (s.slot >= 0) {
     cudaMemsetAsync(d_info.p + 2 * s.slot, 0, 2 * sizeof(int), stream);
     free_slots.push_back(s.slot);

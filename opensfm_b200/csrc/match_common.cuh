@@ -44,6 +44,111 @@ __host__ __device__ inline void top2_merge(Top2& t, const Top2& o) {
   if (o.i2 >= 0) top2_insert(t, o.s2, o.i2);
 }
 
+// cv2's float32 L2 distances of one tile: the shared-memory halves and the arithmetic of bf_top2_f32_cv
+// (match.cu), also used by the word assignment of bow.cu.
+//
+// cv2::batchDistance -> normL2Sqr_(const float*, const float*, int) (OpenCV core, the x86-64 baseline
+// build of the opencv-python wheels: 4-lane universal intrinsics, no FMA) accumulates
+//     acc[a][l] += t*t   for element e = 16*blk + 4*a + l   (four 4-lane accumulators, mul then add),
+// combines  v[l] = ((acc[0][l] + acc[1][l]) + acc[2][l]) + acc[3][l],
+// reduces   d = (v[0] + v[2]) + (v[1] + v[3]),
+// and adds the dim % 16 tail sequentially, d += t*t.  (Probed against live cv2 4.13 in
+// tests/test_match_oracle.py::test_cv2_float_sum_order; integer-valued descriptors are exact in any order.)
+// Every accumulator receives one term per 16-element block, so the tile walks the 16 (a, l) slots in
+// the outer loop and the blocks in the inner loop: one live accumulator per pair instead of sixteen.
+// Both operand tiles hold whole rows in shared memory ([element][row], 128-bit conflict-free reads).
+// MT = micro-tile edge per thread of a 256-thread CTA (TS = 16 MT rows per tile side), LD = floats per element row.
+
+// rows r0 .. min(r0 + TS, rend) of src (D floats per row) -> dst[e * LD + row], zero rows beyond rend
+template <int TS, int LD>
+__device__ __forceinline__ void cv_load_tile(float* dst, const float* __restrict__ src, int r0, int rend, int D) {
+  const int nvec = D >> 2;
+  for (int idx = threadIdx.x; idx < TS * nvec; idx += 256) {
+    const int row = idx % TS, v = idx / TS;
+    float4 x = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (r0 + row < rend) x = *reinterpret_cast<const float4*>(src + (size_t)(r0 + row) * D + v * 4);
+    dst[(v * 4 + 0) * LD + row] = x.x;
+    dst[(v * 4 + 1) * LD + row] = x.y;
+    dst[(v * 4 + 2) * LD + row] = x.z;
+    dst[(v * 4 + 3) * LD + row] = x.w;
+  }
+}
+
+// d2[i][j] = squared distance of tile rows (As row ty * MT + i, Bs row tx * MT + j) over D padded elements,
+// nblk = full 16-element blocks of the true dimension
+template <int MT, int LD>
+__device__ __forceinline__ void cv_tile_d2(const float* As, const float* Bs, int D, int nblk, int ty, int tx,
+                                           float (&d2)[MT][MT]) {
+  float u[MT][MT], w[MT][MT];
+#pragma unroll
+  for (int li = 0; li < 4; ++li) {
+    const int l = (li == 0) ? 0 : (li == 1) ? 2 : (li == 2) ? 1 : 3;  // lanes 0, 2 feed u; 1, 3 feed w
+    float s[MT][MT];
+#pragma unroll
+    for (int a = 0; a < 4; ++a) {
+      float acc[MT][MT];
+#pragma unroll
+      for (int i = 0; i < MT; ++i)
+#pragma unroll
+        for (int j = 0; j < MT; ++j) acc[i][j] = 0.f;
+      const float* pa = As + (size_t)(4 * a + l) * LD + ty * MT;
+      const float* pb = Bs + (size_t)(4 * a + l) * LD + tx * MT;
+      for (int blk = 0; blk < nblk; ++blk) {
+        float av[MT], bv[MT];
+        if constexpr (MT == 4) {
+          const float4 a4 = *reinterpret_cast<const float4*>(pa);
+          const float4 b4 = *reinterpret_cast<const float4*>(pb);
+          av[0] = a4.x; av[1] = a4.y; av[2] = a4.z; av[3] = a4.w;
+          bv[0] = b4.x; bv[1] = b4.y; bv[2] = b4.z; bv[3] = b4.w;
+        } else {
+          const float2 a2 = *reinterpret_cast<const float2*>(pa);
+          const float2 b2 = *reinterpret_cast<const float2*>(pb);
+          av[0] = a2.x; av[1] = a2.y; bv[0] = b2.x; bv[1] = b2.y;
+        }
+#pragma unroll
+        for (int i = 0; i < MT; ++i)
+#pragma unroll
+          for (int j = 0; j < MT; ++j) {
+            const float t = __fsub_rn(av[i], bv[j]);
+            acc[i][j] = __fadd_rn(acc[i][j], __fmul_rn(t, t));   // mul, then add: no FMA contraction
+          }
+        pa += 16 * LD;
+        pb += 16 * LD;
+      }
+#pragma unroll
+      for (int i = 0; i < MT; ++i)
+#pragma unroll
+        for (int j = 0; j < MT; ++j) s[i][j] = a == 0 ? acc[i][j] : __fadd_rn(s[i][j], acc[i][j]);
+    }
+#pragma unroll
+    for (int i = 0; i < MT; ++i)
+#pragma unroll
+      for (int j = 0; j < MT; ++j) {
+        if (li == 0) u[i][j] = s[i][j];
+        else if (li == 1) u[i][j] = __fadd_rn(u[i][j], s[i][j]);
+        else if (li == 2) w[i][j] = s[i][j];
+        else w[i][j] = __fadd_rn(w[i][j], s[i][j]);
+      }
+  }
+#pragma unroll
+  for (int i = 0; i < MT; ++i)
+#pragma unroll
+    for (int j = 0; j < MT; ++j) d2[i][j] = __fadd_rn(u[i][j], w[i][j]);
+  // scalar tail of the true dimension (zero padding beyond it adds +0)
+  for (int e = nblk * 16; e < D; ++e) {
+    float av[MT], bv[MT];
+#pragma unroll
+    for (int i = 0; i < MT; ++i) { av[i] = As[(size_t)e * LD + ty * MT + i]; bv[i] = Bs[(size_t)e * LD + tx * MT + i]; }
+#pragma unroll
+    for (int i = 0; i < MT; ++i)
+#pragma unroll
+      for (int j = 0; j < MT; ++j) {
+        const float t = __fsub_rn(av[i], bv[j]);
+        d2[i][j] = __fadd_rn(d2[i][j], __fmul_rn(t, t));
+      }
+  }
+}
+
 // One direction of one image pair.
 struct MatchJob {
   const void* q;  // queries, padded rows (float32 or packed uint8 words)
@@ -94,6 +199,14 @@ struct DescSet {
   float* vlad = nullptr;
   int vlad_len = 0, vlad_slab = -1;
   size_t vlad_bytes = 0;
+  // BoW state (bow.cu): the nearest visual word of every row (n ints, words of a bow_nwords-word vocabulary) and
+  // the weighted, normalised word histogram (bow_len doubles); null until computed
+  int* bow_words = nullptr;
+  int bow_nwords = 0, bow_words_slab = -1;
+  size_t bow_words_bytes = 0;
+  double* bow_hist = nullptr;
+  int bow_len = 0, bow_hist_slab = -1;
+  size_t bow_hist_bytes = 0;
 };
 
 // The two layouts of one pair's epipolar bitmask in the last guided submission (the test hook reads them back).
@@ -149,6 +262,12 @@ struct Matcher {
   DevBuf<int> d_vlad_assign, d_vlad_flags;
   DevBuf<double> d_vlad_dist;
   DevBuf<uint8_t> d_vlad_tab;
+  // BoW workspaces (bow.cu): padded vocabulary, per-chunk top-k lists + words of a batch, error flags, distance block,
+  // job / selection tables
+  DevBuf<float> d_bow_vocab;
+  DevBuf<uint8_t> d_bow_work, d_bow_tab;
+  DevBuf<int> d_bow_flags;
+  DevBuf<double> d_bow_dist;
 
   explicit Matcher(int dev);
   ~Matcher();

@@ -15,10 +15,9 @@
 #include <mutex>
 #include <vector>
 
-#include <cub/cub.cuh>
-
 #include "common.cuh"
 #include "match_common.cuh"
+#include "select_common.cuh"
 
 namespace osfm {
 
@@ -28,7 +27,6 @@ constexpr int VA_THREADS = 128;          // word assignment: one thread per feat
 constexpr int VA_CH = 32;                // centres whose distance chains one thread interleaves
 constexpr int VN_THREADS_MAX = 256;      // accumulation + normalisation: one CTA per set
 constexpr int VD_TM = 32, VD_TN = 64, VD_TK = 32;   // distance tile: reference rows x candidate rows x elements
-constexpr int VS_THREADS = 256;          // selection: one CTA per reference row
 constexpr size_t VLAD_SMEM_MAX = 200 * 1024;
 
 struct VladJob {
@@ -206,105 +204,6 @@ __global__ void __launch_bounds__(256)
       const int ia = a0 + ty + 16 * i, jb = b0 + tx + 16 * j;
       if (ia < na && jb < nb) out[(size_t)ia * ldo + jb] = sqrt(acc[i][j]);
     }
-}
-
-// Order-preserving key of a distance: ascending for numbers, every NaN after them (np.argsort's order).
-__device__ __forceinline__ unsigned long long dist_key(double d) {
-  if (isnan(d)) return ~0ull;
-  const unsigned long long b = (unsigned long long)__double_as_longlong(d);
-  return (b >> 63) ? ~b : (b | (1ull << 63));
-}
-
-// One CTA per reference row of the block: the k smallest eligible candidates by (distance, column) -- the order a
-// stable argsort over the reference's sorted candidate list gives -- per camera group.  With camera labels there are
-// two groups, the candidates of the reference's camera and the others (pairs_from_neighbors), otherwise one.
-// Selection: radix select of the k-th key over eight 8-bit digits, then one pass in column order that keeps every
-// key below it and the first `need` keys equal to it.  Output: the selected columns in ascending order.
-__global__ void __launch_bounds__(VS_THREADS)
-    vlad_select_kernel(const double* __restrict__ dist, int ncand, int row0, int nref, const int* __restrict__ ref_ids,
-                       const int* __restrict__ cand_ids, const uint32_t* __restrict__ mask, int mask_words,
-                       const int* __restrict__ labels, int k, int stride, int* __restrict__ out_count,
-                       int* __restrict__ out_cols, double* __restrict__ out_dist) {
-  using Scan = cub::BlockScan<int, VS_THREADS>;
-  __shared__ typename Scan::TempStorage scan_tmp;
-  __shared__ int hist[256];
-  __shared__ unsigned long long s_prefix;
-  __shared__ int s_need;
-  const int row = row0 + blockIdx.x;
-  const double* d = dist + (size_t)blockIdx.x * ncand;
-  const int self = ref_ids[row];
-  const int ngroups = labels ? 2 : 1;
-  const size_t base = (size_t)row * stride;
-  int written = 0;
-  for (int g = 0; g < ngroups; ++g) {
-    auto eligible = [&](int j) {
-      if (cand_ids[j] == self) return false;
-      if (mask && !((mask[(size_t)row * mask_words + (j >> 5)] >> (j & 31)) & 1u)) return false;
-      if (labels && ((labels[nref + j] == labels[row]) != (g == 0))) return false;
-      return true;
-    };
-    int cnt = 0;
-    for (int j = threadIdx.x; j < ncand; j += VS_THREADS) cnt += eligible(j);
-    int total_elig;
-    Scan(scan_tmp).ExclusiveSum(cnt, cnt, total_elig);
-    __syncthreads();
-    const bool take_all = total_elig <= k;
-    unsigned long long thr = ~0ull;
-    int need = 0;
-    if (!take_all) {
-      if (threadIdx.x == 0) { s_prefix = 0ull; s_need = k; }
-      for (int shift = 56; shift >= 0; shift -= 8) {
-        for (int b = threadIdx.x; b < 256; b += VS_THREADS) hist[b] = 0;
-        __syncthreads();
-        const unsigned long long prefix = s_prefix;
-        const unsigned long long hi = shift == 56 ? 0ull : (~0ull << (shift + 8));
-        for (int j = threadIdx.x; j < ncand; j += VS_THREADS) {
-          if (!eligible(j)) continue;
-          const unsigned long long key = dist_key(d[j]);
-          if ((key & hi) == (prefix & hi)) atomicAdd(&hist[(key >> shift) & 255], 1);
-        }
-        __syncthreads();
-        if (threadIdx.x == 0) {
-          int cum = 0, want = s_need, b = 0;
-          for (; b < 255 && cum + hist[b] < want; ++b) cum += hist[b];
-          s_need = want - cum;
-          s_prefix = prefix | ((unsigned long long)b << shift);
-        }
-        __syncthreads();
-      }
-      thr = s_prefix;
-      need = s_need;   // keys equal to thr to keep, lowest columns first
-    }
-    int eq_before = 0;
-    for (int j0 = 0; j0 < ncand; j0 += VS_THREADS) {
-      const int j = j0 + threadIdx.x;
-      bool lt = false, eq = false;
-      double dj = 0.0;
-      if (j < ncand && eligible(j)) {
-        dj = d[j];
-        if (take_all) lt = true;
-        else {
-          const unsigned long long key = dist_key(dj);
-          lt = key < thr;
-          eq = key == thr;
-        }
-      }
-      int eq_rank, eq_total;
-      Scan(scan_tmp).ExclusiveSum((int)eq, eq_rank, eq_total);
-      __syncthreads();
-      const bool take = lt || (eq && eq_before + eq_rank < need);
-      int pos, ntake;
-      Scan(scan_tmp).ExclusiveSum((int)take, pos, ntake);
-      __syncthreads();
-      if (take) {
-        out_cols[base + written + pos] = j;
-        out_dist[base + written + pos] = dj;
-      }
-      written += ntake;
-      eq_before += eq_total;
-    }
-  }
-  if (threadIdx.x == 0) out_count[row] = written;
 }
 
 }  // namespace
@@ -508,9 +407,9 @@ int osfm_matcher_vlad_select(osfm_matcher* m, int nref, const int* ref_ids, int 
   for (int r0 = 0; r0 < nref; r0 += block) {
     const int nb = std::min(block, nref - r0);
     launch_vlad_distances(M.stream, d_rows + r0, nb, d_rows + nref, ncand, L, M.d_vlad_dist.p, ncand);
-    vlad_select_kernel<<<nb, VS_THREADS, 0, M.stream>>>(
+    neighbor_select_kernel<<<nb, VS_THREADS, 0, M.stream>>>(
         M.d_vlad_dist.p, ncand, r0, nref, d_ids, d_ids + nref,
-        cand_mask_bits ? reinterpret_cast<const uint32_t*>(base + o_mask) : nullptr, mask_words,
+        cand_mask_bits ? reinterpret_cast<const uint32_t*>(base + o_mask) : nullptr, mask_words, nullptr,
         camera_labels ? reinterpret_cast<const int*>(base + o_lab) : nullptr, k, stride, d_cnt, d_cols, d_dist);
     OSFM_LAUNCH_CHECK();
   }

@@ -133,6 +133,8 @@ class PairMatcher:
         self._rows: Optional[np.ndarray] = None
         self._pairs: List[Tuple[Any, Any]] = []
         self._vlad: Dict[Any, int] = {}   # image -> length of its resident VLAD descriptor (0: it has none)
+        self._bow: Dict[Any, int] = {}    # image -> length of its resident BoW histogram (0: it has none)
+        self._words: Dict[Any, int] = {}  # image -> vocabulary size of its resident first words (0: it has none)
         if kernel:
             _lib.check(self._m.L.osfm_matcher_set_kernel(self._m.h, int(kernel)))
 
@@ -152,6 +154,8 @@ class PairMatcher:
         self._ids[key] = out.value
         self._n[key] = d.shape[0]
         self._vlad.pop(key, None)
+        self._bow.pop(key, None)
+        self._words.pop(key, None)
 
     def add_many(self, items: Sequence[Tuple[Any, np.ndarray]], uint8_is_l2: bool = False) -> None:
         """Upload many images' descriptors with a single host synchronisation (same dtype and
@@ -180,6 +184,8 @@ class PairMatcher:
             self._ids[k] = int(i)
             self._n[k] = d.shape[0]
             self._vlad.pop(k, None)
+            self._bow.pop(k, None)
+            self._words.pop(k, None)
 
     def clear(self) -> None:
         """Drop every resident descriptor set (device memory stays with the matcher for reuse)."""
@@ -187,6 +193,8 @@ class PairMatcher:
         self._ids.clear()
         self._n.clear()
         self._vlad.clear()
+        self._bow.clear()
+        self._words.clear()
 
     # -- VLAD (opensfm/vlad.py, pairs_selection.vlad_histograms) ---------------------------------------------------
     def compute_vlad(self, keys: Iterable[Any], centers: np.ndarray) -> List[Any]:
@@ -257,6 +265,88 @@ class PairMatcher:
 
         _lib.check(self._m.L.osfm_matcher_vlad_select(self._m.h, nref, ptr(ri), ncand, ptr(ci), ptr(bits), ptr(lab),
                                                       int(k), ptr(offs), ptr(cols), ptr(dist)))
+        return [(cols[offs[r]:offs[r + 1]], dist[offs[r]:offs[r + 1]]) for r in range(nref)]
+
+    # -- BoW (opensfm/bow.py, pairs_selection.load_histograms) ----------------------------------------------------
+    def compute_words(self, keys: Iterable[Any], bows: Any, k: int) -> Dict[Any, np.ndarray]:
+        """bows.map_to_words(descriptors, k, "BRUTEFORCE") of every resident image in `keys`: {key: int32 n x min(k,
+        nwords)}, the k nearest words of `bows` (a `opensfm_b200.bow.BagOfWords`) exactly as cv2 knnMatch ranks them.
+        The first word of every feature stays on the device for `bow_histograms`.  Hamming images and images of
+        another descriptor length are left out."""
+        keys = list(dict.fromkeys(keys))
+        vocab = bows.words32
+        nw = vocab.shape[0]
+        kout = min(int(k), nw)
+        ids = np.array([self._ids[key] for key in keys], dtype=np.int32)
+        valid = np.zeros(len(keys), dtype=np.int32)
+        offs = np.zeros(len(keys) + 1, dtype=np.int64)
+        words = np.empty((max(sum(self._n[key] for key in keys), 1), kout), dtype=np.int32)
+        for key in keys:
+            self._words.pop(key, None)
+            self._bow.pop(key, None)
+        _lib.check(self._m.L.osfm_matcher_bow_words(self._m.h, len(keys), ids.ctypes.data_as(ctypes.c_void_p),
+                                                    vocab.ctypes.data_as(ctypes.c_void_p), nw, vocab.shape[1], int(k),
+                                                    offs.ctypes.data_as(ctypes.c_void_p),
+                                                    words.ctypes.data_as(ctypes.c_void_p),
+                                                    valid.ctypes.data_as(ctypes.c_void_p)))
+        out: Dict[Any, np.ndarray] = {}
+        for i, (key, v) in enumerate(zip(keys, valid)):
+            self._words[key] = nw if v else 0
+            if v:
+                out[key] = words[offs[i]:offs[i + 1]].copy()
+        return out
+
+    def bow_histograms(self, keys: Iterable[Any], bows: Any) -> Dict[Any, np.ndarray]:
+        """pairs_selection.load_histograms (pairs_selection.py:712-727) for resident images whose words
+        `compute_words` computed: {key: float64 histogram of the first words}, bit for bit BagOfWords.histogram;
+        images with 8 or fewer words are left out.  The histograms stay on the device for
+        `pairs_selection.match_candidates_with_bow`."""
+        keys = list(dict.fromkeys(keys))
+        for key in keys:
+            if self._words.get(key) is None:
+                raise ValueError("image %r has no words: run PairMatcher.compute_words on it first" % (key,))
+        w = np.ascontiguousarray(bows.weights, dtype=np.float64)
+        ids = np.array([self._ids[key] for key in keys], dtype=np.int32)
+        valid = np.zeros(len(keys), dtype=np.int32)
+        _lib.check(self._m.L.osfm_matcher_bow_histograms(self._m.h, len(keys), ids.ctypes.data_as(ctypes.c_void_p),
+                                                         w.ctypes.data_as(ctypes.c_void_p), len(w),
+                                                         valid.ctypes.data_as(ctypes.c_void_p)))
+        out: Dict[Any, np.ndarray] = {}
+        for key, v in zip(keys, valid):
+            self._bow[key] = len(w) if v else 0
+            if v:
+                h = np.empty(len(w), dtype=np.float64)
+                _lib.check(self._m.L.osfm_matcher_bow_get(self._m.h, self._ids[key], h.ctypes.data_as(ctypes.c_void_p)))
+                out[key] = h
+        return out
+
+    def has_bow(self, key: Any) -> Optional[bool]:
+        """None if `bow_histograms` never ran on the image, else whether it has a BoW histogram."""
+        return None if key not in self._bow else bool(self._bow[key])
+
+    def bow_select(self, refs: Sequence[Any], cands: Sequence[Any], k: int, cand_order: Optional[np.ndarray] = None,
+                   labels: Optional[np.ndarray] = None) -> List[Tuple[np.ndarray, np.ndarray]]:
+        """Per reference image, the columns of `cands` (and their BoW distances) that osfm_matcher_bow_select keeps:
+        the k nearest by (distance, column), per camera group when `labels` (len(refs) + len(cands) ints) is given.
+        cand_order: None or a len(refs) x len(cands) int array, the position of each candidate in the reference's own
+        candidate list (-1: not a candidate), which then breaks ties instead of the column."""
+        nref, ncand = len(refs), len(cands)
+        ri = np.array([self._ids[r] for r in refs], dtype=np.int32)
+        ci = np.array([self._ids[c] for c in cands], dtype=np.int32)
+        order = None if cand_order is None else np.ascontiguousarray(cand_order, dtype=np.int32).reshape(nref, ncand)
+        lab = None if labels is None else np.ascontiguousarray(labels, dtype=np.int32)
+        if lab is not None and lab.shape != (nref + ncand,):
+            raise ValueError("labels must hold len(refs) + len(cands) ints")
+        cap = max(nref * min(k, ncand) * (2 if lab is not None else 1), 1)
+        offs = np.zeros(nref + 1, dtype=np.int64)
+        cols = np.empty(cap, dtype=np.int32)
+        dist = np.empty(cap, dtype=np.float64)
+
+        def ptr(a):
+            return None if a is None else a.ctypes.data_as(ctypes.c_void_p)
+
+        _lib.check(self._m.L.osfm_matcher_bow_select(self._m.h, nref, ptr(ri), ncand, ptr(ci), ptr(order), ptr(lab),
+                                                     int(k), ptr(offs), ptr(cols), ptr(dist)))
         return [(cols[offs[r]:offs[r + 1]], dist[offs[r]:offs[r + 1]]) for r in range(nref)]
 
     def submit(self, pairs: Sequence[Tuple[Any, Any]], lowes_ratio: float, symmetric: bool = True) -> None:

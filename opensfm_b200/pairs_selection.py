@@ -1,11 +1,14 @@
-"""VLAD pair selection on the GPU: the `opensfm.vlad` / `opensfm.pairs_selection` names this engine replaces.
+"""VLAD and BoW pair selection on the GPU: the `opensfm.vlad` / `opensfm.pairs_selection` names this engine replaces.
 
     unnormalized_vlad(features, centers)                       opensfm/vlad.py
     PairMatcher.vlad_histograms(keys, centers)                 pairs_selection.py:732-745 (vlad_histograms)
     match_candidates_with_vlad(matcher, images_ref, ...)       pairs_selection.py:351-392, 471-490, 764-795
+    PairMatcher.compute_words / bow_histograms(keys, bows)     features_processing.py:269-336, pairs_selection.py:712-727
+    bow_distances(image, other_images, histograms)             pairs_selection.py:690-708
+    match_candidates_with_bow(matcher, images_ref, ...)        pairs_selection.py:281-348, 471-490, 764-795
 
 The VLAD descriptors are computed from the descriptor sets a `PairMatcher` already holds on the device and stay
-there; the all-pairs distances and the neighbour selection run on the device too, so only the selected pairs come
+there (likewise the BoW words and histograms); the all-pairs distances and the neighbour selection run on the device too, so only the selected pairs come
 back.  The selected pairs go straight into `PairMatcher.match_pairs` on the same matcher.  GPS preemption
 (`preempt_candidates`) needs the dataset's topocentric reference and stays with the caller.
 """
@@ -91,6 +94,70 @@ def match_candidates_with_vlad(matcher: PairMatcher, images_ref: Sequence[Any], 
         labels = np.array([names.setdefault(exifs[im]["camera"], len(names)) for im in list(refs) + cands], dtype=np.int32)
     pairs: Dict[Tuple[Any, Any], float] = {}
     for im, (cols, dist) in zip(refs, matcher.vlad_select(refs, cands, max_neighbors, mask, labels)):
+        for j, d in zip(cols.tolist(), dist.tolist()):
+            pairs[sorted_pair(im, cands[j])] = d
+    return pairs
+
+
+def bow_distances(image: Any, other_images: Sequence[Any], histograms: Dict[Any, np.ndarray], device: int = 0):
+    """pairs_selection.bow_distances: (image, distances, other images) with the candidates that have a histogram, in
+    the order given, `image` itself skipped; each distance np.fabs(h - h2).sum() bit for bit."""
+    from .bow import bow_distance_rows
+
+    if image not in histograms:
+        return image, [], []
+    others = [o for o in other_images if o != image and o in histograms]
+    if not others:
+        return image, [], []
+    d = bow_distance_rows(np.stack([histograms[image]] + [histograms[o] for o in others]), 0, device)
+    return image, d[1:].tolist(), others
+
+
+def match_candidates_with_bow(matcher: PairMatcher, images_ref: Sequence[Any], images_cand: Sequence[Any],
+                              exifs: Dict[Any, Any], max_neighbors: int, enforce_other_cameras: bool,
+                              candidates: Optional[Dict[Any, Sequence[Any]]] = None) -> Dict[Tuple[Any, Any], float]:
+    """pairs_selection.match_candidates_with_bow: {sorted pair: BoW distance} of every reference image with its
+    `max_neighbors` nearest candidates (and as many of other cameras when `enforce_other_cameras`; cameras are
+    `exifs[image]["camera"]`).
+
+    `matcher` holds the images' descriptors and their BoW histograms (`PairMatcher.compute_words`, then
+    `bow_histograms`); images without a histogram (8 or fewer words) are skipped, as the reference skips them.
+    `candidates`: {reference image: candidate images}, the first value `preempt_candidates` returns.  None means
+    every reference image against every candidate image; an empty dict gives no pairs, as the reference has no
+    fallback there.
+
+    Distances are the reference's np.fabs(h - h2).sum(), bit for bit.  Each reference's candidates keep the order
+    given, and a tie goes to the earlier candidate (the reference's unstable np.argsort leaves it open); a candidate
+    listed twice for one reference counts once."""
+    if max_neighbors <= 0:
+        return {}
+
+    def has(im):
+        state = matcher.has_bow(im)
+        if state is None:
+            raise ValueError("image %r has no BoW state: run PairMatcher.bow_histograms on it first" % (im,))
+        return state
+
+    order = None
+    if candidates is None:
+        refs = [im for im in dict.fromkeys(images_ref) if has(im)]
+        cands = [c for c in dict.fromkeys(images_cand) if has(c)]
+    else:
+        refs = [im for im in candidates if has(im)]
+        lists = [[c for c in dict.fromkeys(candidates[im]) if has(c)] for im in refs]
+        cands = list(dict.fromkeys(c for lst in lists for c in lst))
+        col = {c: j for j, c in enumerate(cands)}
+        order = np.full((len(refs), len(cands)), -1, dtype=np.int32)
+        for r, lst in enumerate(lists):
+            order[r, [col[c] for c in lst]] = np.arange(len(lst), dtype=np.int32)
+    if not refs or not cands:
+        return {}
+    labels = None
+    if enforce_other_cameras:
+        names: Dict[Any, int] = {}
+        labels = np.array([names.setdefault(exifs[im]["camera"], len(names)) for im in list(refs) + cands], dtype=np.int32)
+    pairs: Dict[Tuple[Any, Any], float] = {}
+    for im, (cols, dist) in zip(refs, matcher.bow_select(refs, cands, max_neighbors, order, labels)):
         for j, d in zip(cols.tolist(), dist.tolist()):
             pairs[sorted_pair(im, cands[j])] = d
     return pairs

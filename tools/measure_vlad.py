@@ -103,7 +103,7 @@ def main():
             torch.cuda.synchronize()
         per = {}
         for ev in prof.events():
-            m = re.search(r"vlad_\w+_kernel", ev.name)
+            m = re.search(r"(vlad_\w+|neighbor_select)_kernel", ev.name)
             if ev.device_type == torch.autograd.DeviceType.CUDA and m:
                 per[m.group(0)] = per.get(m.group(0), 0.0) + ev.device_time / 1e3 / args.reps
         return {"total": sum(per.values()), "kernels": per}
