@@ -11,6 +11,8 @@
  *          (opensfm/src/bundle/bundle_adjuster.h:178-299,
  *           opensfm/src/bundle/src/bundle_adjuster.cc) behind pybundle /
  *          sfm::BAHelpers (opensfm/src/sfm/src/ba_helpers.cc:117,408,581).
+ * and, between them, TRACKS: linking matches into tracks, replacing
+ *          tracking.create_tracks_manager (opensfm/tracking.py:72-150).
  *
  * There is no CPU fallback: every call needs a CUDA device (H100, sm_90a).
  */
@@ -393,6 +395,48 @@ enum {
 int osfm_ba_get_covariances(osfm_ba* ba, int* valid, int* status, double* out);
 /* Device time of the last covariance pass (CUDA events): the whole pass and the Cholesky of the reduced system. */
 int osfm_ba_get_covariance_timing(osfm_ba* ba, double* pass_ms, double* cholesky_ms);
+
+/* ------------------------------------------------------------------------
+ * TRACKS
+ * ---------------------------------------------------------------------- */
+typedef struct osfm_tracks osfm_tracks;
+
+/* Links pair matches into tracks: tracking.create_tracks_manager (opensfm/tracking.py:72-150) and, for all image
+ * pairs at once, TracksManager::GetAllPairsConnectivity / GetAllCommonObservations (tracks_manager.cc:285-350).
+ * A handle owns one CUDA stream and its workspaces on `device`; they are reused from call to call. */
+int osfm_tracks_create(int device, osfm_tracks** out);
+int osfm_tracks_destroy(osfm_tracks* t);
+/* Connected components of the graph whose nodes are features and whose edges are match rows, filtered like
+ * _good_track (tracking.py:238-244): at least min_length features and no two of one image.
+ * num_features[i] = features of image i; has_features[i] = 0 for an image that occurs in matches but has no
+ * feature file: its features count in the filter and are left out of the output (tracking.py:98 vs :106).  Pair p
+ * owns rows [match_start[p], match_start[p + 1]) of matches (int32 x 2: feature in pair_a[p], feature in
+ * pair_b[p]); a pair may be listed several times and in either order.  Tracks with at least one observation to
+ * output are numbered 0 .. T - 1 by their smallest (image, feature), so the result does not depend on the order of
+ * pairs or rows.  Returns T and the number of observations N.  Fails with OSFM_ERR_RUNTIME, naming the first
+ * offending row, if an image or feature index is out of range, and with OSFM_ERR_ARG for more than 2^31 - 1
+ * features or match rows in all. */
+int osfm_tracks_build(osfm_tracks* t, int num_images, const int32_t* num_features, const uint8_t* has_features,
+                      int64_t num_pairs, const int32_t* pair_a, const int32_t* pair_b, const int64_t* match_start,
+                      const int32_t* matches, int min_length, int64_t* num_tracks, int64_t* num_observations);
+/* The last build's observations sorted by (track, image): obs_track / obs_image / obs_feature have N entries,
+ * track t owns rows [track_start[t], track_start[t + 1]) (T + 1 entries). */
+int osfm_tracks_get(osfm_tracks* t, int32_t* obs_track, int32_t* obs_image, int32_t* obs_feature,
+                    int64_t* track_start);
+/* For the last build, every image pair a < b with a track in common and the observations they share.  Returns the
+ * number of such pairs Q and the total number of shared tracks R over all pairs (a track of L observations counts
+ * L (L - 1) / 2 times).  R is known before the pair lists are built; if the device cannot hold them (about 33 R
+ * bytes) the call fails with OSFM_ERR_CUDA and a message giving R, and the handle stays usable. */
+int osfm_tracks_common(osfm_tracks* t, int64_t* num_pairs, int64_t* num_common);
+/* Pairs ascending by (pair_a, pair_b), Q entries; pair q owns rows [pair_start[q], pair_start[q + 1]) (Q + 1
+ * entries; the run length is the pair's connectivity) of common_obs_a / common_obs_b (R entries): rows of
+ * osfm_tracks_get's arrays, the observation in pair_a[q] and the one of the same track in pair_b[q], tracks
+ * ascending inside a pair. */
+int osfm_tracks_get_common(osfm_tracks* t, int32_t* pair_a, int32_t* pair_b, int64_t* pair_start,
+                           int64_t* common_obs_a, int64_t* common_obs_b);
+/* Device time of the last osfm_tracks_build (kernels, sorts and scans, after the uploads) and the last
+ * osfm_tracks_common (CUDA events on the handle's stream). */
+int osfm_tracks_last_device_ms(osfm_tracks* t, float* ms_build, float* ms_common);
 
 #ifdef __cplusplus
 }

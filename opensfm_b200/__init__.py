@@ -1,0 +1,1 @@
+from . import tracking  # noqa: F401

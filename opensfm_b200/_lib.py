@@ -135,6 +135,14 @@ SIGNATURES = {
     "osfm_ba_set_compute_covariances": (c_int, [c_void_p, c_int]),
     "osfm_ba_get_covariances": (c_int, [c_void_p, POINTER(c_int), POINTER(c_int), c_void_p]),
     "osfm_ba_get_covariance_timing": (c_int, [c_void_p, POINTER(c_double), POINTER(c_double)]),
+    "osfm_tracks_create": (c_int, [c_int, POINTER(c_void_p)]),
+    "osfm_tracks_destroy": (c_int, [c_void_p]),
+    "osfm_tracks_build": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_void_p,
+                                  c_int, POINTER(c_int64), POINTER(c_int64)]),
+    "osfm_tracks_get": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "osfm_tracks_common": (c_int, [c_void_p, POINTER(c_int64), POINTER(c_int64)]),
+    "osfm_tracks_get_common": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "osfm_tracks_last_device_ms": (c_int, [c_void_p, POINTER(c_float), POINTER(c_float)]),
 }
 
 _lib = None

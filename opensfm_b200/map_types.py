@@ -48,6 +48,15 @@ class ShotMeasurements:
         self.capture_time = Measurement()
 
 
+class Depth:
+    """pymap.Depth: a depth prior carried by an observation (value, its standard deviation, radial or along z)."""
+
+    def __init__(self, value: float, std_deviation: float, is_radial: bool = True):
+        self.value = float(value)
+        self.std_deviation = float(std_deviation)
+        self.is_radial = bool(is_radial)
+
+
 class Observation:
     """pymap.Observation: normalised image point, scale (its std-deviation in the bundle), optional depth prior."""
 
