@@ -438,6 +438,40 @@ int osfm_tracks_get_common(osfm_tracks* t, int32_t* pair_a, int32_t* pair_b, int
  * osfm_tracks_common (CUDA events on the handle's stream). */
 int osfm_tracks_last_device_ms(osfm_tracks* t, float* ms_build, float* ms_common);
 
+/* ------------------------------------------------------------------------
+ * ROTATION-ONLY RANSAC OF IMAGE PAIRS
+ * ---------------------------------------------------------------------- */
+typedef struct osfm_rotransac osfm_rotransac;
+
+/* Ranks image pairs for the reconstruction bootstrap: pyrobust's ransac_relative_rotation with RANSAC scoring, as
+ * compute_image_pairs runs it (opensfm/reconstruction.py:208-244), and the chord inliers of its rotation, for many
+ * pairs at once.  The rules, including the one deliberate difference (a 3-row sample takes the proper Kabsch
+ * rotation), are stated in oracle/rotation_ransac_oracle.py.  A handle owns one CUDA stream, its workspaces on
+ * `device` and the shared sample stream of mt19937(42). */
+int osfm_rotransac_create(int device, osfm_rotransac** out);
+int osfm_rotransac_destroy(osfm_rotransac* h);
+/* bearings: num_bearings x 3 fp64 unit vectors.  Pair p owns rows [pair_start[p], pair_start[p + 1]) (pair_start[0]
+ * = 0); row r pairs bearing row_a[r] of the first image with bearing row_b[r] of the second.  threshold is the
+ * angle of compute_image_pairs (4 * five_point_algo_threshold): RANSAC inliers have |1 - (M b1) . b2| below
+ * 1 - cos(threshold), chord inliers ||R b2 - b1|| below threshold with R = lo_model^T.  iterations >= 1 (the
+ * reference passes 1000).  Outputs: lo_model (9 per pair, row-major), the RANSAC inlier count and the chord inlier
+ * count of every pair, and the chord inlier mask of every row.  A pair of fewer than 3 rows, or a row naming a
+ * bearing outside [0, num_bearings), fails with OSFM_ERR_ARG naming it. */
+int osfm_rotransac_run(osfm_rotransac* h, int64_t num_bearings, const double* bearings, int64_t num_pairs,
+                       const int64_t* pair_start, const int64_t* row_a, const int64_t* row_b, double threshold,
+                       int iterations, double* lo_model, int32_t* ransac_inliers, int32_t* chord_inliers,
+                       uint8_t* chord_mask);
+/* Device time of the last osfm_rotransac_run (CUDA events around its kernels, after the uploads). */
+int osfm_rotransac_last_device_ms(osfm_rotransac* h, float* ms);
+/* Test hooks.  The generator outputs kept on the device (65536 unless set; a pair that uses them all continues from
+ * the generator state saved after them).  Tracing: with capacity > 0 the next runs record, per pair, every sample
+ * index drawn (minimal samples: rows; local optimisation: positions in the best inlier list), in order, up to
+ * capacity of them; get_trace returns, per pair, how many were drawn, how many generator outputs were consumed,
+ * and the indices (num_pairs x capacity). */
+int osfm_rotransac_set_stream_prefix(osfm_rotransac* h, int64_t length);
+int osfm_rotransac_set_trace(osfm_rotransac* h, int capacity);
+int osfm_rotransac_get_trace(osfm_rotransac* h, int32_t* count, int64_t* stream_used, int32_t* indices);
+
 #ifdef __cplusplus
 }
 #endif

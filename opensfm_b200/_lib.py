@@ -143,6 +143,14 @@ SIGNATURES = {
     "osfm_tracks_common": (c_int, [c_void_p, POINTER(c_int64), POINTER(c_int64)]),
     "osfm_tracks_get_common": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "osfm_tracks_last_device_ms": (c_int, [c_void_p, POINTER(c_float), POINTER(c_float)]),
+    "osfm_rotransac_create": (c_int, [c_int, POINTER(c_void_p)]),
+    "osfm_rotransac_destroy": (c_int, [c_void_p]),
+    "osfm_rotransac_run": (c_int, [c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_double, c_int,
+                                   c_void_p, c_void_p, c_void_p, c_void_p]),
+    "osfm_rotransac_last_device_ms": (c_int, [c_void_p, POINTER(c_float)]),
+    "osfm_rotransac_set_stream_prefix": (c_int, [c_void_p, c_int64]),
+    "osfm_rotransac_set_trace": (c_int, [c_void_p, c_int]),
+    "osfm_rotransac_get_trace": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p]),
 }
 
 _lib = None

@@ -15,6 +15,15 @@ of `opensfm_b200.bundle.BundleAdjuster`:
 `reconstruction` is duck-typed: `opensfm.types.Reconstruction` or `opensfm_b200.map_types.Reconstruction` (same
 attribute names).  To re-point OpenSfM:  `opensfm.reconstruction.bundle = opensfm_b200.reconstruction.bundle`, etc.
 (INTEGRATION.md §2).  Every call runs on the GPU; there is no CPU fallback.
+
+The ranking of image pairs that `incremental_reconstruction` bootstraps from is here too, batched over all pairs
+by the rotation-only RANSAC of opensfm_b200/rotation_ransac.py:
+
+  compute_image_pairs                     reconstruction.py:208-244
+  compute_image_pairs_sequential          reconstruction.py:1684-1709
+  two_view_reconstruction_rotation_only   reconstruction.py:387-412
+  compute_image_pairs_from_tracks         this engine's fast path: bearings once per image, rows from the device's
+                                          common-track lists
 """
 from __future__ import annotations
 
@@ -25,6 +34,7 @@ from typing import Any, Dict, Iterable, List, Optional, Sequence, Set, Tuple
 import numpy as np
 
 from . import bundle as _bundle
+from . import rotation_ransac as _rr
 from . import types as T
 
 logger = logging.getLogger(__name__)
@@ -532,3 +542,113 @@ def remove_outliers(reconstruction, config: Dict[str, Any], points=None) -> int:
                 reconstruction.map.remove_landmark(lm)
     logger.info("Removed outliers: {}".format(len(outliers)))
     return len(outliers)
+
+
+# ---------------------------------------------------------------------------------------------------------------
+# image pairs for the bootstrap (reconstruction.py:193-244, 377-412, 1668-1709)
+# ---------------------------------------------------------------------------------------------------------------
+def pairwise_reconstructability(common_tracks: int, rotation_inliers: int) -> float:
+    """Likeliness of an image pair giving a good initial reconstruction: the outliers of the rotation-only model if
+    they are at least 30 % of the common tracks, else 0."""
+    outliers = common_tracks - rotation_inliers
+    outlier_ratio = float(outliers) / common_tracks
+    if outlier_ratio >= 0.3:
+        return outliers
+    return 0
+
+
+def two_view_reconstruction_rotation_only(p1: np.ndarray, p2: np.ndarray, camera1, camera2,
+                                          threshold: float) -> Tuple[np.ndarray, np.ndarray]:
+    """(angle-axis of R^T, chord inlier rows) of the rotation-only RANSAC of one pair, R b2 ~ b1."""
+    import cv2
+
+    b1 = camera1.pixel_bearing_many(p1)
+    b2 = camera2.pixel_bearing_many(p2)
+    res = _rr.ransac_pairs_lists([b1], [b2], threshold)
+    R = res.rotations()[0]
+    return cv2.Rodrigues(R.T)[0].ravel(), res.inliers(0)
+
+
+def _ranked_by_argsort(keys: List[Tuple[Any, Any]], scores: List[int]) -> List[Tuple[Any, Any]]:
+    """compute_image_pairs' order: non-zero scores, np.argsort(-score) (numpy's default, unstable sort)."""
+    pairs = [k for k, r in zip(keys, scores) if r > 0]
+    score = [r for r in scores if r > 0]
+    order = np.argsort(-np.array(score))
+    return [pairs[o] for o in order]
+
+
+def compute_image_pairs(track_dict: Dict[Tuple[str, str], Any], data) -> List[Tuple[str, str]]:
+    """All matched image pairs sorted by reconstructability.  track_dict: {(im1, im2): (tracks, p1, p2)} as
+    tracking.all_common_tracks_with_features returns; bearings from the cameras' own pixel_bearing_many."""
+    cameras = data.load_camera_models()
+    threshold = 4 * data.config["five_point_algo_threshold"]
+    keys, b1s, b2s = [], [], []
+    for (im1, im2), (_, p1, p2) in track_dict.items():
+        camera1 = cameras[data.load_exif(im1)["camera"]]
+        camera2 = cameras[data.load_exif(im2)["camera"]]
+        keys.append((im1, im2))
+        b1s.append(camera1.pixel_bearing_many(p1))
+        b2s.append(camera2.pixel_bearing_many(p2))
+    if not keys:
+        return []
+    res = _rr.ransac_pairs_lists(b1s, b2s, threshold)
+    return _ranked_by_argsort(keys, res.scores())
+
+
+def _get_common_feature_arrays(tracks_manager, im1: Any, im2: Any) -> Tuple[np.ndarray, np.ndarray]:
+    """Points of im1 and im2 in their common tracks: from the arrays of this engine's TracksManager, else from
+    get_all_common_observations."""
+    if hasattr(tracks_manager, "_pair_rows"):
+        r1, r2 = tracks_manager._pair_rows(im1, im2)
+        xy = tracks_manager._points()[0]
+        return xy[r1], xy[r2]
+    obs = tracks_manager.get_all_common_observations(im1, im2)
+    return np.array([o1.point for _, o1, _ in obs]), np.array([o2.point for _, _, o2 in obs])
+
+
+def compute_image_pairs_sequential(data, tracks_manager, min_common: int = 50) -> List[Tuple[str, str]]:
+    """Image pairs with at least min_common common tracks sorted by reconstructability, in the reference's
+    connectivity order and with its stable sort; all pairs go to the device in one batch."""
+    cameras = data.load_camera_models()
+    threshold = 4 * data.config["five_point_algo_threshold"]
+    keys, b1s, b2s = [], [], []
+    for (im1, im2), size in tracks_manager.get_all_pairs_connectivity().items():
+        if size < min_common:
+            continue
+        features1, features2 = _get_common_feature_arrays(tracks_manager, im1, im2)
+        keys.append((im1, im2))
+        b1s.append(cameras[data.load_exif(im1)["camera"]].pixel_bearing_many(features1))
+        b2s.append(cameras[data.load_exif(im2)["camera"]].pixel_bearing_many(features2))
+    if not keys:
+        return []
+    res = _rr.ransac_pairs_lists(b1s, b2s, threshold)
+    results = [(im1, im2, r) for (im1, im2), r in zip(keys, res.scores()) if r > 0]
+    results.sort(key=lambda x: x[2], reverse=True)
+    return [(im1, im2) for im1, im2, _ in results]
+
+
+def compute_image_pairs_from_tracks(tracks_manager, cameras_by_image: Dict[Any, Any], config: Dict[str, Any],
+                                    min_common: int = 50) -> List[Tuple[Any, Any]]:
+    """compute_image_pairs(tracking.all_common_tracks_with_features(tracks_manager, min_common), data) for this
+    engine's TracksManager, without the per-pair lists: pixel_bearing_many runs once per image over that image's
+    observations, and the rows come from the device's common-track lists.  cameras_by_image: {image: camera}."""
+    pa, pb, ps, ca, cb = tracks_manager._common_arrays()
+    kept = np.nonzero(np.diff(ps) >= min_common)[0]
+    if not len(kept):
+        return []
+    lens = np.diff(ps)[kept]
+    pair_start = np.zeros(len(kept) + 1, dtype=np.int64)
+    np.cumsum(lens, out=pair_start[1:])
+    src = np.repeat(ps[kept] - pair_start[:-1], lens) + np.arange(pair_start[-1], dtype=np.int64)
+    row_a, row_b = ca[src], cb[src]
+
+    order, start = tracks_manager._shot_order()
+    xy = tracks_manager._points()[0]
+    bearings = np.zeros((len(xy), 3), dtype=np.float64)
+    images = tracks_manager.images
+    for i in np.union1d(pa[kept], pb[kept]).tolist():
+        rows = order[start[i]:start[i + 1]]
+        bearings[rows] = cameras_by_image[images[i]].pixel_bearing_many(xy[rows])
+    res = _rr.ransac_pairs(bearings, pair_start, row_a, row_b, 4 * config["five_point_algo_threshold"])
+    keys = [(images[a], images[b]) for a, b in zip(pa[kept].tolist(), pb[kept].tolist())]
+    return _ranked_by_argsort(keys, res.scores())
