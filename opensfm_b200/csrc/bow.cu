@@ -17,7 +17,6 @@
 // so histograms and distances are the reference's bit for bit.
 #include <cfloat>
 #include <cmath>
-#include <mutex>
 #include <vector>
 
 #include "common.cuh"
@@ -312,17 +311,17 @@ __global__ void __launch_bounds__(256)
   }
 }
 
-}  // namespace
-
 // numpy's pairwise order for a vector of length n: leaves (start, length) left to right and the post-order program
 // (i >= 0: push leaf i's sum, -1: add the two partial sums on top); depth = most partial sums alive at once.
+// On the device: leaves | program, `bytes` in all.
 struct PairwisePlan {
   std::vector<int2> leaves;
   std::vector<int> prog;
   int depth = 0;
+  size_t o_prog = 0, bytes = 0;
 };
 
-static PairwisePlan pairwise_plan(long long n) {
+PairwisePlan pairwise_plan(long long n) {
   PairwisePlan P;
   int sp = 0;
   auto rec = [&](auto&& self, long long start, long long m) -> void {
@@ -341,42 +340,45 @@ static PairwisePlan pairwise_plan(long long n) {
   };
   rec(rec, 0, n);
   if (P.depth > BOW_MAX_DEPTH) throw ArgError("BoW vector too long");
+  P.o_prog = align256(sizeof(int2) * P.leaves.size());
+  P.bytes = P.o_prog + align256(sizeof(int) * P.prog.size());
   return P;
 }
 
-static void launch_bow_distances(cudaStream_t stream, const double* const* arows, int na, const double* const* brows,
-                                 int nb, const int2* leaves, const int* prog, int nprog, int depth, double* out,
-                                 long long ldo) {
-  const size_t smem = sizeof(double) * ((size_t)PW_LEAF * (BD_TM + BD_TN) + (size_t)depth * 512);
-  OSFM_CUDA(cudaFuncSetAttribute(bow_distance_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  dim3 grid((unsigned)((nb + BD_TN - 1) / BD_TN), (unsigned)((na + BD_TM - 1) / BD_TM));
-  bow_distance_kernel<<<grid, 256, smem, stream>>>(arows, na, brows, nb, leaves, prog, nprog, out, ldo);
-  OSFM_LAUNCH_CHECK();
+void upload_plan(Matcher& M, const PairwisePlan& P, uint8_t* dst) {
+  OSFM_CUDA(cudaMemcpyAsync(dst, P.leaves.data(), sizeof(int2) * P.leaves.size(), cudaMemcpyHostToDevice, M.stream));
+  OSFM_CUDA(cudaMemcpyAsync(dst + P.o_prog, P.prog.data(), sizeof(int) * P.prog.size(), cudaMemcpyHostToDevice, M.stream));
 }
 
-}  // namespace osfm
+// BoW rows for select_neighbors / distances_to_row (select_common.cuh): the histograms, with the pairwise plan of
+// their length in the table.
+struct BowRows {
+  using Row = double;
+  static constexpr int TILE_M = BD_TM;
+  PairwisePlan P;
+  static const SlabArray<double>& of(Matcher& M, int id, int len) {
+    return M.resident(id, &DescSet::bow_hist, len, "descriptor set has no BoW histogram (osfm_matcher_bow_histograms)",
+                      "BoW histograms of different lengths");
+  }
+  static const double* row(const SlabArray<double>& h) { return h.p; }
+  size_t table_bytes(int len) {
+    P = pairwise_plan(len);
+    return P.bytes;
+  }
+  void upload(Matcher& M, uint8_t* plan) { upload_plan(M, P, plan); }
+  void distances(Matcher& M, const uint8_t* plan, const double* const* arows, int na, const double* const* brows,
+                 int nb, int, double* out, long long ldo) {
+    const size_t smem = sizeof(double) * ((size_t)PW_LEAF * (BD_TM + BD_TN) + (size_t)P.depth * 512);
+    OSFM_CUDA(cudaFuncSetAttribute(bow_distance_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    dim3 grid((unsigned)((nb + BD_TN - 1) / BD_TN), (unsigned)((na + BD_TM - 1) / BD_TM));
+    bow_distance_kernel<<<grid, 256, smem, M.stream>>>(arows, na, brows, nb, reinterpret_cast<const int2*>(plan),
+                                                        reinterpret_cast<const int*>(plan + P.o_prog),
+                                                        (int)P.prog.size(), out, ldo);
+    OSFM_LAUNCH_CHECK();
+  }
+};
 
-struct osfm_matcher;   // defined in match.cu: { Matcher impl; std::mutex mu; }
-namespace osfm {
-Matcher& matcher_impl(osfm_matcher* m);
-std::mutex& matcher_mutex(osfm_matcher* m);
-
-static void release_bow_hist(Matcher& M, DescSet& s) {   // the caller has synchronised the stream
-  if (s.bow_hist) M.slab_release(s.bow_hist_slab, s.bow_hist, s.bow_hist_bytes);
-  s.bow_hist = nullptr;
-  s.bow_hist_slab = -1;
-  s.bow_len = 0;
-  s.bow_hist_bytes = 0;
-}
-
-static void release_bow(Matcher& M, DescSet& s) {
-  if (s.bow_words) M.slab_release(s.bow_words_slab, s.bow_words, s.bow_words_bytes);
-  s.bow_words = nullptr;
-  s.bow_words_slab = -1;
-  s.bow_nwords = 0;
-  s.bow_words_bytes = 0;
-  release_bow_hist(M, s);
-}
+}  // namespace
 
 static int padded_floats(int dim) { return (int)(((size_t)dim * 4 + 63) / 64 * 64 / 4); }   // match.cu add_async
 
@@ -398,11 +400,10 @@ static void bow_words_run(Matcher& M, int count, const int* set_ids, const float
     DescSet& s = M.sets[set_ids[i]];
     const bool valid = !s.u8 && s.dim == dim;
     out_valid[i] = valid;
-    release_bow(M, s);
+    M.release(s.bow_words);
+    M.release(s.bow_hist);
     if (valid) {
-      s.bow_words_bytes = sizeof(int) * (size_t)std::max(s.n, 1);
-      s.bow_words = static_cast<int*>(M.slab_alloc(s.bow_words_bytes, &s.bow_words_slab));
-      s.bow_nwords = nwords;
+      M.slab_new(s.bow_words, sizeof(int) * (size_t)std::max(s.n, 1), nwords);
       if (s.n > 0) {
         job_set.push_back(set_ids[i]);
         job_out.push_back(rows);
@@ -443,7 +444,7 @@ static void bow_words_run(Matcher& M, int count, const int* set_ids, const float
       if (j1 > j0 && brows + s.n > max_rows) break;
       BowJob b;
       b.f = static_cast<const float*>(s.data);   // float32 zero-padded rows for every non-Hamming set
-      b.first = s.bow_words;
+      b.first = s.bow_words.p;
       b.row0 = brows;
       b.n = s.n;
       jobs.push_back(b);
@@ -452,19 +453,20 @@ static void bow_words_run(Matcher& M, int count, const int* set_ids, const float
       brows += s.n;
       max_n = std::max(max_n, s.n);
     }
-    const size_t o_pre = (sizeof(BowJob) * jobs.size() + 255) / 256 * 256;
-    M.d_bow_tab.reserve(o_pre + sizeof(int) * prefix.size());
+    const size_t o_pre = align256(sizeof(BowJob) * jobs.size());
+    M.d_tab.reserve(o_pre + sizeof(int) * prefix.size());
     const size_t nl = (size_t)brows * nchunks * k;
-    const size_t o_idx = (sizeof(float) * nl + 255) / 256 * 256;
-    const size_t o_w = o_idx + (sizeof(int) * nl + 255) / 256 * 256;
-    M.d_bow_work.reserve(o_w + sizeof(int) * (size_t)brows * kout);
-    const BowJob* d_jobs = reinterpret_cast<const BowJob*>(M.d_bow_tab.p);
-    const int* d_pre = reinterpret_cast<const int*>(M.d_bow_tab.p + o_pre);
+    TableLayout work;
+    work.add(sizeof(float) * nl);
+    const size_t o_idx = work.add(sizeof(int) * nl), o_w = work.add(sizeof(int) * (size_t)brows * kout);
+    M.d_bow_work.reserve(work.size);
+    const BowJob* d_jobs = reinterpret_cast<const BowJob*>(M.d_tab.p);
+    const int* d_pre = reinterpret_cast<const int*>(M.d_tab.p + o_pre);
     float* d_key = reinterpret_cast<float*>(M.d_bow_work.p);
     int* d_idx = reinterpret_cast<int*>(M.d_bow_work.p + o_idx);
     int* d_words = reinterpret_cast<int*>(M.d_bow_work.p + o_w);
-    OSFM_CUDA(cudaMemcpyAsync(M.d_bow_tab.p, jobs.data(), sizeof(BowJob) * jobs.size(), cudaMemcpyHostToDevice, M.stream));
-    OSFM_CUDA(cudaMemcpyAsync(M.d_bow_tab.p + o_pre, prefix.data(), sizeof(int) * prefix.size(), cudaMemcpyHostToDevice,
+    OSFM_CUDA(cudaMemcpyAsync(M.d_tab.p, jobs.data(), sizeof(BowJob) * jobs.size(), cudaMemcpyHostToDevice, M.stream));
+    OSFM_CUDA(cudaMemcpyAsync(M.d_tab.p + o_pre, prefix.data(), sizeof(int) * prefix.size(), cudaMemcpyHostToDevice,
                               M.stream));
     bow_words_kernel<<<(unsigned)ctas, 256, smem, M.stream>>>(d_jobs, d_pre, (int)jobs.size(), M.d_bow_vocab.p, nwords, D,
                                                               nblk, k, nchunks, chunk_len, d_key, d_idx, M.d_bow_flags.p);
@@ -481,7 +483,10 @@ static void bow_words_run(Matcher& M, int count, const int* set_ids, const float
   int flags = 0;
   OSFM_CUDA(cudaMemcpy(&flags, M.d_bow_flags.p, sizeof(int), cudaMemcpyDeviceToHost));
   if (flags) {
-    for (int id : job_set) release_bow(M, M.sets[id]);
+    for (int id : job_set) {
+      M.release(M.sets[id].bow_words);
+      M.release(M.sets[id].bow_hist);
+    }
     throw ArgError("non-finite descriptor element in a BoW input set");
   }
 }
@@ -495,42 +500,23 @@ static void check_word_args(const float* vocab, int nwords, int dim, int k) {
     if (!std::isfinite(vocab[e])) throw ArgError("non-finite BoW vocabulary element");
 }
 
-static const DescSet& bow_hist_set(Matcher& M, int id, int len) {
-  auto it = M.sets.find(id);
-  if (it == M.sets.end()) throw ArgError("unknown descriptor set id");
-  if (!it->second.bow_hist) throw ArgError("descriptor set has no BoW histogram (osfm_matcher_bow_histograms)");
-  if (len >= 0 && it->second.bow_len != len) throw ArgError("BoW histograms of different lengths");
-  return it->second;
-}
-
-// plan tables on the device: leaves | program
-static void upload_plan(Matcher& M, const PairwisePlan& P, uint8_t* dst, size_t* o_prog) {
-  *o_prog = (sizeof(int2) * P.leaves.size() + 255) / 256 * 256;
-  OSFM_CUDA(cudaMemcpyAsync(dst, P.leaves.data(), sizeof(int2) * P.leaves.size(), cudaMemcpyHostToDevice, M.stream));
-  OSFM_CUDA(cudaMemcpyAsync(dst + *o_prog, P.prog.data(), sizeof(int) * P.prog.size(), cudaMemcpyHostToDevice, M.stream));
-}
-
-static size_t plan_bytes(const PairwisePlan& P) {
-  return (sizeof(int2) * P.leaves.size() + 255) / 256 * 256 + (sizeof(int) * P.prog.size() + 255) / 256 * 256;
-}
-
 // device tables (weights | plan | jobs) and one CTA per histogram
 static void launch_bow_histograms(Matcher& M, const std::vector<HistJob>& jobs, const double* weights, int nwords,
                                   const PairwisePlan& P) {
-  const size_t o_plan = (sizeof(double) * (size_t)nwords + 255) / 256 * 256;
-  const size_t o_jobs = o_plan + plan_bytes(P);
-  M.d_bow_tab.reserve(o_jobs + sizeof(HistJob) * jobs.size());
-  uint8_t* base = M.d_bow_tab.p;
-  size_t o_prog;
+  TableLayout tab;
+  tab.add(sizeof(double) * (size_t)nwords);
+  const size_t o_plan = tab.add(P.bytes), o_jobs = tab.add(sizeof(HistJob) * jobs.size());
+  M.d_tab.reserve(tab.size);
+  uint8_t* base = M.d_tab.p;
   OSFM_CUDA(cudaMemcpyAsync(base, weights, sizeof(double) * (size_t)nwords, cudaMemcpyHostToDevice, M.stream));
-  upload_plan(M, P, base + o_plan, &o_prog);
+  upload_plan(M, P, base + o_plan);
   OSFM_CUDA(cudaMemcpyAsync(base + o_jobs, jobs.data(), sizeof(HistJob) * jobs.size(), cudaMemcpyHostToDevice, M.stream));
   const size_t smem = sizeof(double) * P.leaves.size();
   OSFM_CUDA(cudaFuncSetAttribute(bow_histogram_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   bow_histogram_kernel<<<(unsigned)jobs.size(), 256, smem, M.stream>>>(
       reinterpret_cast<const HistJob*>(base + o_jobs), reinterpret_cast<const double*>(base), nwords,
       reinterpret_cast<const int2*>(base + o_plan), (int)P.leaves.size(),
-      reinterpret_cast<const int*>(base + o_plan + o_prog), (int)P.prog.size());
+      reinterpret_cast<const int*>(base + o_plan + P.o_prog), (int)P.prog.size());
   OSFM_LAUNCH_CHECK();
 }
 }  // namespace osfm
@@ -541,14 +527,11 @@ int osfm_matcher_bow_words(osfm_matcher* m, int count, const int* set_ids, const
                            int k, int64_t* out_offsets, int32_t* out_words, int* out_valid) {
   OSFM_API_BEGIN
   using namespace osfm;
-  if (!m) throw ArgError("null matcher");
+  MatcherGuard g(m);
   if (count < 0) throw ArgError("bad BoW set count");
   if (!out_offsets || (count > 0 && (!set_ids || !out_valid))) throw ArgError("null arrays");
   check_word_args(vocab, nwords, dim, k);
-  std::lock_guard<std::mutex> lock(matcher_mutex(m));
-  Matcher& M = matcher_impl(m);
-  OSFM_CUDA(cudaSetDevice(M.device));
-  bow_words_run(M, count, set_ids, vocab, nwords, dim, k, out_offsets, out_words, out_valid);
+  bow_words_run(g.M, count, set_ids, vocab, nwords, dim, k, out_offsets, out_words, out_valid);
   OSFM_API_END
 }
 
@@ -556,12 +539,10 @@ int osfm_bow_map_to_words(osfm_matcher* m, const float* desc, int n, int dim, co
                           int32_t* out) {
   OSFM_API_BEGIN
   using namespace osfm;
-  if (!m) throw ArgError("null matcher");
+  MatcherGuard g(m);
+  Matcher& M = g.M;
   if (n < 0 || (n > 0 && (!desc || !out))) throw ArgError("bad descriptor arguments");
   check_word_args(vocab, nwords, dim, k);
-  std::lock_guard<std::mutex> lock(matcher_mutex(m));
-  Matcher& M = matcher_impl(m);
-  OSFM_CUDA(cudaSetDevice(M.device));
   const int id = M.add(desc, n, dim, false);
   try {
     int64_t offs[2];
@@ -579,13 +560,11 @@ int osfm_matcher_bow_histograms(osfm_matcher* m, int count, const int* set_ids, 
                                 int* out_valid) {
   OSFM_API_BEGIN
   using namespace osfm;
-  if (!m) throw ArgError("null matcher");
+  MatcherGuard g(m);
+  Matcher& M = g.M;
   if (count < 0 || nwords <= 0) throw ArgError("bad BoW histogram sizes");
   if (!weights || (count > 0 && (!set_ids || !out_valid))) throw ArgError("null arrays");
   const PairwisePlan P = pairwise_plan(nwords);
-  std::lock_guard<std::mutex> lock(matcher_mutex(m));
-  Matcher& M = matcher_impl(m);
-  OSFM_CUDA(cudaSetDevice(M.device));
   for (int i = 0; i < count; ++i)
     if (!M.sets.count(set_ids[i])) throw ArgError("unknown descriptor set id");
   OSFM_CUDA(cudaStreamSynchronize(M.stream));   // earlier work may still read histograms released below
@@ -593,14 +572,12 @@ int osfm_matcher_bow_histograms(osfm_matcher* m, int count, const int* set_ids, 
   std::vector<HistJob> jobs;
   for (int i = 0; i < count; ++i) {
     DescSet& s = M.sets[set_ids[i]];
-    release_bow_hist(M, s);
-    const bool valid = s.bow_words && s.bow_nwords == nwords && s.n > 8;
+    M.release(s.bow_hist);
+    const bool valid = s.bow_words.p && s.bow_words.len == nwords && s.n > 8;
     out_valid[i] = valid;
     if (!valid) continue;
-    s.bow_hist_bytes = sizeof(double) * (size_t)nwords;
-    s.bow_hist = static_cast<double*>(M.slab_alloc(s.bow_hist_bytes, &s.bow_hist_slab));
-    s.bow_len = nwords;
-    jobs.push_back(HistJob{s.bow_words, s.bow_hist, s.n});
+    M.slab_new(s.bow_hist, sizeof(double) * (size_t)nwords, nwords);
+    jobs.push_back(HistJob{s.bow_words.p, s.bow_hist.p, s.n});
   }
   if (jobs.empty()) return OSFM_OK;
   launch_bow_histograms(M, jobs, weights, nwords, P);
@@ -611,18 +588,16 @@ int osfm_matcher_bow_histograms(osfm_matcher* m, int count, const int* set_ids, 
 int osfm_bow_histogram(osfm_matcher* m, const int32_t* words, int n, const double* weights, int nwords, double* out) {
   OSFM_API_BEGIN
   using namespace osfm;
-  if (!m) throw ArgError("null matcher");
+  MatcherGuard g(m);
+  Matcher& M = g.M;
   if (n < 0 || nwords <= 0 || !weights || !out || (n > 0 && !words)) throw ArgError("bad BoW histogram arguments");
   for (int i = 0; i < n; ++i)
     if (words[i] < 0 || words[i] >= nwords) throw ArgError("word index out of range");
   const PairwisePlan P = pairwise_plan(nwords);
-  std::lock_guard<std::mutex> lock(matcher_mutex(m));
-  Matcher& M = matcher_impl(m);
-  OSFM_CUDA(cudaSetDevice(M.device));
-  const size_t b_w = (sizeof(int) * (size_t)std::max(n, 1) + 255) / 256 * 256;
-  M.staging.reserve(b_w + sizeof(double) * (size_t)nwords);
+  const size_t o_h = align256(sizeof(int) * (size_t)std::max(n, 1));
+  M.staging.reserve(o_h + sizeof(double) * (size_t)nwords);
   int* d_w = reinterpret_cast<int*>(M.staging.p);
-  double* d_h = reinterpret_cast<double*>(M.staging.p + b_w);
+  double* d_h = reinterpret_cast<double*>(M.staging.p + o_h);
   if (n > 0) OSFM_CUDA(cudaMemcpyAsync(d_w, words, sizeof(int) * (size_t)n, cudaMemcpyHostToDevice, M.stream));
   launch_bow_histograms(M, {HistJob{d_w, d_h, n}}, weights, nwords, P);
   OSFM_CUDA(cudaMemcpyAsync(out, d_h, sizeof(double) * (size_t)nwords, cudaMemcpyDeviceToHost, M.stream));
@@ -634,137 +609,32 @@ int osfm_matcher_bow_get(osfm_matcher* m, int set_id, double* out) {
   OSFM_API_BEGIN
   using namespace osfm;
   if (!m || !out) throw ArgError("null arguments");
-  std::lock_guard<std::mutex> lock(matcher_mutex(m));
-  Matcher& M = matcher_impl(m);
-  OSFM_CUDA(cudaSetDevice(M.device));
-  const DescSet& s = bow_hist_set(M, set_id, -1);
-  OSFM_CUDA(cudaMemcpyAsync(out, s.bow_hist, sizeof(double) * (size_t)s.bow_len, cudaMemcpyDeviceToHost, M.stream));
-  OSFM_CUDA(cudaStreamSynchronize(M.stream));
+  MatcherGuard g(m);
+  const SlabArray<double>& h = BowRows::of(g.M, set_id, -1);
+  OSFM_CUDA(cudaMemcpyAsync(out, h.p, sizeof(double) * (size_t)h.len, cudaMemcpyDeviceToHost, g.M.stream));
+  OSFM_CUDA(cudaStreamSynchronize(g.M.stream));
   OSFM_API_END
 }
 
 int osfm_matcher_bow_select(osfm_matcher* m, int nref, const int* ref_ids, int ncand, const int* cand_ids,
                             const int32_t* cand_order, const int* camera_labels, int k, int64_t* out_offsets,
                             int32_t* out_cols, double* out_dist) {
-  OSFM_API_BEGIN
   using namespace osfm;
-  if (!m) throw ArgError("null matcher");
-  if (nref < 0 || ncand < 0 || k < 0) throw ArgError("bad BoW selection sizes");
-  if ((nref > 0 && (!ref_ids || !out_offsets)) || (ncand > 0 && !cand_ids)) throw ArgError("null arrays");
-  std::lock_guard<std::mutex> lock(matcher_mutex(m));
-  Matcher& M = matcher_impl(m);
-  OSFM_CUDA(cudaSetDevice(M.device));
-  if (nref == 0) return OSFM_OK;
-  out_offsets[0] = 0;
-  const int ngroups = camera_labels ? 2 : 1;
-  const int stride = ngroups * std::min(k, ncand);
-  if (ncand == 0 || stride == 0) {
-    for (int r = 0; r < nref; ++r) out_offsets[r + 1] = 0;
-    return OSFM_OK;
-  }
-  if (!out_cols || !out_dist) throw ArgError("null output arrays");
-  int L = -1;
-  std::vector<const double*> rows((size_t)nref + ncand);
-  for (int r = 0; r < nref; ++r) {
-    const DescSet& s = bow_hist_set(M, ref_ids[r], L);
-    L = s.bow_len;
-    rows[r] = s.bow_hist;
-  }
-  for (int j = 0; j < ncand; ++j) rows[(size_t)nref + j] = bow_hist_set(M, cand_ids[j], L).bow_hist;
-  const PairwisePlan P = pairwise_plan(L);
-  // device tables: row pointers | ids | labels | order | plan | counts | columns | distances
-  auto up256 = [](size_t x) { return (x + 255) / 256 * 256; };
-  const size_t o_ids = up256(sizeof(double*) * rows.size());
-  const size_t o_lab = o_ids + up256(sizeof(int) * rows.size());
-  const size_t o_ord = o_lab + up256(camera_labels ? sizeof(int) * rows.size() : 0);
-  const size_t o_plan = o_ord + up256(cand_order ? sizeof(int) * (size_t)nref * ncand : 0);
-  const size_t o_cnt = o_plan + plan_bytes(P);
-  const size_t o_cols = o_cnt + up256(sizeof(int) * (size_t)nref);
-  const size_t o_dist = o_cols + up256(sizeof(int) * (size_t)nref * stride);
-  const size_t total = o_dist + sizeof(double) * (size_t)nref * stride;
-  M.d_bow_tab.reserve(total);
-  uint8_t* base = M.d_bow_tab.p;
-  std::vector<int> ids((size_t)nref + ncand);
-  std::copy(ref_ids, ref_ids + nref, ids.begin());
-  std::copy(cand_ids, cand_ids + ncand, ids.begin() + nref);
-  OSFM_CUDA(cudaMemcpyAsync(base, rows.data(), sizeof(double*) * rows.size(), cudaMemcpyHostToDevice, M.stream));
-  OSFM_CUDA(cudaMemcpyAsync(base + o_ids, ids.data(), sizeof(int) * ids.size(), cudaMemcpyHostToDevice, M.stream));
-  if (camera_labels)
-    OSFM_CUDA(cudaMemcpyAsync(base + o_lab, camera_labels, sizeof(int) * rows.size(), cudaMemcpyHostToDevice, M.stream));
-  if (cand_order)
-    OSFM_CUDA(cudaMemcpyAsync(base + o_ord, cand_order, sizeof(int) * (size_t)nref * ncand, cudaMemcpyHostToDevice,
-                              M.stream));
-  size_t o_prog;
-  upload_plan(M, P, base + o_plan, &o_prog);
-  const double* const* d_rows = reinterpret_cast<const double* const*>(base);
-  const int* d_ids = reinterpret_cast<const int*>(base + o_ids);
-  const int2* d_leaves = reinterpret_cast<const int2*>(base + o_plan);
-  const int* d_prog = reinterpret_cast<const int*>(base + o_plan + o_prog);
-  int* d_cnt = reinterpret_cast<int*>(base + o_cnt);
-  int* d_cols = reinterpret_cast<int*>(base + o_cols);
-  double* d_dist = reinterpret_cast<double*>(base + o_dist);
-  // reference rows in blocks: the distance block stays under 256 MB (a multiple of the tile height)
-  // and the distance grid's y dimension within 65535
-  const long long budget = (256ll << 20) / (long long)(sizeof(double) * ncand);
-  const long long cap = std::min<long long>(budget / BD_TM * BD_TM, 65535ll * BD_TM);
-  const int block = (int)std::max<long long>(BD_TM, std::min<long long>(nref, cap));
-  M.d_bow_dist.reserve((size_t)block * ncand);
-  for (int r0 = 0; r0 < nref; r0 += block) {
-    const int nb = std::min(block, nref - r0);
-    launch_bow_distances(M.stream, d_rows + r0, nb, d_rows + nref, ncand, d_leaves, d_prog, (int)P.prog.size(), P.depth,
-                         M.d_bow_dist.p, ncand);
-    neighbor_select_kernel<<<nb, VS_THREADS, 0, M.stream>>>(
-        M.d_bow_dist.p, ncand, r0, nref, d_ids, d_ids + nref, nullptr, 0,
-        cand_order ? reinterpret_cast<const int*>(base + o_ord) : nullptr,
-        camera_labels ? reinterpret_cast<const int*>(base + o_lab) : nullptr, k, stride, d_cnt, d_cols, d_dist);
-    OSFM_LAUNCH_CHECK();
-  }
-  std::vector<int> cnt(nref);
-  std::vector<int> cols((size_t)nref * stride);
-  std::vector<double> dist((size_t)nref * stride);
-  OSFM_CUDA(cudaMemcpyAsync(cnt.data(), d_cnt, sizeof(int) * nref, cudaMemcpyDeviceToHost, M.stream));
-  OSFM_CUDA(cudaMemcpyAsync(cols.data(), d_cols, sizeof(int) * cols.size(), cudaMemcpyDeviceToHost, M.stream));
-  OSFM_CUDA(cudaMemcpyAsync(dist.data(), d_dist, sizeof(double) * dist.size(), cudaMemcpyDeviceToHost, M.stream));
-  OSFM_CUDA(cudaStreamSynchronize(M.stream));
-  int64_t o = 0;
-  for (int r = 0; r < nref; ++r) {
-    std::copy(cols.begin() + (size_t)r * stride, cols.begin() + (size_t)r * stride + cnt[r], out_cols + o);
-    std::copy(dist.begin() + (size_t)r * stride, dist.begin() + (size_t)r * stride + cnt[r], out_dist + o);
-    o += cnt[r];
-    out_offsets[r + 1] = o;
-  }
-  OSFM_API_END
+  return with_matcher(m, [&](Matcher& M) {
+    if (nref < 0 || ncand < 0 || k < 0) throw ArgError("bad BoW selection sizes");
+    BowRows kind;
+    select_neighbors(M, kind, nref, ref_ids, ncand, cand_ids, nullptr, cand_order, camera_labels, k, out_offsets,
+                     out_cols, out_dist);
+  });
 }
 
 int osfm_bow_distances(osfm_matcher* m, const double* hist, int n, int len, int query, double* out_n) {
-  OSFM_API_BEGIN
   using namespace osfm;
-  if (!m) throw ArgError("null matcher");
-  if (n <= 0 || len <= 0 || query < 0 || query >= n || !hist || !out_n) throw ArgError("bad BoW distance arguments");
-  const PairwisePlan P = pairwise_plan(len);
-  std::lock_guard<std::mutex> lock(matcher_mutex(m));
-  Matcher& M = matcher_impl(m);
-  OSFM_CUDA(cudaSetDevice(M.device));
-  // the 1 x n block of the selection's distance kernel over the uploaded rows
-  const size_t b_h = (sizeof(double) * (size_t)n * len + 255) / 256 * 256;
-  const size_t b_p = (sizeof(double*) * (size_t)n + 255) / 256 * 256;
-  const size_t b_o = (sizeof(double) * (size_t)n + 255) / 256 * 256;
-  M.staging.reserve(b_h + b_p + b_o + plan_bytes(P));
-  double* d_h = reinterpret_cast<double*>(M.staging.p);
-  const double** d_p = reinterpret_cast<const double**>(M.staging.p + b_h);
-  double* d_out = reinterpret_cast<double*>(M.staging.p + b_h + b_p);
-  uint8_t* d_plan = M.staging.p + b_h + b_p + b_o;
-  std::vector<const double*> rows(n);
-  for (int i = 0; i < n; ++i) rows[i] = d_h + (size_t)i * len;
-  OSFM_CUDA(cudaMemcpyAsync(d_h, hist, sizeof(double) * (size_t)n * len, cudaMemcpyHostToDevice, M.stream));
-  OSFM_CUDA(cudaMemcpyAsync(d_p, rows.data(), sizeof(double*) * (size_t)n, cudaMemcpyHostToDevice, M.stream));
-  size_t o_prog;
-  upload_plan(M, P, d_plan, &o_prog);
-  launch_bow_distances(M.stream, d_p + query, 1, d_p, n, reinterpret_cast<const int2*>(d_plan),
-                       reinterpret_cast<const int*>(d_plan + o_prog), (int)P.prog.size(), P.depth, d_out, n);
-  OSFM_CUDA(cudaMemcpyAsync(out_n, d_out, sizeof(double) * (size_t)n, cudaMemcpyDeviceToHost, M.stream));
-  OSFM_CUDA(cudaStreamSynchronize(M.stream));
-  OSFM_API_END
+  return with_matcher(m, [&](Matcher& M) {
+    if (n <= 0 || len <= 0 || query < 0 || query >= n || !hist || !out_n) throw ArgError("bad BoW distance arguments");
+    BowRows kind;
+    distances_to_row(M, kind, hist, n, len, query, out_n);
+  });
 }
 
 }  // extern "C"

@@ -21,7 +21,6 @@
 #include <algorithm>
 #include <cmath>
 #include <map>
-#include <mutex>
 #include <vector>
 
 #include "common.cuh"
@@ -469,7 +468,7 @@ __global__ void __launch_bounds__(256) epi_mask_bits(const EpiPair* __restrict__
 }
 
 // ---------------------------------------------------------------------------
-// Matcher object
+// Matcher object (its methods run under the C ABI's MatcherGuard, which makes the device current)
 // ---------------------------------------------------------------------------
 Matcher::Matcher(int dev) : device(dev) {
   OSFM_CUDA(cudaSetDevice(device));
@@ -489,7 +488,7 @@ Matcher::~Matcher() {
 }
 
 void* Matcher::slab_alloc(size_t bytes, int* slab_idx) {
-  bytes = (bytes + 255) / 256 * 256;
+  bytes = align256(bytes);
   // first fit in the released ranges, then the bump pointers, then a new slab
   for (size_t i = 0; i < slabs.size(); ++i) {
     Slab& sl = slabs[i];
@@ -531,7 +530,7 @@ void Matcher::slab_release(int idx, void* ptr, size_t bytes) {   // callers sync
   if (idx < 0) return;
   Slab& sl = slabs[idx];
   if (--sl.live == 0) { sl.used = 0; sl.free_ranges.clear(); return; }
-  bytes = (bytes + 255) / 256 * 256;
+  bytes = align256(bytes);
   if (!ptr || bytes == 0) return;
   size_t off = (size_t)(static_cast<char*>(ptr) - sl.base);
   auto& fr = sl.free_ranges;
@@ -561,10 +560,10 @@ void Matcher::refresh_info() {
 
 void Matcher::free_set(DescSet& s) {
   slab_release(s.slab, s.data, s.slab_bytes);
-  if (s.bearings) { slab_release(s.bear_slab, s.bearings, s.bear_bytes); s.bearings = nullptr; s.bear_slab = -1; }
-  if (s.vlad) { slab_release(s.vlad_slab, s.vlad, s.vlad_bytes); s.vlad = nullptr; s.vlad_slab = -1; }
-  if (s.bow_words) { slab_release(s.bow_words_slab, s.bow_words, s.bow_words_bytes); s.bow_words = nullptr; s.bow_words_slab = -1; }
-  if (s.bow_hist) { slab_release(s.bow_hist_slab, s.bow_hist, s.bow_hist_bytes); s.bow_hist = nullptr; s.bow_hist_slab = -1; }
+  release(s.bearings);
+  release(s.vlad);
+  release(s.bow_words);
+  release(s.bow_hist);
   if (s.slot >= 0) {
     cudaMemsetAsync(d_info.p + 2 * s.slot, 0, 2 * sizeof(int), stream);
     free_slots.push_back(s.slot);
@@ -587,7 +586,6 @@ __global__ void widen_rows_kernel(const uint8_t* __restrict__ src, int n, int di
 int Matcher::add_async(const void* host, int n, int dim, bool u8, bool u8_as_l2) {
   if (n < 0 || dim <= 0) throw ArgError("descriptor matrix must be n x dim with dim > 0");
   if (!host && n > 0) throw ArgError("null descriptor pointer");
-  OSFM_CUDA(cudaSetDevice(device));
   DescSet s;
   s.n = n;
   s.dim = dim;
@@ -601,7 +599,7 @@ int Matcher::add_async(const void* host, int n, int dim, bool u8, bool u8_as_l2)
   s.row_bytes = row_bytes;
   const bool tc = tc_capable(dim, u8);
   const bool h8 = u8 && h8_capable(dim);     // Hamming on the tensor cores: +-1 fp8 operands
-  const size_t data_bytes = ((size_t)std::max(n, 1) * row_bytes + 255) / 256 * 256;
+  const size_t data_bytes = align256((size_t)std::max(n, 1) * row_bytes);
   s.rows_padded = (tc || h8) ? tc_rows_padded(n) : 0;
   const size_t tc_bytes = tc ? tc_operand_bytes(s.rows_padded) : h8 ? h8_operand_bytes(s.rows_padded) : 0;
   s.slab_bytes = data_bytes + tc_bytes;
@@ -660,14 +658,10 @@ void Matcher::set_bearings(int id, const float* host_n_by_3) {
   auto it = sets.find(id);
   if (it == sets.end()) throw ArgError("unknown descriptor set id");
   if (!host_n_by_3) throw ArgError("null bearings");
-  OSFM_CUDA(cudaSetDevice(device));
   DescSet& s = it->second;
-  if (!s.bearings) {
-    s.bear_bytes = sizeof(float) * 3 * (size_t)std::max(s.n, 1);
-    s.bearings = static_cast<float*>(slab_alloc(s.bear_bytes, &s.bear_slab));
-  }
+  if (!s.bearings.p) slab_new(s.bearings, sizeof(float) * 3 * (size_t)std::max(s.n, 1), s.n);
   if (s.n > 0) {
-    OSFM_CUDA(cudaMemcpyAsync(s.bearings, host_n_by_3, sizeof(float) * 3 * (size_t)s.n, cudaMemcpyHostToDevice, stream));
+    OSFM_CUDA(cudaMemcpyAsync(s.bearings.p, host_n_by_3, sizeof(float) * 3 * (size_t)s.n, cudaMemcpyHostToDevice, stream));
     OSFM_CUDA(cudaStreamSynchronize(stream));
   }
 }
@@ -681,14 +675,12 @@ int Matcher::add(const void* host, int n, int dim, bool u8, bool u8_as_l2) {
 void Matcher::remove(int id) {
   auto it = sets.find(id);
   if (it == sets.end()) throw ArgError("unknown descriptor set id");
-  OSFM_CUDA(cudaSetDevice(device));
   OSFM_CUDA(cudaStreamSynchronize(stream));
   free_set(it->second);
   sets.erase(it);
 }
 
 void Matcher::clear() {
-  OSFM_CUDA(cudaSetDevice(device));
   OSFM_CUDA(cudaStreamSynchronize(stream));
   for (auto& kv : sets) free_set(kv.second);
   sets.clear();
@@ -696,7 +688,6 @@ void Matcher::clear() {
 
 void Matcher::match_pairs_async(int npairs, const int* ids_a, const int* ids_b, double ratio, bool symmetric,
                                 const uint8_t* dmask, const double* pose12, double epi_threshold) {
-  OSFM_CUDA(cudaSetDevice(device));
   refresh_info();
   if (npairs < 0) throw ArgError("npairs < 0");
   if (npairs > 30000) throw ArgError("at most 30000 pairs per submission");
@@ -756,9 +747,9 @@ void Matcher::match_pairs_async(int npairs, const int* ids_a, const int* ids_b, 
     for (int p = 0; p < npairs; ++p) {
       const DescSet& A = sets.find(ids_a[p])->second;
       const DescSet& B = sets.find(ids_b[p])->second;
-      if (!A.bearings || !B.bearings) throw ArgError("guided matching needs bearings for both images (osfm_matcher_set_bearings)");
+      if (!A.bearings.p || !B.bearings.p) throw ArgError("guided matching needs bearings for both images (osfm_matcher_set_bearings)");
       EpiPair& e = epi[p];
-      e.b1 = A.bearings; e.b2 = B.bearings; e.n1 = A.n; e.n2 = B.n;
+      e.b1 = A.bearings.p; e.b2 = B.bearings.p; e.n1 = A.n; e.n2 = B.n;
       e.w1 = (A.n + 31) / 32; e.w2 = (B.n + 31) / 32;
       e.F = reinterpret_cast<uint32_t*>(words); words += (size_t)A.n * e.w2;
       e.T = reinterpret_cast<uint32_t*>(words); words += (size_t)B.n * e.w1;
@@ -829,9 +820,7 @@ void Matcher::match_pairs_async(int npairs, const int* ids_a, const int* ids_b, 
     j.chunk_len = chunk_len;
     j.partial_off = partial_total;
     partial_total += (long long)nchunks * j.nq;
-    const bool direct = !symmetric;  // one-way: the forward match buffer is the result
     j.match_off = match_total;
-    (void)direct;
     match_total += j.nq;
     h_prefix[i] = (int)tiles_total;
     tiles_total += (long long)j.qtiles * nchunks;
@@ -920,7 +909,6 @@ void Matcher::get_epipolar_masks(int pair, uint32_t* F, uint32_t* T) {
   if (last_masks.empty()) throw ArgError("the last submission was not guided");
   if (pair < 0 || pair >= (int)last_masks.size()) throw ArgError("pair index out of range");
   if (!F || !T) throw ArgError("null output");
-  OSFM_CUDA(cudaSetDevice(device));
   const EpiMasks& e = last_masks[pair];
   const size_t fw = (size_t)e.n1 * e.w2, tw = (size_t)e.n2 * e.w1;
   if (fw) OSFM_CUDA(cudaMemcpyAsync(F, e.F, sizeof(uint32_t) * fw, cudaMemcpyDeviceToHost, stream));
@@ -928,13 +916,7 @@ void Matcher::get_epipolar_masks(int pair, uint32_t* F, uint32_t* T) {
   OSFM_CUDA(cudaStreamSynchronize(stream));
 }
 
-void Matcher::sync() {
-  OSFM_CUDA(cudaSetDevice(device));
-  OSFM_CUDA(cudaStreamSynchronize(stream));
-}
-
 void Matcher::fetch(int32_t* out, int64_t capacity) {
-  OSFM_CUDA(cudaSetDevice(device));
   if (capacity < last_total_results) throw ArgError("output buffer too small for the last batch");
   if (last_total_results > 0) {
     // one-way results are laid out per job == per pair in d_match (match_off == out_off)
@@ -947,7 +929,6 @@ void Matcher::fetch(int32_t* out, int64_t capacity) {
 // offsets_out[npairs + 1]: first row of every pair in the packed list; pairs_out: (query, train) int32 rows.
 // Returns the number of rows; throws if capacity_rows is too small.
 long long Matcher::fetch_pairs(long long* offsets_out, int32_t* pairs_out, long long capacity_rows) {
-  OSFM_CUDA(cudaSetDevice(device));
   const int npairs = last_npairs;
   if (npairs == 0) { if (offsets_out) offsets_out[0] = 0; return 0; }
   const int32_t* src = results_in_match_buf ? d_match.p : d_out.p;
@@ -972,7 +953,6 @@ long long Matcher::fetch_pairs(long long* offsets_out, int32_t* pairs_out, long 
 }
 
 void Matcher::last_ms(float* total, float* kernel) {
-  OSFM_CUDA(cudaSetDevice(device));
   OSFM_CUDA(cudaEventSynchronize(ev[3]));
   if (total) OSFM_CUDA(cudaEventElapsedTime(total, ev[0], ev[3]));
   if (kernel) OSFM_CUDA(cudaEventElapsedTime(kernel, ev[1], ev[2]));
@@ -1009,16 +989,6 @@ void Matcher::one_shot(const void* f1, int n1, const void* f2, int n2, int dim, 
 // C ABI
 // ---------------------------------------------------------------------------
 using osfm::Matcher;
-struct osfm_matcher {
-  Matcher impl;
-  std::mutex mu;
-  explicit osfm_matcher(int dev) : impl(dev) {}
-};
-
-namespace osfm {   // accessors for words.cu
-Matcher& matcher_impl(osfm_matcher* m) { return m->impl; }
-std::mutex& matcher_mutex(osfm_matcher* m) { return m->mu; }
-}  // namespace osfm
 
 extern "C" {
 
@@ -1038,57 +1008,45 @@ int osfm_matcher_destroy(osfm_matcher* m) {
   OSFM_API_END
 }
 
-#define OSFM_M_LOCK                                   \
-  if (!m) throw osfm::ArgError("null matcher");       \
-  std::lock_guard<std::mutex> lock(m->mu);
-
 int osfm_bf_match_f32(osfm_matcher* m, const float* f1, int n1, const float* f2, int n2, int dim,
                       double lowes_ratio, const uint8_t* mask, int symmetric, int32_t* out_match) {
-  OSFM_API_BEGIN
-  OSFM_M_LOCK
-  m->impl.one_shot(f1, n1, f2, n2, dim, false, lowes_ratio, mask, symmetric != 0, out_match);
-  OSFM_API_END
+  return osfm::with_matcher(
+      m, [&](Matcher& M) { M.one_shot(f1, n1, f2, n2, dim, false, lowes_ratio, mask, symmetric != 0, out_match); });
 }
 
 int osfm_bf_match_u8(osfm_matcher* m, const uint8_t* f1, int n1, const uint8_t* f2, int n2, int nbytes,
                      double lowes_ratio, const uint8_t* mask, int symmetric, int32_t* out_match) {
-  OSFM_API_BEGIN
-  OSFM_M_LOCK
-  m->impl.one_shot(f1, n1, f2, n2, nbytes, true, lowes_ratio, mask, symmetric != 0, out_match);
-  OSFM_API_END
+  return osfm::with_matcher(
+      m, [&](Matcher& M) { M.one_shot(f1, n1, f2, n2, nbytes, true, lowes_ratio, mask, symmetric != 0, out_match); });
 }
 
+static int add_one(osfm_matcher* m, const void* desc, int n, int dim, bool u8, int* out_id, bool u8_as_l2 = false) {
+  return osfm::with_matcher(m, [&](Matcher& M) {
+    if (!out_id) throw osfm::ArgError("null out_id");
+    *out_id = M.add(desc, n, dim, u8, u8_as_l2);
+  });
+}
 int osfm_matcher_add_f32(osfm_matcher* m, const float* desc, int n, int dim, int* out_id) {
-  OSFM_API_BEGIN
-  OSFM_M_LOCK
-  if (!out_id) throw osfm::ArgError("null out_id");
-  *out_id = m->impl.add(desc, n, dim, false);
-  OSFM_API_END
+  return add_one(m, desc, n, dim, false, out_id);
 }
-
 int osfm_matcher_add_u8(osfm_matcher* m, const uint8_t* desc, int n, int nbytes, int* out_id) {
-  OSFM_API_BEGIN
-  OSFM_M_LOCK
-  if (!out_id) throw osfm::ArgError("null out_id");
-  *out_id = m->impl.add(desc, n, nbytes, true);
-  OSFM_API_END
+  return add_one(m, desc, n, nbytes, true, out_id);
 }
 
 static int add_batch(osfm_matcher* m, int count, const void* const* desc, const int* n, int dim, bool u8, int* out_ids,
                      bool u8_as_l2 = false) {
-  OSFM_API_BEGIN
-  OSFM_M_LOCK
-  if (count < 0 || (count > 0 && (!desc || !n || !out_ids))) throw osfm::ArgError("bad batch arguments");
-  int done = 0;
-  try {
-    for (; done < count; ++done) out_ids[done] = m->impl.add_async(desc[done], n[done], dim, u8, u8_as_l2);
-    OSFM_CUDA(cudaStreamSynchronize(m->impl.stream));
-  } catch (...) {
-    cudaStreamSynchronize(m->impl.stream);
-    for (int i = 0; i < done; ++i) m->impl.remove(out_ids[i]);
-    throw;
-  }
-  OSFM_API_END
+  return osfm::with_matcher(m, [&](Matcher& M) {
+    if (count < 0 || (count > 0 && (!desc || !n || !out_ids))) throw osfm::ArgError("bad batch arguments");
+    int done = 0;
+    try {
+      for (; done < count; ++done) out_ids[done] = M.add_async(desc[done], n[done], dim, u8, u8_as_l2);
+      OSFM_CUDA(cudaStreamSynchronize(M.stream));
+    } catch (...) {
+      cudaStreamSynchronize(M.stream);
+      for (int i = 0; i < done; ++i) M.remove(out_ids[i]);
+      throw;
+    }
+  });
 }
 int osfm_matcher_add_batch_f32(osfm_matcher* m, int count, const float* const* desc, const int* n, int dim, int* out_ids) {
   return add_batch(m, count, reinterpret_cast<const void* const*>(desc), n, dim, false, out_ids);
@@ -1099,11 +1057,7 @@ int osfm_matcher_add_batch_u8(osfm_matcher* m, int count, const uint8_t* const* 
 }
 
 int osfm_matcher_add_u8_l2(osfm_matcher* m, const uint8_t* desc, int n, int dim, int* out_id) {
-  OSFM_API_BEGIN
-  OSFM_M_LOCK
-  if (!out_id) throw osfm::ArgError("null out_id");
-  *out_id = m->impl.add(desc, n, dim, false, true);
-  OSFM_API_END
+  return add_one(m, desc, n, dim, false, out_id, true);
 }
 int osfm_matcher_add_batch_u8_l2(osfm_matcher* m, int count, const uint8_t* const* desc, const int* n, int dim,
                                  int* out_ids) {
@@ -1111,99 +1065,74 @@ int osfm_matcher_add_batch_u8_l2(osfm_matcher* m, int count, const uint8_t* cons
 }
 
 int osfm_matcher_remove(osfm_matcher* m, int id) {
-  OSFM_API_BEGIN
-  OSFM_M_LOCK
-  m->impl.remove(id);
-  OSFM_API_END
+  return osfm::with_matcher(m, [&](Matcher& M) { M.remove(id); });
 }
 
 int osfm_matcher_clear(osfm_matcher* m) {
-  OSFM_API_BEGIN
-  OSFM_M_LOCK
-  m->impl.clear();
-  OSFM_API_END
+  return osfm::with_matcher(m, [&](Matcher& M) { M.clear(); });
 }
 
 int osfm_matcher_match_pairs_async(osfm_matcher* m, int npairs, const int* ids_a, const int* ids_b,
                                    double lowes_ratio, int symmetric) {
-  OSFM_API_BEGIN
-  OSFM_M_LOCK
-  if (npairs > 0 && (!ids_a || !ids_b)) throw osfm::ArgError("null pair list");
-  m->impl.match_pairs_async(npairs, ids_a, ids_b, lowes_ratio, symmetric != 0, nullptr);
-  OSFM_API_END
+  return osfm::with_matcher(m, [&](Matcher& M) {
+    if (npairs > 0 && (!ids_a || !ids_b)) throw osfm::ArgError("null pair list");
+    M.match_pairs_async(npairs, ids_a, ids_b, lowes_ratio, symmetric != 0, nullptr);
+  });
 }
 
 int osfm_matcher_set_bearings(osfm_matcher* m, int id, const float* bearings_n_by_3) {
-  OSFM_API_BEGIN
-  OSFM_M_LOCK
-  m->impl.set_bearings(id, bearings_n_by_3);
-  OSFM_API_END
+  return osfm::with_matcher(m, [&](Matcher& M) { M.set_bearings(id, bearings_n_by_3); });
 }
 
 int osfm_matcher_match_pairs_guided_async(osfm_matcher* m, int npairs, const int* ids_a, const int* ids_b,
                                           const double* pose12, double threshold, double lowes_ratio, int symmetric) {
-  OSFM_API_BEGIN
-  OSFM_M_LOCK
-  if (npairs > 0 && (!ids_a || !ids_b || !pose12)) throw osfm::ArgError("null pair list / poses");
-  // any threshold is the reference's comparison `angle < threshold`: at or below 0 nothing passes
-  if (std::isnan(threshold)) throw osfm::ArgError("guided matching threshold is NaN");
-  m->impl.match_pairs_async(npairs, ids_a, ids_b, lowes_ratio, symmetric != 0, nullptr, pose12, threshold);
-  OSFM_API_END
+  return osfm::with_matcher(m, [&](Matcher& M) {
+    if (npairs > 0 && (!ids_a || !ids_b || !pose12)) throw osfm::ArgError("null pair list / poses");
+    // any threshold is the reference's comparison `angle < threshold`: at or below 0 nothing passes
+    if (std::isnan(threshold)) throw osfm::ArgError("guided matching threshold is NaN");
+    M.match_pairs_async(npairs, ids_a, ids_b, lowes_ratio, symmetric != 0, nullptr, pose12, threshold);
+  });
 }
 
 int osfm_matcher_get_epipolar_masks(osfm_matcher* m, int pair, uint32_t* F, uint32_t* T) {
-  OSFM_API_BEGIN
-  OSFM_M_LOCK
-  m->impl.get_epipolar_masks(pair, F, T);
-  OSFM_API_END
+  return osfm::with_matcher(m, [&](Matcher& M) { M.get_epipolar_masks(pair, F, T); });
 }
 
 int osfm_matcher_sync(osfm_matcher* m) {
-  OSFM_API_BEGIN
-  OSFM_M_LOCK
-  m->impl.sync();
-  OSFM_API_END
+  return osfm::with_matcher(m, [&](Matcher& M) { OSFM_CUDA(cudaStreamSynchronize(M.stream)); });
 }
 
 int osfm_matcher_fetch(osfm_matcher* m, int32_t* out_match, int64_t capacity) {
-  OSFM_API_BEGIN
-  OSFM_M_LOCK
-  m->impl.fetch(out_match, capacity);
-  OSFM_API_END
+  return osfm::with_matcher(m, [&](Matcher& M) { M.fetch(out_match, capacity); });
 }
 
 int osfm_matcher_fetch_pairs(osfm_matcher* m, int64_t* offsets_out, int32_t* pairs_out, int64_t capacity_rows,
                              int64_t* total_rows) {
-  OSFM_API_BEGIN
-  OSFM_M_LOCK
-  if (!offsets_out || !total_rows || (capacity_rows > 0 && !pairs_out)) throw osfm::ArgError("null output");
-  static_assert(sizeof(long long) == sizeof(int64_t), "offsets are 64-bit");
-  *total_rows = m->impl.fetch_pairs(reinterpret_cast<long long*>(offsets_out), pairs_out, capacity_rows);
-  OSFM_API_END
+  return osfm::with_matcher(m, [&](Matcher& M) {
+    if (!offsets_out || !total_rows || (capacity_rows > 0 && !pairs_out)) throw osfm::ArgError("null output");
+    static_assert(sizeof(long long) == sizeof(int64_t), "offsets are 64-bit");
+    *total_rows = M.fetch_pairs(reinterpret_cast<long long*>(offsets_out), pairs_out, capacity_rows);
+  });
 }
 
 int osfm_matcher_last_device_ms(osfm_matcher* m, float* ms_total, float* ms_distance_kernel) {
-  OSFM_API_BEGIN
-  OSFM_M_LOCK
-  m->impl.last_ms(ms_total, ms_distance_kernel);
-  OSFM_API_END
+  return osfm::with_matcher(m, [&](Matcher& M) { M.last_ms(ms_total, ms_distance_kernel); });
 }
 
 int osfm_matcher_set_kernel(osfm_matcher* m, int which) {
-  OSFM_API_BEGIN
-  OSFM_M_LOCK
-  if (which < 0 || which > 2) throw osfm::ArgError("kernel must be 0, 1 or 2");
-  m->impl.kernel_choice = which;
-  OSFM_API_END
+  return osfm::with_matcher(m, [&](Matcher& M) {
+    if (which < 0 || which > 2) throw osfm::ArgError("kernel must be 0, 1 or 2");
+    M.kernel_choice = which;
+  });
 }
 
 int osfm_matcher_last_kernel(osfm_matcher* m) { return m ? m->impl.last_kernel : 0; }
 int osfm_matcher_device_bytes(osfm_matcher* m, int64_t* reserved, int64_t* in_use) {
   OSFM_API_BEGIN
   if (!m || !reserved || !in_use) throw osfm::ArgError("null argument");
-  std::lock_guard<std::mutex> lock(m->mu);
+  osfm::MatcherGuard g(m);
   int64_t cap = 0, used = 0;
-  for (const auto& sl : m->impl.slabs) {
+  for (const auto& sl : g.M.slabs) {
     cap += (int64_t)sl.cap;
     used += (int64_t)sl.used;
     for (const auto& fr : sl.free_ranges) used -= (int64_t)fr.second;

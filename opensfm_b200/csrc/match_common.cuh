@@ -3,6 +3,7 @@
 #include <cuda_bf16.h>
 
 #include <map>
+#include <mutex>
 #include <vector>
 
 #include "common.cuh"
@@ -175,6 +176,15 @@ __device__ __forceinline__ bool job_allows(const MatchJob& job, int gq, int gt) 
   return true;
 }
 
+// An array in the matcher's slabs (Matcher::slab_new / Matcher::release); null until allocated.
+template <class T>
+struct SlabArray {
+  T* p = nullptr;
+  int slab = -1;
+  size_t bytes = 0;
+  int len = 0;   // the length its owner records with it
+};
+
 struct DescSet {
   void* data = nullptr;
   int n = 0, dim = 0, dim_padded = 0, row_bytes = 0;
@@ -190,23 +200,16 @@ struct DescSet {
   // device memory comes from the matcher's slabs; the exactness flag / max norm of a freshly added set
   // live in d_info[slot] until refresh_info() reads them back (no host sync per add)
   int slab = -1, slot = -1;
-  size_t slab_bytes = 0, bear_bytes = 0;   // sizes of the two slab allocations (data + operands; bearings)
+  size_t slab_bytes = 0;   // size of the data + operands allocation
   bool info_pending = false;
-  // unit bearing vectors of the features (n x 3 float32), for guided matching; null until set
-  float* bearings = nullptr;
-  int bear_slab = -1;
-  // VLAD descriptor of the set (vlad.cu): [unnormalised | normalised], vlad_len floats each; null until computed
-  float* vlad = nullptr;
-  int vlad_len = 0, vlad_slab = -1;
-  size_t vlad_bytes = 0;
-  // BoW state (bow.cu): the nearest visual word of every row (n ints, words of a bow_nwords-word vocabulary) and
-  // the weighted, normalised word histogram (bow_len doubles); null until computed
-  int* bow_words = nullptr;
-  int bow_nwords = 0, bow_words_slab = -1;
-  size_t bow_words_bytes = 0;
-  double* bow_hist = nullptr;
-  int bow_len = 0, bow_hist_slab = -1;
-  size_t bow_hist_bytes = 0;
+  // unit bearing vectors of the features (n x 3 float32), for guided matching
+  SlabArray<float> bearings;
+  // VLAD descriptor of the set (vlad.cu): [unnormalised | normalised], len floats each
+  SlabArray<float> vlad;
+  // BoW state (bow.cu): the nearest visual word of every row (n ints, words of a len-word vocabulary) and
+  // the weighted, normalised word histogram (len doubles)
+  SlabArray<int> bow_words;
+  SlabArray<double> bow_hist;
 };
 
 // The two layouts of one pair's epipolar bitmask in the last guided submission (the test hook reads them back).
@@ -224,6 +227,7 @@ struct Slab {
   std::vector<std::pair<size_t, size_t>> free_ranges;
 };
 
+// Its methods expect the device to be current; the C entry points make it so (MatcherGuard, with_matcher below).
 struct Matcher {
   int device;
   cudaStream_t stream = nullptr;
@@ -257,17 +261,17 @@ struct Matcher {
   PinnedBuf<MatchJob> p_jobs;
   PinnedBuf<int> p_prefix;
   PinnedBuf<long long> p_out_off;
-  // VLAD workspaces (vlad.cu): centres, per-feature nearest centre, error flags, distance block, job / selection tables
+  // VLAD workspaces (vlad.cu): centres, per-feature nearest centre, error flags
   DevBuf<float> d_vlad_centers;
   DevBuf<int> d_vlad_assign, d_vlad_flags;
-  DevBuf<double> d_vlad_dist;
-  DevBuf<uint8_t> d_vlad_tab;
-  // BoW workspaces (bow.cu): padded vocabulary, per-chunk top-k lists + words of a batch, error flags, distance block,
-  // job / selection tables
+  // BoW workspaces (bow.cu): padded vocabulary, per-chunk top-k lists + words of a batch, error flags
   DevBuf<float> d_bow_vocab;
-  DevBuf<uint8_t> d_bow_work, d_bow_tab;
+  DevBuf<uint8_t> d_bow_work;
   DevBuf<int> d_bow_flags;
-  DevBuf<double> d_bow_dist;
+  // VLAD and BoW: job / plan / selection tables and the selection's distance block.  Every call that uses them
+  // synchronises the stream before it returns.
+  DevBuf<uint8_t> d_tab;
+  DevBuf<double> d_dist;
 
   explicit Matcher(int dev);
   ~Matcher();
@@ -282,6 +286,29 @@ struct Matcher {
   static constexpr int MAX_SLOTS = 1 << 16;
   void* slab_alloc(size_t bytes, int* slab_idx);
   void slab_release(int idx, void* ptr, size_t bytes);
+  template <class T>
+  void slab_new(SlabArray<T>& a, size_t bytes, int len) {
+    a.p = static_cast<T*>(slab_alloc(bytes, &a.slab));
+    a.bytes = bytes;
+    a.len = len;
+  }
+  // callers synchronise the stream first; slab_release counts a release even of a null pointer, so only what was
+  // allocated goes back
+  template <class T>
+  void release(SlabArray<T>& a) {
+    if (a.p) slab_release(a.slab, a.p, a.bytes);
+    a = SlabArray<T>();
+  }
+  // the array `field` of set `id`, whose len must equal `len` when len >= 0
+  template <class T>
+  const SlabArray<T>& resident(int id, SlabArray<T> DescSet::*field, int len, const char* missing, const char* mismatch) {
+    auto it = sets.find(id);
+    if (it == sets.end()) throw ArgError("unknown descriptor set id");
+    const SlabArray<T>& a = it->second.*field;
+    if (!a.p) throw ArgError(missing);
+    if (len >= 0 && a.len != len) throw ArgError(mismatch);
+    return a;
+  }
   void refresh_info();
   // u8: Hamming descriptors.  u8_as_l2: uint8 storage of an L2 descriptor (widened to float32 on the device).
   int add_async(const void* host, int n, int dim, bool u8, bool u8_as_l2 = false);  // no host sync; the host buffer must stay valid
@@ -295,7 +322,6 @@ struct Matcher {
                          const uint8_t* dmask, const double* pose12 = nullptr, double epi_threshold = 0.0);
   void set_bearings(int id, const float* host_n_by_3);
   void get_epipolar_masks(int pair, uint32_t* F, uint32_t* T);
-  void sync();
   void fetch(int32_t* out, int64_t capacity);
   long long fetch_pairs(long long* offsets_out, int32_t* pairs_out, long long capacity_rows);
   void last_ms(float* total, float* kernel);
@@ -321,4 +347,42 @@ size_t h8_operand_bytes(int rows_padded);
 bool h8_capable(int nbytes);
 void launch_tc_h8(Matcher& m, int njobs, int ntiles);
 
+// Offsets of arrays packed into one device table, each on a 256-byte boundary.
+inline size_t align256(size_t bytes) { return (bytes + 255) / 256 * 256; }
+struct TableLayout {
+  size_t size = 0;
+  size_t add(size_t bytes) {
+    const size_t o = size;
+    size += align256(bytes);
+    return o;
+  }
+};
+
+}  // namespace osfm
+
+// The C ABI's matcher handle.
+struct osfm_matcher {
+  osfm::Matcher impl;
+  std::mutex mu;
+  explicit osfm_matcher(int dev) : impl(dev) {}
+};
+
+namespace osfm {
+// The preamble of every matcher entry point: a null check, the matcher's lock and its device made current.
+struct MatcherGuard {
+  std::lock_guard<std::mutex> lock;
+  Matcher& M;
+  explicit MatcherGuard(osfm_matcher* m) : lock((m ? m : throw ArgError("null matcher"))->mu), M(m->impl) {
+    OSFM_CUDA(cudaSetDevice(M.device));
+  }
+};
+
+// A matcher entry point: body(M) under MatcherGuard, its exceptions turned into error codes.
+template <class F>
+int with_matcher(osfm_matcher* m, F&& body) {
+  OSFM_API_BEGIN
+  MatcherGuard g(m);
+  body(g.M);
+  OSFM_API_END
+}
 }  // namespace osfm

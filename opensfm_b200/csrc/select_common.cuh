@@ -3,7 +3,11 @@
 #pragma once
 #include <cub/cub.cuh>
 
+#include <algorithm>
+#include <vector>
+
 #include "common.cuh"
+#include "match_common.cuh"
 
 namespace osfm {
 namespace {
@@ -130,6 +134,123 @@ __global__ void __launch_bounds__(VS_THREADS)
     }
   }
   if (threadIdx.x == 0) out_count[row] = written;
+}
+
+// A kind of pair selection (VladRows in vlad.cu, BowRows in bow.cu) supplies its row type, its distance kernel's tile
+// height, the lookup of a set's resident array (`of`) and the row in it, and its own device tables (BoW: the pairwise
+// plan).  The calls come in this order: table_bytes(len) for rows of length len, upload() into the table, then
+// distances(), which launches one block of distances.
+
+// Host side of the selection: the rows of the listed sets, one device table, the reference rows in blocks (the
+// distance block stays under 256 MB as a multiple of the tile height, and the distance grid's y dimension within
+// 65535) of distances + neighbor_select_kernel, and the selected columns compacted into out_offsets / out_cols /
+// out_dist.
+// VLAD passes mask_bits, BoW passes order.
+template <class Kind>
+void select_neighbors(Matcher& M, Kind& kind, int nref, const int* ref_ids, int ncand, const int* cand_ids,
+                      const uint32_t* mask_bits, const int32_t* order, const int* labels, int k, int64_t* out_offsets,
+                      int32_t* out_cols, double* out_dist) {
+  using Row = typename Kind::Row;
+  if ((nref > 0 && (!ref_ids || !out_offsets)) || (ncand > 0 && !cand_ids)) throw ArgError("null arrays");
+  if (nref == 0) return;
+  out_offsets[0] = 0;
+  const int ngroups = labels ? 2 : 1;
+  const int stride = ngroups * std::min(k, ncand);
+  if (ncand == 0 || stride == 0) {
+    for (int r = 0; r < nref; ++r) out_offsets[r + 1] = 0;
+    return;
+  }
+  if (!out_cols || !out_dist) throw ArgError("null output arrays");
+  const size_t nrows = (size_t)nref + ncand;
+  std::vector<int> ids(nrows);
+  std::copy(ref_ids, ref_ids + nref, ids.begin());
+  std::copy(cand_ids, cand_ids + ncand, ids.begin() + nref);
+  int L = -1;
+  std::vector<const Row*> rows(nrows);
+  for (size_t i = 0; i < nrows; ++i) {
+    const auto& a = Kind::of(M, ids[i], L);
+    L = a.len;
+    rows[i] = Kind::row(a);
+  }
+  const int mask_words = (ncand + 31) / 32;
+  const size_t mask_bytes = mask_bits ? sizeof(uint32_t) * (size_t)nref * mask_words : 0;
+  const size_t order_bytes = order ? sizeof(int) * (size_t)nref * ncand : 0;
+  // device table: row pointers | ids | labels | mask | order | the kind's tables | counts | columns | distances
+  TableLayout t;
+  t.add(sizeof(Row*) * nrows);
+  const size_t o_ids = t.add(sizeof(int) * nrows);
+  const size_t o_lab = t.add(labels ? sizeof(int) * nrows : 0);
+  const size_t o_mask = t.add(mask_bytes), o_ord = t.add(order_bytes), o_kind = t.add(kind.table_bytes(L));
+  const size_t o_cnt = t.add(sizeof(int) * (size_t)nref);
+  const size_t o_cols = t.add(sizeof(int) * (size_t)nref * stride);
+  const size_t o_dist = t.add(sizeof(double) * (size_t)nref * stride);
+  M.d_tab.reserve(t.size);
+  uint8_t* base = M.d_tab.p;
+  auto upload = [&](size_t off, const void* src, size_t bytes) {
+    if (src) OSFM_CUDA(cudaMemcpyAsync(base + off, src, bytes, cudaMemcpyHostToDevice, M.stream));
+  };
+  upload(0, rows.data(), sizeof(Row*) * nrows);
+  upload(o_ids, ids.data(), sizeof(int) * nrows);
+  upload(o_lab, labels, sizeof(int) * nrows);
+  upload(o_mask, mask_bits, mask_bytes);
+  upload(o_ord, order, order_bytes);
+  kind.upload(M, base + o_kind);
+  const Row* const* d_rows = reinterpret_cast<const Row* const*>(base);
+  const int* d_ids = reinterpret_cast<const int*>(base + o_ids);
+  int* d_cnt = reinterpret_cast<int*>(base + o_cnt);
+  int* d_cols = reinterpret_cast<int*>(base + o_cols);
+  double* d_dist = reinterpret_cast<double*>(base + o_dist);
+  const long long budget = (256ll << 20) / (long long)(sizeof(double) * ncand);
+  const long long cap = std::min<long long>(budget / Kind::TILE_M * Kind::TILE_M, 65535ll * Kind::TILE_M);
+  const int block = (int)std::max<long long>(Kind::TILE_M, std::min<long long>(nref, cap));
+  M.d_dist.reserve((size_t)block * ncand);
+  for (int r0 = 0; r0 < nref; r0 += block) {
+    const int nb = std::min(block, nref - r0);
+    kind.distances(M, base + o_kind, d_rows + r0, nb, d_rows + nref, ncand, L, M.d_dist.p, ncand);
+    neighbor_select_kernel<<<nb, VS_THREADS, 0, M.stream>>>(
+        M.d_dist.p, ncand, r0, nref, d_ids, d_ids + nref,
+        mask_bits ? reinterpret_cast<const uint32_t*>(base + o_mask) : nullptr, mask_words,
+        order ? reinterpret_cast<const int*>(base + o_ord) : nullptr,
+        labels ? reinterpret_cast<const int*>(base + o_lab) : nullptr, k, stride, d_cnt, d_cols, d_dist);
+    OSFM_LAUNCH_CHECK();
+  }
+  std::vector<int> cnt(nref);
+  std::vector<int> cols((size_t)nref * stride);
+  std::vector<double> dist((size_t)nref * stride);
+  OSFM_CUDA(cudaMemcpyAsync(cnt.data(), d_cnt, sizeof(int) * nref, cudaMemcpyDeviceToHost, M.stream));
+  OSFM_CUDA(cudaMemcpyAsync(cols.data(), d_cols, sizeof(int) * cols.size(), cudaMemcpyDeviceToHost, M.stream));
+  OSFM_CUDA(cudaMemcpyAsync(dist.data(), d_dist, sizeof(double) * dist.size(), cudaMemcpyDeviceToHost, M.stream));
+  OSFM_CUDA(cudaStreamSynchronize(M.stream));
+  int64_t o = 0;
+  for (int r = 0; r < nref; ++r) {
+    std::copy(cols.begin() + (size_t)r * stride, cols.begin() + (size_t)r * stride + cnt[r], out_cols + o);
+    std::copy(dist.begin() + (size_t)r * stride, dist.begin() + (size_t)r * stride + cnt[r], out_dist + o);
+    o += cnt[r];
+    out_offsets[r + 1] = o;
+  }
+}
+
+// The distances of host row `query` to all n host rows of len elements (osfm_vlad_distances, osfm_bow_distances):
+// the rows, their pointers and the kind's tables go to the staging buffer, one 1 x n block runs.
+template <class Kind>
+void distances_to_row(Matcher& M, Kind& kind, const typename Kind::Row* host, int n, int len, int query, double* out_n) {
+  using Row = typename Kind::Row;
+  TableLayout t;
+  t.add(sizeof(Row) * (size_t)n * len);
+  const size_t o_ptr = t.add(sizeof(Row*) * (size_t)n), o_out = t.add(sizeof(double) * (size_t)n);
+  const size_t o_kind = t.add(kind.table_bytes(len));
+  M.staging.reserve(t.size);
+  Row* d_v = reinterpret_cast<Row*>(M.staging.p);
+  const Row** d_p = reinterpret_cast<const Row**>(M.staging.p + o_ptr);
+  double* d_out = reinterpret_cast<double*>(M.staging.p + o_out);
+  std::vector<const Row*> rows(n);
+  for (int i = 0; i < n; ++i) rows[i] = d_v + (size_t)i * len;
+  OSFM_CUDA(cudaMemcpyAsync(d_v, host, sizeof(Row) * (size_t)n * len, cudaMemcpyHostToDevice, M.stream));
+  OSFM_CUDA(cudaMemcpyAsync(d_p, rows.data(), sizeof(Row*) * (size_t)n, cudaMemcpyHostToDevice, M.stream));
+  kind.upload(M, M.staging.p + o_kind);
+  kind.distances(M, M.staging.p + o_kind, d_p + query, 1, d_p, n, len, d_out, n);
+  OSFM_CUDA(cudaMemcpyAsync(out_n, d_out, sizeof(double) * (size_t)n, cudaMemcpyDeviceToHost, M.stream));
+  OSFM_CUDA(cudaStreamSynchronize(M.stream));
 }
 
 }  // namespace

@@ -12,7 +12,6 @@
 // operations in the same order, so the unnormalised vector is bit for bit the reference's.
 #include <cfloat>
 #include <cmath>
-#include <mutex>
 #include <vector>
 
 #include "common.cuh"
@@ -206,38 +205,26 @@ __global__ void __launch_bounds__(256)
     }
 }
 
+// VLAD rows for select_neighbors / distances_to_row (select_common.cuh): the normalised half of each descriptor.
+struct VladRows {
+  using Row = float;
+  static constexpr int TILE_M = VD_TM;
+  static const SlabArray<float>& of(Matcher& M, int id, int len) {
+    return M.resident(id, &DescSet::vlad, len, "descriptor set has no VLAD descriptor (osfm_matcher_vlad_compute)",
+                      "VLAD descriptors of different lengths");
+  }
+  static const float* row(const SlabArray<float>& v) { return v.p + v.len; }
+  size_t table_bytes(int) { return 0; }
+  void upload(Matcher&, uint8_t*) {}
+  void distances(Matcher& M, const uint8_t*, const float* const* arows, int na, const float* const* brows, int nb,
+                 int L, double* out, long long ldo) {
+    dim3 grid((unsigned)((nb + VD_TN - 1) / VD_TN), (unsigned)((na + VD_TM - 1) / VD_TM));
+    vlad_distance_kernel<<<grid, 256, 0, M.stream>>>(arows, na, brows, nb, L, out, ldo);
+    OSFM_LAUNCH_CHECK();
+  }
+};
+
 }  // namespace
-
-// Launch the distance kernel for na reference rows x nb candidate rows into out (na rows of ldo doubles).
-static void launch_vlad_distances(cudaStream_t stream, const float* const* arows, int na, const float* const* brows,
-                                  int nb, int L, double* out, long long ldo) {
-  dim3 grid((unsigned)((nb + VD_TN - 1) / VD_TN), (unsigned)((na + VD_TM - 1) / VD_TM));
-  vlad_distance_kernel<<<grid, 256, 0, stream>>>(arows, na, brows, nb, L, out, ldo);
-  OSFM_LAUNCH_CHECK();
-}
-
-}  // namespace osfm
-
-struct osfm_matcher;   // defined in match.cu: { Matcher impl; std::mutex mu; }
-namespace osfm {
-Matcher& matcher_impl(osfm_matcher* m);
-std::mutex& matcher_mutex(osfm_matcher* m);
-
-static void release_vlad(Matcher& M, DescSet& s) {   // the caller has synchronised the stream
-  if (s.vlad) M.slab_release(s.vlad_slab, s.vlad, s.vlad_bytes);
-  s.vlad = nullptr;
-  s.vlad_slab = -1;
-  s.vlad_len = 0;
-  s.vlad_bytes = 0;
-}
-
-static const DescSet& vlad_set(Matcher& M, int id, int L) {
-  auto it = M.sets.find(id);
-  if (it == M.sets.end()) throw ArgError("unknown descriptor set id");
-  if (!it->second.vlad) throw ArgError("descriptor set has no VLAD descriptor (osfm_matcher_vlad_compute)");
-  if (L >= 0 && it->second.vlad_len != L) throw ArgError("VLAD descriptors of different lengths");
-  return it->second;
-}
 }  // namespace osfm
 
 extern "C" {
@@ -246,7 +233,8 @@ int osfm_matcher_vlad_compute(osfm_matcher* m, int count, const int* set_ids, co
                               int* out_valid) {
   OSFM_API_BEGIN
   using namespace osfm;
-  if (!m) throw ArgError("null matcher");
+  MatcherGuard g(m);
+  Matcher& M = g.M;
   if (count < 0 || ncenters <= 0 || dim <= 0) throw ArgError("bad VLAD sizes");
   if ((count > 0 && (!set_ids || !out_valid)) || !centers) throw ArgError("null arrays");
   const int ncp = (ncenters + VA_CH - 1) / VA_CH * VA_CH;
@@ -255,9 +243,6 @@ int osfm_matcher_vlad_compute(osfm_matcher* m, int count, const int* set_ids, co
     throw ArgError("VLAD vocabulary too large: ncenters x dim float32 must fit in 200 KB of shared memory");
   for (size_t e = 0; e < L; ++e)
     if (!std::isfinite(centers[e])) throw ArgError("non-finite VLAD centre");
-  std::lock_guard<std::mutex> lock(matcher_mutex(m));
-  Matcher& M = matcher_impl(m);
-  OSFM_CUDA(cudaSetDevice(M.device));
   for (int i = 0; i < count; ++i)
     if (!M.sets.count(set_ids[i])) throw ArgError("unknown descriptor set id");
   OSFM_CUDA(cudaStreamSynchronize(M.stream));   // earlier work may still read VLADs released below
@@ -270,16 +255,12 @@ int osfm_matcher_vlad_compute(osfm_matcher* m, int count, const int* set_ids, co
     DescSet& s = M.sets[set_ids[i]];
     const bool valid = !s.u8 && s.dim == dim;
     out_valid[i] = valid;
-    if (s.vlad && (!valid || (size_t)s.vlad_len != L)) release_vlad(M, s);
+    if (!valid || (size_t)s.vlad.len != L) M.release(s.vlad);
     if (!valid) continue;
-    if (!s.vlad) {
-      s.vlad_bytes = 2 * L * sizeof(float);
-      s.vlad = static_cast<float*>(M.slab_alloc(s.vlad_bytes, &s.vlad_slab));
-      s.vlad_len = (int)L;
-    }
+    if (!s.vlad.p) M.slab_new(s.vlad, 2 * L * sizeof(float), (int)L);
     VladJob j;
     j.f = static_cast<const float*>(s.data);   // float32 zero-padded rows for every non-Hamming set (match.cu add_async)
-    j.v = s.vlad;
+    j.v = s.vlad.p;
     j.aoff = nfeat;
     j.n = s.n;
     j.ld = s.dim_padded;
@@ -297,11 +278,11 @@ int osfm_matcher_vlad_compute(osfm_matcher* m, int count, const int* set_ids, co
   M.d_vlad_centers.reserve(hc.size());
   M.d_vlad_assign.reserve((size_t)std::max<long long>(nfeat, 1));
   M.d_vlad_flags.reserve(1);
-  M.d_vlad_tab.reserve(sizeof(VladJob) * jobs.size());
+  M.d_tab.reserve(sizeof(VladJob) * jobs.size());
   OSFM_CUDA(cudaMemcpyAsync(M.d_vlad_centers.p, hc.data(), sizeof(float) * hc.size(), cudaMemcpyHostToDevice, M.stream));
-  OSFM_CUDA(cudaMemcpyAsync(M.d_vlad_tab.p, jobs.data(), sizeof(VladJob) * jobs.size(), cudaMemcpyHostToDevice, M.stream));
+  OSFM_CUDA(cudaMemcpyAsync(M.d_tab.p, jobs.data(), sizeof(VladJob) * jobs.size(), cudaMemcpyHostToDevice, M.stream));
   OSFM_CUDA(cudaMemsetAsync(M.d_vlad_flags.p, 0, sizeof(int), M.stream));
-  const VladJob* d_jobs = reinterpret_cast<const VladJob*>(M.d_vlad_tab.p);
+  const VladJob* d_jobs = reinterpret_cast<const VladJob*>(M.d_tab.p);
   const size_t smem_a = (size_t)dim * ncp * sizeof(float), smem_n = L * sizeof(float);
   OSFM_CUDA(cudaFuncSetAttribute(vlad_assign_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_a));
   OSFM_CUDA(cudaFuncSetAttribute(vlad_accumulate_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_n));
@@ -322,7 +303,7 @@ int osfm_matcher_vlad_compute(osfm_matcher* m, int count, const int* set_ids, co
   OSFM_CUDA(cudaMemcpyAsync(&flags, M.d_vlad_flags.p, sizeof(int), cudaMemcpyDeviceToHost, M.stream));
   OSFM_CUDA(cudaStreamSynchronize(M.stream));
   if (flags) {
-    for (int id : job_set) release_vlad(M, M.sets[id]);
+    for (int id : job_set) M.release(M.sets[id].vlad);
     throw ArgError(flags & 1 ? "non-finite descriptor element in a VLAD input set"
                              : "a feature's squared distance to every VLAD centre overflows float32");
   }
@@ -333,126 +314,33 @@ int osfm_matcher_vlad_get(osfm_matcher* m, int set_id, int unnormalized, float* 
   OSFM_API_BEGIN
   using namespace osfm;
   if (!m || !out) throw ArgError("null arguments");
-  std::lock_guard<std::mutex> lock(matcher_mutex(m));
-  Matcher& M = matcher_impl(m);
-  OSFM_CUDA(cudaSetDevice(M.device));
-  const DescSet& s = vlad_set(M, set_id, -1);
-  const float* src = s.vlad + (unnormalized ? 0 : s.vlad_len);
-  OSFM_CUDA(cudaMemcpyAsync(out, src, sizeof(float) * (size_t)s.vlad_len, cudaMemcpyDeviceToHost, M.stream));
-  OSFM_CUDA(cudaStreamSynchronize(M.stream));
+  MatcherGuard g(m);
+  const SlabArray<float>& v = VladRows::of(g.M, set_id, -1);
+  OSFM_CUDA(cudaMemcpyAsync(out, v.p + (unnormalized ? 0 : v.len), sizeof(float) * (size_t)v.len, cudaMemcpyDeviceToHost,
+                            g.M.stream));
+  OSFM_CUDA(cudaStreamSynchronize(g.M.stream));
   OSFM_API_END
 }
 
 int osfm_matcher_vlad_select(osfm_matcher* m, int nref, const int* ref_ids, int ncand, const int* cand_ids,
                              const uint32_t* cand_mask_bits, const int* camera_labels, int k, int64_t* out_offsets,
                              int32_t* out_cols, double* out_dist) {
-  OSFM_API_BEGIN
   using namespace osfm;
-  if (!m) throw ArgError("null matcher");
-  if (nref < 0 || ncand < 0 || k < 0) throw ArgError("bad VLAD selection sizes");
-  if ((nref > 0 && (!ref_ids || !out_offsets)) || (ncand > 0 && !cand_ids)) throw ArgError("null arrays");
-  std::lock_guard<std::mutex> lock(matcher_mutex(m));
-  Matcher& M = matcher_impl(m);
-  OSFM_CUDA(cudaSetDevice(M.device));
-  if (nref == 0) return OSFM_OK;
-  out_offsets[0] = 0;
-  const int ngroups = camera_labels ? 2 : 1;
-  const int stride = ngroups * std::min(k, ncand);
-  if (ncand == 0 || stride == 0) {
-    for (int r = 0; r < nref; ++r) out_offsets[r + 1] = 0;
-    return OSFM_OK;
-  }
-  if (!out_cols || !out_dist) throw ArgError("null output arrays");
-  int L = -1;
-  std::vector<const float*> rows((size_t)nref + ncand);
-  for (int r = 0; r < nref; ++r) {
-    const DescSet& s = vlad_set(M, ref_ids[r], L);
-    L = s.vlad_len;
-    rows[r] = s.vlad + L;
-  }
-  for (int j = 0; j < ncand; ++j) rows[(size_t)nref + j] = vlad_set(M, cand_ids[j], L).vlad + L;
-  const int mask_words = (ncand + 31) / 32;
-  // device tables: row pointers | ids | labels | mask | counts | columns | distances
-  auto up256 = [](size_t x) { return (x + 255) / 256 * 256; };
-  const size_t o_ids = up256(sizeof(float*) * rows.size());
-  const size_t o_lab = o_ids + up256(sizeof(int) * rows.size());
-  const size_t o_mask = o_lab + up256(camera_labels ? sizeof(int) * rows.size() : 0);
-  const size_t o_cnt = o_mask + up256(cand_mask_bits ? sizeof(uint32_t) * (size_t)nref * mask_words : 0);
-  const size_t o_cols = o_cnt + up256(sizeof(int) * (size_t)nref);
-  const size_t o_dist = o_cols + up256(sizeof(int) * (size_t)nref * stride);
-  const size_t total = o_dist + sizeof(double) * (size_t)nref * stride;
-  M.d_vlad_tab.reserve(total);
-  uint8_t* base = M.d_vlad_tab.p;
-  std::vector<int> ids((size_t)nref + ncand);
-  std::copy(ref_ids, ref_ids + nref, ids.begin());
-  std::copy(cand_ids, cand_ids + ncand, ids.begin() + nref);
-  OSFM_CUDA(cudaMemcpyAsync(base, rows.data(), sizeof(float*) * rows.size(), cudaMemcpyHostToDevice, M.stream));
-  OSFM_CUDA(cudaMemcpyAsync(base + o_ids, ids.data(), sizeof(int) * ids.size(), cudaMemcpyHostToDevice, M.stream));
-  if (camera_labels)
-    OSFM_CUDA(cudaMemcpyAsync(base + o_lab, camera_labels, sizeof(int) * rows.size(), cudaMemcpyHostToDevice, M.stream));
-  if (cand_mask_bits)
-    OSFM_CUDA(cudaMemcpyAsync(base + o_mask, cand_mask_bits, sizeof(uint32_t) * (size_t)nref * mask_words,
-                              cudaMemcpyHostToDevice, M.stream));
-  const float* const* d_rows = reinterpret_cast<const float* const*>(base);
-  const int* d_ids = reinterpret_cast<const int*>(base + o_ids);
-  int* d_cnt = reinterpret_cast<int*>(base + o_cnt);
-  int* d_cols = reinterpret_cast<int*>(base + o_cols);
-  double* d_dist = reinterpret_cast<double*>(base + o_dist);
-  // reference rows in blocks: the distance block stays under 256 MB (a multiple of the tile height)
-  // and the distance grid's y dimension (block / VD_TM tiles) within 65535
-  const long long budget = (256ll << 20) / (long long)(sizeof(double) * ncand);
-  const long long cap = std::min<long long>(budget / VD_TM * VD_TM, 65535ll * VD_TM);
-  const int block = (int)std::max<long long>(VD_TM, std::min<long long>(nref, cap));
-  M.d_vlad_dist.reserve((size_t)block * ncand);
-  for (int r0 = 0; r0 < nref; r0 += block) {
-    const int nb = std::min(block, nref - r0);
-    launch_vlad_distances(M.stream, d_rows + r0, nb, d_rows + nref, ncand, L, M.d_vlad_dist.p, ncand);
-    neighbor_select_kernel<<<nb, VS_THREADS, 0, M.stream>>>(
-        M.d_vlad_dist.p, ncand, r0, nref, d_ids, d_ids + nref,
-        cand_mask_bits ? reinterpret_cast<const uint32_t*>(base + o_mask) : nullptr, mask_words, nullptr,
-        camera_labels ? reinterpret_cast<const int*>(base + o_lab) : nullptr, k, stride, d_cnt, d_cols, d_dist);
-    OSFM_LAUNCH_CHECK();
-  }
-  std::vector<int> cnt(nref);
-  std::vector<int> cols((size_t)nref * stride);
-  std::vector<double> dist((size_t)nref * stride);
-  OSFM_CUDA(cudaMemcpyAsync(cnt.data(), d_cnt, sizeof(int) * nref, cudaMemcpyDeviceToHost, M.stream));
-  OSFM_CUDA(cudaMemcpyAsync(cols.data(), d_cols, sizeof(int) * cols.size(), cudaMemcpyDeviceToHost, M.stream));
-  OSFM_CUDA(cudaMemcpyAsync(dist.data(), d_dist, sizeof(double) * dist.size(), cudaMemcpyDeviceToHost, M.stream));
-  OSFM_CUDA(cudaStreamSynchronize(M.stream));
-  int64_t o = 0;
-  for (int r = 0; r < nref; ++r) {
-    std::copy(cols.begin() + (size_t)r * stride, cols.begin() + (size_t)r * stride + cnt[r], out_cols + o);
-    std::copy(dist.begin() + (size_t)r * stride, dist.begin() + (size_t)r * stride + cnt[r], out_dist + o);
-    o += cnt[r];
-    out_offsets[r + 1] = o;
-  }
-  OSFM_API_END
+  return with_matcher(m, [&](Matcher& M) {
+    if (nref < 0 || ncand < 0 || k < 0) throw ArgError("bad VLAD selection sizes");
+    VladRows kind;
+    select_neighbors(M, kind, nref, ref_ids, ncand, cand_ids, cand_mask_bits, nullptr, camera_labels, k, out_offsets,
+                     out_cols, out_dist);
+  });
 }
 
 int osfm_vlad_distances(osfm_matcher* m, const float* vlad, int n, int dim, int query, double* out_n) {
-  OSFM_API_BEGIN
   using namespace osfm;
-  if (!m) throw ArgError("null matcher");
-  if (n <= 0 || dim <= 0 || query < 0 || query >= n || !vlad || !out_n) throw ArgError("bad VLAD arguments");
-  std::lock_guard<std::mutex> lock(matcher_mutex(m));
-  Matcher& M = matcher_impl(m);
-  OSFM_CUDA(cudaSetDevice(M.device));
-  // the 1 x n block of the selection's distance kernel over the uploaded rows
-  const size_t b_v = (sizeof(float) * (size_t)n * dim + 255) / 256 * 256;
-  const size_t b_p = (sizeof(float*) * (size_t)n + 255) / 256 * 256;
-  M.staging.reserve(b_v + b_p + sizeof(double) * (size_t)n);
-  float* d_v = reinterpret_cast<float*>(M.staging.p);
-  const float** d_p = reinterpret_cast<const float**>(M.staging.p + b_v);
-  double* d_out = reinterpret_cast<double*>(M.staging.p + b_v + b_p);
-  std::vector<const float*> rows(n);
-  for (int i = 0; i < n; ++i) rows[i] = d_v + (size_t)i * dim;
-  OSFM_CUDA(cudaMemcpyAsync(d_v, vlad, sizeof(float) * (size_t)n * dim, cudaMemcpyHostToDevice, M.stream));
-  OSFM_CUDA(cudaMemcpyAsync(d_p, rows.data(), sizeof(float*) * (size_t)n, cudaMemcpyHostToDevice, M.stream));
-  launch_vlad_distances(M.stream, d_p + query, 1, d_p, n, dim, d_out, n);
-  OSFM_CUDA(cudaMemcpyAsync(out_n, d_out, sizeof(double) * (size_t)n, cudaMemcpyDeviceToHost, M.stream));
-  OSFM_CUDA(cudaStreamSynchronize(M.stream));
-  OSFM_API_END
+  return with_matcher(m, [&](Matcher& M) {
+    if (n <= 0 || dim <= 0 || query < 0 || query >= n || !vlad || !out_n) throw ArgError("bad VLAD arguments");
+    VladRows kind;
+    distances_to_row(M, kind, vlad, n, dim, query, out_n);
+  });
 }
 
 }  // extern "C"

@@ -13,7 +13,6 @@
 // and one thread walks the candidates of one feature with the same sequence of float32 operations (separate
 // multiply and add, no FMA contraction, like the reference's x86-64 baseline build).
 #include <algorithm>
-#include <mutex>
 #include <vector>
 
 #include "common.cuh"
@@ -54,24 +53,16 @@ __global__ void __launch_bounds__(128)
 
 }  // namespace osfm
 
-struct osfm_matcher;   // defined in match.cu: { Matcher impl; std::mutex mu; }
-namespace osfm {
-Matcher& matcher_impl(osfm_matcher* m);
-std::mutex& matcher_mutex(osfm_matcher* m);
-}  // namespace osfm
-
 extern "C" {
 
 int osfm_match_words(osfm_matcher* m, const float* f1, int n1, const int32_t* words1, int words_per_feature,
                      const float* f2, int n2, const int32_t* words2, int dim, float lowes_ratio, int max_checks,
                      int32_t* out_match) {
   OSFM_API_BEGIN
-  if (!m) throw osfm::ArgError("null matcher");
+  osfm::MatcherGuard g(m);
+  osfm::Matcher& M = g.M;
   if (n1 < 0 || n2 < 0 || dim <= 0 || words_per_feature <= 0) throw osfm::ArgError("bad sizes");
   if ((n1 > 0 && (!f1 || !words1 || !out_match)) || (n2 > 0 && (!f2 || !words2))) throw osfm::ArgError("null arrays");
-  std::lock_guard<std::mutex> lock(osfm::matcher_mutex(m));
-  osfm::Matcher& M = osfm::matcher_impl(m);
-  OSFM_CUDA(cudaSetDevice(M.device));
   if (n1 == 0) return OSFM_OK;
   // CSR of image 2's features by word: stable counting sort = the multimap's order among equal words
   int nwords = 0;
@@ -85,11 +76,11 @@ int osfm_match_words(osfm_matcher* m, const float* f1, int n1, const int32_t* wo
   }
   const size_t b_f1 = sizeof(float) * (size_t)n1 * dim, b_f2 = sizeof(float) * (size_t)std::max(n2, 1) * dim;
   const size_t b_w1 = sizeof(int) * (size_t)n1 * words_per_feature;
-  auto up256 = [](size_t x) { return (x + 255) / 256 * 256; };
-  const size_t o_f2 = up256(b_f1), o_w1 = o_f2 + up256(b_f2), o_st = o_w1 + up256(b_w1);
-  const size_t o_or = o_st + up256(sizeof(int) * start.size()), o_out = o_or + up256(sizeof(int) * order.size());
-  const size_t total = o_out + up256(sizeof(int) * (size_t)n1);
-  M.staging.reserve(total);
+  osfm::TableLayout tab;
+  tab.add(b_f1);
+  const size_t o_f2 = tab.add(b_f2), o_w1 = tab.add(b_w1), o_st = tab.add(sizeof(int) * start.size());
+  const size_t o_or = tab.add(sizeof(int) * order.size()), o_out = tab.add(sizeof(int) * (size_t)n1);
+  M.staging.reserve(tab.size);
   uint8_t* base = M.staging.p;
   OSFM_CUDA(cudaMemcpyAsync(base, f1, b_f1, cudaMemcpyHostToDevice, M.stream));
   if (n2 > 0) OSFM_CUDA(cudaMemcpyAsync(base + o_f2, f2, sizeof(float) * (size_t)n2 * dim, cudaMemcpyHostToDevice, M.stream));

@@ -51,6 +51,10 @@ def _thread_matcher(device: int = 0) -> _Matcher:
     return m
 
 
+def _ptr(a: Optional[np.ndarray]) -> Optional[ctypes.c_void_p]:
+    return None if a is None else a.ctypes.data_as(ctypes.c_void_p)
+
+
 def _prep(f: np.ndarray) -> np.ndarray:
     if f.dtype.type == np.uint8:
         return np.ascontiguousarray(f)
@@ -153,9 +157,7 @@ class PairMatcher:
             _lib.check(self._m.L.osfm_matcher_remove(self._m.h, self._ids[key]))
         self._ids[key] = out.value
         self._n[key] = d.shape[0]
-        self._vlad.pop(key, None)
-        self._bow.pop(key, None)
-        self._words.pop(key, None)
+        self._forget(key)
 
     def add_many(self, items: Sequence[Tuple[Any, np.ndarray]], uint8_is_l2: bool = False) -> None:
         """Upload many images' descriptors with a single host synchronisation (same dtype and
@@ -183,18 +185,18 @@ class PairMatcher:
                 _lib.check(self._m.L.osfm_matcher_remove(self._m.h, self._ids[k]))
             self._ids[k] = int(i)
             self._n[k] = d.shape[0]
-            self._vlad.pop(k, None)
-            self._bow.pop(k, None)
-            self._words.pop(k, None)
+            self._forget(k)
 
     def clear(self) -> None:
         """Drop every resident descriptor set (device memory stays with the matcher for reuse)."""
         _lib.check(self._m.L.osfm_matcher_clear(self._m.h))
-        self._ids.clear()
-        self._n.clear()
-        self._vlad.clear()
-        self._bow.clear()
-        self._words.clear()
+        for d in (self._ids, self._n, self._vlad, self._bow, self._words):
+            d.clear()
+
+    def _forget(self, key: Any) -> None:
+        """Drop the VLAD / BoW state of an image whose descriptor set was replaced or removed."""
+        for state in (self._vlad, self._bow, self._words):
+            state.pop(key, None)
 
     # -- VLAD (opensfm/vlad.py, pairs_selection.vlad_histograms) ---------------------------------------------------
     def compute_vlad(self, keys: Iterable[Any], centers: np.ndarray) -> List[Any]:
@@ -209,9 +211,8 @@ class PairMatcher:
         valid = np.zeros(len(keys), dtype=np.int32)
         for k in keys:
             self._vlad.pop(k, None)
-        _lib.check(self._m.L.osfm_matcher_vlad_compute(self._m.h, len(keys), ids.ctypes.data_as(ctypes.c_void_p),
-                                                       c.ctypes.data_as(ctypes.c_void_p), c.shape[0], c.shape[1],
-                                                       valid.ctypes.data_as(ctypes.c_void_p)))
+        _lib.check(self._m.L.osfm_matcher_vlad_compute(self._m.h, len(keys), _ptr(ids), _ptr(c), c.shape[0], c.shape[1],
+                                                       _ptr(valid)))
         for k, v in zip(keys, valid):
             self._vlad[k] = c.size if v else 0
         return [k for k, v in zip(keys, valid) if v]
@@ -222,8 +223,7 @@ class PairMatcher:
         if not self._vlad.get(key):
             raise KeyError("no VLAD descriptor for image %r" % (key,))
         out = np.empty(self._vlad[key], dtype=np.float32)
-        _lib.check(self._m.L.osfm_matcher_vlad_get(self._m.h, self._ids[key], int(not normalized),
-                                                   out.ctypes.data_as(ctypes.c_void_p)))
+        _lib.check(self._m.L.osfm_matcher_vlad_get(self._m.h, self._ids[key], int(not normalized), _ptr(out)))
         return out
 
     def has_vlad(self, key: Any) -> Optional[bool]:
@@ -242,8 +242,6 @@ class PairMatcher:
         the k nearest by (distance, column), per camera group when `labels` (len(refs) + len(cands) ints) is given.
         cand_mask: None or a len(refs) x len(cands) boolean array of allowed candidates."""
         nref, ncand = len(refs), len(cands)
-        ri = np.array([self._ids[r] for r in refs], dtype=np.int32)
-        ci = np.array([self._ids[c] for c in cands], dtype=np.int32)
         bits = None
         if cand_mask is not None:
             m = np.asarray(cand_mask, dtype=bool).reshape(nref, ncand)
@@ -252,6 +250,15 @@ class PairMatcher:
             padded = np.zeros((nref, 4 * words), dtype=np.uint8)
             padded[:, :packed.shape[1]] = packed
             bits = np.ascontiguousarray(padded).view("<u4")
+        return self._select(self._m.L.osfm_matcher_vlad_select, refs, cands, k, bits, labels)
+
+    def _select(self, fn, refs: Sequence[Any], cands: Sequence[Any], k: int, per_ref: Optional[np.ndarray],
+                labels: Optional[np.ndarray]) -> List[Tuple[np.ndarray, np.ndarray]]:
+        """Run a selection entry point, `fn` (osfm_matcher_vlad_select or osfm_matcher_bow_select), whose
+        per-reference argument is `per_ref` (the VLAD mask bits or the BoW candidate order)."""
+        nref, ncand = len(refs), len(cands)
+        ri = np.array([self._ids[r] for r in refs], dtype=np.int32)
+        ci = np.array([self._ids[c] for c in cands], dtype=np.int32)
         lab = None if labels is None else np.ascontiguousarray(labels, dtype=np.int32)
         if lab is not None and lab.shape != (nref + ncand,):
             raise ValueError("labels must hold len(refs) + len(cands) ints")
@@ -259,12 +266,8 @@ class PairMatcher:
         offs = np.zeros(nref + 1, dtype=np.int64)
         cols = np.empty(cap, dtype=np.int32)
         dist = np.empty(cap, dtype=np.float64)
-
-        def ptr(a):
-            return None if a is None else a.ctypes.data_as(ctypes.c_void_p)
-
-        _lib.check(self._m.L.osfm_matcher_vlad_select(self._m.h, nref, ptr(ri), ncand, ptr(ci), ptr(bits), ptr(lab),
-                                                      int(k), ptr(offs), ptr(cols), ptr(dist)))
+        _lib.check(fn(self._m.h, nref, _ptr(ri), ncand, _ptr(ci), _ptr(per_ref), _ptr(lab), int(k), _ptr(offs),
+                      _ptr(cols), _ptr(dist)))
         return [(cols[offs[r]:offs[r + 1]], dist[offs[r]:offs[r + 1]]) for r in range(nref)]
 
     # -- BoW (opensfm/bow.py, pairs_selection.load_histograms) ----------------------------------------------------
@@ -284,11 +287,8 @@ class PairMatcher:
         for key in keys:
             self._words.pop(key, None)
             self._bow.pop(key, None)
-        _lib.check(self._m.L.osfm_matcher_bow_words(self._m.h, len(keys), ids.ctypes.data_as(ctypes.c_void_p),
-                                                    vocab.ctypes.data_as(ctypes.c_void_p), nw, vocab.shape[1], int(k),
-                                                    offs.ctypes.data_as(ctypes.c_void_p),
-                                                    words.ctypes.data_as(ctypes.c_void_p),
-                                                    valid.ctypes.data_as(ctypes.c_void_p)))
+        _lib.check(self._m.L.osfm_matcher_bow_words(self._m.h, len(keys), _ptr(ids), _ptr(vocab), nw, vocab.shape[1],
+                                                    int(k), _ptr(offs), _ptr(words), _ptr(valid)))
         out: Dict[Any, np.ndarray] = {}
         for i, (key, v) in enumerate(zip(keys, valid)):
             self._words[key] = nw if v else 0
@@ -308,15 +308,13 @@ class PairMatcher:
         w = np.ascontiguousarray(bows.weights, dtype=np.float64)
         ids = np.array([self._ids[key] for key in keys], dtype=np.int32)
         valid = np.zeros(len(keys), dtype=np.int32)
-        _lib.check(self._m.L.osfm_matcher_bow_histograms(self._m.h, len(keys), ids.ctypes.data_as(ctypes.c_void_p),
-                                                         w.ctypes.data_as(ctypes.c_void_p), len(w),
-                                                         valid.ctypes.data_as(ctypes.c_void_p)))
+        _lib.check(self._m.L.osfm_matcher_bow_histograms(self._m.h, len(keys), _ptr(ids), _ptr(w), len(w), _ptr(valid)))
         out: Dict[Any, np.ndarray] = {}
         for key, v in zip(keys, valid):
             self._bow[key] = len(w) if v else 0
             if v:
                 h = np.empty(len(w), dtype=np.float64)
-                _lib.check(self._m.L.osfm_matcher_bow_get(self._m.h, self._ids[key], h.ctypes.data_as(ctypes.c_void_p)))
+                _lib.check(self._m.L.osfm_matcher_bow_get(self._m.h, self._ids[key], _ptr(h)))
                 out[key] = h
         return out
 
@@ -330,24 +328,10 @@ class PairMatcher:
         the k nearest by (distance, column), per camera group when `labels` (len(refs) + len(cands) ints) is given.
         cand_order: None or a len(refs) x len(cands) int array, the position of each candidate in the reference's own
         candidate list (-1: not a candidate), which then breaks ties instead of the column."""
-        nref, ncand = len(refs), len(cands)
-        ri = np.array([self._ids[r] for r in refs], dtype=np.int32)
-        ci = np.array([self._ids[c] for c in cands], dtype=np.int32)
-        order = None if cand_order is None else np.ascontiguousarray(cand_order, dtype=np.int32).reshape(nref, ncand)
-        lab = None if labels is None else np.ascontiguousarray(labels, dtype=np.int32)
-        if lab is not None and lab.shape != (nref + ncand,):
-            raise ValueError("labels must hold len(refs) + len(cands) ints")
-        cap = max(nref * min(k, ncand) * (2 if lab is not None else 1), 1)
-        offs = np.zeros(nref + 1, dtype=np.int64)
-        cols = np.empty(cap, dtype=np.int32)
-        dist = np.empty(cap, dtype=np.float64)
-
-        def ptr(a):
-            return None if a is None else a.ctypes.data_as(ctypes.c_void_p)
-
-        _lib.check(self._m.L.osfm_matcher_bow_select(self._m.h, nref, ptr(ri), ncand, ptr(ci), ptr(order), ptr(lab),
-                                                     int(k), ptr(offs), ptr(cols), ptr(dist)))
-        return [(cols[offs[r]:offs[r + 1]], dist[offs[r]:offs[r + 1]]) for r in range(nref)]
+        order = None
+        if cand_order is not None:
+            order = np.ascontiguousarray(cand_order, dtype=np.int32).reshape(len(refs), len(cands))
+        return self._select(self._m.L.osfm_matcher_bow_select, refs, cands, k, order, labels)
 
     def submit(self, pairs: Sequence[Tuple[Any, Any]], lowes_ratio: float, symmetric: bool = True) -> None:
         ia = np.array([self._ids[a] for a, _ in pairs], dtype=np.int32)
@@ -507,8 +491,7 @@ def vlad_distances(image: Any, other_images: Sequence[Any], histograms: Dict[Any
     mat = np.ascontiguousarray(np.stack([histograms[image]] + [histograms[o] for o in others]), dtype=np.float32)
     out = np.zeros(len(mat), dtype=np.float64)
     m = _thread_matcher(device)
-    _lib.check(m.L.osfm_vlad_distances(m.h, mat.ctypes.data_as(ctypes.c_void_p), mat.shape[0], mat.shape[1], 0,
-                                       out.ctypes.data_as(ctypes.c_void_p)))
+    _lib.check(m.L.osfm_vlad_distances(m.h, _ptr(mat), mat.shape[0], mat.shape[1], 0, _ptr(out)))
     return image, out[1:].tolist(), others
 
 

@@ -20,7 +20,7 @@ from typing import Any, Dict, Optional, Sequence, Tuple
 import numpy as np
 
 from . import _lib
-from .matching import PairMatcher, _thread_matcher
+from .matching import PairMatcher, _ptr, _thread_matcher
 
 
 def unnormalized_vlad(features: np.ndarray, centers: np.ndarray, device: int = 0) -> Optional[np.ndarray]:
@@ -32,14 +32,13 @@ def unnormalized_vlad(features: np.ndarray, centers: np.ndarray, device: int = 0
     c = np.ascontiguousarray(centers, dtype=np.float32)
     m = _thread_matcher(device)
     sid = ctypes.c_int()
-    _lib.check(m.L.osfm_matcher_add_f32(m.h, f.ctypes.data_as(ctypes.c_void_p), f.shape[0], f.shape[1], ctypes.byref(sid)))
+    _lib.check(m.L.osfm_matcher_add_f32(m.h, _ptr(f), f.shape[0], f.shape[1], ctypes.byref(sid)))
     try:
         ids = np.array([sid.value], dtype=np.int32)
         valid = np.zeros(1, dtype=np.int32)
-        _lib.check(m.L.osfm_matcher_vlad_compute(m.h, 1, ids.ctypes.data_as(ctypes.c_void_p), c.ctypes.data_as(ctypes.c_void_p),
-                                                 c.shape[0], c.shape[1], valid.ctypes.data_as(ctypes.c_void_p)))
+        _lib.check(m.L.osfm_matcher_vlad_compute(m.h, 1, _ptr(ids), _ptr(c), c.shape[0], c.shape[1], _ptr(valid)))
         out = np.empty(c.size, dtype=np.float32)
-        _lib.check(m.L.osfm_matcher_vlad_get(m.h, sid.value, 1, out.ctypes.data_as(ctypes.c_void_p)))
+        _lib.check(m.L.osfm_matcher_vlad_get(m.h, sid.value, 1, _ptr(out)))
     finally:
         _lib.check(m.L.osfm_matcher_remove(m.h, sid.value))
     return out
@@ -48,6 +47,36 @@ def unnormalized_vlad(features: np.ndarray, centers: np.ndarray, device: int = 0
 def sorted_pair(im1: Any, im2: Any) -> Tuple[Any, Any]:
     """pairs_selection.sorted_pair."""
     return (im1, im2) if im1 < im2 else (im2, im1)
+
+
+def _state_check(state_of, kind: str, producer: str):
+    """has(image): whether the image has a VLAD descriptor / BoW histogram; raises if `producer` never ran on it."""
+
+    def has(im):
+        state = state_of(im)
+        if state is None:
+            raise ValueError("image %r has no %s state: run PairMatcher.%s on it first" % (im, kind, producer))
+        return state
+
+    return has
+
+
+def _selected_pairs(select, refs: Sequence[Any], cands: Sequence[Any], per_ref: Optional[np.ndarray],
+                    exifs: Dict[Any, Any], max_neighbors: int,
+                    enforce_other_cameras: bool) -> Dict[Tuple[Any, Any], float]:
+    """{sorted pair: distance} of the candidates `select` (PairMatcher.vlad_select / bow_select) keeps for each
+    reference, with camera labels from `exifs` when `enforce_other_cameras`."""
+    if not refs or not cands:
+        return {}
+    labels = None
+    if enforce_other_cameras:
+        names: Dict[Any, int] = {}
+        labels = np.array([names.setdefault(exifs[im]["camera"], len(names)) for im in list(refs) + cands], dtype=np.int32)
+    pairs: Dict[Tuple[Any, Any], float] = {}
+    for im, (cols, dist) in zip(refs, select(refs, cands, max_neighbors, per_ref, labels)):
+        for j, d in zip(cols.tolist(), dist.tolist()):
+            pairs[sorted_pair(im, cands[j])] = d
+    return pairs
 
 
 def match_candidates_with_vlad(matcher: PairMatcher, images_ref: Sequence[Any], images_cand: Sequence[Any],
@@ -66,13 +95,7 @@ def match_candidates_with_vlad(matcher: PairMatcher, images_ref: Sequence[Any], 
     the candidate that comes first in sorted order, which is the order compute_vlad_distances lists them in."""
     if max_neighbors <= 0:
         return {}
-
-    def has(im):
-        state = matcher.has_vlad(im)
-        if state is None:
-            raise ValueError("image %r has no VLAD state: run PairMatcher.vlad_histograms on it first" % (im,))
-        return state
-
+    has = _state_check(matcher.has_vlad, "VLAD", "vlad_histograms")
     mask = None
     if not candidates:
         refs = [im for im in dict.fromkeys(images_ref) if has(im)]
@@ -86,17 +109,7 @@ def match_candidates_with_vlad(matcher: PairMatcher, images_ref: Sequence[Any], 
             mask = np.zeros((len(refs), len(cands)), dtype=bool)
             for r, s in enumerate(per_ref):
                 mask[r, [col[c] for c in s]] = True
-    if not refs or not cands:
-        return {}
-    labels = None
-    if enforce_other_cameras:
-        names: Dict[Any, int] = {}
-        labels = np.array([names.setdefault(exifs[im]["camera"], len(names)) for im in list(refs) + cands], dtype=np.int32)
-    pairs: Dict[Tuple[Any, Any], float] = {}
-    for im, (cols, dist) in zip(refs, matcher.vlad_select(refs, cands, max_neighbors, mask, labels)):
-        for j, d in zip(cols.tolist(), dist.tolist()):
-            pairs[sorted_pair(im, cands[j])] = d
-    return pairs
+    return _selected_pairs(matcher.vlad_select, refs, cands, mask, exifs, max_neighbors, enforce_other_cameras)
 
 
 def bow_distances(image: Any, other_images: Sequence[Any], histograms: Dict[Any, np.ndarray], device: int = 0):
@@ -131,13 +144,7 @@ def match_candidates_with_bow(matcher: PairMatcher, images_ref: Sequence[Any], i
     listed twice for one reference counts once."""
     if max_neighbors <= 0:
         return {}
-
-    def has(im):
-        state = matcher.has_bow(im)
-        if state is None:
-            raise ValueError("image %r has no BoW state: run PairMatcher.bow_histograms on it first" % (im,))
-        return state
-
+    has = _state_check(matcher.has_bow, "BoW", "bow_histograms")
     order = None
     if candidates is None:
         refs = [im for im in dict.fromkeys(images_ref) if has(im)]
@@ -150,14 +157,4 @@ def match_candidates_with_bow(matcher: PairMatcher, images_ref: Sequence[Any], i
         order = np.full((len(refs), len(cands)), -1, dtype=np.int32)
         for r, lst in enumerate(lists):
             order[r, [col[c] for c in lst]] = np.arange(len(lst), dtype=np.int32)
-    if not refs or not cands:
-        return {}
-    labels = None
-    if enforce_other_cameras:
-        names: Dict[Any, int] = {}
-        labels = np.array([names.setdefault(exifs[im]["camera"], len(names)) for im in list(refs) + cands], dtype=np.int32)
-    pairs: Dict[Tuple[Any, Any], float] = {}
-    for im, (cols, dist) in zip(refs, matcher.bow_select(refs, cands, max_neighbors, order, labels)):
-        for j, d in zip(cols.tolist(), dist.tolist()):
-            pairs[sorted_pair(im, cands[j])] = d
-    return pairs
+    return _selected_pairs(matcher.bow_select, refs, cands, order, exifs, max_neighbors, enforce_other_cameras)
