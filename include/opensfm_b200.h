@@ -15,6 +15,11 @@
  *          tracking.create_tracks_manager (opensfm/tracking.py:72-150).
  *
  * There is no CPU fallback: every call needs a CUDA device (H100, sm_90a).
+ *
+ * Handles (osfm_matcher, osfm_ba, osfm_tracks, osfm_rotransac) own a CUDA stream and workspaces on the device they
+ * were created on, and every call on a handle makes that device current on the calling thread.  Calls on one handle
+ * are serialised and may come from any thread; calls on different handles do not wait for each other.  A callback
+ * (today only the all-reduce of osfm_ba_set_distributed) must not call into the handle that called it.
  */
 #ifndef OPENSFM_B200_H_
 #define OPENSFM_B200_H_
@@ -41,9 +46,9 @@ int64_t osfm_kernel_launch_count(void);
  * ---------------------------------------------------------------------- */
 typedef struct osfm_matcher osfm_matcher;
 
-/* A matcher owns one CUDA stream and its workspaces on `device`.  One matcher
- * per host thread: matching.match_brute_force is called concurrently from
- * joblib threads (opensfm/context.py:59-64). */
+/* A matcher owns one CUDA stream and its workspaces on `device`.  Threads that
+ * match at the same time use a matcher each: matching.match_brute_force is
+ * called concurrently from joblib threads (opensfm/context.py:59-64). */
 int osfm_matcher_create(int device, osfm_matcher** out);
 int osfm_matcher_destroy(osfm_matcher* m);
 

@@ -5,9 +5,14 @@ present, calls raise.  (The library is built in-tree by `__graft_entry__.build()
 """
 from __future__ import annotations
 
+import contextlib
 import ctypes
 import os
+import threading
 from ctypes import POINTER, c_char_p, c_double, c_float, c_int, c_int32, c_int64, c_uint8, c_void_p
+from typing import Dict, Iterator, List, Optional, Tuple
+
+import numpy as np
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(HERE, "lib", "libopensfm_b200.so")
@@ -179,3 +184,55 @@ def check(code: int) -> None:
         if code == 2:
             raise ValueError(msg)
         raise RuntimeError(msg)
+
+
+def ptr(a: Optional[np.ndarray]) -> Optional[ctypes.c_void_p]:
+    """The data pointer of a C-contiguous array, or None for None."""
+    return None if a is None else a.ctypes.data_as(ctypes.c_void_p)
+
+
+class Handle:
+    """One engine object of the C ABI, `osfm_<kind>_create(device)` .. `osfm_<kind>_destroy`, with kind one of "ba",
+    "matcher", "tracks" and "rotransac".  It keeps its stream and device workspaces between calls.  The library
+    serialises calls on one handle, so callers that should not wait for one another use handles of their own."""
+
+    def __init__(self, kind: str, device: int = 0):
+        self.kind, self.device, self.L = kind, int(device), load()
+        self.h = ctypes.c_void_p()
+        check(getattr(self.L, "osfm_%s_create" % kind)(self.device, ctypes.byref(self.h)))
+
+    def __del__(self):
+        try:
+            getattr(self.L, "osfm_%s_destroy" % self.kind)(self.h)
+        except Exception:
+            pass
+
+
+# Released handles by (kind, device).  A caller that asks again gets the handle it released last, so one thread
+# calling repeatedly reuses the same stream, HBM workspaces and, for bundle adjustment, NCCL communicator.
+_pool_lock = threading.Lock()
+_pool: Dict[Tuple[str, int], List[Handle]] = {}
+
+
+def acquire(kind: str, device: int = 0) -> Handle:
+    """A handle of `kind` on `device` that is the caller's alone until it calls release()."""
+    with _pool_lock:
+        free = _pool.get((kind, int(device)))
+        if free:
+            return free.pop()
+    return Handle(kind, device)
+
+
+def release(handle: Handle) -> None:
+    with _pool_lock:
+        _pool.setdefault((handle.kind, handle.device), []).append(handle)
+
+
+@contextlib.contextmanager
+def pooled(kind: str, device: int = 0) -> Iterator[Handle]:
+    """acquire() for the duration of a `with` block, released however the block ends."""
+    h = acquire(kind, device)
+    try:
+        yield h
+    finally:
+        release(h)

@@ -19,7 +19,6 @@ from typing import Optional
 import numpy as np
 
 from . import _lib
-from .matching import _thread_matcher
 
 
 class BagOfWords:
@@ -39,10 +38,10 @@ class BagOfWords:
         if d.ndim != 2 or d.shape[1] != self.words32.shape[1]:
             raise ValueError("descriptors must be n x %d" % self.words32.shape[1])
         out = np.empty((d.shape[0], min(int(k), len(self.words32))), dtype=np.int32)
-        m = _thread_matcher(self.device)
-        _lib.check(m.L.osfm_bow_map_to_words(m.h, d.ctypes.data_as(ctypes.c_void_p), d.shape[0], d.shape[1],
-                                             self.words32.ctypes.data_as(ctypes.c_void_p), len(self.words32), int(k),
-                                             out.ctypes.data_as(ctypes.c_void_p)))
+        with _lib.pooled("matcher", self.device) as m:
+            _lib.check(m.L.osfm_bow_map_to_words(m.h, d.ctypes.data_as(ctypes.c_void_p), d.shape[0], d.shape[1],
+                                                 self.words32.ctypes.data_as(ctypes.c_void_p), len(self.words32),
+                                                 int(k), out.ctypes.data_as(ctypes.c_void_p)))
         return out
 
     def histogram(self, words: np.ndarray) -> np.ndarray:
@@ -52,9 +51,10 @@ class BagOfWords:
             raise ValueError("word index out of range")
         wt = np.ascontiguousarray(self.weights, dtype=np.float64)
         out = np.empty(len(wt), dtype=np.float64)
-        m = _thread_matcher(self.device)
-        _lib.check(m.L.osfm_bow_histogram(m.h, w.ctypes.data_as(ctypes.c_void_p), len(w),
-                                          wt.ctypes.data_as(ctypes.c_void_p), len(wt), out.ctypes.data_as(ctypes.c_void_p)))
+        with _lib.pooled("matcher", self.device) as m:
+            _lib.check(m.L.osfm_bow_histogram(m.h, w.ctypes.data_as(ctypes.c_void_p), len(w),
+                                              wt.ctypes.data_as(ctypes.c_void_p), len(wt),
+                                              out.ctypes.data_as(ctypes.c_void_p)))
         return out
 
     def bow_distance(self, w1: np.ndarray, w2: np.ndarray, h1: Optional[np.ndarray] = None,
@@ -71,7 +71,7 @@ def bow_distance_rows(hist: np.ndarray, query: int, device: int = 0) -> np.ndarr
     """np.fabs(hist[query] - hist[i]).sum() for every row i, on the device (osfm_bow_distances)."""
     h = np.ascontiguousarray(hist, dtype=np.float64)
     out = np.zeros(h.shape[0], dtype=np.float64)
-    m = _thread_matcher(device)
-    _lib.check(m.L.osfm_bow_distances(m.h, h.ctypes.data_as(ctypes.c_void_p), h.shape[0], h.shape[1], int(query),
-                                      out.ctypes.data_as(ctypes.c_void_p)))
+    with _lib.pooled("matcher", device) as m:
+        _lib.check(m.L.osfm_bow_distances(m.h, h.ctypes.data_as(ctypes.c_void_p), h.shape[0], h.shape[1], int(query),
+                                          out.ctypes.data_as(ctypes.c_void_p)))
     return out

@@ -15,7 +15,6 @@ No CPU fallback: every `run()` goes to the GPU library.
 from __future__ import annotations
 
 import ctypes
-import threading
 from typing import Any, Dict, List, Optional, Sequence
 
 import numpy as np
@@ -23,38 +22,9 @@ import numpy as np
 from . import _lib
 from . import ba_problem as bp
 from . import types as T
+from ._lib import ptr
 
 _TERMINATION = {0: "CONVERGENCE", 1: "NO_CONVERGENCE", 2: "FAILURE"}
-
-# One engine handle per (thread, device): its HBM workspaces (Jacobian planes, reduced system, ...)
-# are kept between solves, so repeated bundle() calls do not pay cudaMalloc/cudaFree every time.
-_tls = threading.local()
-
-
-class _Handle:
-    def __init__(self, device: int):
-        self.L = _lib.load()
-        self.h = ctypes.c_void_p()
-        _lib.check(self.L.osfm_ba_create(int(device), ctypes.byref(self.h)))
-
-    def __del__(self):
-        try:
-            self.L.osfm_ba_destroy(self.h)
-        except Exception:
-            pass
-
-
-def _handle(device: int) -> "_Handle":
-    cache = getattr(_tls, "handles", None)
-    if cache is None:
-        cache = _tls.handles = {}
-    if device not in cache:
-        cache[device] = _Handle(device)
-    return cache[device]
-
-
-def _p(a: np.ndarray):
-    return a.ctypes.data_as(ctypes.c_void_p)
 
 
 def solve(pb: bp.BAProblem, device: int = 0, rank: int = 0, world: int = 1, allreduce=None,
@@ -77,43 +47,43 @@ def solve(pb: bp.BAProblem, device: int = 0, rank: int = 0, world: int = 1, allr
     (1-based) as the PCG received it, the PCG solution, the Jacobi scale, the LM diagonal, the gradient and the
     kernel paths that ran (osfm_ba_get_captured_system); raises if the solve ended before that iteration.
     `compute_covariances` (single GPU): the result gains "covariances" (NI x 6 x 6, the rig-instance pose covariances
-    in the problem's instance order, zeros for constant instances), "covariance_valid" and "covariance_status" (one of
-    _lib.COVARIANCE_STATUS).  As in the reference, an invalid estimate leaves every instance with the default
-    diag(1e-5, 1e-5, 1e-5, 1e-2, 1e-2, 1e-2)."""
+    in the problem's instance order, zeros for constant instances), "covariance_valid", "covariance_status" (one of
+    _lib.COVARIANCE_STATUS) and "covariance_ms", the device times (ms) of the covariance pass and of its Cholesky
+    factorisation (osfm_ba_get_covariance_timing).  As in the reference, an invalid estimate leaves every instance with
+    the default diag(1e-5, 1e-5, 1e-5, 1e-2, 1e-2, 1e-2)."""
     pb.validate(check_indices=False)
-    L = _lib.load()
-    h = _handle(int(device)).h
-    if True:
+    with _lib.pooled("ba", device) as hd:
+        L, h = hd.L, hd.h
         i32 = lambda a: np.ascontiguousarray(a, dtype=np.int32)
         f64 = lambda a: np.ascontiguousarray(a, dtype=np.float64)
         K, NI, NR = len(pb.cam_type), len(pb.inst), len(pb.rigcam)
         S, P, N = len(pb.shot_inst), len(pb.points), len(pb.obs_shot)
         keep = [i32(pb.cam_type), f64(pb.cam_params), i32(pb.cam_const), f64(pb.cam_prior), f64(pb.cam_prior_sigma),
                 i32(pb.cam_prior_log)]
-        _lib.check(L.osfm_ba_set_cameras(h, K, *[_p(a) for a in keep]))
+        _lib.check(L.osfm_ba_set_cameras(h, K, *[ptr(a) for a in keep]))
         k2 = [f64(pb.inst), i32(pb.inst_const), i32(pb.inst_has_prior), f64(pb.inst_prior_pos), f64(pb.inst_prior_std)]
-        _lib.check(L.osfm_ba_set_rig_instances(h, NI, *[_p(a) for a in k2]))
+        _lib.check(L.osfm_ba_set_rig_instances(h, NI, *[ptr(a) for a in k2]))
         k3 = [f64(pb.rigcam), i32(pb.rigcam_const)]
-        _lib.check(L.osfm_ba_set_rig_cameras(h, NR, *[_p(a) for a in k3]))
+        _lib.check(L.osfm_ba_set_rig_cameras(h, NR, *[ptr(a) for a in k3]))
         k4 = [i32(pb.shot_inst), i32(pb.shot_cam), i32(pb.shot_rc), i32(pb.shot_use_rc)]
-        _lib.check(L.osfm_ba_set_shots(h, S, *[_p(a) for a in k4]))
+        _lib.check(L.osfm_ba_set_shots(h, S, *[ptr(a) for a in k4]))
         k5 = [f64(pb.points), i32(pb.point_const)]
-        _lib.check(L.osfm_ba_set_points(h, P, *[_p(a) for a in k5]))
+        _lib.check(L.osfm_ba_set_points(h, P, *[ptr(a) for a in k5]))
         k6 = [i32(pb.obs_shot), i32(pb.obs_point), f64(pb.obs_xy), f64(pb.obs_sigma)]
         set_obs = L.osfm_ba_set_observations_async if pinned_inputs else L.osfm_ba_set_observations
-        _lib.check(set_obs(h, N, *[_p(a) for a in k6]))
+        _lib.check(set_obs(h, N, *[ptr(a) for a in k6]))
         # secondary residuals: always (re)set, the handle is reused between solves
         if pb.rigcam_prior is not None:
             k7 = [f64(pb.rigcam_prior), f64(pb.rigcam_prior_sigma)]
             if k7[0].shape != (NR, 6) or k7[1].shape != (NR, 6):
                 raise ValueError("rigcam_prior / rigcam_prior_sigma must be NR x 6")
-            _lib.check(L.osfm_ba_set_rig_camera_priors(h, _p(k7[0]), _p(k7[1])))
+            _lib.check(L.osfm_ba_set_rig_camera_priors(h, ptr(k7[0]), ptr(k7[1])))
         else:
             _lib.check(L.osfm_ba_set_rig_camera_priors(h, None, None))
         k8 = [i32(pb.pp_point), f64(pb.pp_prior), f64(pb.pp_sigma), i32(pb.pp_alt)]
-        _lib.check(L.osfm_ba_set_point_priors(h, len(k8[0]), *[_p(a) for a in k8]))
+        _lib.check(L.osfm_ba_set_point_priors(h, len(k8[0]), *[ptr(a) for a in k8]))
         k9 = [i32(pb.ext_size), f64(pb.ext_values), i32(pb.ext_const), f64(pb.ext_lower)]
-        _lib.check(L.osfm_ba_set_ext_blocks(h, len(k9[0]), *[_p(a) for a in k9]))
+        _lib.check(L.osfm_ba_set_ext_blocks(h, len(k9[0]), *[ptr(a) for a in k9]))
         recs, consts = pb.packed_side_terms()
         terms = (_lib.SideTerm * max(len(recs), 1))()
         for t, (ty, nres, nb, kind, idx, loss, loss_a, cofs, aux) in zip(terms, recs):
@@ -122,7 +92,8 @@ def solve(pb: bp.BAProblem, device: int = 0, rank: int = 0, world: int = 1, allr
             t.idx[:] = idx
             t.aux[:] = aux
         consts = f64(consts)
-        _lib.check(L.osfm_ba_set_side_terms(h, len(recs), ctypes.cast(terms, ctypes.c_void_p), len(consts), _p(consts)))
+        _lib.check(L.osfm_ba_set_side_terms(h, len(recs), ctypes.cast(terms, ctypes.c_void_p), len(consts),
+                                            ptr(consts)))
         if pb.loss_name not in _lib.LOSS_IDS:
             raise RuntimeError("ceres::LossFunction with name %s not found." % pb.loss_name)  # bundle_adjuster.cc:427
         _lib.check(L.osfm_ba_set_options(h, _lib.LOSS_IDS[pb.loss_name], float(pb.loss_threshold),
@@ -136,7 +107,6 @@ def solve(pb: bp.BAProblem, device: int = 0, rank: int = 0, world: int = 1, allr
                 if allreduce != "nccl":
                     raise ValueError("allreduce must be a callable or 'nccl'")
                 # the library's own NCCL communicator (one per handle; the 128-byte id travels over torch.distributed)
-                hd = _handle(int(device))
                 if getattr(hd, "nccl", None) != (int(rank), int(world)):
                     import torch.distributed as tdist
 
@@ -192,15 +162,15 @@ def solve(pb: bp.BAProblem, device: int = 0, rank: int = 0, world: int = 1, allr
         rep = _out("reprojection_errors", (N, 3))
         if not compute_reprojection_errors:
             rep[:] = 0.0
-        _lib.check(L.osfm_ba_get_cameras(h, _p(cam)))
-        _lib.check(L.osfm_ba_get_rig_instances(h, _p(inst)))
-        _lib.check(L.osfm_ba_get_rig_cameras(h, _p(rc)))
-        _lib.check(L.osfm_ba_get_points(h, _p(pts)))
+        _lib.check(L.osfm_ba_get_cameras(h, ptr(cam)))
+        _lib.check(L.osfm_ba_get_rig_instances(h, ptr(inst)))
+        _lib.check(L.osfm_ba_get_rig_cameras(h, ptr(rc)))
+        _lib.check(L.osfm_ba_get_points(h, ptr(pts)))
         if compute_reprojection_errors:
-            _lib.check(L.osfm_ba_get_reprojection_errors(h, _p(rep)))
+            _lib.check(L.osfm_ba_get_reprojection_errors(h, ptr(rep)))
         ext = np.zeros(len(k9[1]))
         if len(ext):
-            _lib.check(L.osfm_ba_get_ext_blocks(h, _p(ext)))
+            _lib.check(L.osfm_ba_get_ext_blocks(h, ptr(ext)))
         s = _lib.BASummary()
         _lib.check(L.osfm_ba_get_summary(h, ctypes.byref(s)))
         summary = {f[0]: getattr(s, f[0]) for f in s._fields_}
@@ -213,10 +183,13 @@ def solve(pb: bp.BAProblem, device: int = 0, rank: int = 0, world: int = 1, allr
         if compute_covariances:
             cov = np.zeros((NI, 6, 6))
             valid, status = ctypes.c_int(0), ctypes.c_int(0)
-            _lib.check(L.osfm_ba_get_covariances(h, ctypes.byref(valid), ctypes.byref(status), _p(cov)))
+            _lib.check(L.osfm_ba_get_covariances(h, ctypes.byref(valid), ctypes.byref(status), ptr(cov)))
             res["covariances"] = cov
             res["covariance_valid"] = bool(valid.value)
             res["covariance_status"] = _lib.COVARIANCE_STATUS[status.value]
+            pass_ms, chol_ms = ctypes.c_double(), ctypes.c_double()
+            _lib.check(L.osfm_ba_get_covariance_timing(h, ctypes.byref(pass_ms), ctypes.byref(chol_ms)))
+            res["covariance_ms"] = (pass_ms.value, chol_ms.value)
         return res
 
 
@@ -229,12 +202,13 @@ def _get_capture(L, h, ncam: int, NI: int, NR: int, P: int, next_: int) -> Dict[
     cap["pcg_kernel"] = _lib.PCG_KERNELS[info.pcg_kernel]
     arrs = {"S": np.zeros((nc, nc)), "rhs": np.zeros(nc), "y": np.zeros(nc), "scale": np.zeros(n), "diag": np.zeros(n),
             "grad": np.zeros(n)}
-    _lib.check(L.osfm_ba_get_captured_system(h, None, *[_p(arrs[k]) for k in ("S", "rhs", "y", "scale", "diag", "grad")]))
+    _lib.check(L.osfm_ba_get_captured_system(h, None, *[ptr(arrs[k]) for k in ("S", "rhs", "y", "scale", "diag",
+                                                                                 "grad")]))
     # the linearisation point of the captured iteration
     x = {"cam_params": np.zeros(ncam), "inst": np.zeros((NI, 6)), "rigcam": np.zeros((NR, 6)), "points": np.zeros((P, 3)),
          "ext_values": np.zeros(next_)}
-    _lib.check(L.osfm_ba_get_captured_parameters(h, *[_p(x[k]) for k in ("cam_params", "inst", "rigcam", "points",
-                                                                       "ext_values")]))
+    _lib.check(L.osfm_ba_get_captured_parameters(h, *[ptr(x[k]) for k in ("cam_params", "inst", "rigcam", "points",
+                                                                        "ext_values")]))
     cap.update(arrs)
     cap["x"] = x
     return cap
@@ -250,9 +224,9 @@ def eval_observation(projection_type: int, camera, rig_instance, rig_camera, use
     rc = f64(rig_camera if rig_camera is not None else np.zeros(6))
     r, jc, ji, jrc, jp = np.zeros(3), np.zeros(3 * 16), np.zeros(18), np.zeros(18), np.zeros(9)
     n = ctypes.c_int()
-    _lib.check(L.osfm_ba_eval_observation(device, int(projection_type), _p(cam), _p(ri), _p(rc), int(bool(use_rig_camera)),
-                                          _p(pt), _p(ob), float(std_deviation), _p(r), _p(jc), _p(ji), _p(jrc), _p(jp),
-                                          ctypes.byref(n)))
+    _lib.check(L.osfm_ba_eval_observation(device, int(projection_type), ptr(cam), ptr(ri), ptr(rc),
+                                          int(bool(use_rig_camera)), ptr(pt), ptr(ob), float(std_deviation), ptr(r),
+                                          ptr(jc), ptr(ji), ptr(jrc), ptr(jp), ctypes.byref(n)))
     k = n.value
     return (r[:k].copy(), jc[:k * C].reshape(k, C).copy(), ji[:k * 6].reshape(k, 6).copy(),
             jrc[:k * 6].reshape(k, 6).copy(), jp[:k * 3].reshape(k, 3).copy())

@@ -525,102 +525,94 @@ extern "C" {
 
 int osfm_matcher_bow_words(osfm_matcher* m, int count, const int* set_ids, const float* vocab, int nwords, int dim,
                            int k, int64_t* out_offsets, int32_t* out_words, int* out_valid) {
-  OSFM_API_BEGIN
   using namespace osfm;
-  MatcherGuard g(m);
-  if (count < 0) throw ArgError("bad BoW set count");
-  if (!out_offsets || (count > 0 && (!set_ids || !out_valid))) throw ArgError("null arrays");
-  check_word_args(vocab, nwords, dim, k);
-  bow_words_run(g.M, count, set_ids, vocab, nwords, dim, k, out_offsets, out_words, out_valid);
-  OSFM_API_END
+  return with_handle(m, [&](Matcher& M) {
+    if (count < 0) throw ArgError("bad BoW set count");
+    if (!out_offsets || (count > 0 && (!set_ids || !out_valid))) throw ArgError("null arrays");
+    check_word_args(vocab, nwords, dim, k);
+    bow_words_run(M, count, set_ids, vocab, nwords, dim, k, out_offsets, out_words, out_valid);
+  });
 }
 
 int osfm_bow_map_to_words(osfm_matcher* m, const float* desc, int n, int dim, const float* vocab, int nwords, int k,
                           int32_t* out) {
-  OSFM_API_BEGIN
   using namespace osfm;
-  MatcherGuard g(m);
-  Matcher& M = g.M;
-  if (n < 0 || (n > 0 && (!desc || !out))) throw ArgError("bad descriptor arguments");
-  check_word_args(vocab, nwords, dim, k);
-  const int id = M.add(desc, n, dim, false);
-  try {
-    int64_t offs[2];
-    int valid = 0;
-    bow_words_run(M, 1, &id, vocab, nwords, dim, k, offs, out, &valid);
-  } catch (...) {
+  return with_handle(m, [&](Matcher& M) {
+    if (n < 0 || (n > 0 && (!desc || !out))) throw ArgError("bad descriptor arguments");
+    check_word_args(vocab, nwords, dim, k);
+    const int id = M.add(desc, n, dim, false);
+    try {
+      int64_t offs[2];
+      int valid = 0;
+      bow_words_run(M, 1, &id, vocab, nwords, dim, k, offs, out, &valid);
+    } catch (...) {
+      M.remove(id);
+      throw;
+    }
     M.remove(id);
-    throw;
-  }
-  M.remove(id);
-  OSFM_API_END
+  });
 }
 
 int osfm_matcher_bow_histograms(osfm_matcher* m, int count, const int* set_ids, const double* weights, int nwords,
                                 int* out_valid) {
-  OSFM_API_BEGIN
   using namespace osfm;
-  MatcherGuard g(m);
-  Matcher& M = g.M;
-  if (count < 0 || nwords <= 0) throw ArgError("bad BoW histogram sizes");
-  if (!weights || (count > 0 && (!set_ids || !out_valid))) throw ArgError("null arrays");
-  const PairwisePlan P = pairwise_plan(nwords);
-  for (int i = 0; i < count; ++i)
-    if (!M.sets.count(set_ids[i])) throw ArgError("unknown descriptor set id");
-  OSFM_CUDA(cudaStreamSynchronize(M.stream));   // earlier work may still read histograms released below
-  // load_histograms: a set needs more than 8 words (pairs_selection.py:712-727)
-  std::vector<HistJob> jobs;
-  for (int i = 0; i < count; ++i) {
-    DescSet& s = M.sets[set_ids[i]];
-    M.release(s.bow_hist);
-    const bool valid = s.bow_words.p && s.bow_words.len == nwords && s.n > 8;
-    out_valid[i] = valid;
-    if (!valid) continue;
-    M.slab_new(s.bow_hist, sizeof(double) * (size_t)nwords, nwords);
-    jobs.push_back(HistJob{s.bow_words.p, s.bow_hist.p, s.n});
-  }
-  if (jobs.empty()) return OSFM_OK;
-  launch_bow_histograms(M, jobs, weights, nwords, P);
-  OSFM_CUDA(cudaStreamSynchronize(M.stream));
-  OSFM_API_END
+  return with_handle(m, [&](Matcher& M) {
+    if (count < 0 || nwords <= 0) throw ArgError("bad BoW histogram sizes");
+    if (!weights || (count > 0 && (!set_ids || !out_valid))) throw ArgError("null arrays");
+    const PairwisePlan P = pairwise_plan(nwords);
+    for (int i = 0; i < count; ++i)
+      if (!M.sets.count(set_ids[i])) throw ArgError("unknown descriptor set id");
+    OSFM_CUDA(cudaStreamSynchronize(M.stream));   // earlier work may still read histograms released below
+    // load_histograms: a set needs more than 8 words (pairs_selection.py:712-727)
+    std::vector<HistJob> jobs;
+    for (int i = 0; i < count; ++i) {
+      DescSet& s = M.sets[set_ids[i]];
+      M.release(s.bow_hist);
+      const bool valid = s.bow_words.p && s.bow_words.len == nwords && s.n > 8;
+      out_valid[i] = valid;
+      if (!valid) continue;
+      M.slab_new(s.bow_hist, sizeof(double) * (size_t)nwords, nwords);
+      jobs.push_back(HistJob{s.bow_words.p, s.bow_hist.p, s.n});
+    }
+    if (jobs.empty()) return;
+    launch_bow_histograms(M, jobs, weights, nwords, P);
+    OSFM_CUDA(cudaStreamSynchronize(M.stream));
+  });
 }
 
 int osfm_bow_histogram(osfm_matcher* m, const int32_t* words, int n, const double* weights, int nwords, double* out) {
-  OSFM_API_BEGIN
   using namespace osfm;
-  MatcherGuard g(m);
-  Matcher& M = g.M;
-  if (n < 0 || nwords <= 0 || !weights || !out || (n > 0 && !words)) throw ArgError("bad BoW histogram arguments");
-  for (int i = 0; i < n; ++i)
-    if (words[i] < 0 || words[i] >= nwords) throw ArgError("word index out of range");
-  const PairwisePlan P = pairwise_plan(nwords);
-  const size_t o_h = align256(sizeof(int) * (size_t)std::max(n, 1));
-  M.staging.reserve(o_h + sizeof(double) * (size_t)nwords);
-  int* d_w = reinterpret_cast<int*>(M.staging.p);
-  double* d_h = reinterpret_cast<double*>(M.staging.p + o_h);
-  if (n > 0) OSFM_CUDA(cudaMemcpyAsync(d_w, words, sizeof(int) * (size_t)n, cudaMemcpyHostToDevice, M.stream));
-  launch_bow_histograms(M, {HistJob{d_w, d_h, n}}, weights, nwords, P);
-  OSFM_CUDA(cudaMemcpyAsync(out, d_h, sizeof(double) * (size_t)nwords, cudaMemcpyDeviceToHost, M.stream));
-  OSFM_CUDA(cudaStreamSynchronize(M.stream));
-  OSFM_API_END
+  return with_handle(m, [&](Matcher& M) {
+    if (n < 0 || nwords <= 0 || !weights || !out || (n > 0 && !words)) throw ArgError("bad BoW histogram arguments");
+    for (int i = 0; i < n; ++i)
+      if (words[i] < 0 || words[i] >= nwords) throw ArgError("word index out of range");
+    const PairwisePlan P = pairwise_plan(nwords);
+    const size_t o_h = align256(sizeof(int) * (size_t)std::max(n, 1));
+    M.staging.reserve(o_h + sizeof(double) * (size_t)nwords);
+    int* d_w = reinterpret_cast<int*>(M.staging.p);
+    double* d_h = reinterpret_cast<double*>(M.staging.p + o_h);
+    if (n > 0) OSFM_CUDA(cudaMemcpyAsync(d_w, words, sizeof(int) * (size_t)n, cudaMemcpyHostToDevice, M.stream));
+    launch_bow_histograms(M, {HistJob{d_w, d_h, n}}, weights, nwords, P);
+    OSFM_CUDA(cudaMemcpyAsync(out, d_h, sizeof(double) * (size_t)nwords, cudaMemcpyDeviceToHost, M.stream));
+    OSFM_CUDA(cudaStreamSynchronize(M.stream));
+  });
 }
 
 int osfm_matcher_bow_get(osfm_matcher* m, int set_id, double* out) {
-  OSFM_API_BEGIN
   using namespace osfm;
-  if (!m || !out) throw ArgError("null arguments");
-  MatcherGuard g(m);
-  const SlabArray<double>& h = BowRows::of(g.M, set_id, -1);
-  OSFM_CUDA(cudaMemcpyAsync(out, h.p, sizeof(double) * (size_t)h.len, cudaMemcpyDeviceToHost, g.M.stream));
-  OSFM_CUDA(cudaStreamSynchronize(g.M.stream));
-  OSFM_API_END
+  return with_handle(m, [&](Matcher& M) {
+    if (!out) throw ArgError("null arguments");
+    const SlabArray<double>& h = BowRows::of(M, set_id, -1);
+    OSFM_CUDA(cudaMemcpyAsync(out, h.p, sizeof(double) * (size_t)h.len, cudaMemcpyDeviceToHost, M.stream));
+    OSFM_CUDA(cudaStreamSynchronize(M.stream));
+  });
 }
 
 int osfm_matcher_bow_select(osfm_matcher* m, int nref, const int* ref_ids, int ncand, const int* cand_ids,
                             const int32_t* cand_order, const int* camera_labels, int k, int64_t* out_offsets,
                             int32_t* out_cols, double* out_dist) {
   using namespace osfm;
-  return with_matcher(m, [&](Matcher& M) {
+  return with_handle(m, [&](Matcher& M) {
     if (nref < 0 || ncand < 0 || k < 0) throw ArgError("bad BoW selection sizes");
     BowRows kind;
     select_neighbors(M, kind, nref, ref_ids, ncand, cand_ids, nullptr, cand_order, camera_labels, k, out_offsets,
@@ -630,7 +622,7 @@ int osfm_matcher_bow_select(osfm_matcher* m, int nref, const int* ref_ids, int n
 
 int osfm_bow_distances(osfm_matcher* m, const double* hist, int n, int len, int query, double* out_n) {
   using namespace osfm;
-  return with_matcher(m, [&](Matcher& M) {
+  return with_handle(m, [&](Matcher& M) {
     if (n <= 0 || len <= 0 || query < 0 || query >= n || !hist || !out_n) throw ArgError("bad BoW distance arguments");
     BowRows kind;
     distances_to_row(M, kind, hist, n, len, query, out_n);

@@ -2,13 +2,16 @@
 #pragma once
 #include <cuda_runtime.h>
 
+#include <algorithm>
 #include <atomic>
 #include <cstdarg>
 #include <cstdint>
 #include <cstdio>
 #include <cstring>
+#include <mutex>
 #include <stdexcept>
 #include <string>
+#include <vector>
 
 #include "../../include/opensfm_b200.h"
 
@@ -96,5 +99,97 @@ struct PinnedBuf {
     cap = want;
   }
 };
+
+// Copies of n elements on stream st.  The device buffer grows to hold at least one element, so that its pointer is
+// never null, even for an empty upload.
+template <class T>
+void upload(DevBuf<T>& d, const T* h, size_t n, cudaStream_t st) {
+  d.reserve(std::max<size_t>(n, 1));
+  if (n) OSFM_CUDA(cudaMemcpyAsync(d.p, h, sizeof(T) * n, cudaMemcpyHostToDevice, st));
+}
+template <class T>
+void upload(DevBuf<T>& d, const std::vector<T>& h, cudaStream_t st) {
+  upload(d, h.data(), h.size(), st);
+}
+template <class T>
+void download(T* h, const T* d, size_t n, cudaStream_t st) {
+  if (n) OSFM_CUDA(cudaMemcpyAsync(h, d, sizeof(T) * n, cudaMemcpyDeviceToHost, st));
+}
+template <class T>
+void download(std::vector<T>& h, const T* d, size_t n, cudaStream_t st) {
+  h.resize(n);
+  download(h.data(), d, n, st);
+}
+
+// An engine's device, its non-blocking stream there and NEV timing events, with the copies on that stream.
+template <int NEV>
+struct DeviceStream {
+  int device;
+  cudaStream_t stream = nullptr;
+  cudaEvent_t ev[NEV] = {};
+
+  explicit DeviceStream(int dev) : device(dev) {
+    OSFM_CUDA(cudaSetDevice(device));
+    OSFM_CUDA(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));
+    for (auto& e : ev) OSFM_CUDA(cudaEventCreate(&e));
+  }
+  ~DeviceStream() {
+    for (auto& e : ev)
+      if (e) cudaEventDestroy(e);
+    if (stream) cudaStreamDestroy(stream);
+  }
+  DeviceStream(const DeviceStream&) = delete;
+  DeviceStream& operator=(const DeviceStream&) = delete;
+
+  template <class T>
+  void upload(DevBuf<T>& d, const T* h, size_t n) {
+    ::osfm::upload(d, h, n, stream);
+  }
+  template <class T>
+  void download(T* h, const T* d, size_t n) {
+    ::osfm::download(h, d, n, stream);
+  }
+};
+
+// What stands behind one C-ABI handle (osfm_ba, osfm_matcher, osfm_tracks, osfm_rotransac): the engine object and the
+// lock that serialises calls on it.  The engine's methods expect its device to be current: with_handle makes it so
+// for every entry point, and the destructor for the engine's own destructor, which frees its device memory.
+template <class Engine>
+struct Handle {
+  std::mutex mu;
+  Engine impl;
+  explicit Handle(int device) : impl(device) {}
+  ~Handle() { cudaSetDevice(impl.device); }
+};
+
+// osfm_<kind>_create and osfm_<kind>_destroy.
+template <class H>
+int create_handle(int device, H** out) {
+  OSFM_API_BEGIN
+  if (!out) throw ArgError("null out");
+  int count = 0;
+  OSFM_CUDA(cudaGetDeviceCount(&count));
+  if (device < 0 || device >= count) throw ArgError("no such CUDA device");
+  *out = new H(device);
+  OSFM_API_END
+}
+template <class H>
+int destroy_handle(H* h) {
+  OSFM_API_BEGIN
+  delete h;
+  OSFM_API_END
+}
+
+// Every other entry point on a handle: body(engine) under the handle's lock with its device current, exceptions
+// turned into error codes.  The lock is not recursive, so body must not re-enter the same handle.
+template <class H, class F>
+int with_handle(H* h, F&& body) {
+  OSFM_API_BEGIN
+  if (!h) throw ArgError(H::null_message);
+  std::lock_guard<std::mutex> lock(h->mu);
+  OSFM_CUDA(cudaSetDevice(h->impl.device));
+  body(h->impl);
+  OSFM_API_END
+}
 
 }  // namespace osfm

@@ -468,23 +468,17 @@ __global__ void __launch_bounds__(256) epi_mask_bits(const EpiPair* __restrict__
 }
 
 // ---------------------------------------------------------------------------
-// Matcher object (its methods run under the C ABI's MatcherGuard, which makes the device current)
+// Matcher object (its methods run under the C ABI's with_handle, which makes the device current)
 // ---------------------------------------------------------------------------
-Matcher::Matcher(int dev) : device(dev) {
-  OSFM_CUDA(cudaSetDevice(device));
-  OSFM_CUDA(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));
-  for (auto& e : ev) OSFM_CUDA(cudaEventCreate(&e));
+Matcher::Matcher(int dev) : DeviceStream(dev) {
   cudaDeviceProp prop;
   OSFM_CUDA(cudaGetDeviceProperties(&prop, device));
   num_sms = prop.multiProcessorCount;
 }
 
 Matcher::~Matcher() {
-  cudaSetDevice(device);
   cudaStreamSynchronize(stream);
   for (auto& sl : slabs) cudaFree(sl.base);
-  for (auto& e : ev) cudaEventDestroy(e);
-  cudaStreamDestroy(stream);
 }
 
 void* Matcher::slab_alloc(size_t bytes, int* slab_idx) {
@@ -992,36 +986,23 @@ using osfm::Matcher;
 
 extern "C" {
 
-int osfm_matcher_create(int device, osfm_matcher** out) {
-  OSFM_API_BEGIN
-  if (!out) throw osfm::ArgError("null out");
-  int count = 0;
-  OSFM_CUDA(cudaGetDeviceCount(&count));
-  if (device < 0 || device >= count) throw osfm::ArgError("no such CUDA device");
-  *out = new osfm_matcher(device);
-  OSFM_API_END
-}
-
-int osfm_matcher_destroy(osfm_matcher* m) {
-  OSFM_API_BEGIN
-  delete m;
-  OSFM_API_END
-}
+int osfm_matcher_create(int device, osfm_matcher** out) { return osfm::create_handle(device, out); }
+int osfm_matcher_destroy(osfm_matcher* m) { return osfm::destroy_handle(m); }
 
 int osfm_bf_match_f32(osfm_matcher* m, const float* f1, int n1, const float* f2, int n2, int dim,
                       double lowes_ratio, const uint8_t* mask, int symmetric, int32_t* out_match) {
-  return osfm::with_matcher(
+  return osfm::with_handle(
       m, [&](Matcher& M) { M.one_shot(f1, n1, f2, n2, dim, false, lowes_ratio, mask, symmetric != 0, out_match); });
 }
 
 int osfm_bf_match_u8(osfm_matcher* m, const uint8_t* f1, int n1, const uint8_t* f2, int n2, int nbytes,
                      double lowes_ratio, const uint8_t* mask, int symmetric, int32_t* out_match) {
-  return osfm::with_matcher(
+  return osfm::with_handle(
       m, [&](Matcher& M) { M.one_shot(f1, n1, f2, n2, nbytes, true, lowes_ratio, mask, symmetric != 0, out_match); });
 }
 
 static int add_one(osfm_matcher* m, const void* desc, int n, int dim, bool u8, int* out_id, bool u8_as_l2 = false) {
-  return osfm::with_matcher(m, [&](Matcher& M) {
+  return osfm::with_handle(m, [&](Matcher& M) {
     if (!out_id) throw osfm::ArgError("null out_id");
     *out_id = M.add(desc, n, dim, u8, u8_as_l2);
   });
@@ -1035,7 +1016,7 @@ int osfm_matcher_add_u8(osfm_matcher* m, const uint8_t* desc, int n, int nbytes,
 
 static int add_batch(osfm_matcher* m, int count, const void* const* desc, const int* n, int dim, bool u8, int* out_ids,
                      bool u8_as_l2 = false) {
-  return osfm::with_matcher(m, [&](Matcher& M) {
+  return osfm::with_handle(m, [&](Matcher& M) {
     if (count < 0 || (count > 0 && (!desc || !n || !out_ids))) throw osfm::ArgError("bad batch arguments");
     int done = 0;
     try {
@@ -1065,28 +1046,28 @@ int osfm_matcher_add_batch_u8_l2(osfm_matcher* m, int count, const uint8_t* cons
 }
 
 int osfm_matcher_remove(osfm_matcher* m, int id) {
-  return osfm::with_matcher(m, [&](Matcher& M) { M.remove(id); });
+  return osfm::with_handle(m, [&](Matcher& M) { M.remove(id); });
 }
 
 int osfm_matcher_clear(osfm_matcher* m) {
-  return osfm::with_matcher(m, [&](Matcher& M) { M.clear(); });
+  return osfm::with_handle(m, [&](Matcher& M) { M.clear(); });
 }
 
 int osfm_matcher_match_pairs_async(osfm_matcher* m, int npairs, const int* ids_a, const int* ids_b,
                                    double lowes_ratio, int symmetric) {
-  return osfm::with_matcher(m, [&](Matcher& M) {
+  return osfm::with_handle(m, [&](Matcher& M) {
     if (npairs > 0 && (!ids_a || !ids_b)) throw osfm::ArgError("null pair list");
     M.match_pairs_async(npairs, ids_a, ids_b, lowes_ratio, symmetric != 0, nullptr);
   });
 }
 
 int osfm_matcher_set_bearings(osfm_matcher* m, int id, const float* bearings_n_by_3) {
-  return osfm::with_matcher(m, [&](Matcher& M) { M.set_bearings(id, bearings_n_by_3); });
+  return osfm::with_handle(m, [&](Matcher& M) { M.set_bearings(id, bearings_n_by_3); });
 }
 
 int osfm_matcher_match_pairs_guided_async(osfm_matcher* m, int npairs, const int* ids_a, const int* ids_b,
                                           const double* pose12, double threshold, double lowes_ratio, int symmetric) {
-  return osfm::with_matcher(m, [&](Matcher& M) {
+  return osfm::with_handle(m, [&](Matcher& M) {
     if (npairs > 0 && (!ids_a || !ids_b || !pose12)) throw osfm::ArgError("null pair list / poses");
     // any threshold is the reference's comparison `angle < threshold`: at or below 0 nothing passes
     if (std::isnan(threshold)) throw osfm::ArgError("guided matching threshold is NaN");
@@ -1095,20 +1076,20 @@ int osfm_matcher_match_pairs_guided_async(osfm_matcher* m, int npairs, const int
 }
 
 int osfm_matcher_get_epipolar_masks(osfm_matcher* m, int pair, uint32_t* F, uint32_t* T) {
-  return osfm::with_matcher(m, [&](Matcher& M) { M.get_epipolar_masks(pair, F, T); });
+  return osfm::with_handle(m, [&](Matcher& M) { M.get_epipolar_masks(pair, F, T); });
 }
 
 int osfm_matcher_sync(osfm_matcher* m) {
-  return osfm::with_matcher(m, [&](Matcher& M) { OSFM_CUDA(cudaStreamSynchronize(M.stream)); });
+  return osfm::with_handle(m, [&](Matcher& M) { OSFM_CUDA(cudaStreamSynchronize(M.stream)); });
 }
 
 int osfm_matcher_fetch(osfm_matcher* m, int32_t* out_match, int64_t capacity) {
-  return osfm::with_matcher(m, [&](Matcher& M) { M.fetch(out_match, capacity); });
+  return osfm::with_handle(m, [&](Matcher& M) { M.fetch(out_match, capacity); });
 }
 
 int osfm_matcher_fetch_pairs(osfm_matcher* m, int64_t* offsets_out, int32_t* pairs_out, int64_t capacity_rows,
                              int64_t* total_rows) {
-  return osfm::with_matcher(m, [&](Matcher& M) {
+  return osfm::with_handle(m, [&](Matcher& M) {
     if (!offsets_out || !total_rows || (capacity_rows > 0 && !pairs_out)) throw osfm::ArgError("null output");
     static_assert(sizeof(long long) == sizeof(int64_t), "offsets are 64-bit");
     *total_rows = M.fetch_pairs(reinterpret_cast<long long*>(offsets_out), pairs_out, capacity_rows);
@@ -1116,30 +1097,35 @@ int osfm_matcher_fetch_pairs(osfm_matcher* m, int64_t* offsets_out, int32_t* pai
 }
 
 int osfm_matcher_last_device_ms(osfm_matcher* m, float* ms_total, float* ms_distance_kernel) {
-  return osfm::with_matcher(m, [&](Matcher& M) { M.last_ms(ms_total, ms_distance_kernel); });
+  return osfm::with_handle(m, [&](Matcher& M) { M.last_ms(ms_total, ms_distance_kernel); });
 }
 
 int osfm_matcher_set_kernel(osfm_matcher* m, int which) {
-  return osfm::with_matcher(m, [&](Matcher& M) {
+  return osfm::with_handle(m, [&](Matcher& M) {
     if (which < 0 || which > 2) throw osfm::ArgError("kernel must be 0, 1 or 2");
     M.kernel_choice = which;
   });
 }
 
-int osfm_matcher_last_kernel(osfm_matcher* m) { return m ? m->impl.last_kernel : 0; }
+// returns the kernel, not an error code, and 0 when the call fails (a null matcher, for one)
+int osfm_matcher_last_kernel(osfm_matcher* m) {
+  int kernel = 0;
+  osfm::with_handle(m, [&](Matcher& M) { kernel = M.last_kernel; });
+  return kernel;
+}
+
 int osfm_matcher_device_bytes(osfm_matcher* m, int64_t* reserved, int64_t* in_use) {
-  OSFM_API_BEGIN
-  if (!m || !reserved || !in_use) throw osfm::ArgError("null argument");
-  osfm::MatcherGuard g(m);
-  int64_t cap = 0, used = 0;
-  for (const auto& sl : g.M.slabs) {
-    cap += (int64_t)sl.cap;
-    used += (int64_t)sl.used;
-    for (const auto& fr : sl.free_ranges) used -= (int64_t)fr.second;
-  }
-  *reserved = cap;
-  *in_use = used;
-  OSFM_API_END
+  return osfm::with_handle(m, [&](Matcher& M) {
+    if (!reserved || !in_use) throw osfm::ArgError("null argument");
+    int64_t cap = 0, used = 0;
+    for (const auto& sl : M.slabs) {
+      cap += (int64_t)sl.cap;
+      used += (int64_t)sl.used;
+      for (const auto& fr : sl.free_ranges) used -= (int64_t)fr.second;
+    }
+    *reserved = cap;
+    *in_use = used;
+  });
 }
 
 }  // extern "C"

@@ -3,7 +3,6 @@
 #include <cuda_bf16.h>
 
 #include <map>
-#include <mutex>
 #include <vector>
 
 #include "common.cuh"
@@ -227,11 +226,8 @@ struct Slab {
   std::vector<std::pair<size_t, size_t>> free_ranges;
 };
 
-// Its methods expect the device to be current; the C entry points make it so (MatcherGuard, with_matcher below).
-struct Matcher {
-  int device;
-  cudaStream_t stream = nullptr;
-  cudaEvent_t ev[4];
+// Its methods expect the device to be current; the C entry points make it so (with_handle).
+struct Matcher : DeviceStream<4> {
   int num_sms = 132;
   int next_id = 1;
   int kernel_choice = 0;
@@ -275,8 +271,6 @@ struct Matcher {
 
   explicit Matcher(int dev);
   ~Matcher();
-  Matcher(const Matcher&) = delete;
-  Matcher& operator=(const Matcher&) = delete;
 
   std::vector<Slab> slabs;
   DevBuf<int> d_info;                 // [MAX_SLOTS][2]: not-exact flag, max |x|^2 (float bits)
@@ -360,29 +354,7 @@ struct TableLayout {
 
 }  // namespace osfm
 
-// The C ABI's matcher handle.
-struct osfm_matcher {
-  osfm::Matcher impl;
-  std::mutex mu;
-  explicit osfm_matcher(int dev) : impl(dev) {}
+struct osfm_matcher : osfm::Handle<osfm::Matcher> {
+  using Handle::Handle;
+  static constexpr const char* null_message = "null matcher";
 };
-
-namespace osfm {
-// The preamble of every matcher entry point: a null check, the matcher's lock and its device made current.
-struct MatcherGuard {
-  std::lock_guard<std::mutex> lock;
-  Matcher& M;
-  explicit MatcherGuard(osfm_matcher* m) : lock((m ? m : throw ArgError("null matcher"))->mu), M(m->impl) {
-    OSFM_CUDA(cudaSetDevice(M.device));
-  }
-};
-
-// A matcher entry point: body(M) under MatcherGuard, its exceptions turned into error codes.
-template <class F>
-int with_matcher(osfm_matcher* m, F&& body) {
-  OSFM_API_BEGIN
-  MatcherGuard g(m);
-  body(g.M);
-  OSFM_API_END
-}
-}  // namespace osfm

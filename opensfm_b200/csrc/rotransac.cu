@@ -19,7 +19,6 @@
 #include <climits>
 #include <cmath>
 #include <memory>
-#include <mutex>
 #include <numeric>
 #include <vector>
 
@@ -425,10 +424,7 @@ __global__ void __launch_bounds__(RR_THREADS) rr_ransac(RrArgs a, int staged) {
   }
 }
 
-struct RotRansac {
-  int device;
-  cudaStream_t stream = nullptr;
-  cudaEvent_t ev[2] = {nullptr, nullptr};
+struct RotRansac : DeviceStream<2> {
   bool timed = false;
   long long prefix_len = 0, prefix_want = RR_DEFAULT_PREFIX;
   int trace_cap = 0;
@@ -441,27 +437,7 @@ struct RotRansac {
   DevBuf<int> d_order, d_best_rows, d_ransac, d_chord, d_trace, d_trace_count;
   DevBuf<unsigned char> d_mask;
 
-  explicit RotRansac(int dev) : device(dev) {
-    OSFM_CUDA(cudaSetDevice(device));
-    OSFM_CUDA(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));
-    for (auto& e : ev) OSFM_CUDA(cudaEventCreate(&e));
-  }
-  ~RotRansac() {
-    cudaSetDevice(device);
-    for (auto& e : ev)
-      if (e) cudaEventDestroy(e);
-    if (stream) cudaStreamDestroy(stream);
-  }
-
-  template <class T>
-  void upload(DevBuf<T>& d, const T* h, size_t n) {
-    d.reserve(std::max<size_t>(n, 1));
-    if (n) OSFM_CUDA(cudaMemcpyAsync(d.p, h, sizeof(T) * n, cudaMemcpyHostToDevice, stream));
-  }
-  template <class T>
-  void download(T* h, const T* d, size_t n) {
-    if (n) OSFM_CUDA(cudaMemcpyAsync(h, d, sizeof(T) * n, cudaMemcpyDeviceToHost, stream));
-  }
+  explicit RotRansac(int dev) : DeviceStream(dev) {}
 
   // the first prefix_want outputs of mt19937(42) and the generator after them
   void make_prefix() {
@@ -585,82 +561,57 @@ void RotRansac::run(int64_t num_bearings, const double* bearings, int64_t num_pa
 }  // namespace
 }  // namespace osfm
 
-struct osfm_rotransac {
-  std::mutex mu;
-  osfm::RotRansac impl;
-  explicit osfm_rotransac(int device) : impl(device) {}
+struct osfm_rotransac : osfm::Handle<osfm::RotRansac> {
+  using Handle::Handle;
+  static constexpr const char* null_message = "null rotation RANSAC";
 };
-
-#define OSFM_RR_LOCK                                       \
-  if (!h) throw osfm::ArgError("null rotation RANSAC");    \
-  std::lock_guard<std::mutex> lock(h->mu);                 \
-  osfm::RotRansac& K = h->impl;                            \
-  OSFM_CUDA(cudaSetDevice(K.device));
 
 extern "C" {
 
-int osfm_rotransac_create(int device, osfm_rotransac** out) {
-  OSFM_API_BEGIN
-  if (!out) throw osfm::ArgError("null out");
-  int count = 0;
-  OSFM_CUDA(cudaGetDeviceCount(&count));
-  if (device < 0 || device >= count) throw osfm::ArgError("no such CUDA device");
-  *out = new osfm_rotransac(device);
-  OSFM_API_END
-}
-
-int osfm_rotransac_destroy(osfm_rotransac* h) {
-  OSFM_API_BEGIN
-  delete h;
-  OSFM_API_END
-}
+int osfm_rotransac_create(int device, osfm_rotransac** out) { return osfm::create_handle(device, out); }
+int osfm_rotransac_destroy(osfm_rotransac* h) { return osfm::destroy_handle(h); }
 
 int osfm_rotransac_run(osfm_rotransac* h, int64_t num_bearings, const double* bearings, int64_t num_pairs,
                        const int64_t* pair_start, const int64_t* row_a, const int64_t* row_b, double threshold,
                        int iterations, double* lo_model, int32_t* ransac_inliers, int32_t* chord_inliers,
                        uint8_t* chord_mask) {
-  OSFM_API_BEGIN
-  OSFM_RR_LOCK
-  K.run(num_bearings, bearings, num_pairs, pair_start, row_a, row_b, threshold, iterations, lo_model, ransac_inliers,
-        chord_inliers, chord_mask);
-  OSFM_API_END
+  return osfm::with_handle(h, [&](osfm::RotRansac& K) {
+    K.run(num_bearings, bearings, num_pairs, pair_start, row_a, row_b, threshold, iterations, lo_model, ransac_inliers,
+          chord_inliers, chord_mask);
+  });
 }
 
 int osfm_rotransac_set_stream_prefix(osfm_rotransac* h, int64_t length) {
-  OSFM_API_BEGIN
-  OSFM_RR_LOCK
-  if (length < 1 || length > (1LL << 28)) throw osfm::ArgError("stream prefix length must be in [1, 2^28]");
-  K.prefix_want = length;
-  OSFM_API_END
+  return osfm::with_handle(h, [&](osfm::RotRansac& K) {
+    if (length < 1 || length > (1LL << 28)) throw osfm::ArgError("stream prefix length must be in [1, 2^28]");
+    K.prefix_want = length;
+  });
 }
 
 int osfm_rotransac_set_trace(osfm_rotransac* h, int capacity) {
-  OSFM_API_BEGIN
-  OSFM_RR_LOCK
-  if (capacity < 0) throw osfm::ArgError("negative trace capacity");
-  K.trace_cap = capacity;
-  OSFM_API_END
+  return osfm::with_handle(h, [&](osfm::RotRansac& K) {
+    if (capacity < 0) throw osfm::ArgError("negative trace capacity");
+    K.trace_cap = capacity;
+  });
 }
 
 int osfm_rotransac_get_trace(osfm_rotransac* h, int32_t* count, int64_t* stream_used, int32_t* indices) {
-  OSFM_API_BEGIN
-  OSFM_RR_LOCK
-  if (!K.timed || K.trace_cap == 0) throw std::runtime_error("rotation RANSAC: no traced run");
-  if (!count || !stream_used || !indices) throw osfm::ArgError("null outputs");
-  K.download(count, K.d_trace_count.p, (size_t)K.P);
-  K.download(reinterpret_cast<long long*>(stream_used), K.d_stream_used.p, (size_t)K.P);
-  K.download(indices, K.d_trace.p, (size_t)K.P * K.trace_cap);
-  OSFM_CUDA(cudaStreamSynchronize(K.stream));
-  OSFM_API_END
+  return osfm::with_handle(h, [&](osfm::RotRansac& K) {
+    if (!K.timed || K.trace_cap == 0) throw std::runtime_error("rotation RANSAC: no traced run");
+    if (!count || !stream_used || !indices) throw osfm::ArgError("null outputs");
+    K.download(count, K.d_trace_count.p, (size_t)K.P);
+    K.download(reinterpret_cast<long long*>(stream_used), K.d_stream_used.p, (size_t)K.P);
+    K.download(indices, K.d_trace.p, (size_t)K.P * K.trace_cap);
+    OSFM_CUDA(cudaStreamSynchronize(K.stream));
+  });
 }
 
 int osfm_rotransac_last_device_ms(osfm_rotransac* h, float* ms) {
-  OSFM_API_BEGIN
-  OSFM_RR_LOCK
-  if (!ms) throw osfm::ArgError("null ms");
-  *ms = 0.f;
-  if (K.timed) OSFM_CUDA(cudaEventElapsedTime(ms, K.ev[0], K.ev[1]));
-  OSFM_API_END
+  return osfm::with_handle(h, [&](osfm::RotRansac& K) {
+    if (!ms) throw osfm::ArgError("null ms");
+    *ms = 0.f;
+    if (K.timed) OSFM_CUDA(cudaEventElapsedTime(ms, K.ev[0], K.ev[1]));
+  });
 }
 
 }  // extern "C"

@@ -20,7 +20,6 @@
 
 #include <algorithm>
 #include <cub/cub.cuh>
-#include <mutex>
 #include <vector>
 
 #include "common.cuh"
@@ -250,10 +249,7 @@ int trk_bits(unsigned long long max_value) {
   return b;
 }
 
-struct Tracks {
-  int device;
-  cudaStream_t stream = nullptr;
-  cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};   // build start / end, common start / end
+struct Tracks : DeviceStream<4> {   // events: build start / end, common start / end
   bool built = false, common_built = false, timed_build = false, timed_common = false;
   int I = 0, T = 0, Q = 0;
   long long nobs = 0, R = 0;
@@ -277,31 +273,13 @@ struct Tracks {
   PinnedBuf<TrkCounts> h_counts;
   PinnedBuf<long long> h_ll;
 
-  explicit Tracks(int dev) : device(dev) {
-    OSFM_CUDA(cudaSetDevice(device));
-    OSFM_CUDA(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));
-    for (auto& e : ev) OSFM_CUDA(cudaEventCreate(&e));
+  explicit Tracks(int dev) : DeviceStream(dev) {
     d_counts.reserve(1);
     d_num_selected.reserve(1);
     h_counts.reserve(1);
     h_ll.reserve(1);
   }
-  ~Tracks() {
-    cudaSetDevice(device);
-    for (auto& e : ev)
-      if (e) cudaEventDestroy(e);
-    if (stream) cudaStreamDestroy(stream);
-  }
 
-  template <class T>
-  void upload(DevBuf<T>& d, const T* h, size_t n) {
-    d.reserve(n);
-    if (n) OSFM_CUDA(cudaMemcpyAsync(d.p, h, sizeof(T) * n, cudaMemcpyHostToDevice, stream));
-  }
-  template <class T>
-  void download(T* h, const T* d, size_t n) {
-    if (n) OSFM_CUDA(cudaMemcpyAsync(h, d, sizeof(T) * n, cudaMemcpyDeviceToHost, stream));
-  }
   const TrkCounts& read_counts() {
     OSFM_CUDA(cudaMemcpyAsync(h_counts.p, d_counts.p, sizeof(TrkCounts), cudaMemcpyDeviceToHost, stream));
     OSFM_CUDA(cudaStreamSynchronize(stream));
@@ -531,99 +509,73 @@ void Tracks::common(int64_t* num_pairs, int64_t* num_common) {
 }  // namespace
 }  // namespace osfm
 
-struct osfm_tracks {
-  std::mutex mu;
-  osfm::Tracks impl;
-  explicit osfm_tracks(int device) : impl(device) {}
+struct osfm_tracks : osfm::Handle<osfm::Tracks> {
+  using Handle::Handle;
+  static constexpr const char* null_message = "null tracks";
 };
-
-#define OSFM_T_LOCK                              \
-  if (!t) throw osfm::ArgError("null tracks");   \
-  std::lock_guard<std::mutex> lock(t->mu);       \
-  osfm::Tracks& K = t->impl;                     \
-  OSFM_CUDA(cudaSetDevice(K.device));
 
 extern "C" {
 
-int osfm_tracks_create(int device, osfm_tracks** out) {
-  OSFM_API_BEGIN
-  if (!out) throw osfm::ArgError("null out");
-  int count = 0;
-  OSFM_CUDA(cudaGetDeviceCount(&count));
-  if (device < 0 || device >= count) throw osfm::ArgError("no such CUDA device");
-  *out = new osfm_tracks(device);
-  OSFM_API_END
-}
-
-int osfm_tracks_destroy(osfm_tracks* t) {
-  OSFM_API_BEGIN
-  delete t;
-  OSFM_API_END
-}
+int osfm_tracks_create(int device, osfm_tracks** out) { return osfm::create_handle(device, out); }
+int osfm_tracks_destroy(osfm_tracks* t) { return osfm::destroy_handle(t); }
 
 int osfm_tracks_build(osfm_tracks* t, int num_images, const int32_t* num_features, const uint8_t* has_features,
                       int64_t num_pairs, const int32_t* pair_a, const int32_t* pair_b, const int64_t* match_start,
                       const int32_t* matches, int min_length, int64_t* num_tracks, int64_t* num_observations) {
-  OSFM_API_BEGIN
-  OSFM_T_LOCK
-  K.build(num_images, num_features, has_features, num_pairs, pair_a, pair_b, match_start, matches, min_length,
-          num_tracks, num_observations);
-  OSFM_API_END
+  return osfm::with_handle(t, [&](osfm::Tracks& K) {
+    K.build(num_images, num_features, has_features, num_pairs, pair_a, pair_b, match_start, matches, min_length,
+            num_tracks, num_observations);
+  });
 }
 
 int osfm_tracks_get(osfm_tracks* t, int32_t* obs_track, int32_t* obs_image, int32_t* obs_feature,
                     int64_t* track_start) {
-  OSFM_API_BEGIN
-  OSFM_T_LOCK
-  if (!K.built) throw std::runtime_error("tracks: osfm_tracks_get needs a successful osfm_tracks_build");
-  if (!track_start || (K.nobs > 0 && (!obs_track || !obs_image || !obs_feature))) throw osfm::ArgError("null outputs");
-  K.download(obs_track, K.d_obs_track.p, (size_t)K.nobs);
-  K.download(obs_image, K.d_obs_image.p, (size_t)K.nobs);
-  K.download(obs_feature, K.d_obs_feature.p, (size_t)K.nobs);
-  K.download(reinterpret_cast<long long*>(track_start), K.d_track_start.p, (size_t)K.T + 1);
-  OSFM_CUDA(cudaStreamSynchronize(K.stream));
-  OSFM_API_END
+  return osfm::with_handle(t, [&](osfm::Tracks& K) {
+    if (!K.built) throw std::runtime_error("tracks: osfm_tracks_get needs a successful osfm_tracks_build");
+    if (!track_start || (K.nobs > 0 && (!obs_track || !obs_image || !obs_feature))) throw osfm::ArgError("null outputs");
+    K.download(obs_track, K.d_obs_track.p, (size_t)K.nobs);
+    K.download(obs_image, K.d_obs_image.p, (size_t)K.nobs);
+    K.download(obs_feature, K.d_obs_feature.p, (size_t)K.nobs);
+    K.download(reinterpret_cast<long long*>(track_start), K.d_track_start.p, (size_t)K.T + 1);
+    OSFM_CUDA(cudaStreamSynchronize(K.stream));
+  });
 }
 
 int osfm_tracks_common(osfm_tracks* t, int64_t* num_pairs, int64_t* num_common) {
-  OSFM_API_BEGIN
-  OSFM_T_LOCK
-  K.common(num_pairs, num_common);
-  OSFM_API_END
+  return osfm::with_handle(t, [&](osfm::Tracks& K) { K.common(num_pairs, num_common); });
 }
 
 int osfm_tracks_get_common(osfm_tracks* t, int32_t* pair_a, int32_t* pair_b, int64_t* pair_start,
                            int64_t* common_obs_a, int64_t* common_obs_b) {
-  OSFM_API_BEGIN
-  OSFM_T_LOCK
-  if (!K.common_built) throw std::runtime_error("tracks: osfm_tracks_get_common needs a successful osfm_tracks_common");
-  if (!pair_start || (K.Q > 0 && (!pair_a || !pair_b)) || (K.R > 0 && (!common_obs_a || !common_obs_b)))
-    throw osfm::ArgError("null outputs");
-  if (K.R == 0) {
-    pair_start[0] = 0;
-    return OSFM_OK;
-  }
-  K.download(pair_a, K.d_cpair_a.p, (size_t)K.Q);
-  K.download(pair_b, K.d_cpair_b.p, (size_t)K.Q);
-  K.download(reinterpret_cast<long long*>(pair_start), K.d_pair_start.p, (size_t)K.Q + 1);
-  K.download(reinterpret_cast<long long*>(common_obs_a), reinterpret_cast<long long*>(K.d_key.p), (size_t)K.R);
-  K.download(reinterpret_cast<long long*>(common_obs_b), reinterpret_cast<long long*>(K.d_val.p), (size_t)K.R);
-  OSFM_CUDA(cudaStreamSynchronize(K.stream));
-  OSFM_API_END
+  return osfm::with_handle(t, [&](osfm::Tracks& K) {
+    if (!K.common_built)
+      throw std::runtime_error("tracks: osfm_tracks_get_common needs a successful osfm_tracks_common");
+    if (!pair_start || (K.Q > 0 && (!pair_a || !pair_b)) || (K.R > 0 && (!common_obs_a || !common_obs_b)))
+      throw osfm::ArgError("null outputs");
+    if (K.R == 0) {
+      pair_start[0] = 0;
+      return;
+    }
+    K.download(pair_a, K.d_cpair_a.p, (size_t)K.Q);
+    K.download(pair_b, K.d_cpair_b.p, (size_t)K.Q);
+    K.download(reinterpret_cast<long long*>(pair_start), K.d_pair_start.p, (size_t)K.Q + 1);
+    K.download(reinterpret_cast<long long*>(common_obs_a), reinterpret_cast<long long*>(K.d_key.p), (size_t)K.R);
+    K.download(reinterpret_cast<long long*>(common_obs_b), reinterpret_cast<long long*>(K.d_val.p), (size_t)K.R);
+    OSFM_CUDA(cudaStreamSynchronize(K.stream));
+  });
 }
 
 int osfm_tracks_last_device_ms(osfm_tracks* t, float* ms_build, float* ms_common) {
-  OSFM_API_BEGIN
-  OSFM_T_LOCK
-  if (ms_build) {
-    *ms_build = 0.f;
-    if (K.timed_build) OSFM_CUDA(cudaEventElapsedTime(ms_build, K.ev[0], K.ev[1]));
-  }
-  if (ms_common) {
-    *ms_common = 0.f;
-    if (K.timed_common) OSFM_CUDA(cudaEventElapsedTime(ms_common, K.ev[2], K.ev[3]));
-  }
-  OSFM_API_END
+  return osfm::with_handle(t, [&](osfm::Tracks& K) {
+    if (ms_build) {
+      *ms_build = 0.f;
+      if (K.timed_build) OSFM_CUDA(cudaEventElapsedTime(ms_build, K.ev[0], K.ev[1]));
+    }
+    if (ms_common) {
+      *ms_common = 0.f;
+      if (K.timed_common) OSFM_CUDA(cudaEventElapsedTime(ms_common, K.ev[2], K.ev[3]));
+    }
+  });
 }
 
 }  // extern "C"

@@ -231,102 +231,99 @@ extern "C" {
 
 int osfm_matcher_vlad_compute(osfm_matcher* m, int count, const int* set_ids, const float* centers, int ncenters, int dim,
                               int* out_valid) {
-  OSFM_API_BEGIN
   using namespace osfm;
-  MatcherGuard g(m);
-  Matcher& M = g.M;
-  if (count < 0 || ncenters <= 0 || dim <= 0) throw ArgError("bad VLAD sizes");
-  if ((count > 0 && (!set_ids || !out_valid)) || !centers) throw ArgError("null arrays");
-  const int ncp = (ncenters + VA_CH - 1) / VA_CH * VA_CH;
-  const size_t L = (size_t)ncenters * dim;
-  if ((size_t)dim * ncp * sizeof(float) > VLAD_SMEM_MAX || L * sizeof(float) > VLAD_SMEM_MAX)
-    throw ArgError("VLAD vocabulary too large: ncenters x dim float32 must fit in 200 KB of shared memory");
-  for (size_t e = 0; e < L; ++e)
-    if (!std::isfinite(centers[e])) throw ArgError("non-finite VLAD centre");
-  for (int i = 0; i < count; ++i)
-    if (!M.sets.count(set_ids[i])) throw ArgError("unknown descriptor set id");
-  OSFM_CUDA(cudaStreamSynchronize(M.stream));   // earlier work may still read VLADs released below
-  // one descriptor per set; Hamming sets and sets of another dimension have none (unnormalized_vlad -> None)
-  std::vector<VladJob> jobs;
-  std::vector<int> job_set;
-  long long nfeat = 0;
-  int max_n = 0;
-  for (int i = 0; i < count; ++i) {
-    DescSet& s = M.sets[set_ids[i]];
-    const bool valid = !s.u8 && s.dim == dim;
-    out_valid[i] = valid;
-    if (!valid || (size_t)s.vlad.len != L) M.release(s.vlad);
-    if (!valid) continue;
-    if (!s.vlad.p) M.slab_new(s.vlad, 2 * L * sizeof(float), (int)L);
-    VladJob j;
-    j.f = static_cast<const float*>(s.data);   // float32 zero-padded rows for every non-Hamming set (match.cu add_async)
-    j.v = s.vlad.p;
-    j.aoff = nfeat;
-    j.n = s.n;
-    j.ld = s.dim_padded;
-    jobs.push_back(j);
-    job_set.push_back(set_ids[i]);
-    nfeat += s.n;
-    max_n = std::max(max_n, s.n);
-  }
-  if (jobs.empty()) return OSFM_OK;
-  // centres: row-major for the residuals, transposed and padded with +inf for the assignment
-  std::vector<float> hc(L + (size_t)dim * ncp, __builtin_huge_valf());
-  std::copy(centers, centers + L, hc.begin());
-  for (int c = 0; c < ncenters; ++c)
-    for (int k = 0; k < dim; ++k) hc[L + (size_t)k * ncp + c] = centers[(size_t)c * dim + k];
-  M.d_vlad_centers.reserve(hc.size());
-  M.d_vlad_assign.reserve((size_t)std::max<long long>(nfeat, 1));
-  M.d_vlad_flags.reserve(1);
-  M.d_tab.reserve(sizeof(VladJob) * jobs.size());
-  OSFM_CUDA(cudaMemcpyAsync(M.d_vlad_centers.p, hc.data(), sizeof(float) * hc.size(), cudaMemcpyHostToDevice, M.stream));
-  OSFM_CUDA(cudaMemcpyAsync(M.d_tab.p, jobs.data(), sizeof(VladJob) * jobs.size(), cudaMemcpyHostToDevice, M.stream));
-  OSFM_CUDA(cudaMemsetAsync(M.d_vlad_flags.p, 0, sizeof(int), M.stream));
-  const VladJob* d_jobs = reinterpret_cast<const VladJob*>(M.d_tab.p);
-  const size_t smem_a = (size_t)dim * ncp * sizeof(float), smem_n = L * sizeof(float);
-  OSFM_CUDA(cudaFuncSetAttribute(vlad_assign_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_a));
-  OSFM_CUDA(cudaFuncSetAttribute(vlad_accumulate_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_n));
-  const int nthreads = std::min(VN_THREADS_MAX, std::max(32, (dim + 31) / 32 * 32));
-  for (size_t j0 = 0; j0 < jobs.size(); j0 += 32768) {   // gridDim.y <= 65535
-    const int nj = (int)std::min<size_t>(32768, jobs.size() - j0);
-    if (max_n > 0) {
-      dim3 grid((unsigned)((max_n + VA_THREADS - 1) / VA_THREADS), (unsigned)nj);
-      vlad_assign_kernel<<<grid, VA_THREADS, smem_a, M.stream>>>(d_jobs + j0, M.d_vlad_centers.p + L, ncp, dim,
-                                                                 M.d_vlad_assign.p, M.d_vlad_flags.p);
+  return with_handle(m, [&](Matcher& M) {
+    if (count < 0 || ncenters <= 0 || dim <= 0) throw ArgError("bad VLAD sizes");
+    if ((count > 0 && (!set_ids || !out_valid)) || !centers) throw ArgError("null arrays");
+    const int ncp = (ncenters + VA_CH - 1) / VA_CH * VA_CH;
+    const size_t L = (size_t)ncenters * dim;
+    if ((size_t)dim * ncp * sizeof(float) > VLAD_SMEM_MAX || L * sizeof(float) > VLAD_SMEM_MAX)
+      throw ArgError("VLAD vocabulary too large: ncenters x dim float32 must fit in 200 KB of shared memory");
+    for (size_t e = 0; e < L; ++e)
+      if (!std::isfinite(centers[e])) throw ArgError("non-finite VLAD centre");
+    for (int i = 0; i < count; ++i)
+      if (!M.sets.count(set_ids[i])) throw ArgError("unknown descriptor set id");
+    OSFM_CUDA(cudaStreamSynchronize(M.stream));   // earlier work may still read VLADs released below
+    // one descriptor per set; Hamming sets and sets of another dimension have none (unnormalized_vlad -> None)
+    std::vector<VladJob> jobs;
+    std::vector<int> job_set;
+    long long nfeat = 0;
+    int max_n = 0;
+    for (int i = 0; i < count; ++i) {
+      DescSet& s = M.sets[set_ids[i]];
+      const bool valid = !s.u8 && s.dim == dim;
+      out_valid[i] = valid;
+      if (!valid || (size_t)s.vlad.len != L) M.release(s.vlad);
+      if (!valid) continue;
+      if (!s.vlad.p) M.slab_new(s.vlad, 2 * L * sizeof(float), (int)L);
+      VladJob j;
+      j.f = static_cast<const float*>(s.data);   // float32 zero-padded rows for every non-Hamming set (match.cu add_async)
+      j.v = s.vlad.p;
+      j.aoff = nfeat;
+      j.n = s.n;
+      j.ld = s.dim_padded;
+      jobs.push_back(j);
+      job_set.push_back(set_ids[i]);
+      nfeat += s.n;
+      max_n = std::max(max_n, s.n);
+    }
+    if (jobs.empty()) return;
+    // centres: row-major for the residuals, transposed and padded with +inf for the assignment
+    std::vector<float> hc(L + (size_t)dim * ncp, __builtin_huge_valf());
+    std::copy(centers, centers + L, hc.begin());
+    for (int c = 0; c < ncenters; ++c)
+      for (int k = 0; k < dim; ++k) hc[L + (size_t)k * ncp + c] = centers[(size_t)c * dim + k];
+    M.d_vlad_centers.reserve(hc.size());
+    M.d_vlad_assign.reserve((size_t)std::max<long long>(nfeat, 1));
+    M.d_vlad_flags.reserve(1);
+    M.d_tab.reserve(sizeof(VladJob) * jobs.size());
+    OSFM_CUDA(cudaMemcpyAsync(M.d_vlad_centers.p, hc.data(), sizeof(float) * hc.size(), cudaMemcpyHostToDevice, M.stream));
+    OSFM_CUDA(cudaMemcpyAsync(M.d_tab.p, jobs.data(), sizeof(VladJob) * jobs.size(), cudaMemcpyHostToDevice, M.stream));
+    OSFM_CUDA(cudaMemsetAsync(M.d_vlad_flags.p, 0, sizeof(int), M.stream));
+    const VladJob* d_jobs = reinterpret_cast<const VladJob*>(M.d_tab.p);
+    const size_t smem_a = (size_t)dim * ncp * sizeof(float), smem_n = L * sizeof(float);
+    OSFM_CUDA(cudaFuncSetAttribute(vlad_assign_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_a));
+    OSFM_CUDA(cudaFuncSetAttribute(vlad_accumulate_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_n));
+    const int nthreads = std::min(VN_THREADS_MAX, std::max(32, (dim + 31) / 32 * 32));
+    for (size_t j0 = 0; j0 < jobs.size(); j0 += 32768) {   // gridDim.y <= 65535
+      const int nj = (int)std::min<size_t>(32768, jobs.size() - j0);
+      if (max_n > 0) {
+        dim3 grid((unsigned)((max_n + VA_THREADS - 1) / VA_THREADS), (unsigned)nj);
+        vlad_assign_kernel<<<grid, VA_THREADS, smem_a, M.stream>>>(d_jobs + j0, M.d_vlad_centers.p + L, ncp, dim,
+                                                                   M.d_vlad_assign.p, M.d_vlad_flags.p);
+        OSFM_LAUNCH_CHECK();
+      }
+      vlad_accumulate_kernel<<<nj, nthreads, smem_n, M.stream>>>(d_jobs + j0, M.d_vlad_centers.p, ncenters, dim,
+                                                                M.d_vlad_assign.p, M.d_vlad_flags.p);
       OSFM_LAUNCH_CHECK();
     }
-    vlad_accumulate_kernel<<<nj, nthreads, smem_n, M.stream>>>(d_jobs + j0, M.d_vlad_centers.p, ncenters, dim,
-                                                              M.d_vlad_assign.p, M.d_vlad_flags.p);
-    OSFM_LAUNCH_CHECK();
-  }
-  int flags = 0;
-  OSFM_CUDA(cudaMemcpyAsync(&flags, M.d_vlad_flags.p, sizeof(int), cudaMemcpyDeviceToHost, M.stream));
-  OSFM_CUDA(cudaStreamSynchronize(M.stream));
-  if (flags) {
-    for (int id : job_set) M.release(M.sets[id].vlad);
-    throw ArgError(flags & 1 ? "non-finite descriptor element in a VLAD input set"
-                             : "a feature's squared distance to every VLAD centre overflows float32");
-  }
-  OSFM_API_END
+    int flags = 0;
+    OSFM_CUDA(cudaMemcpyAsync(&flags, M.d_vlad_flags.p, sizeof(int), cudaMemcpyDeviceToHost, M.stream));
+    OSFM_CUDA(cudaStreamSynchronize(M.stream));
+    if (flags) {
+      for (int id : job_set) M.release(M.sets[id].vlad);
+      throw ArgError(flags & 1 ? "non-finite descriptor element in a VLAD input set"
+                               : "a feature's squared distance to every VLAD centre overflows float32");
+    }
+  });
 }
 
 int osfm_matcher_vlad_get(osfm_matcher* m, int set_id, int unnormalized, float* out) {
-  OSFM_API_BEGIN
   using namespace osfm;
-  if (!m || !out) throw ArgError("null arguments");
-  MatcherGuard g(m);
-  const SlabArray<float>& v = VladRows::of(g.M, set_id, -1);
-  OSFM_CUDA(cudaMemcpyAsync(out, v.p + (unnormalized ? 0 : v.len), sizeof(float) * (size_t)v.len, cudaMemcpyDeviceToHost,
-                            g.M.stream));
-  OSFM_CUDA(cudaStreamSynchronize(g.M.stream));
-  OSFM_API_END
+  return with_handle(m, [&](Matcher& M) {
+    if (!out) throw ArgError("null arguments");
+    const SlabArray<float>& v = VladRows::of(M, set_id, -1);
+    OSFM_CUDA(cudaMemcpyAsync(out, v.p + (unnormalized ? 0 : v.len), sizeof(float) * (size_t)v.len,
+                              cudaMemcpyDeviceToHost, M.stream));
+    OSFM_CUDA(cudaStreamSynchronize(M.stream));
+  });
 }
 
 int osfm_matcher_vlad_select(osfm_matcher* m, int nref, const int* ref_ids, int ncand, const int* cand_ids,
                              const uint32_t* cand_mask_bits, const int* camera_labels, int k, int64_t* out_offsets,
                              int32_t* out_cols, double* out_dist) {
   using namespace osfm;
-  return with_matcher(m, [&](Matcher& M) {
+  return with_handle(m, [&](Matcher& M) {
     if (nref < 0 || ncand < 0 || k < 0) throw ArgError("bad VLAD selection sizes");
     VladRows kind;
     select_neighbors(M, kind, nref, ref_ids, ncand, cand_ids, cand_mask_bits, nullptr, camera_labels, k, out_offsets,
@@ -336,7 +333,7 @@ int osfm_matcher_vlad_select(osfm_matcher* m, int nref, const int* ref_ids, int 
 
 int osfm_vlad_distances(osfm_matcher* m, const float* vlad, int n, int dim, int query, double* out_n) {
   using namespace osfm;
-  return with_matcher(m, [&](Matcher& M) {
+  return with_handle(m, [&](Matcher& M) {
     if (n <= 0 || dim <= 0 || query < 0 || query >= n || !vlad || !out_n) throw ArgError("bad VLAD arguments");
     VladRows kind;
     distances_to_row(M, kind, vlad, n, dim, query, out_n);

@@ -10,49 +10,19 @@ arithmetic happens in the CUDA library (opensfm_b200/csrc/match*.cu) through the
 C ABI; there is no CPU path here.
 
 Thread safety: the reference calls these from a joblib *threading* pool
-(opensfm/context.py:59-64).  Each Python thread gets its own matcher (own CUDA
-stream); ctypes releases the GIL for the duration of the call.
+(opensfm/context.py:59-64).  Each call takes a matcher (own CUDA stream) that no
+other thread holds meanwhile from the library's handle pool; ctypes releases the
+GIL for the duration of the call.
 """
 from __future__ import annotations
 
 import ctypes
-import threading
 from typing import Any, Dict, Iterable, List, Optional, Sequence, Tuple
 
 import numpy as np
 
 from . import _lib
-
-_tls = threading.local()
-
-
-class _Matcher:
-    def __init__(self, device: int = 0):
-        L = _lib.load()
-        h = ctypes.c_void_p()
-        _lib.check(L.osfm_matcher_create(int(device), ctypes.byref(h)))
-        self.h = h
-        self.device = device
-        self.L = L
-
-    def __del__(self):
-        try:
-            self.L.osfm_matcher_destroy(self.h)
-        except Exception:
-            pass
-
-
-def _thread_matcher(device: int = 0) -> _Matcher:
-    key = "m%d" % device
-    m = getattr(_tls, key, None)
-    if m is None:
-        m = _Matcher(device)
-        setattr(_tls, key, m)
-    return m
-
-
-def _ptr(a: Optional[np.ndarray]) -> Optional[ctypes.c_void_p]:
-    return None if a is None else a.ctypes.data_as(ctypes.c_void_p)
+from ._lib import ptr
 
 
 def _prep(f: np.ndarray) -> np.ndarray:
@@ -79,10 +49,10 @@ def _match_raw(f1: np.ndarray, f2: np.ndarray, ratio: float, maskij: Optional[np
         if mask.shape != (n1, n2):
             raise ValueError("maskij must be len(f1) x len(f2)")
         mask_p = mask.ctypes.data_as(ctypes.c_void_p)
-    m = _thread_matcher(device)
-    fn = m.L.osfm_bf_match_u8 if a.dtype == np.uint8 else m.L.osfm_bf_match_f32
-    _lib.check(fn(m.h, a.ctypes.data_as(ctypes.c_void_p), n1, b.ctypes.data_as(ctypes.c_void_p), n2, dim,
-                  float(ratio), mask_p, int(symmetric), out.ctypes.data_as(ctypes.c_void_p)))
+    with _lib.pooled("matcher", device) as m:
+        fn = m.L.osfm_bf_match_u8 if a.dtype == np.uint8 else m.L.osfm_bf_match_f32
+        _lib.check(fn(m.h, a.ctypes.data_as(ctypes.c_void_p), n1, b.ctypes.data_as(ctypes.c_void_p), n2, dim,
+                      float(ratio), mask_p, int(symmetric), out.ctypes.data_as(ctypes.c_void_p)))
     return out
 
 
@@ -130,7 +100,7 @@ class PairMatcher:
     """
 
     def __init__(self, device: int = 0, kernel: int = 0):
-        self._m = _Matcher(device)
+        self._m = _lib.Handle("matcher", device)
         self._ids: Dict[Any, int] = {}
         self._n: Dict[Any, int] = {}
         self._keep: Dict[Any, np.ndarray] = {}
@@ -211,8 +181,8 @@ class PairMatcher:
         valid = np.zeros(len(keys), dtype=np.int32)
         for k in keys:
             self._vlad.pop(k, None)
-        _lib.check(self._m.L.osfm_matcher_vlad_compute(self._m.h, len(keys), _ptr(ids), _ptr(c), c.shape[0], c.shape[1],
-                                                       _ptr(valid)))
+        _lib.check(self._m.L.osfm_matcher_vlad_compute(self._m.h, len(keys), ptr(ids), ptr(c), c.shape[0], c.shape[1],
+                                                       ptr(valid)))
         for k, v in zip(keys, valid):
             self._vlad[k] = c.size if v else 0
         return [k for k, v in zip(keys, valid) if v]
@@ -223,7 +193,7 @@ class PairMatcher:
         if not self._vlad.get(key):
             raise KeyError("no VLAD descriptor for image %r" % (key,))
         out = np.empty(self._vlad[key], dtype=np.float32)
-        _lib.check(self._m.L.osfm_matcher_vlad_get(self._m.h, self._ids[key], int(not normalized), _ptr(out)))
+        _lib.check(self._m.L.osfm_matcher_vlad_get(self._m.h, self._ids[key], int(not normalized), ptr(out)))
         return out
 
     def has_vlad(self, key: Any) -> Optional[bool]:
@@ -266,8 +236,8 @@ class PairMatcher:
         offs = np.zeros(nref + 1, dtype=np.int64)
         cols = np.empty(cap, dtype=np.int32)
         dist = np.empty(cap, dtype=np.float64)
-        _lib.check(fn(self._m.h, nref, _ptr(ri), ncand, _ptr(ci), _ptr(per_ref), _ptr(lab), int(k), _ptr(offs),
-                      _ptr(cols), _ptr(dist)))
+        _lib.check(fn(self._m.h, nref, ptr(ri), ncand, ptr(ci), ptr(per_ref), ptr(lab), int(k), ptr(offs),
+                      ptr(cols), ptr(dist)))
         return [(cols[offs[r]:offs[r + 1]], dist[offs[r]:offs[r + 1]]) for r in range(nref)]
 
     # -- BoW (opensfm/bow.py, pairs_selection.load_histograms) ----------------------------------------------------
@@ -287,8 +257,8 @@ class PairMatcher:
         for key in keys:
             self._words.pop(key, None)
             self._bow.pop(key, None)
-        _lib.check(self._m.L.osfm_matcher_bow_words(self._m.h, len(keys), _ptr(ids), _ptr(vocab), nw, vocab.shape[1],
-                                                    int(k), _ptr(offs), _ptr(words), _ptr(valid)))
+        _lib.check(self._m.L.osfm_matcher_bow_words(self._m.h, len(keys), ptr(ids), ptr(vocab), nw, vocab.shape[1],
+                                                    int(k), ptr(offs), ptr(words), ptr(valid)))
         out: Dict[Any, np.ndarray] = {}
         for i, (key, v) in enumerate(zip(keys, valid)):
             self._words[key] = nw if v else 0
@@ -308,13 +278,13 @@ class PairMatcher:
         w = np.ascontiguousarray(bows.weights, dtype=np.float64)
         ids = np.array([self._ids[key] for key in keys], dtype=np.int32)
         valid = np.zeros(len(keys), dtype=np.int32)
-        _lib.check(self._m.L.osfm_matcher_bow_histograms(self._m.h, len(keys), _ptr(ids), _ptr(w), len(w), _ptr(valid)))
+        _lib.check(self._m.L.osfm_matcher_bow_histograms(self._m.h, len(keys), ptr(ids), ptr(w), len(w), ptr(valid)))
         out: Dict[Any, np.ndarray] = {}
         for key, v in zip(keys, valid):
             self._bow[key] = len(w) if v else 0
             if v:
                 h = np.empty(len(w), dtype=np.float64)
-                _lib.check(self._m.L.osfm_matcher_bow_get(self._m.h, self._ids[key], _ptr(h)))
+                _lib.check(self._m.L.osfm_matcher_bow_get(self._m.h, self._ids[key], ptr(h)))
                 out[key] = h
         return out
 
@@ -462,11 +432,10 @@ def match_words(f1: np.ndarray, words1: np.ndarray, f2: np.ndarray, words2: np.n
     if f1.ndim != 2 or f2.ndim != 2 or f1.shape[1] != f2.shape[1]:
         raise ValueError("descriptor matrices must be n x dim with the same dim")
     out = np.full(len(f1), -1, dtype=np.int32)
-    m = _thread_matcher(device)
-    _lib.check(m.L.osfm_match_words(m.h, f1.ctypes.data_as(ctypes.c_void_p), len(f1), w1.ctypes.data_as(ctypes.c_void_p),
-                                    w1.shape[1], f2.ctypes.data_as(ctypes.c_void_p), len(f2),
-                                    w2.ctypes.data_as(ctypes.c_void_p), f1.shape[1], float(config["lowes_ratio"]),
-                                    int(config["bow_num_checks"]), out.ctypes.data_as(ctypes.c_void_p)))
+    with _lib.pooled("matcher", device) as m:
+        _lib.check(m.L.osfm_match_words(m.h, ptr(f1), len(f1), ptr(w1), w1.shape[1], ptr(f2), len(f2), ptr(w2),
+                                        f1.shape[1], float(config["lowes_ratio"]), int(config["bow_num_checks"]),
+                                        ptr(out)))
     q = np.flatnonzero(out >= 0)
     return np.stack([q, out[q]], axis=1).astype(np.int32)
 
@@ -490,8 +459,8 @@ def vlad_distances(image: Any, other_images: Sequence[Any], histograms: Dict[Any
         return image, [], []
     mat = np.ascontiguousarray(np.stack([histograms[image]] + [histograms[o] for o in others]), dtype=np.float32)
     out = np.zeros(len(mat), dtype=np.float64)
-    m = _thread_matcher(device)
-    _lib.check(m.L.osfm_vlad_distances(m.h, _ptr(mat), mat.shape[0], mat.shape[1], 0, _ptr(out)))
+    with _lib.pooled("matcher", device) as m:
+        _lib.check(m.L.osfm_vlad_distances(m.h, ptr(mat), mat.shape[0], mat.shape[1], 0, ptr(out)))
     return image, out[1:].tolist(), others
 
 

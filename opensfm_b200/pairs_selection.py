@@ -20,7 +20,8 @@ from typing import Any, Dict, Optional, Sequence, Tuple
 import numpy as np
 
 from . import _lib
-from .matching import PairMatcher, _ptr, _thread_matcher
+from ._lib import ptr
+from .matching import PairMatcher
 
 
 def unnormalized_vlad(features: np.ndarray, centers: np.ndarray, device: int = 0) -> Optional[np.ndarray]:
@@ -30,17 +31,17 @@ def unnormalized_vlad(features: np.ndarray, centers: np.ndarray, device: int = 0
         return None
     f = np.ascontiguousarray(features, dtype=np.float32)
     c = np.ascontiguousarray(centers, dtype=np.float32)
-    m = _thread_matcher(device)
-    sid = ctypes.c_int()
-    _lib.check(m.L.osfm_matcher_add_f32(m.h, _ptr(f), f.shape[0], f.shape[1], ctypes.byref(sid)))
-    try:
-        ids = np.array([sid.value], dtype=np.int32)
-        valid = np.zeros(1, dtype=np.int32)
-        _lib.check(m.L.osfm_matcher_vlad_compute(m.h, 1, _ptr(ids), _ptr(c), c.shape[0], c.shape[1], _ptr(valid)))
-        out = np.empty(c.size, dtype=np.float32)
-        _lib.check(m.L.osfm_matcher_vlad_get(m.h, sid.value, 1, _ptr(out)))
-    finally:
-        _lib.check(m.L.osfm_matcher_remove(m.h, sid.value))
+    with _lib.pooled("matcher", device) as m:
+        sid = ctypes.c_int()
+        _lib.check(m.L.osfm_matcher_add_f32(m.h, ptr(f), f.shape[0], f.shape[1], ctypes.byref(sid)))
+        try:
+            ids = np.array([sid.value], dtype=np.int32)
+            valid = np.zeros(1, dtype=np.int32)
+            _lib.check(m.L.osfm_matcher_vlad_compute(m.h, 1, ptr(ids), ptr(c), c.shape[0], c.shape[1], ptr(valid)))
+            out = np.empty(c.size, dtype=np.float32)
+            _lib.check(m.L.osfm_matcher_vlad_get(m.h, sid.value, 1, ptr(out)))
+        finally:
+            _lib.check(m.L.osfm_matcher_remove(m.h, sid.value))
     return out
 
 

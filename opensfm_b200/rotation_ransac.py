@@ -9,23 +9,17 @@ consecutive rows (`pair_start`).  `ransac_pairs_lists` builds that from per-pair
 from __future__ import annotations
 
 import ctypes
-import threading
 from dataclasses import dataclass
-from typing import Dict, List, Sequence
+from typing import List, Optional, Sequence
 
 import numpy as np
 
 from . import _lib
+from ._lib import ptr
 
 ITERATIONS = 1000   # what two_view_reconstruction_rotation_only passes
 
-_pool_lock = threading.Lock()
-_pool: Dict[int, List["RotationRansac"]] = {}
 _last_device_ms = 0.0
-
-
-def _ptr(a: np.ndarray):
-    return a.ctypes.data_as(ctypes.c_void_p)
 
 
 @dataclass
@@ -58,21 +52,14 @@ def reconstructability(common: np.ndarray, rotation_inliers: np.ndarray) -> List
 
 
 class RotationRansac:
-    """osfm_rotransac: one stream, its workspaces and the sample stream kept on the device."""
+    """osfm_rotransac: one stream, its workspaces and the sample stream kept on the device; a new handle, or `handle`
+    when given."""
 
-    def __init__(self, device: int = 0):
-        L = _lib.load()
-        h = ctypes.c_void_p()
-        _lib.check(L.osfm_rotransac_create(int(device), ctypes.byref(h)))
-        self.h, self.L, self.device = h, L, int(device)
+    def __init__(self, device: int = 0, handle: Optional[_lib.Handle] = None):
+        self.handle = handle if handle is not None else _lib.Handle("rotransac", device)
+        self.h, self.L, self.device = self.handle.h, self.handle.L, self.handle.device
         self._trace_cap = 0
         self._num_pairs = 0
-
-    def __del__(self):
-        try:
-            self.L.osfm_rotransac_destroy(self.h)
-        except Exception:
-            pass
 
     def set_stream_prefix(self, length: int) -> None:
         """How many generator outputs the device keeps (a test hook: pairs that use them all continue from the saved
@@ -90,7 +77,7 @@ class RotationRansac:
         count = np.zeros(P, dtype=np.int32)
         used = np.zeros(P, dtype=np.int64)
         idx = np.zeros(P * cap, dtype=np.int32)
-        _lib.check(self.L.osfm_rotransac_get_trace(self.h, _ptr(count), _ptr(used), _ptr(idx)))
+        _lib.check(self.L.osfm_rotransac_get_trace(self.h, ptr(count), ptr(used), ptr(idx)))
         idx = idx.reshape(P, cap)
         return [idx[p, :min(int(count[p]), cap)] for p in range(P)], count, used
 
@@ -108,37 +95,21 @@ class RotationRansac:
         ransac = np.zeros(P, dtype=np.int32)
         chord = np.zeros(P, dtype=np.int32)
         mask = np.zeros(R, dtype=np.uint8)
-        _lib.check(self.L.osfm_rotransac_run(self.h, len(bearings), _ptr(bearings), P, _ptr(pair_start), _ptr(row_a),
-                                             _ptr(row_b), float(threshold), int(iterations), _ptr(lo), _ptr(ransac),
-                                             _ptr(chord), _ptr(mask)))
+        _lib.check(self.L.osfm_rotransac_run(self.h, len(bearings), ptr(bearings), P, ptr(pair_start), ptr(row_a),
+                                             ptr(row_b), float(threshold), int(iterations), ptr(lo), ptr(ransac),
+                                             ptr(chord), ptr(mask)))
         self._num_pairs = P
         ms = ctypes.c_float(0)
         _lib.check(self.L.osfm_rotransac_last_device_ms(self.h, ctypes.byref(ms)))
         return PairsResult(lo, ransac, chord, mask.view(bool), pair_start, float(ms.value))
 
 
-def _acquire(device: int) -> RotationRansac:
-    with _pool_lock:
-        free = _pool.get(int(device))
-        if free:
-            return free.pop()
-    return RotationRansac(device)
-
-
-def _release(h: RotationRansac) -> None:
-    with _pool_lock:
-        _pool.setdefault(h.device, []).append(h)
-
-
 def ransac_pairs(bearings: np.ndarray, pair_start: np.ndarray, row_a: np.ndarray, row_b: np.ndarray,
                  threshold: float, iterations: int = ITERATIONS, device: int = 0) -> PairsResult:
     """Every pair's rotation-only RANSAC and chord inliers; rows index one bearing table."""
     global _last_device_ms
-    h = _acquire(device)
-    try:
-        res = h.run(bearings, pair_start, row_a, row_b, threshold, iterations)
-    finally:
-        _release(h)
+    with _lib.pooled("rotransac", device) as h:
+        res = RotationRansac(handle=h).run(bearings, pair_start, row_a, row_b, threshold, iterations)
     _last_device_ms = res.device_ms
     return res
 

@@ -17,61 +17,25 @@ Track ids are opaque strings in both; the partition of the features into tracks 
 from __future__ import annotations
 
 import ctypes
-import threading
 from typing import Any, Dict, Iterable, List, Optional, Sequence, Tuple
 
 import numpy as np
 
 from . import _lib
+from ._lib import ptr
 from .map_types import Depth, Observation
 
 NO_SEMANTIC_VALUE = -1   # pymap.Observation.NO_SEMANTIC_VALUE
-
-_pool_lock = threading.Lock()
-_pool: Dict[int, List["_Handle"]] = {}
-
-
-class _Handle:
-    """osfm_tracks: one stream and the workspaces, reused by the next TracksManager once this one has its arrays."""
-
-    def __init__(self, device: int):
-        L = _lib.load()
-        h = ctypes.c_void_p()
-        _lib.check(L.osfm_tracks_create(int(device), ctypes.byref(h)))
-        self.h, self.L, self.device = h, L, int(device)
-
-    def __del__(self):
-        try:
-            self.L.osfm_tracks_destroy(self.h)
-        except Exception:
-            pass
-
-
-def _acquire(device: int) -> _Handle:
-    with _pool_lock:
-        free = _pool.get(int(device))
-        if free:
-            return free.pop()
-    return _Handle(device)
-
-
-def _release(h: _Handle) -> None:
-    with _pool_lock:
-        _pool.setdefault(h.device, []).append(h)
-
-
-def _ptr(a: np.ndarray):
-    return a.ctypes.data_as(ctypes.c_void_p)
 
 
 class TracksManager:
     """Array-backed, read-only mirror of the part of pymap.TracksManager the pipeline reads.  Observations are
     kept as arrays sorted by (track, image); `Observation` objects are made when an accessor returns them."""
 
-    def __init__(self, handle: _Handle, images: List[Any], obs_track: np.ndarray, obs_image: np.ndarray,
+    def __init__(self, handle: _lib.Handle, images: List[Any], obs_track: np.ndarray, obs_image: np.ndarray,
                  obs_feature: np.ndarray, track_start: np.ndarray, features, colors, segmentations, instances, depths,
                  depth_is_radial: bool, depth_std_deviation: float, device_ms: float):
-        self._handle: Optional[_Handle] = handle
+        self._handle: Optional[_lib.Handle] = handle   # released once the common tracks are read
         self.images = images
         self.obs_track, self.obs_image, self.obs_feature, self.track_start = obs_track, obs_image, obs_feature, track_start
         self._features, self._colors, self._segmentations, self._instances = features, colors, segmentations, instances
@@ -92,7 +56,7 @@ class TracksManager:
     def _give_back(self) -> None:
         h, self._handle = self._handle, None
         if h is not None:
-            _release(h)
+            _lib.release(h)
 
     # -- structure-of-arrays views ----------------------------------------------------------------------------
     def _shot_order(self) -> Tuple[np.ndarray, np.ndarray]:
@@ -200,7 +164,7 @@ class TracksManager:
             pa, pb = np.zeros(nq.value, dtype=np.int32), np.zeros(nq.value, dtype=np.int32)
             ps = np.zeros(nq.value + 1, dtype=np.int64)
             ca, cb = np.zeros(nr.value, dtype=np.int64), np.zeros(nr.value, dtype=np.int64)
-            _lib.check(h.L.osfm_tracks_get_common(h.h, _ptr(pa), _ptr(pb), _ptr(ps), _ptr(ca), _ptr(cb)))
+            _lib.check(h.L.osfm_tracks_get_common(h.h, ptr(pa), ptr(pb), ptr(ps), ptr(ca), ptr(cb)))
             ms = ctypes.c_float(0)
             _lib.check(h.L.osfm_tracks_last_device_ms(h.h, None, ctypes.byref(ms)))
             self.common_device_ms = float(ms.value)
@@ -285,19 +249,19 @@ def create_tracks_manager(features: Dict[Any, np.ndarray], colors: Dict[Any, np.
                     num_features[index[im]] = max(num_features[index[im]], int(r[:, col].max()) + 1)
     allrows = np.ascontiguousarray(np.concatenate(rows)) if rows else np.zeros((0, 2), dtype=np.int32)
 
-    h = _acquire(device)
+    h = _lib.acquire("tracks", device)
     try:
         nt, no = ctypes.c_int64(0), ctypes.c_int64(0)
-        _lib.check(h.L.osfm_tracks_build(h.h, len(images), _ptr(num_features), _ptr(has_features), len(rows),
-                                         _ptr(pair_a), _ptr(pair_b), _ptr(match_start), _ptr(allrows),
+        _lib.check(h.L.osfm_tracks_build(h.h, len(images), ptr(num_features), ptr(has_features), len(rows),
+                                         ptr(pair_a), ptr(pair_b), ptr(match_start), ptr(allrows),
                                          int(min_length), ctypes.byref(nt), ctypes.byref(no)))
         obs_track, obs_image, obs_feature = (np.zeros(no.value, dtype=np.int32) for _ in range(3))
         track_start = np.zeros(nt.value + 1, dtype=np.int64)
-        _lib.check(h.L.osfm_tracks_get(h.h, _ptr(obs_track), _ptr(obs_image), _ptr(obs_feature), _ptr(track_start)))
+        _lib.check(h.L.osfm_tracks_get(h.h, ptr(obs_track), ptr(obs_image), ptr(obs_feature), ptr(track_start)))
         ms = ctypes.c_float(0)
         _lib.check(h.L.osfm_tracks_last_device_ms(h.h, ctypes.byref(ms), None))
     except Exception:
-        _release(h)
+        _lib.release(h)
         raise
     return TracksManager(h, images, obs_track, obs_image, obs_feature, track_start, features, colors, segmentations,
                          instances, depths, depth_is_radial, depth_std_deviation, float(ms.value))

@@ -76,6 +76,8 @@ def measure(name):
          "valid": on["covariance_valid"],
          "status": on["covariance_status"], "valid_o": valid, "status_o": status, "termination": on["summary"]["termination"]}
     const = np.asarray(pb.inst_const) != 0
+    pass_ms, chol_ms = on["covariance_ms"]   # device times of the pass and of its Cholesky factorisation
+    m["timing_ok"] = bool(np.isfinite([pass_ms, chol_ms]).all() and pass_ms > 0.0 and chol_ms >= 0.0)
     m["const_zero"] = bool(np.all(Ce[const] == 0.0)) if valid else True
     m["default_exact"] = bool(np.array_equal(Ce, np.tile(co.DEFAULT, (len(pb.inst), 1, 1)))) if not on["covariance_valid"] else True
     m["ratio"] = 0.0
@@ -92,7 +94,7 @@ def measure(name):
 def _check(m):
     print(json.dumps(m))
     assert m["valid"] == m["valid_o"] and m["status"] == m["status_o"], m
-    assert m["const_zero"] and m["default_exact"], m
+    assert m["const_zero"] and m["default_exact"] and m["timing_ok"], m
     assert m["ratio"] <= 1.0, m
     if m["name"] in FULL_RANK:
         assert m["valid"], m

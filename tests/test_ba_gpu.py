@@ -104,6 +104,20 @@ def test_async_observation_upload_gives_the_same_solve():
         assert np.abs(got["points"] - ref["points"]).max() < 1e-9
 
 
+def test_solve_on_a_caller_stream():
+    """stream=: the solve runs on the caller's CUDA stream (osfm_ba_set_stream) and gives the default path's result;
+    the next solve without it runs on the handle's own stream again."""
+    import torch
+
+    sc = syn.cube_scene(10, 1000, 1.0, with_descriptors=False)
+    pb = syn.scene_to_problem(sc)
+    ref = bundle.solve(pb)
+    s = torch.cuda.Stream()
+    for got in (bundle.solve(pb, stream=s.cuda_stream), bundle.solve(pb)):
+        assert abs(got["summary"]["final_cost"] - ref["summary"]["final_cost"]) <= 1e-12 * ref["summary"]["final_cost"]
+        assert np.abs(got["points"] - ref["points"]).max() < 1e-9
+
+
 def test_pose_only_and_point_only():
     sc = syn.cube_scene(6, 400, 1.0, with_descriptors=False)
     pb = syn.scene_to_problem(sc, optimize_cameras=False)

@@ -6,7 +6,6 @@ covariances, the pass time and the Cholesky time from the CUDA events around the
 rate n_c^3 / 3 over its kernel time next to the H100 SXM data-sheet FP64 tensor-core figure (67 TFLOP/s at 700 W).
 Fails without a GPU.  Usage: python tools/measure_covariance.py [--repeats N]"""
 import argparse
-import ctypes
 import json
 import os
 import subprocess
@@ -18,7 +17,7 @@ sys.path.insert(0, ROOT)
 
 import numpy as np  # noqa: E402
 
-from opensfm_b200 import _lib, bundle  # noqa: E402
+from opensfm_b200 import bundle  # noqa: E402
 from opensfm_b200 import synthetic as syn  # noqa: E402
 
 FP64_TC_PEAK = 67e12   # H100 SXM data sheet, dense FP64 tensor core, 700 W
@@ -41,7 +40,6 @@ def main():
     pb.inst_has_prior[:] = 1
     pb.inst_prior_pos = pb.inst[:, 3:] + rng.normal(0, 0.02, (len(pb.inst), 3))
     pb.inst_prior_std = np.full((len(pb.inst), 3), 0.05)
-    L = _lib.load()
     bundle.solve(pb, compute_covariances=True)   # warm-up: module load, allocations, shared-memory opt-ins
     bundle.solve(pb)
     rows = []
@@ -53,14 +51,12 @@ def main():
             row = {"covariances": cov, "run_wall_s": wall, "run_device_ms": res["summary"]["time_device_ms"],
                    "iterations": res["summary"]["iterations"]}
             if cov:
-                pass_ms, chol_ms = ctypes.c_double(), ctypes.c_double()
-                _lib.check(L.osfm_ba_get_covariance_timing(bundle._handle(0).h, ctypes.byref(pass_ms),
-                                                            ctypes.byref(chol_ms)))
+                pass_ms, chol_ms = res["covariance_ms"]
                 nc = res["summary"]["reduced_dim"]
-                row.update(pass_ms=pass_ms.value, cholesky_ms=chol_ms.value, n_c=nc,
+                row.update(pass_ms=pass_ms, cholesky_ms=chol_ms, n_c=nc,
                            status=res["covariance_status"],
-                           cholesky_tflops=nc ** 3 / 3 / (chol_ms.value * 1e-3) / 1e12,
-                           cholesky_share_of_fp64_tc_datasheet=nc ** 3 / 3 / (chol_ms.value * 1e-3) / FP64_TC_PEAK)
+                           cholesky_tflops=nc ** 3 / 3 / (chol_ms * 1e-3) / 1e12,
+                           cholesky_share_of_fp64_tc_datasheet=nc ** 3 / 3 / (chol_ms * 1e-3) / FP64_TC_PEAK)
             rows.append(row)
     print(json.dumps({"card": card(), "runs": rows}, indent=1))
 
