@@ -1029,7 +1029,7 @@ struct BA {
   DevBuf<int> d_sp_ftab;                   // flush destinations per segment (sp_flush_tables)
   DevBuf<int> d_tab;
   DevBuf<double> d_ptsum;                  // [9][npf] unscaled Jp^T Jp (upper) and Jp^T r per point (ba_linearize_fused)
-  std::vector<const void*> smem_opted;     // kernels opted into their dynamic shared memory (per handle = per device)
+  SmemOptIn opt_in_smem;                   // opt_in_smem(kernel, bytes): above 48 KB, once per handle
   int num_sms = 132;
   DevBuf<int> d_pr_cam_param, d_pr_cam_col, d_pr_cam_log, d_pr_pos_inst, d_pr_pos_axis, d_pr_pos_col;
   DevBuf<double> d_pr_cam_prior, d_pr_cam_scale, d_pr_pos_prior, d_pr_pos_scale;
@@ -1155,13 +1155,6 @@ struct BA {
         throw ArgError("world > 1 but neither an all-reduce callback nor an NCCL communicator is set");
       }
     }
-  }
-  template <class Kernel>
-  void opt_in_smem(Kernel* kernel, int bytes) {   // dynamic shared memory above 48 KB, once per handle
-    const void* k = (const void*)kernel;
-    if (std::find(smem_opted.begin(), smem_opted.end(), k) != smem_opted.end()) return;
-    OSFM_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
-    smem_opted.push_back(k);
   }
   void trace(const char* what) {   // OSFM_BA_TRACE=1: host wall-clock per phase of run() on stderr (diagnostics only)
     if (!switches().trace) return;

@@ -443,7 +443,7 @@ static void bow_words_run(Matcher& M, int count, const int* set_ids, const float
       const DescSet& s = M.sets[job_set[j1]];
       if (j1 > j0 && brows + s.n > max_rows) break;
       BowJob b;
-      b.f = static_cast<const float*>(s.data);   // float32 zero-padded rows for every non-Hamming set
+      b.f = reinterpret_cast<const float*>(s.rows.p);   // float32 zero-padded rows for every non-Hamming set
       b.first = s.bow_words.p;
       b.row0 = brows;
       b.n = s.n;

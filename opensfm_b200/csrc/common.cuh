@@ -121,6 +121,19 @@ void download(std::vector<T>& h, const T* d, size_t n, cudaStream_t st) {
   download(h.data(), d, n, st);
 }
 
+// The kernels an engine has opted into more than 48 KB of dynamic shared memory, each once, at a fixed byte count.
+// The attribute is set for the current device, so an engine keeps one record per handle (= per device).
+struct SmemOptIn {
+  std::vector<const void*> opted;
+  template <class Kernel>
+  void operator()(Kernel* kernel, int bytes) {
+    const void* k = (const void*)kernel;
+    if (std::find(opted.begin(), opted.end(), k) != opted.end()) return;
+    OSFM_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
+    opted.push_back(k);
+  }
+};
+
 // An engine's device, its non-blocking stream there and NEV timing events, with the copies on that stream.
 template <int NEV>
 struct DeviceStream {

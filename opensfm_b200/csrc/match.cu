@@ -14,9 +14,10 @@
 //    distances (matching.py:754).
 //
 // Kernels in this file:
-//  bf_top2_simt<U8>   exact SIMT tile kernel (any float32 values, masks, Hamming)
-//  bf_top2_finalize   merge train chunks per query + ratio test
-//  bf_symmetric       keep (i,j) iff j's match is i (matching.py:775-777)
+//  bf_top2_simt        Hamming SIMT tile kernel (XOR + popcount)
+//  bf_top2_f32_cv<MT>  float32 SIMT tile kernel in cv2's summation order
+//  bf_top2_finalize    merge train chunks per query + ratio test
+//  bf_symmetric        keep (i,j) iff j's match is i (matching.py:775-777)
 // The wgmma tensor-core distance kernels live in match_tc.cu.
 #include <algorithm>
 #include <cmath>
@@ -29,40 +30,26 @@
 namespace osfm {
 
 // ---------------------------------------------------------------------------
-// SIMT tile kernel
+// Hamming SIMT tile kernel
 // ---------------------------------------------------------------------------
 constexpr int BM = 64;       // queries per CTA tile
 constexpr int BN = 64;       // trains per inner tile
-constexpr int DK = 16;       // elements (float or u32 word) per k-step
+constexpr int DK = 16;       // u32 words per k-step
 constexpr int LDS_STRIDE = 68;
 
-template <bool U8>
 __global__ void __launch_bounds__(256) bf_top2_simt(const MatchJob* __restrict__ jobs,
                                                     const int* __restrict__ tile_prefix, int njobs,
                                                     Top2* __restrict__ partial) {
-  using Elem = typename std::conditional<U8, uint32_t, float>::type;
-  using Acc = typename std::conditional<U8, int, float>::type;
-  __shared__ __align__(16) Elem As[DK][LDS_STRIDE];
-  __shared__ __align__(16) Elem Bs[DK][LDS_STRIDE];
+  __shared__ __align__(16) uint32_t As[DK][LDS_STRIDE];
+  __shared__ __align__(16) uint32_t Bs[DK][LDS_STRIDE];
   __shared__ Top2 cand[BM][16];
 
-  // locate the job of this CTA (binary search over the tile prefix sums)
-  int lo = 0, hi = njobs - 1;
-  const int cta = blockIdx.x;
-  while (lo < hi) {
-    const int mid = (lo + hi + 1) >> 1;
-    if (tile_prefix[mid] <= cta) lo = mid; else hi = mid - 1;
-  }
-  const MatchJob job = jobs[lo];
-  const int local = cta - tile_prefix[lo];
-  const int qtile = local / job.nchunks;
-  const int chunk = local % job.nchunks;
-  const int q0 = qtile * BM;
-  const int t_begin = chunk * job.chunk_len;
-  const int t_end = min(job.nt, t_begin + job.chunk_len);
-  const int D = job.dim_padded;  // elements per row (multiple of DK)
-  const Elem* __restrict__ Q = static_cast<const Elem*>(job.q);
-  const Elem* __restrict__ T = static_cast<const Elem*>(job.t);
+  const MatchTile tile = decode_tile<BM>(jobs, tile_prefix, njobs, blockIdx.x);
+  const MatchJob& job = tile.job;
+  const int q0 = tile.q0, t_begin = tile.t_begin, t_end = tile.t_end, chunk = tile.chunk;
+  const int D = job.dim_padded;  // words per row (multiple of DK)
+  const uint32_t* __restrict__ Q = static_cast<const uint32_t*>(job.q);
+  const uint32_t* __restrict__ T = static_cast<const uint32_t*>(job.t);
 
   const int tid = threadIdx.x;
   const int ty = tid >> 4, tx = tid & 15;
@@ -72,7 +59,7 @@ __global__ void __launch_bounds__(256) bf_top2_simt(const MatchJob* __restrict__
   for (int i = 0; i < 4; ++i) best[i] = top2_empty();
 
   for (int t0 = t_begin; t0 < t_end; t0 += BN) {
-    Acc acc[4][4];
+    int acc[4][4];
 #pragma unroll
     for (int i = 0; i < 4; ++i)
 #pragma unroll
@@ -86,8 +73,8 @@ __global__ void __launch_bounds__(256) bf_top2_simt(const MatchJob* __restrict__
         uint4 va = make_uint4(0, 0, 0, 0), vb = make_uint4(0, 0, 0, 0);
         if (gq < job.nq) va = *reinterpret_cast<const uint4*>(Q + (size_t)gq * D + k0 + kq * 4);
         if (gt < t_end) vb = *reinterpret_cast<const uint4*>(T + (size_t)gt * D + k0 + kq * 4);
-        const Elem* ea = reinterpret_cast<const Elem*>(&va);
-        const Elem* eb = reinterpret_cast<const Elem*>(&vb);
+        const uint32_t* ea = reinterpret_cast<const uint32_t*>(&va);
+        const uint32_t* eb = reinterpret_cast<const uint32_t*>(&vb);
 #pragma unroll
         for (int e = 0; e < 4; ++e) {
           As[kq * 4 + e][row] = ea[e];
@@ -99,19 +86,12 @@ __global__ void __launch_bounds__(256) bf_top2_simt(const MatchJob* __restrict__
       for (int k = 0; k < DK; ++k) {
         const uint4 a4 = *reinterpret_cast<const uint4*>(&As[k][ty * 4]);
         const uint4 b4 = *reinterpret_cast<const uint4*>(&Bs[k][tx * 4]);
-        const Elem* a = reinterpret_cast<const Elem*>(&a4);
-        const Elem* b = reinterpret_cast<const Elem*>(&b4);
+        const uint32_t* a = reinterpret_cast<const uint32_t*>(&a4);
+        const uint32_t* b = reinterpret_cast<const uint32_t*>(&b4);
 #pragma unroll
         for (int i = 0; i < 4; ++i)
 #pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            if constexpr (U8) {
-              acc[i][j] += __popc(a[i] ^ b[j]);
-            } else {
-              const float d = a[i] - b[j];
-              acc[i][j] = fmaf(d, d, acc[i][j]);
-            }
-          }
+          for (int j = 0; j < 4; ++j) acc[i][j] += __popc(a[i] ^ b[j]);
       }
       __syncthreads();
     }
@@ -124,9 +104,7 @@ __global__ void __launch_bounds__(256) bf_top2_simt(const MatchJob* __restrict__
         const int gt = t0 + tx * 4 + j;
         if (gq >= job.nq || gt >= t_end) continue;
         if (!job_allows(job, gq, gt)) continue;
-        float s;
-        if constexpr (U8) s = (float)acc[i][j]; else s = __fsqrt_rn(acc[i][j]);
-        top2_insert(best[i], s, gt);
+        top2_insert(best[i], (float)acc[i][j], gt);
       }
     }
   }
@@ -157,19 +135,9 @@ __global__ void __launch_bounds__(256) bf_top2_f32_cv(const MatchJob* __restrict
   extern __shared__ __align__(16) float fx_smem[];
   __shared__ Top2 cand[TS][16];
 
-  int lo = 0, hi = njobs - 1;
-  const int cta = blockIdx.x;
-  while (lo < hi) {
-    const int mid = (lo + hi + 1) >> 1;
-    if (tile_prefix[mid] <= cta) lo = mid; else hi = mid - 1;
-  }
-  const MatchJob job = jobs[lo];
-  const int local = cta - tile_prefix[lo];
-  const int qtile = local / job.nchunks;
-  const int chunk = local % job.nchunks;
-  const int q0 = qtile * TS;
-  const int t_begin = chunk * job.chunk_len;
-  const int t_end = min(job.nt, t_begin + job.chunk_len);
+  const MatchTile tile = decode_tile<TS>(jobs, tile_prefix, njobs, blockIdx.x);
+  const MatchJob& job = tile.job;
+  const int q0 = tile.q0, t_begin = tile.t_begin, t_end = tile.t_end, chunk = tile.chunk;
   const int D = job.dim_padded;
   const int nblk = job.dim / 16;   // full 16-element blocks of the TRUE dimension; the rest is cv2's scalar tail
   const float* __restrict__ Q = static_cast<const float*>(job.q);
@@ -217,6 +185,29 @@ __global__ void __launch_bounds__(256) bf_top2_f32_cv(const MatchJob* __restrict
 }
 constexpr int FX_MAX_DIM_T64 = 320;   // padded elements: 2 * 320 * 68 * 4 B = 174 KB of shared memory
 constexpr int FX_MAX_DIM_T32 = 704;   // 2 * 704 * 36 * 4 B = 203 KB
+
+static void launch_simt(Matcher& m, int njobs, int ntiles, int) {
+  bf_top2_simt<<<(unsigned)ntiles, 256, 0, m.stream>>>(m.d_jobs.p, m.d_prefix.p, njobs, m.d_partial.p);
+  OSFM_LAUNCH_CHECK();
+}
+template <int MT>
+static void launch_f32_cv(Matcher& m, int njobs, int ntiles, int smem) {
+  constexpr int max_dim = MT == 4 ? FX_MAX_DIM_T64 : FX_MAX_DIM_T32;
+  m.opt_in_smem(bf_top2_f32_cv<MT>, 2 * max_dim * (16 * MT + 4) * (int)sizeof(float));
+  bf_top2_f32_cv<MT><<<(unsigned)ntiles, 256, smem, m.stream>>>(m.d_jobs.p, m.d_prefix.p, njobs, m.d_partial.p);
+  OSFM_LAUNCH_CHECK();
+}
+
+// The SIMT kernels split the trains until there are four tiles per SM.  The float32 kernel keeps whole rows in
+// shared memory, so its tile edge follows the longest padded row of the submission.
+static KernelPlan simt_plan(bool u8, int max_dim_padded) {
+  if (u8) return {BM, BM, 4, false, 0, launch_simt};
+  if (max_dim_padded > FX_MAX_DIM_T32)
+    throw ArgError("float32 descriptors longer than 704 elements are not supported by the exact matcher");
+  const int tile = max_dim_padded > FX_MAX_DIM_T64 ? 32 : 64;
+  const int smem = 2 * max_dim_padded * (tile + 4) * (int)sizeof(float);
+  return {tile, tile, 4, false, smem, tile == 64 ? launch_f32_cv<4> : launch_f32_cv<2>};
+}
 
 // ---------------------------------------------------------------------------
 // Merge chunks + ratio test.  grid = (ceil(max_nq/256), njobs)
@@ -553,7 +544,7 @@ void Matcher::refresh_info() {
 }
 
 void Matcher::free_set(DescSet& s) {
-  slab_release(s.slab, s.data, s.slab_bytes);
+  release(s.rows);
   release(s.bearings);
   release(s.vlad);
   release(s.bow_words);
@@ -562,10 +553,7 @@ void Matcher::free_set(DescSet& s) {
     cudaMemsetAsync(d_info.p + 2 * s.slot, 0, 2 * sizeof(int), stream);
     free_slots.push_back(s.slot);
   }
-  s.data = nullptr;
-  s.tc_data = nullptr;
   s.tc_ok = false;
-  s.slab = -1;
   s.slot = -1;
 }
 
@@ -596,10 +584,7 @@ int Matcher::add_async(const void* host, int n, int dim, bool u8, bool u8_as_l2)
   const size_t data_bytes = align256((size_t)std::max(n, 1) * row_bytes);
   s.rows_padded = (tc || h8) ? tc_rows_padded(n) : 0;
   const size_t tc_bytes = tc ? tc_operand_bytes(s.rows_padded) : h8 ? h8_operand_bytes(s.rows_padded) : 0;
-  s.slab_bytes = data_bytes + tc_bytes;
-  char* chunk = static_cast<char*>(slab_alloc(s.slab_bytes, &s.slab));
-  s.data = chunk;
-  s.tc_data = (tc || h8) ? chunk + data_bytes : nullptr;
+  slab_new(s.rows, data_bytes + tc_bytes, n);
   if (tc) {
     if (d_info.p == nullptr) {
       d_info.reserve(2 * (size_t)MAX_SLOTS);
@@ -607,13 +592,13 @@ int Matcher::add_async(const void* host, int n, int dim, bool u8, bool u8_as_l2)
     }
     if (!free_slots.empty()) { s.slot = free_slots.back(); free_slots.pop_back(); }
     else if (next_slot < MAX_SLOTS) s.slot = next_slot++;
-    else { slab_release(s.slab, chunk, s.slab_bytes); throw std::runtime_error("too many resident descriptor sets"); }
+    else { release(s.rows); throw std::runtime_error("too many resident descriptor sets"); }
   }
   if (n > 0) {
     const bool dense = !u8_as_l2 && (size_t)dim * esz == (size_t)row_bytes;  // the upload already is the padded copy
-    const void* src = s.data;
+    const void* src = s.rows.p;
     if (dense) {
-      OSFM_CUDA(cudaMemcpyAsync(s.data, host, (size_t)n * row_bytes, cudaMemcpyHostToDevice, stream));
+      OSFM_CUDA(cudaMemcpyAsync(s.rows.p, host, (size_t)n * row_bytes, cudaMemcpyHostToDevice, stream));
     } else {
       staging.reserve(std::max<size_t>((size_t)n * dim * hsz, (size_t)4 << 20));
       OSFM_CUDA(cudaMemcpyAsync(staging.p, host, (size_t)n * dim * hsz, cudaMemcpyHostToDevice, stream));
@@ -621,22 +606,22 @@ int Matcher::add_async(const void* host, int n, int dim, bool u8, bool u8_as_l2)
     }
     if (tc) {
       // one fused pass: padded copy (if needed) + exactness + norms + bf16 operands (match_tc.cu)
-      prepare_tc(s, src, u8_as_l2, dense ? nullptr : static_cast<float*>(s.data));
+      prepare_tc(s, src, u8_as_l2, dense ? nullptr : reinterpret_cast<float*>(s.rows.p));
     } else if (u8_as_l2) {
       const size_t total = (size_t)n * s.dim_padded;
-      widen_rows_kernel<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(staging.p, n, dim, (float*)s.data, s.dim_padded);
+      widen_rows_kernel<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(staging.p, n, dim, (float*)s.rows.p, s.dim_padded);
       OSFM_LAUNCH_CHECK();
     } else if (!dense) {
       const size_t total = (size_t)n * row_bytes / esz;
       const int threads = 256;
       const unsigned blocks = (unsigned)((total + threads - 1) / threads);
       if (u8)
-        pad_rows_kernel<uint8_t><<<blocks, threads, 0, stream>>>(staging.p, n, dim, (uint8_t*)s.data, row_bytes);
+        pad_rows_kernel<uint8_t><<<blocks, threads, 0, stream>>>(staging.p, n, dim, (uint8_t*)s.rows.p, row_bytes);
       else
-        pad_rows_kernel<float><<<blocks, threads, 0, stream>>>((const float*)staging.p, n, dim, (float*)s.data, row_bytes / 4);
+        pad_rows_kernel<float><<<blocks, threads, 0, stream>>>((const float*)staging.p, n, dim, (float*)s.rows.p, row_bytes / 4);
       OSFM_LAUNCH_CHECK();
     }
-    if (h8) prepare_h8(s, static_cast<const uint8_t*>(s.data), row_bytes);
+    if (h8) prepare_h8(s, reinterpret_cast<const uint8_t*>(s.rows.p), row_bytes);
   } else {
     // a set without rows is trivially exact: its jobs have no query tiles or no train tiles, so it must not move
     // the rest of a submission off the tensor cores
@@ -680,153 +665,183 @@ void Matcher::clear() {
   sets.clear();
 }
 
-void Matcher::match_pairs_async(int npairs, const int* ids_a, const int* ids_b, double ratio, bool symmetric,
-                                const uint8_t* dmask, const double* pose12, double epi_threshold) {
-  refresh_info();
-  if (npairs < 0) throw ArgError("npairs < 0");
-  if (npairs > 30000) throw ArgError("at most 30000 pairs per submission");
-  const int ndir = symmetric ? 2 : 1;
-  const int njobs = npairs * ndir;
-  last_masks.clear();
-  h_jobs.assign(njobs, MatchJob());
-  h_prefix.assign(njobs + 1, 0);
-  h_out_off.assign(npairs + 1, 0);
-  bool any_u8 = false, any_f32 = false, all_tc = true, all_h8 = true;
-  long long total_qtiles = 0;
+// ---------------------------------------------------------------------------
+// A submission, step by step: build_jobs, plan_guided_masks, choose_kernel, cut_chunks, then upload and launch
+// (Matcher::match_pairs_async).
+// ---------------------------------------------------------------------------
+// What the jobs of a submission have in common.
+struct JobSummary {
+  bool any_u8 = false, any_f32 = false;
+  bool all_tc = true;   // every pair bf16-exact and norm-bounded: the tensor-core L2 kernel ranks as cv2 does
+  bool all_h8 = true;   // every set has the fp8 operands of the tensor-core Hamming kernel
   int max_nq = 0, max_dim_padded = 0;
+};
+
+// m.h_jobs: one job per pair and direction (job 2p is a->b, 2p+1 is b->a when symmetric); m.h_out_off: the first
+// result of every pair.
+static JobSummary build_jobs(Matcher& m, int npairs, const int* ids_a, const int* ids_b, bool symmetric,
+                             const uint8_t* dmask) {
+  const int ndir = symmetric ? 2 : 1;
+  m.h_jobs.assign(npairs * ndir, MatchJob());
+  m.h_out_off.assign(npairs + 1, 0);
+  JobSummary js;
   for (int p = 0; p < npairs; ++p) {
-    auto ia = sets.find(ids_a[p]), ib = sets.find(ids_b[p]);
-    if (ia == sets.end() || ib == sets.end()) throw ArgError("unknown descriptor set id in pair list");
+    auto ia = m.sets.find(ids_a[p]), ib = m.sets.find(ids_b[p]);
+    if (ia == m.sets.end() || ib == m.sets.end()) throw ArgError("unknown descriptor set id in pair list");
     const DescSet& A = ia->second;
     const DescSet& B = ib->second;
     // matching.py:737: assert f1.dtype.type == f2.dtype.type
     if (A.u8 != B.u8 || A.dim != B.dim) throw ArgError("descriptor sets of a pair differ in dtype or dimension");
-    any_u8 |= A.u8;
-    any_f32 |= !A.u8;
-    max_dim_padded = std::max(max_dim_padded, A.dim_padded);
+    js.any_u8 |= A.u8;
+    js.any_f32 |= !A.u8;
+    js.max_dim_padded = std::max(js.max_dim_padded, A.dim_padded);
     // d^2 <= (|a| + |b|)^2 <= 2 (|a|^2 + |b|^2) must stay below 2^22 for the d^2-space ranking of the
     // tensor-core kernel to equal cv2's sqrt-space ranking (float32 sqrt injective on integers < 2^22)
-    all_tc &= (!A.u8 && A.tc_ok && B.tc_ok && 2.0f * (A.tc_max_norm + B.tc_max_norm) < 4194304.0f);
-    all_h8 &= (A.u8 && A.tc_ok && B.tc_ok);
-    h_out_off[p + 1] = h_out_off[p] + A.n;
+    js.all_tc &= (!A.u8 && A.tc_ok && B.tc_ok && 2.0f * (A.tc_max_norm + B.tc_max_norm) < 4194304.0f);
+    js.all_h8 &= (A.u8 && A.tc_ok && B.tc_ok);
+    m.h_out_off[p + 1] = m.h_out_off[p] + A.n;
     for (int d = 0; d < ndir; ++d) {
-      MatchJob& j = h_jobs[p * ndir + d];
+      MatchJob& j = m.h_jobs[p * ndir + d];
       const DescSet& Qs = d == 0 ? A : B;
       const DescSet& Ts = d == 0 ? B : A;
-      j.q = Qs.data; j.t = Ts.data;
+      j.q = Qs.rows.p; j.t = Ts.rows.p;
       j.q_tc = Qs.tc_q; j.t_tc = Ts.tc_t;
       j.q_norm = Qs.tc_norm; j.t_norm = Ts.tc_norm;
       j.nq = Qs.n; j.nt = Ts.n;
       j.dim = A.dim;
       j.dim_padded = A.dim_padded;
-      j.qtiles = (j.nq + BM - 1) / BM;
       j.mask = dmask;
       if (dmask) {
         // forward: mask[q*n2 + t]; backward reads the transpose (matching.py:774)
         j.mask_sq = d == 0 ? B.n : 1;
         j.mask_st = d == 0 ? 1 : B.n;
       }
-      total_qtiles += j.qtiles;
-      max_nq = std::max(max_nq, j.nq);
+      js.max_nq = std::max(js.max_nq, j.nq);
     }
   }
-  if (any_u8 && any_f32) throw ArgError("mixed float32 / uint8 pairs in one submission");
-  // ---- guided matching: per-pair bitmasks (both layouts) built on the device ----
+  if (js.any_u8 && js.any_f32) throw ArgError("mixed float32 / uint8 pairs in one submission");
+  return js;
+}
+
+// Guided matching: places both layouts of every pair's bitmask in m.d_mask_bits and its epipolar vectors in
+// m.d_epi_vec, and points the jobs at their masks.  Returns the records epi_vectors / epi_mask_bits fill them from.
+static std::vector<EpiPair> plan_guided_masks(Matcher& m, int npairs, const int* ids_a, const int* ids_b,
+                                              bool symmetric, const double* pose12) {
+  const int ndir = symmetric ? 2 : 1;
+  size_t words = 0, vecs = 0;
+  std::vector<EpiPair> epi(npairs);
+  for (int p = 0; p < npairs; ++p) {   // offsets first: the buffers are sized by the whole submission
+    const DescSet& A = m.sets.find(ids_a[p])->second;
+    const DescSet& B = m.sets.find(ids_b[p])->second;
+    if (!A.bearings.p || !B.bearings.p) throw ArgError("guided matching needs bearings for both images (osfm_matcher_set_bearings)");
+    EpiPair& e = epi[p];
+    e.b1 = A.bearings.p; e.b2 = B.bearings.p; e.n1 = A.n; e.n2 = B.n;
+    e.w1 = (A.n + 31) / 32; e.w2 = (B.n + 31) / 32;
+    e.F = reinterpret_cast<uint32_t*>(words); words += (size_t)A.n * e.w2;
+    e.T = reinterpret_cast<uint32_t*>(words); words += (size_t)B.n * e.w1;
+    e.v1 = reinterpret_cast<double*>(vecs); vecs += 6 * (size_t)A.n;
+    e.v2 = reinterpret_cast<double*>(vecs); vecs += 6 * (size_t)B.n;
+    std::memcpy(e.pose, pose12 + 12 * (size_t)p, sizeof(double) * 12);
+  }
+  if (words > ((size_t)1 << 29)) throw ArgError("guided submission needs more than 2 GiB of mask bits: split the pair list");
+  m.d_mask_bits.reserve(std::max<size_t>(words, 1));
+  m.d_epi_vec.reserve(std::max<size_t>(vecs, 1));
+  for (int p = 0; p < npairs; ++p) {   // offsets -> pointers
+    EpiPair& e = epi[p];
+    e.F = m.d_mask_bits.p + reinterpret_cast<size_t>(e.F);
+    e.T = m.d_mask_bits.p + reinterpret_cast<size_t>(e.T);
+    e.v1 = m.d_epi_vec.p + reinterpret_cast<size_t>(e.v1);
+    e.v2 = m.d_epi_vec.p + reinterpret_cast<size_t>(e.v2);
+    for (int d = 0; d < ndir; ++d) {
+      MatchJob& j = m.h_jobs[p * ndir + d];
+      j.mask_bits = d == 0 ? e.F : e.T;
+      j.mask_words = d == 0 ? e.w2 : e.w1;
+    }
+    m.last_masks.push_back(EpiMasks{e.F, e.T, e.n1, e.n2, e.w1, e.w2});
+  }
+  return epi;
+}
+
+// choice (osfm_matcher_set_kernel): 0 takes the tensor cores wherever they rank as cv2 does, 1 the SIMT kernels,
+// 2 the tensor-core L2 kernel or an error.
+static DistKernel choose_kernel(int choice, const JobSummary& js, bool byte_mask, bool guided, int npairs) {
+  if (choice == 2) {
+    if (!js.all_tc || byte_mask)
+      throw ArgError("tensor-core kernel forced but descriptors are not bf16-exact / norm-bounded, or a mask is set");
+    return DistKernel::TC_L2;
+  }
+  if (choice == 0 && js.all_tc && !byte_mask && js.any_f32 && tc_available())
+    return DistKernel::TC_L2;   // (guided pairs too: the tensor-core epilogue applies the bitmask)
+  if (choice == 0 && js.all_h8 && js.any_u8 && !byte_mask && !guided && npairs > 0 && tc_available())
+    return DistKernel::TC_HAMMING;   // Hamming as a +-1 fp8 contraction
+  return DistKernel::SIMT;
+}
+
+struct TileCounts {
+  long long tiles = 0, partials = 0, matches = 0;
+};
+// Query tiles of the kernel's height; when they are too few to fill the GPU, the trains of every job are split into
+// chunks (whole multiples of chunk_unit).  Lays out the partials and results of the jobs, and m.h_prefix: the first
+// tile of every job, then the total.
+static TileCounts cut_chunks(Matcher& m, const KernelPlan& k) {
+  const int njobs = (int)m.h_jobs.size();
+  long long total_qtiles = 0;
+  for (auto& j : m.h_jobs) { j.qtiles = (j.nq + k.tile_m - 1) / k.tile_m; total_qtiles += j.qtiles; }
+  const long long target = (long long)m.num_sms * k.ctas_per_sm;
+  m.h_prefix.assign(njobs + 1, 0);
+  TileCounts c;
+  for (int i = 0; i < njobs; ++i) {
+    MatchJob& j = m.h_jobs[i];
+    int nchunks = 1;
+    if (total_qtiles < target && total_qtiles > 0) {
+      const int want = (int)((target + total_qtiles - 1) / total_qtiles);
+      const int maxc = std::max(1, (j.nt + k.chunk_unit - 1) / k.chunk_unit);
+      nchunks = std::min(want, maxc);
+    }
+    int chunk_len = (j.nt + nchunks - 1) / nchunks;
+    chunk_len = std::max(k.chunk_unit, (chunk_len + k.chunk_unit - 1) / k.chunk_unit * k.chunk_unit);
+    nchunks = std::max(1, (j.nt + chunk_len - 1) / chunk_len);
+    j.nchunks = nchunks;
+    j.chunk_len = chunk_len;
+    j.partial_off = c.partials;
+    c.partials += (long long)nchunks * j.nq;
+    j.match_off = c.matches;
+    c.matches += j.nq;
+    m.h_prefix[i] = (int)c.tiles;
+    c.tiles += (long long)j.qtiles * nchunks;
+    if (c.tiles > 0x7fffffffLL) throw ArgError("too many tiles in one submission");
+  }
+  m.h_prefix[njobs] = (int)c.tiles;
+  return c;
+}
+
+void Matcher::match_pairs_async(int npairs, const int* ids_a, const int* ids_b, double ratio, bool symmetric,
+                                const uint8_t* dmask, const double* pose12, double epi_threshold) {
+  refresh_info();
+  if (npairs < 0) throw ArgError("npairs < 0");
+  if (npairs > 30000) throw ArgError("at most 30000 pairs per submission");
+  last_masks.clear();
+  const JobSummary js = build_jobs(*this, npairs, ids_a, ids_b, symmetric, dmask);
+  const int njobs = (int)h_jobs.size();
   const bool guided = pose12 != nullptr;
   std::vector<EpiPair> epi;
   if (guided) {
     if (dmask) throw ArgError("guided matching builds its own mask");
-    size_t words = 0, vecs = 0;
-    epi.resize(npairs);
-    for (int p = 0; p < npairs; ++p) {
-      const DescSet& A = sets.find(ids_a[p])->second;
-      const DescSet& B = sets.find(ids_b[p])->second;
-      if (!A.bearings.p || !B.bearings.p) throw ArgError("guided matching needs bearings for both images (osfm_matcher_set_bearings)");
-      EpiPair& e = epi[p];
-      e.b1 = A.bearings.p; e.b2 = B.bearings.p; e.n1 = A.n; e.n2 = B.n;
-      e.w1 = (A.n + 31) / 32; e.w2 = (B.n + 31) / 32;
-      e.F = reinterpret_cast<uint32_t*>(words); words += (size_t)A.n * e.w2;
-      e.T = reinterpret_cast<uint32_t*>(words); words += (size_t)B.n * e.w1;
-      e.v1 = reinterpret_cast<double*>(vecs); vecs += 6 * (size_t)A.n;
-      e.v2 = reinterpret_cast<double*>(vecs); vecs += 6 * (size_t)B.n;
-      std::memcpy(e.pose, pose12 + 12 * (size_t)p, sizeof(double) * 12);
-    }
-    if (words > ((size_t)1 << 29)) throw ArgError("guided submission needs more than 2 GiB of mask bits: split the pair list");
-    d_mask_bits.reserve(std::max<size_t>(words, 1));
-    d_epi_vec.reserve(std::max<size_t>(vecs, 1));
-    for (int p = 0; p < npairs; ++p) {   // offsets -> pointers
-      EpiPair& e = epi[p];
-      e.F = d_mask_bits.p + reinterpret_cast<size_t>(e.F);
-      e.T = d_mask_bits.p + reinterpret_cast<size_t>(e.T);
-      e.v1 = d_epi_vec.p + reinterpret_cast<size_t>(e.v1);
-      e.v2 = d_epi_vec.p + reinterpret_cast<size_t>(e.v2);
-      for (int d = 0; d < ndir; ++d) {
-        MatchJob& j = h_jobs[p * ndir + d];
-        j.mask_bits = d == 0 ? e.F : e.T;
-        j.mask_words = d == 0 ? e.w2 : e.w1;
-      }
-      last_masks.push_back(EpiMasks{e.F, e.T, e.n1, e.n2, e.w1, e.w2});
-    }
+    epi = plan_guided_masks(*this, npairs, ids_a, ids_b, symmetric, pose12);
   }
-  // kernel choice
-  int use = 1;
-  if (kernel_choice == 2) {
-    if (!all_tc || dmask) throw ArgError("tensor-core kernel forced but descriptors are not bf16-exact / norm-bounded, or a mask is set");
-    use = 2;
-  } else if (kernel_choice == 0 && all_tc && !dmask && any_f32 && tc_available()) {
-    use = 2;   // (guided pairs too: the tensor-core epilogue applies the bitmask)
-  } else if (kernel_choice == 0 && all_h8 && any_u8 && !dmask && !guided && npairs > 0 && tc_available()) {
-    use = 3;   // Hamming as a +-1 fp8 contraction (match_tc.cu bf_top2_wg<KIND_HAMMING>)
-  }
-  last_kernel = use;
+  const DistKernel kernel = choose_kernel(kernel_choice, js, dmask != nullptr, guided, npairs);
+  last_kernel = (int)kernel;
   last_total_results = h_out_off[npairs];
   last_npairs = npairs;
+  const KernelPlan plan = kernel == DistKernel::SIMT ? simt_plan(js.any_u8, js.max_dim_padded) : tc_plan(kernel, guided);
+  const TileCounts counts = cut_chunks(*this, plan);
 
-  // split the train dimension when there are too few query tiles to fill the GPU
-  // float32 SIMT path: the cv2-order kernel keeps whole rows in shared memory -> tile edge by descriptor length
-  int simt_tile = BM;
-  if (use == 1 && any_f32) {
-    if (max_dim_padded > FX_MAX_DIM_T32)
-      throw ArgError("float32 descriptors longer than 704 elements are not supported by the exact matcher");
-    simt_tile = max_dim_padded > FX_MAX_DIM_T64 ? 32 : 64;
-  }
-  const int tile_m = use == 2 ? tc_tile_m() : use == 3 ? h8_tile_m() : simt_tile;
-  const int chunk_unit = use == 2 ? tc_tile_n() : use == 3 ? h8_tile_n() : simt_tile;
-  long long tiles_total = 0;
-  if (use >= 2 || simt_tile != BM) {
-    total_qtiles = 0;
-    for (auto& j : h_jobs) { j.qtiles = (j.nq + tile_m - 1) / tile_m; total_qtiles += j.qtiles; }
-  }
-  const long long target = (long long)num_sms * (use >= 2 ? 2 : 4);
-  long long partial_total = 0, match_total = 0;
-  for (int i = 0; i < njobs; ++i) {
-    MatchJob& j = h_jobs[i];
-    int nchunks = 1;
-    if (total_qtiles < target && total_qtiles > 0) {
-      const int want = (int)((target + total_qtiles - 1) / total_qtiles);
-      const int maxc = std::max(1, (j.nt + chunk_unit - 1) / chunk_unit);
-      nchunks = std::min(want, maxc);
-    }
-    int chunk_len = (j.nt + nchunks - 1) / nchunks;
-    chunk_len = std::max(chunk_unit, (chunk_len + chunk_unit - 1) / chunk_unit * chunk_unit);
-    nchunks = std::max(1, (j.nt + chunk_len - 1) / chunk_len);
-    j.nchunks = nchunks;
-    j.chunk_len = chunk_len;
-    j.partial_off = partial_total;
-    partial_total += (long long)nchunks * j.nq;
-    j.match_off = match_total;
-    match_total += j.nq;
-    h_prefix[i] = (int)tiles_total;
-    tiles_total += (long long)j.qtiles * nchunks;
-    if (tiles_total > 0x7fffffffLL) throw ArgError("too many tiles in one submission");
-  }
-  h_prefix[njobs] = (int)tiles_total;
-
+  // ---- upload and launch ----
   d_jobs.reserve(njobs + 1);
   d_prefix.reserve(njobs + 1);
   d_out_off.reserve(npairs + 1);
-  d_partial.reserve(std::max<long long>(partial_total, 1));
-  d_match.reserve(std::max<long long>(match_total, 1));
+  d_partial.reserve(std::max<long long>(counts.partials, 1));
+  d_match.reserve(std::max<long long>(counts.matches, 1));
   d_out.reserve(std::max<long long>(last_total_results, 1));
   p_jobs.reserve(njobs + 1);
   p_prefix.reserve(njobs + 1);
@@ -860,37 +875,14 @@ void Matcher::match_pairs_async(int npairs, const int* ids_a, const int* ids_b, 
     OSFM_LAUNCH_CHECK();
   }
   OSFM_CUDA(cudaEventRecord(ev[1], stream));
-  if (tiles_total > 0) {
-    if (use == 2) {
-      launch_tc(*this, njobs, (int)tiles_total, guided);
-    } else if (use == 3) {
-      launch_tc_h8(*this, njobs, (int)tiles_total);
-    } else if (any_u8) {
-      bf_top2_simt<true><<<(unsigned)tiles_total, 256, 0, stream>>>(d_jobs.p, d_prefix.p, njobs, d_partial.p);
-      OSFM_LAUNCH_CHECK();
-    } else {
-      const size_t smem = 2 * (size_t)max_dim_padded * (simt_tile + 4) * sizeof(float);
-      if (!fx_attr_set) {
-        OSFM_CUDA(cudaFuncSetAttribute(bf_top2_f32_cv<4>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       2 * FX_MAX_DIM_T64 * 68 * (int)sizeof(float)));
-        OSFM_CUDA(cudaFuncSetAttribute(bf_top2_f32_cv<2>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       2 * FX_MAX_DIM_T32 * 36 * (int)sizeof(float)));
-        fx_attr_set = true;
-      }
-      if (simt_tile == 64)
-        bf_top2_f32_cv<4><<<(unsigned)tiles_total, 256, smem, stream>>>(d_jobs.p, d_prefix.p, njobs, d_partial.p);
-      else
-        bf_top2_f32_cv<2><<<(unsigned)tiles_total, 256, smem, stream>>>(d_jobs.p, d_prefix.p, njobs, d_partial.p);
-      OSFM_LAUNCH_CHECK();
-    }
-  }
+  if (counts.tiles > 0) plan.launch(*this, njobs, (int)counts.tiles, plan.smem);
   OSFM_CUDA(cudaEventRecord(ev[2], stream));
-  if (njobs > 0 && max_nq > 0) {
-    dim3 grid((max_nq + 255) / 256, njobs);
-    bf_top2_finalize<<<grid, 256, 0, stream>>>(d_jobs.p, d_partial.p, d_match.p, ratio, use == 2 ? 1 : 0);
+  if (njobs > 0 && js.max_nq > 0) {
+    dim3 grid((js.max_nq + 255) / 256, njobs);
+    bf_top2_finalize<<<grid, 256, 0, stream>>>(d_jobs.p, d_partial.p, d_match.p, ratio, plan.squared ? 1 : 0);
     OSFM_LAUNCH_CHECK();
     if (symmetric) {
-      dim3 g2((max_nq + 255) / 256, npairs);
+      dim3 g2((js.max_nq + 255) / 256, npairs);
       bf_symmetric<<<g2, 256, 0, stream>>>(d_jobs.p, d_match.p, d_out.p, d_out_off.p);
       OSFM_LAUNCH_CHECK();
     }

@@ -175,6 +175,41 @@ __device__ __forceinline__ bool job_allows(const MatchJob& job, int gq, int gt) 
   return true;
 }
 
+// Tile `tile` of a submission: queries q0 .. q0 + M - 1 of `job` against its trains t_begin .. t_end - 1 (chunk
+// `chunk`).  A job's tiles are its query tiles times its chunks, chunk fastest; tile_prefix[i] is job i's first tile.
+struct MatchTile {
+  MatchJob job;
+  int q0, t_begin, t_end, chunk;
+};
+template <int M>
+__device__ __forceinline__ MatchTile decode_tile(const MatchJob* __restrict__ jobs, const int* __restrict__ tile_prefix,
+                                                 int njobs, int tile) {
+  int lo = 0, hi = njobs - 1;
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (tile_prefix[mid] <= tile) lo = mid; else hi = mid - 1;
+  }
+  MatchTile t;
+  t.job = jobs[lo];
+  const int local = tile - tile_prefix[lo];
+  t.q0 = local / t.job.nchunks * M;
+  t.chunk = local % t.job.nchunks;
+  t.t_begin = t.chunk * t.job.chunk_len;
+  t.t_end = min(t.job.nt, t.t_begin + t.job.chunk_len);
+  return t;
+}
+
+// Offsets of arrays packed into one device table, each on a 256-byte boundary.
+inline size_t align256(size_t bytes) { return (bytes + 255) / 256 * 256; }
+struct TableLayout {
+  size_t size = 0;
+  size_t add(size_t bytes) {
+    const size_t o = size;
+    size += align256(bytes);
+    return o;
+  }
+};
+
 // An array in the matcher's slabs (Matcher::slab_new / Matcher::release); null until allocated.
 template <class T>
 struct SlabArray {
@@ -185,11 +220,13 @@ struct SlabArray {
 };
 
 struct DescSet {
-  void* data = nullptr;
+  // one allocation: the zero-padded rows (n x row_bytes), then the tensor-core operands of a set that has them
+  SlabArray<char> rows;
   int n = 0, dim = 0, dim_padded = 0, row_bytes = 0;
   bool u8 = false;
-  // tensor-core operands (float32 sets with integer values in [0,255] and dim <= 128 only)
-  void* tc_data = nullptr;  // one allocation: [A-role | B-role | norms]
+  // tensor-core operands (float32 sets with integer values in [0,255] and dim <= 128, Hamming sets of <= 63 bytes):
+  // L2 [A-role | B-role | norms], Hamming [A-role | B-role]
+  char* tc_data() const { return rows.p + align256((size_t)std::max(n, 1) * row_bytes); }
   const __nv_bfloat16* tc_q = nullptr;
   const __nv_bfloat16* tc_t = nullptr;
   const float* tc_norm = nullptr;
@@ -198,8 +235,7 @@ struct DescSet {
   int rows_padded = 0;
   // device memory comes from the matcher's slabs; the exactness flag / max norm of a freshly added set
   // live in d_info[slot] until refresh_info() reads them back (no host sync per add)
-  int slab = -1, slot = -1;
-  size_t slab_bytes = 0;   // size of the data + operands allocation
+  int slot = -1;
   bool info_pending = false;
   // unit bearing vectors of the features (n x 3 float32), for guided matching
   SlabArray<float> bearings;
@@ -235,7 +271,7 @@ struct Matcher : DeviceStream<4> {
   long long last_total_results = 0;
   int last_npairs = 0;
   bool results_in_match_buf = true;
-  bool tc_attr_set = false, tcm_attr_set = false, fx_attr_set = false, h8_attr_set = false;
+  SmemOptIn opt_in_smem;
   std::map<int, DescSet> sets;
   std::vector<MatchJob> h_jobs;
   std::vector<int> h_prefix;
@@ -326,31 +362,32 @@ struct Matcher : DeviceStream<4> {
   void prepare_h8(DescSet& s, const uint8_t* src, int src_stride);   // +-1 fp8 operands of a Hamming set
 };
 
+// The distance kernel of a submission; the values are those osfm_matcher_last_kernel returns.
+enum class DistKernel : int {
+  SIMT = 1,         // bf_top2_simt (Hamming), bf_top2_f32_cv (float32)
+  TC_L2 = 2,        // bf_top2_wg<KIND_L2> (match_tc.cu)
+  TC_HAMMING = 3,   // bf_top2_wg<KIND_HAMMING>
+};
+
+// What the distance kernel fixes in a submission's plan.
+struct KernelPlan {
+  int tile_m;        // query rows per tile
+  int chunk_unit;    // train chunks are whole multiples of this many rows
+  int ctas_per_sm;   // the trains are split into chunks until the tiles reach this many per SM
+  bool squared;      // the partials hold d^2, which bf_top2_finalize takes the square root of
+  int smem;          // dynamic shared memory of a CTA
+  void (*launch)(Matcher& m, int njobs, int ntiles, int smem);
+};
+
 // match_tc.cu
 bool tc_available();
-int tc_tile_m();
-int tc_tile_n();
-void launch_tc(Matcher& m, int njobs, int ntiles, bool masked);
+KernelPlan tc_plan(DistKernel kernel, bool masked);   // kernel: TC_L2 or TC_HAMMING; masked: guided L2
 int tc_rows_padded(int n);
 size_t tc_operand_bytes(int rows_padded);
 bool tc_capable(int dim, bool u8);
 // tensor-core Hamming (match_tc.cu)
-int h8_tile_m();
-int h8_tile_n();
 size_t h8_operand_bytes(int rows_padded);
 bool h8_capable(int nbytes);
-void launch_tc_h8(Matcher& m, int njobs, int ntiles);
-
-// Offsets of arrays packed into one device table, each on a 256-byte boundary.
-inline size_t align256(size_t bytes) { return (bytes + 255) / 256 * 256; }
-struct TableLayout {
-  size_t size = 0;
-  size_t add(size_t bytes) {
-    const size_t o = size;
-    size += align256(bytes);
-    return o;
-  }
-};
 
 }  // namespace osfm
 

@@ -82,9 +82,6 @@ static_assert(WgGeom<KIND_L2>::SMEM <= 227 * 1024 - 1024, "L2 kernel exceeds the
 static_assert(WgGeom<KIND_HAMMING>::SMEM <= 227 * 1024 - 1024, "Hamming kernel exceeds the H100 shared memory of a block");
 static_assert(WgGeom<KIND_L2>::M == 256, "tc_rows_padded pads sets to whole L2 query tiles");
 
-int tc_tile_m() { return WgGeom<KIND_L2>::M; }
-int tc_tile_n() { return WG_N; }
-
 // The library is built for sm_90a only, so this is the H100 class (compute capability 9.0) it can run on.
 bool tc_available() {
   int dev = 0;
@@ -187,9 +184,9 @@ __global__ void __launch_bounds__(256)
 void Matcher::prepare_tc(DescSet& s, const void* src, bool src_u8, float* padded_dst) {
   const int rows_padded = s.rows_padded;
   const size_t op_bytes = (size_t)rows_padded * TC_ROW_BYTES;
-  __nv_bfloat16* qa = reinterpret_cast<__nv_bfloat16*>(s.tc_data);
-  __nv_bfloat16* tb = reinterpret_cast<__nv_bfloat16*>(reinterpret_cast<char*>(s.tc_data) + op_bytes);
-  float* norm = reinterpret_cast<float*>(reinterpret_cast<char*>(s.tc_data) + 2 * op_bytes);
+  __nv_bfloat16* qa = reinterpret_cast<__nv_bfloat16*>(s.tc_data());
+  __nv_bfloat16* tb = reinterpret_cast<__nv_bfloat16*>(s.tc_data() + op_bytes);
+  float* norm = reinterpret_cast<float*>(s.tc_data() + 2 * op_bytes);
   if (src_u8)
     tc_prepare_set<uint8_t><<<(rows_padded + 7) / 8, 256, 0, stream>>>(static_cast<const uint8_t*>(src), s.n, s.dim, rows_padded,
                                                                       padded_dst, s.dim_padded, norm, qa, tb, d_info.p + 2 * s.slot);
@@ -265,35 +262,11 @@ __device__ __forceinline__ void wg_mma<KIND_HAMMING>(float (&d)[64], uint64_t ad
       : "memory");
 }
 
-struct TcTask {
-  MatchJob job;
-  int q0, t_begin, ntiles, chunk;
-};
-
-template <int M>
-__device__ __forceinline__ TcTask tc_decode(const MatchJob* jobs, const int* tile_prefix, int njobs, int task) {
-  int lo = 0, hi = njobs - 1;
-  while (lo < hi) {
-    const int mid = (lo + hi + 1) >> 1;
-    if (tile_prefix[mid] <= task) lo = mid; else hi = mid - 1;
-  }
-  TcTask t;
-  t.job = jobs[lo];
-  const int local = task - tile_prefix[lo];
-  const int qtile = local / t.job.nchunks;
-  t.chunk = local % t.job.nchunks;
-  t.q0 = qtile * M;
-  t.t_begin = t.chunk * t.job.chunk_len;
-  const int t_end = min(t.job.nt, t.t_begin + t.job.chunk_len);
-  t.ntiles = (t_end - t.t_begin + WG_N - 1) / WG_N;
-  return t;
-}
-
 // Epilogue state of one query row: the two smallest accumulator values (L2: d^2 - |a|^2; Hamming: 2 H - nbits;
 // exact integers either way) with their train indices.  For L2, ranking in d^2 is the ranking cv2 uses (sqrt'd
 // float32 distance, ties -> lowest index) as long as float32 sqrt is injective on the integers involved, i.e.
 // d^2 < 2^22; the host only selects this kernel for descriptor sets whose norms guarantee that bound
-// (Matcher::match_pairs_async), everything else goes to the exact SIMT kernel.
+// (choose_kernel, match.cu), everything else goes to the exact SIMT kernel.
 struct RowState {
   float q1, q2;
   int i1, i2;
@@ -367,7 +340,8 @@ __global__ void __launch_bounds__(WG_THREADS, 1)
     if (warp == CONSUMER_WARPS && lane == 0) {
       int stage = 0, ph = 0, n = 0;
       for (int task = blockIdx.x; task < ntasks; task += gridDim.x, ++n) {
-        const TcTask t = tc_decode<G::M>(jobs, tile_prefix, njobs, task);
+        const MatchTile t = decode_tile<G::M>(jobs, tile_prefix, njobs, task);
+        const int ntiles = (t.t_end - t.t_begin + WG_N - 1) / WG_N;
         const int b = n % QBUF, qph = (n / QBUF) & 1;
         mbar_wait(&bar_qempty[b], qph ^ 1, err_flag);
         // the last query tile of a job may hold no rows for the second warpgroup: only the first half is loaded
@@ -375,7 +349,7 @@ __global__ void __launch_bounds__(WG_THREADS, 1)
         mbar_expect_tx(&bar_qfull[b], qbytes);
         bulk_copy_g2s(smem + b * G::Q_BYTES, reinterpret_cast<const uint8_t*>(t.job.q_tc) + (size_t)t.q0 * C::ROW_BYTES,
                       qbytes, &bar_qfull[b]);
-        for (int i = 0; i < t.ntiles; ++i) {
+        for (int i = 0; i < ntiles; ++i) {
           mbar_wait(&bar_empty[stage], ph ^ 1, err_flag);
           mbar_expect_tx(&bar_full[stage], G::T_BYTES);
           bulk_copy_g2s(smem + QBUF * G::Q_BYTES + stage * G::T_BYTES,
@@ -399,7 +373,8 @@ __global__ void __launch_bounds__(WG_THREADS, 1)
     for (int i = 0; i < 64; ++i) acc[mb][i] = 0.0f;
   int stage = 0, ph = 0, n = 0;
   for (int task = blockIdx.x; task < ntasks; task += gridDim.x, ++n) {
-    const TcTask t = tc_decode<G::M>(jobs, tile_prefix, njobs, task);
+    const MatchTile t = decode_tile<G::M>(jobs, tile_prefix, njobs, task);
+    const int ntiles = (t.t_end - t.t_begin + WG_N - 1) / WG_N;
     const int b = n % QBUF, qph = (n / QBUF) & 1;
     const bool active = t.job.nq - t.q0 > wg_row0;
     RowState st[2 * MB];
@@ -410,7 +385,7 @@ __global__ void __launch_bounds__(WG_THREADS, 1)
     }
     mbar_wait(&bar_qfull[b], qph, err_flag);
     const uint32_t q_addr = smem_u32(smem + b * G::Q_BYTES) + (wg_row0 / 8) * G::SBO;
-    for (int i = 0; i < t.ntiles; ++i) {
+    for (int i = 0; i < ntiles; ++i) {
       mbar_wait(&bar_full[stage], ph, err_flag);
       if (active) {
         const uint32_t t_addr = smem_u32(smem + QBUF * G::Q_BYTES + stage * G::T_BYTES);
@@ -511,8 +486,6 @@ __global__ void __launch_bounds__(WG_THREADS, 1)
 // positions: nbytes <= 63); the epilogue drops the padding trains a query with fewer than two real ones keeps.  wgmma m64 n128 k32 e4m3, operands in the same no-swizzle K-major core-matrix order as
 // the bf16 kernel (a core matrix row is 16 bytes = 16 fp8), 512 B per row.
 // ===========================================================================================================
-int h8_tile_m() { return WgGeom<KIND_HAMMING>::M; }
-int h8_tile_n() { return WG_N; }
 size_t h8_operand_bytes(int rows_padded) { return 2 * (size_t)rows_padded * H8_ROW_BYTES; }
 bool h8_capable(int nbytes) { return nbytes >= 1 && nbytes <= 63 && tc_available(); }
 
@@ -549,7 +522,7 @@ __global__ void __launch_bounds__(256)
 
 void Matcher::prepare_h8(DescSet& s, const uint8_t* src, int src_stride) {
   const size_t op_bytes = (size_t)s.rows_padded * H8_ROW_BYTES;
-  uint8_t* qa = reinterpret_cast<uint8_t*>(s.tc_data);
+  uint8_t* qa = reinterpret_cast<uint8_t*>(s.tc_data());
   uint8_t* tb = qa + op_bytes;
   const size_t total = (size_t)s.rows_padded * H8_KCH;
   h8_prepare_set<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(src, s.n, s.dim, src_stride, s.rows_padded, qa, tb);
@@ -561,36 +534,22 @@ void Matcher::prepare_h8(DescSet& s, const uint8_t* src, int src_stride) {
 }
 
 template <int KIND, bool MASKED>
-static void launch_wg(Matcher& m, int njobs, int ntasks) {
+static void launch_wg(Matcher& m, int njobs, int ntasks, int smem) {
+  m.opt_in_smem(bf_top2_wg<KIND, MASKED>, smem);
   m.d_flags.reserve(4);
   OSFM_CUDA(cudaMemsetAsync(m.d_flags.p + 1, 0, sizeof(int), m.stream));
   const int grid = std::min(ntasks, m.num_sms);
-  bf_top2_wg<KIND, MASKED><<<grid, WG_THREADS, WgGeom<KIND>::SMEM, m.stream>>>(m.d_jobs.p, m.d_prefix.p, njobs, ntasks,
-                                                                             m.d_partial.p, m.d_flags.p + 1);
+  bf_top2_wg<KIND, MASKED><<<grid, WG_THREADS, smem, m.stream>>>(m.d_jobs.p, m.d_prefix.p, njobs, ntasks, m.d_partial.p,
+                                                                 m.d_flags.p + 1);
   OSFM_LAUNCH_CHECK();
 }
 
-void launch_tc_h8(Matcher& m, int njobs, int ntasks) {
-  if (!m.h8_attr_set) {
-    OSFM_CUDA(cudaFuncSetAttribute(bf_top2_wg<KIND_HAMMING, false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                   WgGeom<KIND_HAMMING>::SMEM));
-    m.h8_attr_set = true;
-  }
-  launch_wg<KIND_HAMMING, false>(m, njobs, ntasks);
-}
-
-void launch_tc(Matcher& m, int njobs, int ntasks, bool masked) {
-  if (!m.tc_attr_set) {   // per matcher (= per device)
-    OSFM_CUDA(cudaFuncSetAttribute(bf_top2_wg<KIND_L2, false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                   WgGeom<KIND_L2>::SMEM));
-    OSFM_CUDA(cudaFuncSetAttribute(bf_top2_wg<KIND_L2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                   WgGeom<KIND_L2>::SMEM));
-    m.tc_attr_set = true;
-  }
-  if (masked)
-    launch_wg<KIND_L2, true>(m, njobs, ntasks);
-  else
-    launch_wg<KIND_L2, false>(m, njobs, ntasks);
+// Persistent CTAs over WG_N-row train tiles; the trains are split until there are two tasks per SM.
+KernelPlan tc_plan(DistKernel kernel, bool masked) {
+  if (kernel == DistKernel::TC_HAMMING)
+    return {WgGeom<KIND_HAMMING>::M, WG_N, 2, false, WgGeom<KIND_HAMMING>::SMEM, launch_wg<KIND_HAMMING, false>};
+  return {WgGeom<KIND_L2>::M, WG_N, 2, true, WgGeom<KIND_L2>::SMEM,
+          masked ? launch_wg<KIND_L2, true> : launch_wg<KIND_L2, false>};
 }
 
 }  // namespace osfm

@@ -257,7 +257,7 @@ int osfm_matcher_vlad_compute(osfm_matcher* m, int count, const int* set_ids, co
       if (!valid) continue;
       if (!s.vlad.p) M.slab_new(s.vlad, 2 * L * sizeof(float), (int)L);
       VladJob j;
-      j.f = static_cast<const float*>(s.data);   // float32 zero-padded rows for every non-Hamming set (match.cu add_async)
+      j.f = reinterpret_cast<const float*>(s.rows.p);   // float32 zero-padded rows for every non-Hamming set (match.cu add_async)
       j.v = s.vlad.p;
       j.aoff = nfeat;
       j.n = s.n;
