@@ -12,7 +12,9 @@
  *           opensfm/src/bundle/src/bundle_adjuster.cc) behind pybundle /
  *          sfm::BAHelpers (opensfm/src/sfm/src/ba_helpers.cc:117,408,581).
  * and, between them, TRACKS: linking matches into tracks, replacing
- *          tracking.create_tracks_manager (opensfm/tracking.py:72-150).
+ *          tracking.create_tracks_manager (opensfm/tracking.py:72-150), and
+ *          triangulating them, replacing TrackTriangulator.triangulate
+ *          (opensfm/reconstruction.py:1032-1073).
  *
  * There is no CPU fallback: every call needs a CUDA device (H100, sm_90a).
  *
@@ -442,6 +444,27 @@ int osfm_tracks_get_common(osfm_tracks* t, int32_t* pair_a, int32_t* pair_b, int
 /* Device time of the last osfm_tracks_build (kernels, sorts and scans, after the uploads) and the last
  * osfm_tracks_common (CUDA events on the handle's stream). */
 int osfm_tracks_last_device_ms(osfm_tracks* t, float* ms_build, float* ms_common);
+
+/* Triangulates the handle's tracks from its device-resident observations: TrackTriangulator.triangulate
+ * (opensfm/reconstruction.py:1032-1073) of every selected track, i.e. TriangulateBearingsMidpoint with its angle,
+ * reprojection and depth tests (geometry/src/triangulation.cc:137-177) and PointRefinement (:221-233), in fp64.
+ * num_images / num_observations / num_tracks must be the handle's (osfm_tracks_build).  Per image: image_rt
+ * (row-major R^T of the world-to-camera rotation, 9), image_origin (3), image_in (1 if the image is in the
+ * reconstruction); only observations in such images are used.  Per observation, in osfm_tracks_get's order:
+ * bearings (camera frame, 3; read only in images of the reconstruction).  Per track: selected (0 / 1).
+ * threshold is the reprojection angle and min_ray_angle the least ray angle, both in radians; iterations bounds the
+ * refinement.  Out per track: status (OSFM_TRI_*) and points (3; NaN unless the status is OSFM_TRI_OK). */
+#define OSFM_TRI_NOT_SELECTED 0
+#define OSFM_TRI_TOO_FEW 1          /* fewer than 2 observations in images of the reconstruction */
+#define OSFM_TRI_BAD_ANGLE 2        /* no pair of rays at an angle in [min_ray_angle, pi - min_ray_angle] */
+#define OSFM_TRI_BAD_REPROJECTION 3 /* the midpoint fails the reprojection or the depth test */
+#define OSFM_TRI_OK 4
+int osfm_tracks_triangulate(osfm_tracks* t, int num_images, const double* image_rt, const double* image_origin,
+                            const uint8_t* image_in, int64_t num_observations, const double* bearings,
+                            int64_t num_tracks, const uint8_t* selected, double threshold, double min_ray_angle,
+                            double min_depth, int iterations, int8_t* status, double* points);
+/* Device time of the last osfm_tracks_triangulate (CUDA events around its kernel, after the uploads). */
+int osfm_tracks_last_triangulate_ms(osfm_tracks* t, float* ms);
 
 /* ------------------------------------------------------------------------
  * ROTATION-ONLY RANSAC OF IMAGE PAIRS

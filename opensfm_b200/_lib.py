@@ -148,6 +148,9 @@ SIGNATURES = {
     "osfm_tracks_common": (c_int, [c_void_p, POINTER(c_int64), POINTER(c_int64)]),
     "osfm_tracks_get_common": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "osfm_tracks_last_device_ms": (c_int, [c_void_p, POINTER(c_float), POINTER(c_float)]),
+    "osfm_tracks_triangulate": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_int64,
+                                        c_void_p, c_double, c_double, c_double, c_int, c_void_p, c_void_p]),
+    "osfm_tracks_last_triangulate_ms": (c_int, [c_void_p, POINTER(c_float)]),
     "osfm_rotransac_create": (c_int, [c_int, POINTER(c_void_p)]),
     "osfm_rotransac_destroy": (c_int, [c_void_p]),
     "osfm_rotransac_run": (c_int, [c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_double, c_int,

@@ -16,6 +16,7 @@
 //   common: trk_pair_counts .. trk_pair_finish   every (track, image a < image b) keyed by the image pair, one
 //                            radix sort, run lengths = connectivity
 // The host reads back only counts (TrkCounts).
+//   triangulate: triangulate.cu, on the observation arrays built here
 #include <thrust/iterator/counting_iterator.h>
 
 #include <algorithm>
@@ -23,6 +24,7 @@
 #include <vector>
 
 #include "common.cuh"
+#include "triangulate.cuh"
 
 namespace osfm {
 namespace {
@@ -249,7 +251,7 @@ int trk_bits(unsigned long long max_value) {
   return b;
 }
 
-struct Tracks : DeviceStream<4> {   // events: build start / end, common start / end
+struct Tracks : DeviceStream<6> {   // events: build start / end, common start / end, triangulate start / end
   bool built = false, common_built = false, timed_build = false, timed_common = false;
   int I = 0, T = 0, Q = 0;
   long long nobs = 0, R = 0;
@@ -272,6 +274,7 @@ struct Tracks : DeviceStream<4> {   // events: build start / end, common start /
   DevBuf<int> d_cpair_a, d_cpair_b;
   PinnedBuf<TrkCounts> h_counts;
   PinnedBuf<long long> h_ll;
+  TriWorkspace tri;
 
   explicit Tracks(int dev) : DeviceStream(dev) {
     d_counts.reserve(1);
@@ -295,7 +298,7 @@ struct Tracks : DeviceStream<4> {   // events: build start / end, common start /
 void Tracks::build(int num_images, const int32_t* num_features, const uint8_t* has_features, int64_t num_pairs,
                    const int32_t* pair_a, const int32_t* pair_b, const int64_t* match_start, const int32_t* matches,
                    int min_length, int64_t* num_tracks, int64_t* num_observations) {
-  built = common_built = timed_build = timed_common = false;
+  built = common_built = timed_build = timed_common = tri.timed = false;
   if (num_images < 0 || num_pairs < 0 || num_pairs > TRK_MAX_ITEMS) throw ArgError("bad tracks sizes");
   if (!num_tracks || !num_observations) throw ArgError("null outputs");
   if ((num_images > 0 && (!num_features || !has_features)) || (num_pairs > 0 && (!pair_a || !pair_b)) || !match_start)
@@ -562,6 +565,31 @@ int osfm_tracks_get_common(osfm_tracks* t, int32_t* pair_a, int32_t* pair_b, int
     K.download(reinterpret_cast<long long*>(common_obs_a), reinterpret_cast<long long*>(K.d_key.p), (size_t)K.R);
     K.download(reinterpret_cast<long long*>(common_obs_b), reinterpret_cast<long long*>(K.d_val.p), (size_t)K.R);
     OSFM_CUDA(cudaStreamSynchronize(K.stream));
+  });
+}
+
+int osfm_tracks_triangulate(osfm_tracks* t, int num_images, const double* image_rt, const double* image_origin,
+                            const uint8_t* image_in, int64_t num_observations, const double* bearings,
+                            int64_t num_tracks, const uint8_t* selected, double threshold, double min_ray_angle,
+                            double min_depth, int iterations, int8_t* status, double* points) {
+  return osfm::with_handle(t, [&](osfm::Tracks& K) {
+    if (!K.built) throw std::runtime_error("tracks: osfm_tracks_triangulate needs a successful osfm_tracks_build");
+    if (num_images != K.I || num_observations != K.nobs || num_tracks != K.T)
+      throw osfm::ArgError("tracks: osfm_tracks_triangulate sizes (" + std::to_string(num_images) + " images, " +
+                           std::to_string(num_observations) + " observations, " + std::to_string(num_tracks) +
+                           " tracks) differ from the handle's (" + std::to_string(K.I) + ", " +
+                           std::to_string(K.nobs) + ", " + std::to_string(K.T) + ")");
+    const osfm::TriTopology topo{K.I, K.T, K.nobs, K.d_obs_image.p, K.d_track_start.p};
+    osfm::triangulate_tracks(K.tri, K.stream, K.ev[4], K.ev[5], topo, image_rt, image_origin, image_in, bearings,
+                             selected, threshold, min_ray_angle, min_depth, iterations, status, points);
+  });
+}
+
+int osfm_tracks_last_triangulate_ms(osfm_tracks* t, float* ms) {
+  return osfm::with_handle(t, [&](osfm::Tracks& K) {
+    if (!ms) throw osfm::ArgError("null ms");
+    *ms = 0.f;
+    if (K.tri.timed) OSFM_CUDA(cudaEventElapsedTime(ms, K.ev[4], K.ev[5]));
   });
 }
 

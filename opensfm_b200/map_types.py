@@ -224,10 +224,23 @@ class Reconstruction:
         self.rig_cameras: Dict[str, RigCamera] = {}
         self.rig_instances: Dict[str, RigInstance] = {}
         self.shots: Dict[str, Shot] = {}
-        self.points: Dict[str, Landmark] = {}
+        self._points: Dict[str, Landmark] = {}
         self._shot_obs: Dict[str, Dict[str, Observation]] = {}
         self._pt_obs: Dict[str, Dict[str, Observation]] = {}
         self.reference = None   # object with to_topocentric(lat, lon, alt) (opensfm.geo.TopocentricConverter)
+
+    @property
+    def points(self) -> Dict[str, Landmark]:
+        return self._points
+
+    @points.setter
+    def points(self, value: Dict[str, Landmark]) -> None:
+        """Replaces every point, dropping all observations, as types.Reconstruction.set_points does."""
+        self._shot_obs.clear()
+        self._pt_obs.clear()
+        self._points = {}
+        for lm in list(value.values()):
+            self.create_point(lm.id, lm.coordinates)
 
     @property
     def map(self) -> "Reconstruction":

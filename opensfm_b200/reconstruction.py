@@ -24,6 +24,11 @@ by the rotation-only RANSAC of opensfm_b200/rotation_ransac.py:
   two_view_reconstruction_rotation_only   reconstruction.py:387-412
   compute_image_pairs_from_tracks         this engine's fast path: bearings once per image, rows from the device's
                                           common-track lists
+
+and the triangulation of tracks after each shot the incremental loop adds, from opensfm_b200/triangulation.py:
+
+  triangulate_shot_features               reconstruction.py:1143-1183
+  retriangulate                           reconstruction.py:1186-1226
 """
 from __future__ import annotations
 
@@ -36,6 +41,7 @@ import numpy as np
 from . import bundle as _bundle
 from . import rotation_ransac as _rr
 from . import types as T
+from .triangulation import retriangulate, triangulate_shot_features  # noqa: F401
 
 logger = logging.getLogger(__name__)
 

@@ -8,7 +8,9 @@
 The connected components of the match graph, the reference's track filter and the common tracks of every image
 pair are computed by the CUDA library (opensfm_b200/csrc/tracks.cu) through the C ABI; there is no CPU path.
 The host side only marshals: it concatenates the per-pair match arrays, and builds `Observation` objects lazily
-from the structure-of-arrays result when an accessor asks for them.
+from the structure-of-arrays result when an accessor asks for them.  A TracksManager keeps the tracks handle that
+built it, with the observations on the device, for as long as it lives: `TracksManager.triangulate`
+(opensfm_b200/triangulation.py) runs on them without uploading the tracks again.
 
 One stated difference from the reference: tracks are numbered 0 .. T - 1 by their smallest (image, feature) with
 images in name order, whereas the reference numbers them in the iteration order of its union-find's dictionary.
@@ -35,7 +37,7 @@ class TracksManager:
     def __init__(self, handle: _lib.Handle, images: List[Any], obs_track: np.ndarray, obs_image: np.ndarray,
                  obs_feature: np.ndarray, track_start: np.ndarray, features, colors, segmentations, instances, depths,
                  depth_is_radial: bool, depth_std_deviation: float, device_ms: float):
-        self._handle: Optional[_lib.Handle] = handle   # released once the common tracks are read
+        self._handle: Optional[_lib.Handle] = handle   # holds the observations on the device; released with self
         self.images = images
         self.obs_track, self.obs_image, self.obs_feature, self.track_start = obs_track, obs_image, obs_feature, track_start
         self._features, self._colors, self._segmentations, self._instances = features, colors, segmentations, instances
@@ -49,6 +51,7 @@ class TracksManager:
         self._ids: Optional[np.ndarray] = None
         self.build_device_ms = device_ms
         self.common_device_ms = 0.0
+        self.triangulate_device_ms = 0.0
 
     def __del__(self):
         self._give_back()
@@ -169,8 +172,35 @@ class TracksManager:
             _lib.check(h.L.osfm_tracks_last_device_ms(h.h, None, ctypes.byref(ms)))
             self.common_device_ms = float(ms.value)
             self._common = (pa, pb, ps, ca, cb)
-            self._give_back()
         return self._common
+
+    def triangulate(self, image_rt: np.ndarray, image_origin: np.ndarray, image_in: np.ndarray, bearings: np.ndarray,
+                    selected: np.ndarray, threshold: float, min_ray_angle: float, min_depth: float, iterations: int
+                    ) -> Tuple[np.ndarray, np.ndarray]:
+        """TrackTriangulator.triangulate (opensfm/reconstruction.py:1032-1073) of every selected track at once, on
+        the device, from the observations the tracks handle keeps there: (X[T, 3], status[T]).
+
+        Per image of `images`: image_rt (R^T of the world-to-camera rotation, 3 x 3), image_origin (3) and image_in
+        (whether the image is in the reconstruction; only its observations are used).  Per observation, in the
+        (track, image) order of `obs_track`: bearings (camera frame, 3; read only in images of the reconstruction).
+        Per track: selected.  threshold and min_ray_angle are in radians.  status is one of the STATUS_* codes of
+        opensfm_b200.triangulation; X is NaN unless the status is STATUS_OK."""
+        h = self._handle
+        I, T, N = len(self.images), self.num_tracks(), len(self.obs_track)
+        rt = np.ascontiguousarray(image_rt, dtype=np.float64).reshape(I, 9)
+        origin = np.ascontiguousarray(image_origin, dtype=np.float64).reshape(I, 3)
+        inn = np.ascontiguousarray(image_in, dtype=np.uint8).reshape(I)
+        b = np.ascontiguousarray(bearings, dtype=np.float64).reshape(N, 3)
+        sel = np.ascontiguousarray(selected, dtype=np.uint8).reshape(T)
+        status = np.zeros(T, dtype=np.int8)
+        X = np.zeros((T, 3), dtype=np.float64)
+        _lib.check(h.L.osfm_tracks_triangulate(h.h, I, ptr(rt), ptr(origin), ptr(inn), N, ptr(b), T, ptr(sel),
+                                               float(threshold), float(min_ray_angle), float(min_depth),
+                                               int(iterations), ptr(status), ptr(X)))
+        ms = ctypes.c_float(0)
+        _lib.check(h.L.osfm_tracks_last_triangulate_ms(h.h, ctypes.byref(ms)))
+        self.triangulate_device_ms = float(ms.value)
+        return X, status
 
     def get_all_pairs_connectivity(self, shots: Sequence[Any] = (), tracks: Sequence[str] = ()
                                    ) -> Dict[Tuple[Any, Any], int]:
