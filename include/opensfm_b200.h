@@ -357,6 +357,18 @@ int osfm_ba_eval_observation(int device, int projection_type, const double* came
  * reduced camera system at LM iteration `iteration` (1-based) of the next osfm_ba_run; 0 disarms.  Single-GPU
  * only (world == 1, else OSFM_ERR_ARG).  Unarmed, run() computes exactly what it computes without the hook. */
 int osfm_ba_capture_linear_system(osfm_ba* ba, int iteration);
+/* Fallback paths (test and A/B hook).  Every run() of the handle takes the kernel paths `mask` names instead of the
+ * product path; each is a path some inputs take anyway, so a test can compare it with the default on any scene.
+ * 0 = the product path; sticky until the next call.  Bits outside the enum fail with OSFM_ERR_ARG. */
+enum { OSFM_BA_FALLBACK_PER_POINT_SCHUR = 1,        /* every point through the per-point ba_schur */
+       OSFM_BA_FALLBACK_SIMT_SEGMENT_SCHUR = 2,     /* SIMT segment kernels instead of the tensor-core ones */
+       OSFM_BA_FALLBACK_CTA_PER_SEGMENT_SCHUR = 4,  /* ba_schur_mma (one CTA per segment), not ba_schur_pipe */
+       OSFM_BA_FALLBACK_GENERIC_LINEARIZE = 8,      /* generic ba_linearize even for uniform scenes */
+       OSFM_BA_FALLBACK_CLASSIC_PCG = 16,           /* the classic PCG only, not the pipelined one */
+       OSFM_BA_FALLBACK_STREAMED_PCG = 32,          /* the classic PCG streams S from memory */
+       OSFM_BA_FALLBACK_UNDEFLATED_PCG = 64,        /* the pipelined PCG without gauge deflation */
+       OSFM_BA_FALLBACK_HOST_LOOP = 128 };          /* the host drives the LM loop, no CUDA graph */
+int osfm_ba_set_fallbacks(osfm_ba* ba, unsigned mask);
 enum { OSFM_SCHUR_NONE = 0, OSFM_SCHUR_PIPE = 1, OSFM_SCHUR_MMA = 2, OSFM_SCHUR_SIMT_SEGMENT = 3 };
 enum { OSFM_PCG_PIPELINED_DEFLATED = 1, OSFM_PCG_PIPELINED = 2, OSFM_PCG_CLASSIC_RESIDENT = 3,
        OSFM_PCG_CLASSIC_STREAMED = 4 };

@@ -9,7 +9,7 @@ import contextlib
 import ctypes
 import os
 import threading
-from ctypes import POINTER, c_char_p, c_double, c_float, c_int, c_int32, c_int64, c_uint8, c_void_p
+from ctypes import POINTER, c_char_p, c_double, c_float, c_int, c_int32, c_int64, c_uint, c_uint8, c_void_p
 from typing import Dict, Iterator, List, Optional, Tuple
 
 import numpy as np
@@ -56,6 +56,9 @@ SCHUR_KERNELS = {0: "none", 1: "pipe", 2: "mma", 3: "simt_segment"}
 PCG_KERNELS = {1: "pipelined_deflated", 2: "pipelined", 3: "classic_resident", 4: "classic_streamed"}
 COVARIANCE_STATUS = {0: "ok", 1: "solver_failure", 2: "point_rank_deficient", 3: "camera_rank_deficient",
                      4: "non_finite"}
+# OSFM_BA_FALLBACK_* bits of osfm_ba_set_fallbacks by name: kernel paths a solve can be made to take (tests, A/B runs)
+BA_FALLBACKS = {"per_point_schur": 1, "simt_segment_schur": 2, "cta_per_segment_schur": 4, "generic_linearize": 8,
+                "classic_pcg": 16, "streamed_pcg": 32, "undeflated_pcg": 64, "host_loop": 128}
 
 ALLREDUCE_FN = ctypes.CFUNCTYPE(c_int, c_void_p, c_int64, c_void_p, c_void_p)
 
@@ -134,6 +137,7 @@ SIGNATURES = {
     "osfm_ba_eval_observation": (c_int, [c_int, c_int, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p,
                                          c_double, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, POINTER(c_int)]),
     "osfm_ba_capture_linear_system": (c_int, [c_void_p, c_int]),
+    "osfm_ba_set_fallbacks": (c_int, [c_void_p, c_uint]),
     "osfm_ba_get_captured_system": (c_int, [c_void_p, POINTER(BACapture), c_void_p, c_void_p, c_void_p, c_void_p,
                                             c_void_p, c_void_p]),
     "osfm_ba_get_captured_parameters": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),

@@ -30,7 +30,8 @@ _TERMINATION = {0: "CONVERGENCE", 1: "NO_CONVERGENCE", 2: "FAILURE"}
 def solve(pb: bp.BAProblem, device: int = 0, rank: int = 0, world: int = 1, allreduce=None,
           stream: Optional[int] = None, compute_reprojection_errors: bool = True,
           out: Optional[Dict[str, np.ndarray]] = None, pinned_inputs: bool = False,
-          capture_iteration: Optional[int] = None, compute_covariances: bool = False) -> Dict[str, Any]:
+          capture_iteration: Optional[int] = None, compute_covariances: bool = False,
+          fallbacks: Sequence[str] = ()) -> Dict[str, Any]:
     """Run the GPU bundle adjustment on a BAProblem.  Returns updated parameter arrays,
     unscaled reprojection errors (bundle_adjuster.cc:1196-1208) and the run summary.
 
@@ -50,8 +51,14 @@ def solve(pb: bp.BAProblem, device: int = 0, rank: int = 0, world: int = 1, allr
     in the problem's instance order, zeros for constant instances), "covariance_valid", "covariance_status" (one of
     _lib.COVARIANCE_STATUS) and "covariance_ms", the device times (ms) of the covariance pass and of its Cholesky
     factorisation (osfm_ba_get_covariance_timing).  As in the reference, an invalid estimate leaves every instance with
-    the default diag(1e-5, 1e-5, 1e-5, 1e-2, 1e-2, 1e-2)."""
+    the default diag(1e-5, 1e-5, 1e-5, 1e-2, 1e-2, 1e-2).
+    `fallbacks` (tests, A/B runs): names from _lib.BA_FALLBACKS of kernel paths this solve takes instead of the product
+    path (osfm_ba_set_fallbacks); each is a path some inputs take anyway."""
     pb.validate(check_indices=False)
+    unknown = sorted(set(fallbacks) - set(_lib.BA_FALLBACKS))
+    if unknown:
+        raise ValueError("unknown fallback paths %s; known: %s" % (unknown, sorted(_lib.BA_FALLBACKS)))
+    fallback_mask = sum(_lib.BA_FALLBACKS[f] for f in set(fallbacks))
     with _lib.pooled("ba", device) as hd:
         L, h = hd.L, hd.h
         i32 = lambda a: np.ascontiguousarray(a, dtype=np.int32)
@@ -137,6 +144,8 @@ def solve(pb: bp.BAProblem, device: int = 0, rank: int = 0, world: int = 1, allr
             _lib.check(L.osfm_ba_set_distributed(h, 0, 1, ctypes.cast(None, _lib.ALLREDUCE_FN), None))
         _lib.check(L.osfm_ba_set_stream(h, ctypes.c_void_p(stream) if stream is not None else None))
         _lib.check(L.osfm_ba_set_compute_covariances(h, int(bool(compute_covariances))))
+        # set on every call, 0 included: the handle is reused, and one caller's paths must not reach another's solve
+        _lib.check(L.osfm_ba_set_fallbacks(h, fallback_mask))
         if capture_iteration is not None:
             if int(capture_iteration) < 1:
                 raise ValueError("capture_iteration must be >= 1")

@@ -851,27 +851,17 @@ static std::vector<int> balanced_cut(const std::vector<long long>& w, int G) {
   }
   return lo;
 }
-// whether environment variable `name` is set and starts with `c`
-static bool env_starts_with(const char* name, char c) {
-  const char* e = getenv(name);
-  return e && e[0] == c;
+// OSFM_BA_TRACE=1, read once per process: host wall-clock per phase of run(), in-kernel clocks and all-reduce counts
+// on stderr (diagnostics only)
+static bool tracing() {
+  static const bool on = [] {
+    const char* e = getenv("OSFM_BA_TRACE");
+    return e && e[0] == '1';
+  }();
+  return on;
 }
-// The OSFM_BA_* switches, read once per process.  The fallbacks (=0) keep older kernel paths for A/B runs and tests.
-struct BaSwitches {
-  bool trace = env_starts_with("OSFM_BA_TRACE", '1');   // host wall-clock per phase of run(), in-kernel clocks on stderr
-  bool seg_schur = !env_starts_with("OSFM_BA_SEGMENT_SCHUR", '0');   // else every point through the per-point ba_schur
-  bool lin_special = !env_starts_with("OSFM_BA_LIN_SPECIAL", '0');   // else generic ba_linearize for uniform scenes
-  bool schur_mma = !env_starts_with("OSFM_BA_SCHUR_MMA", '0');   // else ba_obs_rows + ba_schur_seg, no tensor cores
-  bool schur_pipe = !env_starts_with("OSFM_BA_SCHUR_PIPE", '0');   // else ba_schur_mma, not the persistent ba_schur_pipe
-  bool pcg_resident = !env_starts_with("OSFM_BA_PCG_RESIDENT", '0');   // else the classic PCG streams S from memory
-  bool pcg_pipelined = !env_starts_with("OSFM_BA_PCG_PIPELINED", '0');   // else the classic PCG only
-  bool pcg_deflate = !env_starts_with("OSFM_BA_PCG_DEFLATE", '0');   // else the pipelined PCG without gauge deflation
-  bool host_loop = env_starts_with("OSFM_BA_HOST_LOOP", '1');   // the host drives the LM loop even where a graph could
-};
-static const BaSwitches& switches() {
-  static const BaSwitches s;
-  return s;
-}
+// Every OSFM_BA_FALLBACK_* bit (osfm_ba_set_fallbacks; HOST_LOOP is the highest)
+constexpr unsigned BA_FALLBACKS_ALL = 2 * OSFM_BA_FALLBACK_HOST_LOOP - 1;
 
 // How linearize() forms the camera-side column norms and gradient of the segment observations (RunState::lin)
 enum LinPath {
@@ -967,6 +957,8 @@ struct BA {
   bool reproj_valid = false;
   osfm_ba_summary summary{};
   bool has_run = false;
+  // osfm_ba_set_fallbacks: OSFM_BA_FALLBACK_* bits of the kernel paths every run() takes instead of the product path
+  unsigned fallbacks = 0;
   // osfm_ba_capture_linear_system: raw copies of the reduced system at LM iteration cap_iter (0 = unarmed)
   int cap_iter = 0;
   bool cap_valid = false;
@@ -1134,11 +1126,11 @@ struct BA {
     if (world > 1) {
       const auto t0 = std::chrono::high_resolution_clock::now();
       cudaEvent_t e0 = nullptr, e1 = nullptr;
-      if (switches().trace) { cudaEventCreate(&e0); cudaEventCreate(&e1); cudaEventRecord(e0, stream); }
+      if (tracing()) { cudaEventCreate(&e0); cudaEventCreate(&e1); cudaEventRecord(e0, stream); }
       struct Done {
         BA* self; std::chrono::high_resolution_clock::time_point t0; cudaEvent_t e0, e1;
         ~Done() {
-          if (switches().trace) {
+          if (tracing()) {
             cudaEventRecord(e1, self->stream); cudaEventSynchronize(e1);
             float ms = 0.f; cudaEventElapsedTime(&ms, e0, e1); self->ar_dev_ms += ms;
             cudaEventDestroy(e0); cudaEventDestroy(e1);
@@ -1157,7 +1149,7 @@ struct BA {
     }
   }
   void trace(const char* what) {   // OSFM_BA_TRACE=1: host wall-clock per phase of run() on stderr (diagnostics only)
-    if (!switches().trace) return;
+    if (!tracing()) return;
     const auto now = std::chrono::high_resolution_clock::now();
     fprintf(stderr, "[osfm_ba] %-12s %8.3f ms\n", what, std::chrono::duration<double, std::milli>(now - rs.t_prev).count());
     rs.t_prev = now;
@@ -1303,7 +1295,7 @@ void BA::plan_layout() {
   }
   rs.wc = std::max(rs.wc, 1);
   // one projection type for all cameras and no rig-camera shots -> specialised linearisation kernels
-  if (switches().lin_special && K > 0) {
+  if (!(fallbacks & OSFM_BA_FALLBACK_GENERIC_LINEARIZE) && K > 0) {
     int& t = rs.uniform_type;
     t = cam_type[0];
     for (int k = 1; k < K; ++k) if (cam_type[k] != t) t = -1;
@@ -1365,8 +1357,8 @@ void BA::order_observations() {
   ord_pair_bound<<<grid_for(Pfull, 256), 256, 0, stream>>>(d_g_pt_start.p, Pfull, d_oc.p);
   OSFM_LAUNCH_CHECK();
   ord_signatures<<<grid_for(P, 256), 256, 0, stream>>>(okeys, d_g_pt_start.p, d_ptc_full.p, P, world, rank, wc,
-                                                       switches().seg_schur ? 1 : 0, SEG_KMAX, SEG_NA, SEG_WCMAX, d_pkey.p,
-                                                       d_pval.p);
+                                                       (fallbacks & OSFM_BA_FALLBACK_PER_POINT_SCHUR) ? 0 : 1, SEG_KMAX,
+                                                       SEG_NA, SEG_WCMAX, d_pkey.p, d_pval.p);
   OSFM_LAUNCH_CHECK();
   tmpb = d_cub.cap;
   OSFM_CUDA(cub::DeviceRadixSort::SortPairs(d_cub.p, tmpb, d_pkey.p, d_pkey2.p, d_pval.p, d_order.p, P, 0, 64, stream));
@@ -1422,7 +1414,7 @@ void BA::order_observations() {
   OSFM_CUDA(cudaStreamSynchronize(stream));
   rs.nseg = h_oc.p->nseg; rs.P_fast = h_oc.p->p_fast;
   rs.n_fast_obs = h_oc.p->n_fast; rs.pair_bound = (long long)h_oc.p->pair_bound;
-  if (switches().trace)
+  if (tracing())
     fprintf(stderr, "[osfm_ba] points %d (fast path %d in %d segments), observations %lld (fast path %lld), free points %d\n", P,
             rs.P_fast, rs.nseg, N, rs.n_fast_obs, rs.npf);
 }
@@ -1693,9 +1685,10 @@ void BA::plan_pcg() {
       }
       const long long off_S = up16(8LL * nc), off_cols = off_S + up16(8 * ent_max), off_rows = off_cols + up16(2 * col_max);
       const long long total = off_rows + 12LL * rows_max;
-      rs.pcg_resident = switches().pcg_resident && monotone && nc <= 65535 && total + 1024 <= max_smem;
+      rs.pcg_resident = !(fallbacks & OSFM_BA_FALLBACK_STREAMED_PCG) && monotone && nc <= 65535 &&
+                        total + 1024 <= max_smem;
       rs.pcg_smem = rs.pcg_resident ? (int)total : 0;
-      if (switches().trace)
+      if (tracing())
         fprintf(stderr, "[osfm_ba] pcg plan: classic resident %s, %lld B of shared memory per CTA, %d B available\n",
                 rs.pcg_resident ? "on" : "off", total, max_smem - 1024);
       if (rs.pcg_resident) {
@@ -1718,9 +1711,9 @@ void BA::plan_pcg() {
       OSFM_CUDA(cudaFuncGetAttributes(&pipe_attr, pcg_pipelined));
       const PcgPipePlan plan = plan_pcg_pipelined(rs.grp_b1, rs.grp_b2, rs.blk_sz, row_M, shared, G,
                                                   (long long)max_smem - (long long)pipe_attr.sharedSizeBytes - 1024);
-      rs.pcg_pipe_ok = switches().pcg_pipelined && nc <= 65535 && plan.fits;
+      rs.pcg_pipe_ok = !(fallbacks & OSFM_BA_FALLBACK_CLASSIC_PCG) && nc <= 65535 && plan.fits;
       rs.pcg_pipe_smem = rs.pcg_pipe_ok ? (int)plan.total : 0;
-      if (switches().trace)
+      if (tracing())
         fprintf(stderr, "[osfm_ba] pcg plan: pipelined %s, %lld B of shared memory per CTA, %lld B available (%d CTAs, "
                 "worst CTA: %lld entries, %lld columns, %d rows, %d groups)\n", rs.pcg_pipe_ok ? "on" : "off", plan.total,
                 plan.available, G, plan.max.ent, plan.max.cols, plan.max.rows, plan.max.groups);
@@ -1819,8 +1812,8 @@ void BA::build_segment_tables() {
   }
   // the persistent Schur kernel runs over the chunk list; its flush table holds offset << 2 (the reduced system must
   // stay below 2^29 doubles) and takes 20 KB per segment
-  const bool use_mma = switches().schur_mma && wc <= 9;
-  const bool use_pipe = use_mma && switches().schur_pipe && rs.sp_nchunks > 0 &&
+  const bool use_mma = !(fallbacks & OSFM_BA_FALLBACK_SIMT_SEGMENT_SCHUR) && wc <= 9;
+  const bool use_pipe = use_mma && !(fallbacks & OSFM_BA_FALLBACK_CTA_PER_SEGMENT_SCHUR) && rs.sp_nchunks > 0 &&
                         rs.s_upper_total + (long long)rs.nc_pad < (1LL << 29) &&
                         (long long)nseg * SP_FT_SEG * (long long)sizeof(int) <= (8LL << 30);
   if (use_pipe) {
@@ -1959,7 +1952,7 @@ void BA::linearize(int b, bool timed) {
 // path.  `timed`: into the Schur phase timer.
 void BA::build_system(const double* diag, double inv_radius, int* rank_flag, bool timed) {
   const int nc = rs.nc, P = rs.P, P_fast = rs.P_fast, nseg = rs.nseg, wc = rs.wc;
-  const bool trace_on = switches().trace;
+  const bool trace_on = tracing();
   double *const d_rhs_p = rs.d_rhs_p, *const d_S_p = rs.d_S_p;
   if (nc > 0) OSFM_CUDA(cudaMemsetAsync(d_Sbuf.p, 0, sizeof(double) * ((size_t)rs.nc_pad + (size_t)rs.s_upper_total), stream));
   if (P > 0) {
@@ -2077,7 +2070,7 @@ void BA::solve_reduced() {
                        stream, d_Spcg.p, rs.lay, rs.bsr, d_Minv.p, rs.d_rhs_p, d_px.p, d_pr.p, d_pz.p, d_pp.p, d_pAp.p, d_Ap.p,
                        d_pcg.p, nc, max_pcg, 1e-16, rs.pcg_res);
     OSFM_LAUNCH_CHECK();
-    if (switches().trace) {
+    if (tracing()) {
       OSFM_CUDA(cudaMemcpyAsync(h_pcg.p, d_pcg.p, PCG_STATE_HEADER, cudaMemcpyDeviceToHost, stream));
       OSFM_CUDA(cudaStreamSynchronize(stream));
       const PcgState& h = *h_pcg.p;
@@ -2090,7 +2083,7 @@ void BA::solve_reduced() {
     launch_cooperative(pcg_pipelined, rs.pcg_grid, PCG_THREADS, rs.pcg_pipe_smem, stream, d_Spcg.p, rs.lay, rs.bsr, d_Minv.p,
                        rs.d_rhs_p, d_px.p, d_pz.p, d_pp.p, d_pcg.p, nc, max_pcg, 1e-16, rs.pcg_pipe);
     OSFM_LAUNCH_CHECK();
-    if (switches().trace) {
+    if (tracing()) {
       OSFM_CUDA(cudaMemcpyAsync(h_pcg.p, d_pcg.p, PCG_STATE_HEADER, cudaMemcpyDeviceToHost, stream));
       OSFM_CUDA(cudaStreamSynchronize(stream));
       const PcgState& h = *h_pcg.p;
@@ -2267,7 +2260,7 @@ void BA::covariance_pass(int termination) {
     cov_status = hf[COV_F_POINT_RANK] ? OSFM_COV_POINT_RANK_DEFICIENT
                  : hf[COV_F_CHOL]     ? OSFM_COV_CAMERA_RANK_DEFICIENT
                  : hf[COV_F_NONFINITE] ? OSFM_COV_NON_FINITE : OSFM_COV_OK;
-    if (switches().trace && hf[COV_F_CHOL])
+    if (tracing() && hf[COV_F_CHOL])
       fprintf(stderr, "[osfm_ba] covariances: reduced system rank deficient at dense column %d\n", hf[COV_F_CHOL_COL]);
   }
   cov_valid = cov_status == OSFM_COV_OK;
@@ -2309,7 +2302,7 @@ void BA::write_results(osfm_ba_summary sum) {
   }
   OSFM_CUDA(cudaStreamSynchronize(stream));
   trace("results");
-  if (switches().trace && world > 1)
+  if (tracing() && world > 1)
     fprintf(stderr, "[osfm_ba] rank %d: %d all-reduces, host %.3f ms, device (traced, serialised) %.3f ms\n", rank, ar_calls,
             ar_host_ms, ar_dev_ms);
   float dev_ms = 0.f;
@@ -2483,8 +2476,8 @@ void BA::run() {
   const int n = rs.n, nc = rs.nc;
   // The graph is built for the pipelined PCG with the classic one as its conditional fallback; a problem whose
   // pipelined plan does not fit runs the host-driven loop.
-  rs.device_loop = world == 1 && !rs.constrained && cap_iter == 0 && !switches().trace && !switches().host_loop &&
-                   rs.pcg_pipe_ok && stream != cudaStreamLegacy;
+  rs.device_loop = world == 1 && !rs.constrained && cap_iter == 0 && !tracing() &&
+                   !(fallbacks & OSFM_BA_FALLBACK_HOST_LOOP) && rs.pcg_pipe_ok && stream != cudaStreamLegacy;
   if (world > 1) {  // all ranks enter the timed region together (their set-up times differ)
     OSFM_CUDA(cudaMemsetAsync(d_sc.p, 0, sizeof(Scalars), stream));
     allreduce_dev(&d_sc.p->cost, 1);
@@ -2500,7 +2493,7 @@ void BA::run() {
   }
   segment_table_scales();   // the scale is constant from here on
   // deflation vectors of the reduced solve: the similarity gauge at the initial poses, in the scaled variables
-  if (switches().pcg_deflate && rs.pcg_pipe_ok && rs.NI > 0 && nc > 0) {
+  if (!(fallbacks & OSFM_BA_FALLBACK_UNDEFLATED_PCG) && rs.pcg_pipe_ok && rs.NI > 0 && nc > 0) {
     d_Wdef.reserve((size_t)PCG_ND * nc);
     OSFM_CUDA(cudaMemsetAsync(d_Wdef.p, 0, sizeof(double) * PCG_ND * (size_t)nc, stream));
     pcg_gauge_vectors<<<grid_for(rs.NI, 128), 128, 0, stream>>>(rs.NI, d_inst_poff.p, params_of(0).inst, d_scale.p, nc, d_Wdef.p);
@@ -2843,6 +2836,13 @@ int osfm_ba_capture_linear_system(osfm_ba* ba, int iteration) {
     if (iteration < 0) throw ArgError("capture iteration must be >= 0");
     if (iteration > 0 && b.world != 1) throw ArgError("the linear-system capture supports world == 1 only");
     b.cap_iter = iteration;
+  });
+}
+
+int osfm_ba_set_fallbacks(osfm_ba* ba, unsigned mask) {
+  return osfm::with_handle(ba, [&](osfm::BA& b) {
+    if (mask & ~osfm::BA_FALLBACKS_ALL) throw ArgError("unknown OSFM_BA_FALLBACK_* bits");
+    b.fallbacks = mask;
   });
 }
 

@@ -24,7 +24,7 @@
 //     (scattered fp64 RED into L2 are several times slower than a warp's RED to 32 consecutive elements, and a C4
 //     launch issues 87M of them.)
 // Eligible: wc == 9, nres == 2 (a 3-parameter camera and a pose per shot), the camera side of the chunk list;
-// everything else keeps ba_schur_mma.  OSFM_BA_SCHUR_PIPE=0 switches back for A/B runs.
+// everything else keeps ba_schur_mma.  OSFM_BA_FALLBACK_CTA_PER_SEGMENT_SCHUR switches back for A/B runs.
 #pragma once
 
 #include "async_copy.cuh"

@@ -5,12 +5,8 @@ matrix; valid runs |C_e - C_o|_ij <= 10 * 5e-12 * cond2(S_o) * sqrt(C_o,ii C_o,j
 agreement of the reduced systems (5e-12, tests/test_ba_linear_system_gpu.py), S_o the oracle's scaled S.  The
 solve is the same with covariances on and off (iterations, termination; cost and parameters within the run-to-run
 spread of the Schur atomics that two unarmed solves show as well).  The scenes also
-run under every OSFM_BA_* switch (subprocesses: the switches are read once per process)."""
-import ctypes
+run on every fallback path (bundle.solve(fallbacks=...))."""
 import json
-import os
-import subprocess
-import sys
 
 import numpy as np
 import pytest
@@ -23,8 +19,6 @@ from test_covariance_reference import gps_cube_constant_instances, point_seen_on
 
 pytestmark = pytest.mark.gpu
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(HERE)
 S_TAU = 5e-12
 
 
@@ -48,11 +42,11 @@ FULL_RANK = {"camera_and_position_priors", "fixed_instances", "point_priors_many
              "gps_cube_500"}
 
 
-def measure(name):
+def measure(name, fallbacks=()):
     pb = SCENES[name]()
-    on = bundle.solve(pb, compute_covariances=True)
-    off = bundle.solve(pb)
-    off2 = bundle.solve(pb)
+    on = bundle.solve(pb, compute_covariances=True, fallbacks=fallbacks)
+    off = bundle.solve(pb, fallbacks=fallbacks)
+    off2 = bundle.solve(pb, fallbacks=fallbacks)
 
     def apart(a, b):
         return max(float(np.abs(a[k] - b[k]).max()) if np.size(a[k]) else 0.0
@@ -60,7 +54,7 @@ def measure(name):
 
     # the pass runs after the LM loop and writes none of the returned buffers, so on and off differ only by the
     # run-to-run spread of the Schur atomics, which two unarmed solves (off, off2) show as well.  Measured on an H100
-    # over every scene and switch: equal iterations and termination; between two unarmed solves parameters up to
+    # over every scene and variant: equal iterations and termination; between two unarmed solves parameters up to
     # 9.0e-6 apart (gauge-free scenes drift along the gauge) and costs up to 3.8e-9 relative, on vs off the same.
     # The bars are twice that.
     diff, spread = apart(on, off), apart(off, off2)
@@ -106,21 +100,10 @@ def test_covariances_match_oracle(name):
     _check(measure(name))
 
 
-def _variant_main(out):
-    ms = [measure(n) for n in sorted(scenes.SCENES)]
-    with open(out, "w") as f:
-        json.dump(ms, f)
-
-
 @pytest.mark.parametrize("variant", sorted(VARIANTS))
-def test_covariances_under_kernel_variant(variant, tmp_path):
-    out = str(tmp_path / "metrics.json")
-    code = ("import sys; sys.path[:0] = [%r, %r]\nimport test_ba_covariance_gpu as t\nt._variant_main(sys.argv[1])\n"
-            % (HERE, ROOT))
-    subprocess.run([sys.executable, "-c", code, out], check=True, env=dict(os.environ, **VARIANTS[variant]), timeout=1800)
-    with open(out) as f:
-        for m in json.load(f):
-            _check(m)
+def test_covariances_under_kernel_variant(variant):
+    for name in sorted(scenes.SCENES):
+        _check(measure(name, VARIANTS[variant]))
 
 
 def test_bundle_adjuster_end_to_end():

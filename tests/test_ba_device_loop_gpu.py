@@ -1,51 +1,24 @@
 """The LM loop driven by the device (one CUDA graph launch: a WHILE node around the iteration body, step control in
-ba_lm_* kernels) against the same body driven by the host (OSFM_BA_HOST_LOOP=1, which reads the LM state after
-every decision).  Both must take the same steps: same iterations, successful steps, linear solves, PCG iterations,
-termination and message; costs to 1e-9 relative and parameters to 1e-6 (the Schur atomics are unordered, as in
-test_ba_pcg_path_gpu.py).  Each driver runs in a subprocess: the switches are read once per process."""
-import json
-import os
-import pickle
-import subprocess
-import sys
-
+ba_lm_* kernels) against the same body driven by the host (the host_loop fallback path, which reads the LM state
+after every decision).  Both must take the same steps: same iterations, successful steps, linear solves, PCG
+iterations, termination and message; costs to 1e-9 relative and parameters to 1e-6 (the Schur atomics are unordered,
+as in test_ba_pcg_path_gpu.py)."""
 import numpy as np
 import pytest
 
-from opensfm_b200 import synthetic as syn
+from opensfm_b200 import bundle, synthetic as syn
 
 pytestmark = pytest.mark.gpu
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(HERE)
 KEYS = ("iterations", "successful_steps", "linear_solves", "pcg_iterations", "termination", "message", "initial_cost",
         "final_cost", "device_loop", "kernel_launches", "linearize_launches", "schur_launches")
 
-WORKER = r"""
-import json, pickle, sys
-import numpy as np
-sys.path.insert(0, sys.argv[1])
-from opensfm_b200 import bundle
-with open(sys.argv[2], "rb") as f:
-    pb = pickle.load(f)
-r = bundle.solve(pb)
-s = r["summary"]
-np.savez(sys.argv[3], cam_params=r["cam_params"], inst=r["inst"], points=r["points"],
-         summary=np.array(json.dumps({k: s[k] for k in json.loads(sys.argv[4])})))
-"""
 
-
-def _both(pb, tmp_path):
-    prob = str(tmp_path / "pb.pkl")
-    with open(prob, "wb") as f:
-        pickle.dump(pb, f)
+def _both(pb):
     out = {}
-    for name, host in (("device", "0"), ("host", "1")):
-        path = str(tmp_path / (name + ".npz"))
-        env = dict(os.environ, OSFM_BA_HOST_LOOP=host)
-        subprocess.run([sys.executable, "-c", WORKER, ROOT, prob, path, json.dumps(KEYS)], env=env, check=True)
-        d = np.load(path)
-        out[name] = (json.loads(str(d["summary"])), {k: d[k] for k in ("cam_params", "inst", "points")})
+    for name, fallbacks in (("device", ()), ("host", ("host_loop",))):
+        r = bundle.solve(pb, fallbacks=fallbacks)
+        out[name] = ({k: r["summary"][k] for k in KEYS}, {k: r[k] for k in ("cam_params", "inst", "points")})
     (sd, pd), (sh, ph) = out["device"], out["host"]
     print("device: %s\nhost:   %s" % (sd, sh))
     assert sd["device_loop"] == 1 and sh["device_loop"] == 0
@@ -60,35 +33,35 @@ def _both(pb, tmp_path):
     return sd, sh
 
 
-def test_c4_device_loop(tmp_path):
+def test_c4_device_loop_against_host_loop_fallback():
     pb = syn.scene_to_problem(syn.cube_scene(500, 200000, 1.0, seed=42, max_obs_per_point=10))
-    sd, sh = _both(pb, tmp_path)
+    sd, sh = _both(pb)
     # the graph's kernels are counted per execution: the same kernels as the host-driven loop, whose decisions
     # launch no kernels of their own
     assert sd["kernel_launches"] == sh["kernel_launches"]
 
 
-def test_perturbed_ring(tmp_path):
+def test_perturbed_ring_against_host_loop_fallback():
     pb = syn.scene_to_problem(syn.cube_scene(30, 4000, 1.0, seed=5), point_noise=0.05, position_noise=0.1,
                               rotation_noise=0.03)
-    _both(pb, tmp_path)
+    _both(pb)
 
 
-def test_exact_start(tmp_path):
+def test_exact_start_against_host_loop_fallback():
     """Noise-free observations at the true parameters: the loop stops at its first step."""
     pb = syn.scene_to_problem(syn.cube_scene(12, 1500, 0.0, seed=3), perturb_seed=None)
-    sd, _ = _both(pb, tmp_path)
+    sd, _ = _both(pb)
     assert sd["iterations"] <= 1 and sd["termination"] == "CONVERGENCE"
 
 
-def test_one_iteration(tmp_path):
+def test_one_iteration_against_host_loop_fallback():
     pb = syn.scene_to_problem(syn.cube_scene(20, 3000, 1.0, seed=9), max_iterations=1)
-    sd, _ = _both(pb, tmp_path)
+    sd, _ = _both(pb)
     assert sd["iterations"] == 1 and sd["message"] == "Maximum number of iterations reached."
 
 
-def test_constant_blocks(tmp_path):
+def test_constant_blocks_against_host_loop_fallback():
     pb = syn.scene_to_problem(syn.cube_scene(24, 3000, 1.0, seed=11), optimize_cameras=False)
     pb.inst_const[:3] = 1
     pb.point_const[::7] = 1
-    _both(pb, tmp_path)
+    _both(pb)

@@ -284,27 +284,18 @@ def test_kernel_variants_agree():
     resident in shared memory) and the fallback kernels the input can select (per-point ba_schur, SIMT segment kernels,
     CTA-per-segment ba_schur_mma, generic ba_linearize, pipelined PCG without deflation, classic PCG with S resident or
     streamed) must give the same solve."""
-    import os
-    import subprocess
-    import sys
-
-    code = (
-        "import sys; sys.path.insert(0, %r)\n"
-        "import numpy as np\n"
-        "from opensfm_b200 import bundle, synthetic as syn\n"
-        "sc = syn.cube_scene(30, 4000, 1.0, with_descriptors=False, max_obs_per_point=8)\n"
-        "r = bundle.solve(syn.scene_to_problem(sc))\n"
-        "np.save(sys.argv[1], np.concatenate([[r['summary']['final_cost'], r['summary']['iterations']], r['points'].ravel()]))\n"
-    ) % os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+    pb = syn.scene_to_problem(syn.cube_scene(30, 4000, 1.0, with_descriptors=False, max_obs_per_point=8))
+    variants = {"default": (), "per_point_schur": ("per_point_schur",), "simt_segment_schur": ("simt_segment_schur",),
+                "cta_per_segment_schur": ("cta_per_segment_schur",), "generic_linearize": ("generic_linearize",),
+                "undeflated_pcg": ("undeflated_pcg",), "classic_pcg": ("classic_pcg",),
+                "streamed_pcg": ("classic_pcg", "streamed_pcg")}
     out = {}
-    variants = {"default": {}, "generic_schur": {"OSFM_BA_SEGMENT_SCHUR": "0"}, "simt_seg_schur": {"OSFM_BA_SCHUR_MMA": "0"}, "cta_per_segment_schur": {"OSFM_BA_SCHUR_PIPE": "0"}, "generic_linearize": {"OSFM_BA_LIN_SPECIAL": "0"}, "undeflated_pcg": {"OSFM_BA_PCG_DEFLATE": "0"}, "classic_pcg": {"OSFM_BA_PCG_PIPELINED": "0"},
-                "streamed_pcg": {"OSFM_BA_PCG_PIPELINED": "0", "OSFM_BA_PCG_RESIDENT": "0"}}
-    for name, extra in variants.items():
-        path = "/tmp/osfm_variant_%s.npy" % name
-        env = dict(os.environ, **extra)
-        subprocess.run([sys.executable, "-c", code, path], check=True, env=env, timeout=600)
-        out[name] = np.load(path)
-    for name in ("generic_schur", "simt_seg_schur", "cta_per_segment_schur", "generic_linearize", "undeflated_pcg", "classic_pcg", "streamed_pcg"):
+    for name, fallbacks in variants.items():
+        r = bundle.solve(pb, fallbacks=fallbacks)
+        out[name] = np.concatenate([[r["summary"]["final_cost"], r["summary"]["iterations"]], r["points"].ravel()])
+    for name in variants:
+        if name == "default":
+            continue
         assert out["default"][1] == out[name][1]
         assert abs(out["default"][0] - out[name][0]) <= 1e-9 * out["default"][0]
         # the solvers that do not deflate the gauge directions stop with a different (larger) error along those

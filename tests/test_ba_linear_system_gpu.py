@@ -9,8 +9,7 @@ Every scene captures LM iteration 1 (osfm_ba_capture_linear_system) and checks
     within the margin the difference of the two systems allows, and no rescue by the classic PCG;
   * the camera and point step of a max_iterations=1 solve against the oracle's;
   * the kernel path the scene is named for.
-The same scenes run under the OSFM_BA_* switches (in subprocesses: the switches are read once per process), each
-compared against the oracle.
+The same scenes run on every fallback path (bundle.solve(fallbacks=...)), each compared against the oracle.
 
 The segment chunk list, and with it ba_schur_pipe, ba_linearize_fused and ba_colnorm_grad_chunks, exists for camera
 sides 9 wide with 2 residual rows only (whichever Schur kernel runs): wc < 9 needs a camera with fewer than 3
@@ -18,10 +17,6 @@ parameters, i.e. SPHERICAL (wc = 7, 3 residuals), so such problems run ba_schur_
 Scenes with FISHEYE624 or BROWN plus rig cameras (wc > 16) have no segment-eligible point at all and run the per-point
 ba_schur only."""
 import functools
-import json
-import os
-import subprocess
-import sys
 
 import numpy as np
 import pytest
@@ -33,8 +28,6 @@ from opensfm_b200 import bundle
 
 pytestmark = pytest.mark.gpu
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(HERE)
 PCG_BAR = 1.5e-8
 # worst |S_e - S_o|_ij / sqrt(S_o,ii S_o,jj) and |rhs_e - rhs_o|_i / |rhs_o|_inf measured on every scene and every
 # variant (H100, fp64 sums of at most ~100 terms in a different order): TAU is at most 100x that
@@ -57,11 +50,12 @@ def _oracle_system(pb, cap):
 
 
 def measure(name, variant=""):
-    """Capture iteration 1 of scene `name` with max_iterations=1 and compare with the oracle.  Returns the metrics
-    (floats / strings, JSON-safe); the asserts live in the callers so that subprocess variants report all of them."""
+    """Capture iteration 1 of scene `name` with max_iterations=1 on the fallback paths of `variant` (a key of
+    VARIANTS, "" for the default path) and compare with the oracle.  Returns the metrics; the asserts live in the
+    callers."""
     pb = scenes.SCENES[name]()
     pb.max_iterations = 1
-    res = bundle.solve(pb, capture_iteration=1)
+    res = bundle.solve(pb, capture_iteration=1, fallbacks=VARIANTS[variant] if variant else ())
     cap = res["capture"]
     ob, cost, cn, g, S_o, rhs_o = _oracle_system(pb, cap)
     nc, S_e, rhs_e, y = cap["nc"], cap["S"], cap["rhs"], cap["y"]
@@ -247,9 +241,9 @@ def test_iteration_two_uses_the_chunked_linearisation():
     assert np.max(np.abs(cap["rhs"] - rhs_o)) <= TAU * np.max(np.abs(rhs_o))
 
 
-# Every scene runs under every switch.  The path each switch forces follows from the default path of the scene: the
+# Every scene runs on every variant.  The path each variant forces follows from the default path of the scene: the
 # persistent kernel gives way to the CTA-per-segment tensor-core kernel, the tensor-core kernels to the SIMT segment
-# kernels, the segment kernels to the per-point kernel; the PCG switches replace the solver.
+# kernels, the segment kernels to the per-point kernel; the PCG variants replace the solver.
 def _variant_path(variant, name):
     schur = EXPECT[name].get("schur_kernel")
     if variant == "cta_per_segment_schur":
@@ -266,12 +260,12 @@ def _variant_path(variant, name):
 
 
 VARIANTS = {
-    "cta_per_segment_schur": {"OSFM_BA_SCHUR_PIPE": "0"},
-    "simt_segment_schur": {"OSFM_BA_SCHUR_MMA": "0"},
-    "per_point_schur": {"OSFM_BA_SEGMENT_SCHUR": "0"},
-    "undeflated_pcg": {"OSFM_BA_PCG_DEFLATE": "0"},
-    "classic_pcg": {"OSFM_BA_PCG_PIPELINED": "0"},
-    "streamed_pcg": {"OSFM_BA_PCG_PIPELINED": "0", "OSFM_BA_PCG_RESIDENT": "0"},
+    "cta_per_segment_schur": ("cta_per_segment_schur",),
+    "simt_segment_schur": ("simt_segment_schur",),
+    "per_point_schur": ("per_point_schur",),
+    "undeflated_pcg": ("undeflated_pcg",),
+    "classic_pcg": ("classic_pcg",),
+    "streamed_pcg": ("classic_pcg", "streamed_pcg"),
 }
 
 
@@ -282,30 +276,36 @@ def _default_chunks(name):
     return bundle.solve(pb, capture_iteration=1)["capture"]["sp_nchunks"]
 
 
-def _variant_main(out_path, variant):
-    ms = [measure(s, variant) for s in sorted(scenes.SCENES)]
-    with open(out_path, "w") as f:
-        json.dump(ms, f)
-
-
+@pytest.mark.parametrize("name", sorted(scenes.SCENES))
 @pytest.mark.parametrize("variant", sorted(VARIANTS))
-def test_kernel_variant_matches_oracle(variant, tmp_path):
-    out = str(tmp_path / "metrics.json")
-    code = ("import sys; sys.path[:0] = [%r, %r]\nimport test_ba_linear_system_gpu as t\nt._variant_main(sys.argv[1], %r)\n"
-            % (ROOT, HERE, variant))
-    subprocess.run([sys.executable, "-c", code, out], check=True, env=dict(os.environ, **VARIANTS[variant]), timeout=1800)
-    with open(out) as f:
-        ms = json.load(f)
-    for m in ms:
-        _report(m)
-    assert sorted(m["name"] for m in ms) == sorted(scenes.SCENES)
-    for m in ms:
-        for k, v in _variant_path(variant, m["name"]).items():
-            assert m[k] == v, (variant, m["name"], k, m)
-        if variant in ("cta_per_segment_schur", "simt_segment_schur"):
-            # the Schur switches replace the Schur kernel only: the chunk list (so the linearisation) is the default's,
-            # and the 1e-12 checks of check() cover the chunk-list column norms under the switch
-            want = _default_chunks(m["name"])
-            assert (want > 0) == (m["wc"] == 9 and m["nres"] == 2 and m["nseg"] > 0), (m["name"], want, m)
-            assert m["sp_nchunks"] == want, (variant, m["name"], want, m)
-        check(m)
+def test_kernel_variant_matches_oracle(variant, name):
+    m = measure(name, variant)
+    _report(m)
+    for k, v in _variant_path(variant, name).items():
+        assert m[k] == v, (variant, name, k, m)
+    if variant in ("cta_per_segment_schur", "simt_segment_schur"):
+        # the Schur variants replace the Schur kernel only: the chunk list (so the linearisation) is the default's,
+        # and the 1e-12 checks of check() cover the chunk-list column norms on the variant
+        want = _default_chunks(name)
+        assert (want > 0) == (m["wc"] == 9 and m["nres"] == 2 and m["nseg"] > 0), (name, want, m)
+        assert m["sp_nchunks"] == want, (variant, name, want, m)
+    check(m)
+
+
+def test_pooled_handle_returns_to_the_product_path():
+    """A fallback solve leaves nothing behind on the pooled handle: the next solve without fallbacks, on the same
+    handle, takes the persistent Schur kernel, the deflated pipelined PCG and the device-driven LM loop."""
+    from opensfm_b200 import _lib
+
+    pb = scenes.SCENES["pipe_few_chunks"]()
+    pb.max_iterations = 1
+    with _lib.pooled("ba") as first:
+        pass
+    forced = bundle.solve(pb, capture_iteration=1, fallbacks=("classic_pcg", "host_loop", "per_point_schur"))
+    assert forced["capture"]["schur_kernel"] == "none" and forced["capture"]["pcg_kernel"] == "classic_resident"
+    assert forced["summary"]["device_loop"] == 0
+    cap = bundle.solve(pb, capture_iteration=1)["capture"]
+    assert cap["schur_kernel"] == "pipe" and cap["pcg_kernel"] == "pipelined_deflated", cap
+    assert bundle.solve(pb)["summary"]["device_loop"] == 1
+    with _lib.pooled("ba") as last:
+        assert last is first   # every solve above ran on this one handle

@@ -1,44 +1,16 @@
 """The linearisation that also forms the column norms, the gradient and the per-point sums (ba_linearize_fused, used
-for perspective scenes with the segment chunk list) against the separate plane-reading kernels (OSFM_BA_LIN_SPECIAL=0,
-in a subprocess: the switches are read once per process).  Only summation orders differ: the captured Jacobi scale,
-LM diagonal and gradient agree to 1e-12 at LM iteration 1 (iteration 2: see below), and a full bundle() takes the same
-iterations to the same termination, final cost and parameters."""
-import json
-import os
-import pickle
-import subprocess
-import sys
-
+for perspective scenes with the segment chunk list) against the separate plane-reading kernels (the generic_linearize
+fallback path).  Only summation orders differ: the captured Jacobi scale, LM diagonal and gradient agree to 1e-12 at
+LM iteration 1 (iteration 2: see below), and a full bundle() takes the same iterations to the same termination, final
+cost and parameters."""
 import numpy as np
 import pytest
 
 import ba_linear_system_scenes as scenes
 from opensfm_b200 import ba_problem as bp
+from opensfm_b200 import bundle
 
 pytestmark = pytest.mark.gpu
-
-HERE = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(HERE)
-
-WORKER = r"""
-import json, pickle, sys
-import numpy as np
-sys.path.insert(0, sys.argv[1])
-from opensfm_b200 import bundle
-with open(sys.argv[2], "rb") as f:
-    pb = pickle.load(f)
-out = {}
-for it in (1, 2):
-    pb.max_iterations = it
-    cap = bundle.solve(pb, capture_iteration=it)["capture"]
-    for k in ("scale", "diag", "grad"):
-        out["%s%d" % (k, it)] = cap[k]
-pb.max_iterations = max_its = int(sys.argv[4])
-r = bundle.solve(pb)
-s = r["summary"]
-np.savez(sys.argv[3], cam_params=r["cam_params"], inst=r["inst"], points=r["points"],
-         summary=np.array(json.dumps({k: s[k] for k in ("iterations", "termination", "final_cost")})), **out)
-"""
 
 
 def _c4():
@@ -69,23 +41,25 @@ SCENES = {
 }
 
 
-def _run(pb, tmp_path, name, special, max_its):
-    prob = str(tmp_path / ("%s.pkl" % name))
-    with open(prob, "wb") as f:
-        pickle.dump(pb, f)
-    path = str(tmp_path / ("%s_%s.npz" % (name, special)))
-    env = dict(os.environ, OSFM_BA_LIN_SPECIAL=special)
-    subprocess.run([sys.executable, "-c", WORKER, ROOT, prob, path, str(max_its)], env=env, check=True)
-    d = np.load(path)
-    return json.loads(str(d["summary"])), d
+def _run(pb, fallbacks, max_its):
+    out = {}
+    for it in (1, 2):
+        pb.max_iterations = it
+        cap = bundle.solve(pb, capture_iteration=it, fallbacks=fallbacks)["capture"]
+        for k in ("scale", "diag", "grad"):
+            out["%s%d" % (k, it)] = cap[k]
+    pb.max_iterations = max_its
+    r = bundle.solve(pb, fallbacks=fallbacks)
+    out.update({k: r[k] for k in ("cam_params", "inst", "points")})
+    return {k: r["summary"][k] for k in ("iterations", "termination", "final_cost")}, out
 
 
 @pytest.mark.parametrize("name", sorted(SCENES))
-def test_fused_linearisation_matches_plane_kernels(name, tmp_path):
+def test_fused_linearisation_matches_plane_kernels(name):
     make, max_its = SCENES[name]
     pb = make()
-    sf, df = _run(pb, tmp_path, name, "1", max_its)
-    sg, dg = _run(pb, tmp_path, name, "0", max_its)
+    sf, df = _run(pb, (), max_its)
+    sg, dg = _run(pb, ("generic_linearize",), max_its)
     # Iteration 1 linearises at the input parameters: only summation orders differ.  The Jacobi scale is fixed by that
     # linearisation.  Iteration 2 linearises after one step, whose parameters already differ by the rounding of the
     # Schur atomics and the PCG (two runs of the same build differ there too), so its diagonal and gradient get 1e-8.

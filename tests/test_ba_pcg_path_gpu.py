@@ -1,13 +1,7 @@
 """The flagship C4 scene (bench.py: 500 cameras, 200k points, 2M observations) on the PCG the solver is built around:
 the gauge-deflated pipelined kernel, whose shared-memory plan (ba_pcg_plan.h) has to fit one CTA per SM.  Checks the
-path and the solve of the captured system, then a full bundle() against the classic PCG (OSFM_BA_PCG_PIPELINED=0, in a
-subprocess: the switches are read once per process)."""
-import json
-import os
-import pickle
-import subprocess
-import sys
-
+path and the solve of the captured system, then a full bundle() against the classic PCG (the classic_pcg fallback
+path)."""
 import numpy as np
 import pytest
 
@@ -15,8 +9,6 @@ from opensfm_b200 import bundle, synthetic as syn
 
 pytestmark = pytest.mark.gpu
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(HERE)
 PCG_BAR = 1.5e-8
 
 
@@ -47,32 +39,12 @@ def test_c4_shared_intrinsics_pcg_path(c4_scene):
     assert res <= PCG_BAR
 
 
-WORKER = r"""
-import json, pickle, sys
-import numpy as np
-sys.path.insert(0, sys.argv[1])
-from opensfm_b200 import bundle
-with open(sys.argv[2], "rb") as f:
-    pb = pickle.load(f)
-r = bundle.solve(pb)
-s = r["summary"]
-np.savez(sys.argv[3], cam_params=r["cam_params"], inst=r["inst"], points=r["points"],
-         summary=np.array(json.dumps({k: s[k] for k in ("iterations", "termination", "final_cost", "pcg_iterations")})))
-"""
-
-
-def test_c4_bundle_matches_classic_pcg(c4_scene, tmp_path):
+def test_c4_bundle_matches_classic_pcg_fallback(c4_scene):
     pb = syn.scene_to_problem(c4_scene)
-    prob = str(tmp_path / "c4.pkl")
-    with open(prob, "wb") as f:
-        pickle.dump(pb, f)
     out = {}
-    for name, pipelined in (("pipelined", "1"), ("classic", "0")):
-        path = str(tmp_path / (name + ".npz"))
-        env = dict(os.environ, OSFM_BA_PCG_PIPELINED=pipelined)
-        subprocess.run([sys.executable, "-c", WORKER, ROOT, prob, path], env=env, check=True)
-        d = np.load(path)
-        out[name] = (json.loads(str(d["summary"])), d)
+    for name, fallbacks in (("pipelined", ()), ("classic", ("classic_pcg",))):
+        r = bundle.solve(pb, fallbacks=fallbacks)
+        out[name] = ({k: r["summary"][k] for k in ("iterations", "termination", "final_cost", "pcg_iterations")}, r)
     (sp, dp), (sc, dc) = out["pipelined"], out["classic"]
     print("pipelined: %s | classic: %s" % (sp, sc))
     assert sp["iterations"] == sc["iterations"] and sp["termination"] == sc["termination"]

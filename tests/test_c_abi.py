@@ -30,6 +30,14 @@ def test_every_declared_symbol_is_exported_and_bound():
     assert decl == set(_lib.SIGNATURES), decl ^ set(_lib.SIGNATURES)
 
 
+def test_ba_fallback_names_match_the_header_enum():
+    txt = open(os.path.join(ROOT, "include", "opensfm_b200.h")).read()
+    txt = re.sub(r"/\*.*?\*/", "", txt, flags=re.S)
+    bits = {k.lower(): int(v) for k, v in re.findall(r"\bOSFM_BA_FALLBACK_([A-Z_]+)\s*=\s*(\d+)", txt)}
+    assert len(bits) == 8
+    assert bits == _lib.BA_FALLBACKS
+
+
 def test_version_and_param_counts_without_gpu():
     L = _lib.load()
     assert L.osfm_version() >= 100

@@ -145,6 +145,15 @@ def test_a_dropped_handle_is_destroyed_once(fake):
     assert fake.destroyed == [value]   # the released handle stays alive in the pool
 
 
+def test_unknown_fallback_path_raises_before_a_handle_is_taken(fake):
+    from opensfm_b200 import bundle, synthetic as syn
+
+    pb = syn.scene_to_problem(syn.cube_scene(4, 50, 1.0))
+    with pytest.raises(ValueError, match="no_such_path"):
+        bundle.solve(pb, fallbacks=("classic_pcg", "no_such_path"))
+    assert fake.created == []
+
+
 def test_ptr_passes_none_through():
     assert _lib.ptr(None) is None
     import numpy as np
