@@ -391,6 +391,10 @@ typedef struct {
  * output may be NULL.  Fails when nothing was captured or nc > 8192. */
 int osfm_ba_get_captured_system(osfm_ba* ba, osfm_ba_capture* info, double* S, double* rhs, double* y, double* scale,
                                 double* diag, double* grad);
+/* The side terms' rows of the captured linearisation, robustified (sqrt(rho') r and sqrt(rho') J), terms in the order
+ * osfm_ba_set_side_terms got them: r holds each term's nres residuals, J each term's nres x np block row-major (np =
+ * the sizes of its blocks in the order it lists them; the columns of constant blocks are 0).  Either may be NULL. */
+int osfm_ba_get_captured_side_rows(osfm_ba* ba, double* r, double* J);
 /* The parameters at which the captured system was linearised, laid out like osfm_ba_get_cameras /
  * _rig_instances / _rig_cameras / _points / _ext_blocks.  Any output may be NULL. */
 int osfm_ba_get_captured_parameters(osfm_ba* ba, double* cam_params, double* inst_pose6, double* rig_camera_pose6,

@@ -141,6 +141,7 @@ SIGNATURES = {
     "osfm_ba_get_captured_system": (c_int, [c_void_p, POINTER(BACapture), c_void_p, c_void_p, c_void_p, c_void_p,
                                             c_void_p, c_void_p]),
     "osfm_ba_get_captured_parameters": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "osfm_ba_get_captured_side_rows": (c_int, [c_void_p, c_void_p, c_void_p]),
     "osfm_ba_set_compute_covariances": (c_int, [c_void_p, c_int]),
     "osfm_ba_get_covariances": (c_int, [c_void_p, POINTER(c_int), POINTER(c_int), c_void_p]),
     "osfm_ba_get_covariance_timing": (c_int, [c_void_p, POINTER(c_double), POINTER(c_double)]),

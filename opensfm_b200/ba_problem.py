@@ -266,6 +266,18 @@ class BAProblem:
             cofs += len(c)
         return recs, (np.concatenate(consts) if consts else np.zeros(0))
 
+    def block_size(self, kind: int, idx: int) -> int:
+        if kind == SB_CAM:
+            return camera_num_params(self.cam_type[idx])
+        return int(self.ext_size[idx]) if kind == SB_EXT else 6
+
+    def side_row_sizes(self) -> Tuple[np.ndarray, np.ndarray]:
+        """Per side term: its residual count and the size nres x np of its Jacobian block (np = the sizes of the blocks
+        it lists, in that order), the layout of the captured side rows."""
+        nres = np.array([t.nres for t in self.side_terms], dtype=np.int64)
+        npar = np.array([sum(self.block_size(k, i) for k, i in t.blocks) for t in self.side_terms], dtype=np.int64)
+        return nres, nres * npar
+
     @property
     def cam_off(self) -> np.ndarray:
         sizes = np.array([camera_num_params(t) for t in self.cam_type], dtype=np.int32)

@@ -46,7 +46,9 @@ def solve(pb: bp.BAProblem, device: int = 0, rank: int = 0, world: int = 1, allr
     ordering (osfm_ba_set_observations_async; the arrays are kept alive here until the solve returns).
     `capture_iteration` (single GPU, tests): result["capture"] holds the damped reduced system of that LM iteration
     (1-based) as the PCG received it, the PCG solution, the Jacobi scale, the LM diagonal, the gradient and the
-    kernel paths that ran (osfm_ba_get_captured_system); raises if the solve ended before that iteration.
+    kernel paths that ran (osfm_ba_get_captured_system), and the side terms' robustified rows "side_r" / "side_J", flat
+    in the layout of BAProblem.side_row_sizes (osfm_ba_get_captured_side_rows); raises if the solve ended before that
+    iteration.
     `compute_covariances` (single GPU): the result gains "covariances" (NI x 6 x 6, the rig-instance pose covariances
     in the problem's instance order, zeros for constant instances), "covariance_valid", "covariance_status" (one of
     _lib.COVARIANCE_STATUS) and "covariance_ms", the device times (ms) of the covariance pass and of its Cholesky
@@ -155,7 +157,12 @@ def solve(pb: bp.BAProblem, device: int = 0, rank: int = 0, world: int = 1, allr
         finally:
             if capture_iteration is not None:   # the handle is reused: later solves run unarmed
                 _lib.check(L.osfm_ba_capture_linear_system(h, 0))
-        capture = _get_capture(L, h, len(keep[1]), NI, NR, P, len(k9[1])) if capture_iteration is not None else None
+        capture = None
+        if capture_iteration is not None:
+            capture = _get_capture(L, h, len(keep[1]), NI, NR, P, len(k9[1]))
+            nrow, nJ = pb.side_row_sizes()
+            capture["side_r"], capture["side_J"] = np.zeros(int(nrow.sum())), np.zeros(int(nJ.sum()))
+            _lib.check(L.osfm_ba_get_captured_side_rows(h, ptr(capture["side_r"]), ptr(capture["side_J"])))
         cam = np.zeros_like(keep[1])
         inst = np.zeros((NI, 6))
         rc = np.zeros((NR, 6))

@@ -965,6 +965,7 @@ struct BA {
   osfm_ba_capture cap_info{};
   std::vector<double> cap_sbuf, cap_y, cap_scale, cap_diag, cap_grad;   // cap_sbuf = [rhs (nc_pad) | block values]
   std::vector<double> cap_cam, cap_inst, cap_rc, cap_pts, cap_ext;      // the linearisation point (points engine order)
+  std::vector<double> cap_side_r, cap_side_J;                           // side_linearize's rows (rofs / jofs layout)
   std::vector<int4> cap_upper;
   std::vector<int> cap_blk_off, cap_blk_sz, cap_pt_poff, cap_global_of;
   int cap_nc_pad = 0;
@@ -2140,6 +2141,8 @@ void BA::capture_linear_system(int it, double radius) {
   download(cap_cam, xp.cam, cam_params.size(), stream); download(cap_inst, xp.inst, inst.size(), stream);
   download(cap_rc, xp.rc, rc.size(), stream); download(cap_pts, xp.pts, 3 * (size_t)P, stream);
   download(cap_ext, xp.ext, ext_values.size(), stream);
+  download(cap_side_r, d_side_r.p, rs.side_rofs[rs.NT], stream);
+  download(cap_side_J, d_side_J.p, rs.side_jofs[rs.NT], stream);
   OSFM_CUDA(cudaStreamSynchronize(stream));
   cap_blk_off = rs.blk_off; cap_blk_sz = rs.blk_sz; cap_nc_pad = rs.nc_pad;
   cap_info = osfm_ba_capture{};
@@ -2886,6 +2889,14 @@ int osfm_ba_get_captured_system(osfm_ba* ba, osfm_ba_capture* info, double* S, d
     scatter(b.cap_scale, scale);
     scatter(b.cap_diag, diag);
     scatter(b.cap_grad, grad);
+  });
+}
+
+int osfm_ba_get_captured_side_rows(osfm_ba* ba, double* r, double* J) {
+  return osfm::with_handle(ba, [&](osfm::BA& b) {
+    if (!b.cap_valid) throw std::runtime_error("no linear system was captured (not armed, or the run ended earlier)");
+    if (r) std::copy(b.cap_side_r.begin(), b.cap_side_r.end(), r);
+    if (J) std::copy(b.cap_side_J.begin(), b.cap_side_J.end(), J);
   });
 }
 

@@ -470,6 +470,21 @@ __device__ __forceinline__ int side_block_of(const SideCols& sc, int nblocks, in
   return k;
 }
 
+// A block a term lists twice (two shots of one rig instance) is one set of columns of J: the sum of its local copies.
+// Only the first copy stands for it in the column norms, the gradient and S, so that a column whose copies cancel is 0.
+__device__ __forceinline__ bool side_first_copy(const SideCols& sc, int kb) {
+  for (int k = 0; k < kb; ++k)
+    if (sc.b[k].col == sc.b[kb].col) return false;
+  return true;
+}
+// entry j (in the first copy of block kb) of one row of J, summed over the copies of that block
+__device__ __forceinline__ double side_column(const SideCols& sc, int nblocks, const double* row, int kb, int j) {
+  double a = row[j];
+  for (int k = kb + 1; k < nblocks; ++k)
+    if (sc.b[k].col == sc.b[kb].col) a += row[sc.start[k] + (j - sc.start[kb])];
+  return a;
+}
+
 // One CTA per term.  Thread j < nparams: column j of the Jacobian (dual seed on parameter j); thread 0 also
 // writes the robustified residual and adds the cost.  with_cost = 0 on ranks that do not own the side terms.
 __global__ void __launch_bounds__(SIDE_THREADS)
@@ -542,12 +557,16 @@ __global__ void __launch_bounds__(SIDE_THREADS)
   const int j = threadIdx.x;
   if (j >= NP) return;
   const int kb = side_block_of(sc, t.nblocks, j);
-  if (sc.b[kb].col < 0) return;
+  if (sc.b[kb].col < 0 || !side_first_copy(sc, kb)) return;
   const int col = sc.b[kb].col + (j - sc.start[kb]);
   const double* J = sv.J + sv.jofs[blockIdx.x];
   const double* r = sv.r + sv.rofs[blockIdx.x];
   double n2 = 0.0, g = 0.0;
-  for (int q = 0; q < t.nres; ++q) { const double a = J[q * NP + j]; n2 += a * a; g += a * r[q]; }
+  for (int q = 0; q < t.nres; ++q) {
+    const double a = side_column(sc, t.nblocks, J + q * NP, kb, j);
+    n2 += a * a;
+    g += a * r[q];
+  }
   atomicAdd(&colnorm2[col], n2);
   atomicAdd(&grad[col], g);
 }
@@ -566,17 +585,18 @@ __global__ void __launch_bounds__(SIDE_THREADS)
     const int k1 = side_block_of(sc, t.nblocks, j1), k2 = side_block_of(sc, t.nblocks, j2);
     const SideBlock& b1 = sc.b[k1];
     const SideBlock& b2 = sc.b[k2];
-    if (b1.col < 0 || b2.col < 0) continue;
+    if (b1.col < 0 || b2.col < 0 || !side_first_copy(sc, k1) || !side_first_copy(sc, k2)) continue;
     const int r1 = j1 - sc.start[k1], r2 = j2 - sc.start[k2];
     if (b1.blk > b2.blk || (b1.blk == b2.blk && r2 < r1)) continue;
     double val = 0.0;
-    for (int q = 0; q < t.nres; ++q) val += J[q * NP + j1] * J[q * NP + j2];
+    for (int q = 0; q < t.nres; ++q)
+      val += side_column(sc, t.nblocks, J + q * NP, k1, j1) * side_column(sc, t.nblocks, J + q * NP, k2, j2);
     val *= scale[b1.col + r1] * scale[b2.col + r2];
     const int off = bsr_lookup(h, b1.blk, b2.blk);
     atomicAdd(&Sval[off + r1 * b2.np + r2], val);
     if (j1 == j2) {
       double g = 0.0;
-      for (int q = 0; q < t.nres; ++q) g += J[q * NP + j1] * r[q];
+      for (int q = 0; q < t.nres; ++q) g += side_column(sc, t.nblocks, J + q * NP, k1, j1) * r[q];
       atomicAdd(&rhs[b1.col + r1], g * scale[b1.col + r1]);
     }
   }

@@ -52,7 +52,7 @@ _c_dbl_p = ctypes.POINTER(ctypes.c_double)
 
 def build(force: bool = False) -> str:
     """Compile oracle/_build/libba_oracle.so (g++, a few seconds)."""
-    src = [os.path.join(_HERE, f) for f in ("ba_oracle.cpp", "ba_functors.hpp", "Makefile")]
+    src = [os.path.join(_HERE, f) for f in ("ba_oracle.cpp", "ba_functors.hpp", "ba_side_terms.hpp", "Makefile")]
     if force or not os.path.exists(_LIB_PATH) or any(
         os.path.getmtime(s) > os.path.getmtime(_LIB_PATH) for s in src
     ):
@@ -74,6 +74,7 @@ def lib() -> ctypes.CDLL:
         L.oba_linearize.restype = ctypes.c_double
         L.oba_x_norm.restype = ctypes.c_double
         L.oba_model_cost_change.restype = ctypes.c_double
+        L.oracle_side_rows.restype = ctypes.c_double
         L.oracle_reproj_analytic.restype = ctypes.c_int
         L.oracle_reproj_autodiff.restype = ctypes.c_int
         L.oracle_camera_num_params.restype = ctypes.c_int
@@ -242,6 +243,14 @@ class OracleBA:
         g = np.zeros(self.n)
         lib().oba_colnorm_gradient(self.h, _d(cn), _d(g))
         return cn, g
+
+    def side_rows(self, pb: Any):
+        """(cost, r, J) of the side terms at the current parameters: robustified rows packed per term like
+        BAProblem.side_row_sizes (oracle_side_rows)."""
+        nrow, nJ = pb.side_row_sizes()
+        r, J = np.zeros(int(nrow.sum())), np.zeros(int(nJ.sum()))
+        cost = lib().oracle_side_rows(self.h, _d(r), _d(J))
+        return cost, r, J
 
     def set_scale(self, s):
         lib().oba_set_scale(self.h, _d(np.ascontiguousarray(s)))

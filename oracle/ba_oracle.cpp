@@ -194,6 +194,23 @@ inline double eval_side_terms(Problem* pb, bool with_rows) {
   return cost;
 }
 
+// The columns of a term's distinct blocks: a block the term lists twice (two shots of one rig instance) is one set of
+// columns, the sum of its local copies.  cols[a] = reduced column, Jd[a * nres + k] = entry of row k.
+inline void distinct_columns(const Problem::DenseRows& rows, std::vector<int>& cols, std::vector<double>& Jd) {
+  cols.clear();
+  Jd.clear();
+  for (int j = 0; j < rows.ncols; ++j) {
+    if (rows.cols[j] < 0 || std::find(rows.cols, rows.cols + j, rows.cols[j]) != rows.cols + j) continue;
+    cols.push_back(rows.cols[j]);
+    for (int k = 0; k < rows.nres; ++k) {
+      double v = 0.0;
+      for (int j2 = j; j2 < rows.ncols; ++j2)
+        if (rows.cols[j2] == rows.cols[j]) v += rows.J[k * MAXD + j2];
+      Jd.push_back(v);
+    }
+  }
+}
+
 // Columns of the camera-side Jacobian of one observation:
 // local layout [camera C | instance 6 | rig camera 6].
 struct ObsCols {
@@ -603,15 +620,32 @@ void oba_colnorm_gradient(void* h, double* colnorm2, double* grad) {
     colnorm2[row.col] += row.d * row.d;
     grad[row.col] += row.d * row.r;
   }
-  for (const auto& rows : pb->side_rows)
-    for (int j = 0; j < rows.ncols; ++j) {
-      if (rows.cols[j] < 0) continue;
+  std::vector<int> cols;
+  std::vector<double> Jd;
+  for (const auto& rows : pb->side_rows) {
+    distinct_columns(rows, cols, Jd);
+    for (size_t a = 0; a < cols.size(); ++a)
       for (int k = 0; k < rows.nres; ++k) {
-        const double v = rows.J[k * MAXD + j];
-        colnorm2[rows.cols[j]] += v * v;
-        grad[rows.cols[j]] += v * rows.r[k];
+        const double v = Jd[a * rows.nres + k];
+        colnorm2[cols[a]] += v * v;
+        grad[cols[a]] += v * rows.r[k];
       }
+  }
+}
+
+// The side terms' robustified rows at the current parameters, packed like osfm_ba_get_captured_side_rows: per term its
+// nres residuals into r and its nres x np Jacobian block (row-major, local columns, 0 on constant blocks) into J.
+// Returns their cost.
+double oracle_side_rows(void* h, double* r, double* J) {
+  Problem* pb = static_cast<Problem*>(h);
+  const double cost = eval_side_terms(pb, true);
+  for (const auto& rows : pb->side_rows) {
+    for (int k = 0; k < rows.nres; ++k) {
+      *r++ = rows.r[k];
+      for (int j = 0; j < rows.ncols; ++j) *J++ = rows.cols[j] >= 0 ? rows.J[k * MAXD + j] : 0.0;
     }
+  }
+  return cost;
 }
 
 // Reduced camera system for the *scaled* Jacobian Js = J diag(scale) and LM
@@ -756,19 +790,22 @@ void oba_schur(void* h, const double* diag2, double* Sout, double* rhs) {
     Sout[(size_t)row.col * nc + row.col] += d * d;
     rhs[row.col] += d * row.r;
   }
-  for (const auto& rows : pb->side_rows)
-    for (int j1 = 0; j1 < rows.ncols; ++j1) {
-      const int c1 = rows.cols[j1];
-      if (c1 < 0) continue;
-      for (int k = 0; k < rows.nres; ++k) rhs[c1] += rows.J[k * MAXD + j1] * sc[c1] * rows.r[k];
-      for (int j2 = 0; j2 < rows.ncols; ++j2) {
-        const int c2 = rows.cols[j2];
-        if (c2 < 0) continue;
+  std::vector<int> cols;
+  std::vector<double> Jd;
+  for (const auto& rows : pb->side_rows) {
+    distinct_columns(rows, cols, Jd);
+    const int nd = (int)cols.size();
+    for (int a = 0; a < nd; ++a) {
+      const int c1 = cols[a];
+      for (int k = 0; k < rows.nres; ++k) rhs[c1] += Jd[a * rows.nres + k] * sc[c1] * rows.r[k];
+      for (int b = 0; b < nd; ++b) {
+        const int c2 = cols[b];
         double v = 0.0;
-        for (int k = 0; k < rows.nres; ++k) v += rows.J[k * MAXD + j1] * rows.J[k * MAXD + j2];
+        for (int k = 0; k < rows.nres; ++k) v += Jd[a * rows.nres + k] * Jd[b * rows.nres + k];
         Sout[(size_t)c1 * nc + c2] += v * sc[c1] * sc[c2];
       }
     }
+  }
   for (int i = 0; i < nc; ++i) Sout[(size_t)i * nc + i] += diag2[i];
 }
 
