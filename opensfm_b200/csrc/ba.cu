@@ -677,15 +677,16 @@ __global__ void ba_model_change_alg(int n, int nc, int cam_side, const double* _
 // levenberg_marquardt_strategy: the same tests in the same order.  `cond`: when `set_cond`, the conditional node
 // handle of the device-driven loop's graph that the kernel's decision drives.
 // ---------------------------------------------------------------------------
-// after the first linearisation and the |x| pass (Scalars: cost, max |g|, |x|^2)
-__global__ void ba_lm_init(LmState* st, const Scalars* sc, int n) {
+// after the first linearisation and the |x| pass (Scalars: cost, max |g|, |x|^2); `has_free`: the problem (all ranks)
+// has free parameters
+__global__ void ba_lm_init(LmState* st, const Scalars* sc, int has_free) {
   st->radius = LM_RADIUS0;
   st->decrease_factor = 2.0;
   st->cost = st->initial_cost = sc->cost;
-  st->x_norm = n > 0 ? sqrt(sc->x_norm2) : 0.0;
+  st->x_norm = has_free ? sqrt(sc->x_norm2) : 0.0;
   st->termination = 1;
   st->message = LM_MSG_MAX_ITERATIONS;
-  if (n == 0) { st->termination = 0; st->message = LM_MSG_NO_FREE; }
+  if (!has_free) { st->termination = 0; st->message = LM_MSG_NO_FREE; }
   else if (sc->grad_max_bits <= LM_GTOL) { st->termination = 0; st->message = LM_MSG_GTOL; }
 }
 // head of the loop: whether another iteration runs (the WHILE condition)
@@ -880,6 +881,9 @@ struct RunState {
   long long Nfull = 0, N = 0, n_fast_obs = 0, pair_bound = 0;   // observations: all, this rank's, in segments
   int nc = 0, nc_pad = 0, n = 0, nblk = 0, npf = 0, ngroups = 0, wc = 0, nres = 2, nseg = 0, P_fast = 0;
   size_t nz = 1;                  // max(n, 1)
+  // free parameters of the whole problem (every rank's points): rank-independent, so the decisions that pair the
+  // ranks' all-reduces depend on it, not on n (a rank's shard may hold no free point while other ranks' do)
+  long long n_all = 0;
   int n_upper = 0, n_blocks_all = 0, pcg_grid = 1;
   long long s_upper_total = 0, s_total = 0, vb = 0;   // stored doubles: upper blocks, all blocks, ELL rows
   int uniform_type = -1;          // the projection type of every camera when no shot uses a rig camera, else -1
@@ -1380,6 +1384,8 @@ void BA::order_observations() {
   const long long N = rs.N = h_oc.p->n_local;
   rs.npf = h_oc.p->npf;
   rs.n = rs.nc + 3 * rs.npf;
+  rs.n_all = rs.nc;
+  for (int c : pt_const) rs.n_all += c ? 0 : 3;
   rs.nz = (size_t)std::max(rs.n, 1);
   {
     const size_t Nz0 = (size_t)std::max<long long>(N, 1);
@@ -1969,7 +1975,9 @@ void BA::build_system(const double* diag, double inv_radius, int* rank_flag, boo
                                                                                d_Vinv.p, d_gp.p, d_Vig.p, rank_flag);
       OSFM_LAUNCH_CHECK();
     }
-    if (rs.schur == OSFM_SCHUR_PIPE || rs.schur == OSFM_SCHUR_MMA) {
+    // the segment kernels add the segment points' camera-side blocks: with no free camera-side block (nc == 0) there
+    // are none (and no segment tables or block structure to read); their point blocks are those above
+    if (nc > 0 && (rs.schur == OSFM_SCHUR_PIPE || rs.schur == OSFM_SCHUR_MMA)) {
       unsigned long long* prof = nullptr;
       if (trace_on) {
         d_prof.reserve(16);
@@ -2010,7 +2018,7 @@ void BA::build_system(const double* diag, double inv_radius, int* rank_flag, boo
         fprintf(stderr, "[osfm_ba] ba_schur_mma clocks / segment (thread 0): structure %llu offsets %llu loads %llu rows %llu mma %llu flush %llu\n",
                 hp[0] / nseg, hp[1] / nseg, hp[2] / nseg, hp[3] / nseg, hp[4] / nseg, hp[5] / nseg);
       }
-    } else if (rs.schur == OSFM_SCHUR_SIMT_SEGMENT) {
+    } else if (nc > 0 && rs.schur == OSFM_SCHUR_SIMT_SEGMENT) {
       const long long n_fast = rs.n_fast_obs;
       ba_obs_rows<<<grid_for(n_fast * wc, 256), 256, 0, stream>>>(rs.v, rs.bm, rs.bsr, n_fast, d_scale.p, d_Vinv.p, d_Vig.p,
                                                                 d_rowsJ.p, d_rowsW.p, d_rowsY.p, d_rhs_p);
@@ -2503,8 +2511,9 @@ void BA::run() {
     OSFM_LAUNCH_CHECK();
     rs.pcg_pipe.Wdef = d_Wdef.p;
   }
-  if (n > 0) x_norm_pass(0);
-  ba_lm_init<<<1, 1, 0, stream>>>(d_lm.p, d_sc.p, n);
+  // every rank takes part in the |x| all-reduce and leaves the loop together: decided on the whole problem's size
+  if (rs.n_all > 0) x_norm_pass(0);
+  ba_lm_init<<<1, 1, 0, stream>>>(d_lm.p, d_sc.p, rs.n_all > 0 ? 1 : 0);
   OSFM_LAUNCH_CHECK();
   if (rs.device_loop) {
     run_lm_graph();
