@@ -991,6 +991,7 @@ struct BA {
   DevBuf<double> d_scale, d_colnorm2, d_grad, d_diag, d_y, d_bs_t;
   DevBuf<double> d_px, d_pr, d_pz, d_pp, d_pAp, d_Minv, d_reproj, d_full_pts;
   DevBuf<double> d_Wdef;                   // [PCG_ND][nc] deflation vectors of the pipelined PCG (pcg_gauge_vectors)
+  DevBuf<unsigned long long> d_pm;         // [2][nc][2] m = M^-1 w of the pipelined PCG as flagged words, by parity
   DevBuf<int> d_blk_off, d_blk_sz, d_cam_blk, d_inst_blk, d_rc_blk;
   // block-sparse reduced system (ba_reduced.cuh)
   DevBuf<unsigned long long> d_tkeys, d_skeys, d_skeys2, d_rkeys, d_rkeys2;
@@ -1510,6 +1511,7 @@ void BA::upload_problem() {
   d_scale.reserve(nz); d_colnorm2.reserve(nz); d_grad.reserve(nz); d_diag.reserve(nz); d_diag_r.reserve(nz); d_y.reserve(nz);
   d_px.reserve(std::max(nc, 1)); d_pr.reserve(std::max(nc, 1)); d_pz.reserve(std::max(nc, 1));
   d_pp.reserve(std::max(nc, 1)); d_pAp.reserve(std::max(nc, 1));
+  d_pm.reserve(4 * (size_t)std::max(nc, 1));
   d_pcg.reserve(1);
   d_Minv.reserve((size_t)std::max(rs.ngroups, 1) * MAXB * MAXB);
   d_Ap.reserve(std::max(nc, 1));
@@ -2072,6 +2074,8 @@ void BA::solve_reduced() {
                                                                 rs.ngroups, d_Minv.p);
   OSFM_LAUNCH_CHECK();
   OSFM_CUDA(cudaMemsetAsync(d_pcg.p, 0, sizeof(PcgState), stream));
+  // the flagged words of pcg_pipelined start every solve at generation 0, which no exchange waits for
+  if (rs.pcg_pipe_ok) OSFM_CUDA(cudaMemsetAsync(d_pm.p, 0, sizeof(unsigned long long) * 4 * (size_t)nc, stream));
   const int max_pcg = std::min(2 * nc + 100, 5000);
   const int classic_path = rs.pcg_resident ? OSFM_PCG_CLASSIC_RESIDENT : OSFM_PCG_CLASSIC_STREAMED;
   auto classic = [&]() {
@@ -2090,17 +2094,16 @@ void BA::solve_reduced() {
   };
   if (rs.pcg_pipe_ok) {
     launch_cooperative(pcg_pipelined, rs.pcg_grid, PCG_THREADS, rs.pcg_pipe_smem, stream, d_Spcg.p, rs.lay, rs.bsr, d_Minv.p,
-                       rs.d_rhs_p, d_px.p, d_pz.p, d_pp.p, d_pcg.p, nc, max_pcg, 1e-16, rs.pcg_pipe);
+                       rs.d_rhs_p, d_px.p, d_pm.p, d_pcg.p, nc, max_pcg, 1e-16, rs.pcg_pipe);
     OSFM_LAUNCH_CHECK();
     if (tracing()) {
       OSFM_CUDA(cudaMemcpyAsync(h_pcg.p, d_pcg.p, PCG_STATE_HEADER, cudaMemcpyDeviceToHost, stream));
       OSFM_CUDA(cudaStreamSynchronize(stream));
       const PcgState& h = *h_pcg.p;
       const int its = std::max(h.iterations, 1);
-      fprintf(stderr, "[osfm_ba] pipelined pcg %d its converged %d, CTA0 clocks/it: stage %lld matvec %lld reduce %lld update %lld"
-              " | wide barrier (all calls / its): own sums %lld release %lld collect %lld column sums %lld\n",
-              h.iterations, h.converged, h.prof[0] / its, h.prof[1] / its, h.prof[2] / its, h.prof[3] / its, h.prof[4] / its,
-              h.prof[5] / its, h.prof[6] / its, h.prof[7] / its);
+      fprintf(stderr, "[osfm_ba] pipelined pcg %d its converged %d, CTA0 clocks/it: post %lld stage %lld matvec %lld collect %lld"
+              " update %lld\n", h.iterations, h.converged, h.prof[0] / its, h.prof[1] / its, h.prof[2] / its, h.prof[3] / its,
+              h.prof[4] / its);
     }
     ba_lm_pcg_check<<<1, 1, 0, stream>>>(d_lm.p, d_pcg.p, classic_path, rs.h_pcg, rs.cap_graph != nullptr);
     OSFM_LAUNCH_CHECK();

@@ -1306,6 +1306,12 @@ struct PcgState {
   alignas(16) double slot[2][PCG_MAX_CTAS][4];
   // wide payload of the deflated solver: 3 dot products + PCG_ND projections (double-buffered by generation parity)
   double slotx[2][PCG_MAX_CTAS][12];
+  // the in-loop dot products of pcg_pipelined as flagged words (pcg_post_wide / pcg_collect_wide, pcg_post3 /
+  // pcg_collect3): PCG_NW doubles per CTA, two words each, by value so that one warp reads a value of 32 CTAs in four
+  // lines; double-buffered by exchange parity
+  alignas(16) unsigned long long slotf[2][PCG_NW][PCG_MAX_CTAS][2];
+  // their totals (pcg_collect_wide), one 128-byte line each: every CTA reads all of them
+  alignas(128) unsigned long long totf[2][PCG_NW][16];
   // per-CTA arrival generation, one 128-byte line each (packed flags contend for one line on
   // every arrival; one line per CTA does not)
   unsigned flags[PCG_MAX_CTAS * PCG_FLAG_STRIDE];
@@ -1556,12 +1562,14 @@ __global__ void __launch_bounds__(PCG_THREADS, 1)
 
 
 // ---------------------------------------------------------------------------
-// Pipelined PCG (Ghysels & Vanroose 2014, preconditioned pipelined CG): the reduction of an
-// iteration's dot products and the exchange of the vector the next mat-vec needs ride on the SAME
-// grid barrier, so an iteration costs one barrier instead of two.  Every CTA owns whole
+// Pipelined PCG (Ghysels & Vanroose 2014, preconditioned pipelined CG): the global reduction of an
+// iteration's dot products runs during its mat-vec, which does not need them.  There is no grid barrier
+// in the loop: the dot products and m travel as flagged words (flag_put / flag_wait_all), a CTA starts its
+// mat-vec as soon as the entries of m its columns need have arrived and collects the totals after it.
+// Every CTA owns whole
 // preconditioner groups: their rows of S, the groups' inverse blocks and all eight recurrence
 // vectors of those rows stay in shared memory / registers for the whole solve; the only vector that
-// moves through L2 is m = M^-1 w (nc doubles, double-buffered by iteration parity): after the barrier a
+// moves through L2 is m = M^-1 w (nc flagged pairs, double-buffered by iteration parity): a
 // CTA gathers, per column list of its block rows, the entries of m those columns need into a packed copy
 // (mp), so the rows then stream S and mp from shared memory without bank conflicts.  The two block rows
 // of a group usually store the same block columns (a camera and the rig instance of its only shot); they
@@ -1622,6 +1630,19 @@ __global__ void pcg_gauge_vectors(int NI, const int* __restrict__ inst_poff, con
   }
 }
 
+// warp i sums value i over the CTAs' rows of gather: lane l takes CTAs l, l + 32, ... in order, then a fixed tree
+__device__ __forceinline__ void wide_column_sums(unsigned nblocks, double* vals /* [PCG_NW] */, const double* gather) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  if (warp < PCG_NW) {
+    double sa = 0.0;
+    for (unsigned c = lane; c < nblocks; c += 32) sa += gather[c * PCG_NW + warp];
+#pragma unroll
+    for (int o = 16; o; o >>= 1) sa += __shfl_xor_sync(0xffffffffu, sa, o);
+    if (lane == 0) vals[warp] = sa;
+  }
+  __syncthreads();
+}
+
 // The grid_reduce barrier with PCG_NW doubles per CTA.  Built for latency, the only thing that matters here, and around one
 // measurement: arguments and results must not live in local memory -- every poll of the barrier invalidates L1
 // (ld.acquire -> CCTL.IVALL), so a stack array written before the call and read inside it is an L2 round trip (the
@@ -1630,14 +1651,14 @@ __global__ void pcg_gauge_vectors(int NI, const int* __restrict__ inst_poff, con
 // column i and publishes it in the CTA's slot; thread 0 releases the flag; thread t < nblocks acquires CTA t's flag,
 // loads its slot with independent 16-byte loads and drops it into gather[t][.]; warp i sums column i over the CTAs
 // in a fixed order (bit-identical totals in every CTA) into vals[i], which the caller reads.  Not inlined: the kernel
-// calls it from seven places and the loop body has to stay resident in the instruction cache.
+// calls it from six places and the loop body has to stay resident in the instruction cache.  The loop of pcg_pipelined
+// exchanges its dot products through flagged words instead (pcg_post_wide / pcg_collect_wide below); this barrier
+// serves the once-per-solve exchanges, where the plain stores it orders are what the caller reads next.
 __device__ __noinline__ void grid_reduce_wide(PcgState* st, unsigned nblocks, unsigned* gen_io, double* vals /* [PCG_NW] */,
                                               double* gather /* [nblocks][PCG_NW] */, const double* inrow /* [nactive][PCG_NW] */,
                                               int nactive) {
   const unsigned gen = ++(*gen_io);
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const bool probe = blockIdx.x == 0 && threadIdx.x == 0;   // st->prof[4..7]: own sums, release, collection, column sums
-  long long tq = probe ? clock64() : 0;
   __syncthreads();   // inrow is complete
   if (warp < PCG_NW) {
     double sa = 0.0;
@@ -1647,10 +1668,8 @@ __device__ __noinline__ void grid_reduce_wide(PcgState* st, unsigned nblocks, un
     if (lane == 0) __stcg(&st->slotx[gen & 1][blockIdx.x][warp], sa);
   }
   __syncthreads();  // the slot (and every other global write of this CTA) happens-before thread 0's release
-  if (probe) { const long long now = clock64(); st->prof[4] += now - tq; tq = now; }
   if (threadIdx.x == 0)
     asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(&st->flags[blockIdx.x * PCG_FLAG_STRIDE]), "r"(gen) : "memory");
-  if (probe) { const long long now = clock64(); st->prof[5] += now - tq; tq = now; }
   if (threadIdx.x < nblocks) {
     const long long t0 = clock64();
     unsigned cur;
@@ -1667,22 +1686,153 @@ __device__ __noinline__ void grid_reduce_wide(PcgState* st, unsigned nblocks, un
     for (int i = 0; i < PCG_NW / 2; ++i) dst[i] = v[i];
   }
   __syncthreads();
-  if (probe) { const long long now = clock64(); st->prof[6] += now - tq; tq = now; }
-  if (warp < PCG_NW) {   // warp i sums value i over the CTAs: lane l takes CTAs l, l + 32, ... in order, then a fixed tree
-    double sa = 0.0;
-    for (unsigned c = lane; c < nblocks; c += 32) sa += gather[c * PCG_NW + warp];
-#pragma unroll
-    for (int o = 16; o; o >>= 1) sa += __shfl_xor_sync(0xffffffffu, sa, o);
-    if (lane == 0) vals[warp] = sa;
-  }
-  __syncthreads();
-  if (probe) st->prof[7] += clock64() - tq;
+  wide_column_sums(nblocks, vals, gather);
 }
 static_assert(PCG_THREADS / 32 >= PCG_NW, "a warp per value of the wide barrier");
 
+// Flagged words (the LL protocol of NCCL): a double travels as two 8-byte words {low 32 bits | gen << 32} and
+// {high 32 bits | gen << 32}.  Each word is single-copy atomic, so a reader that sees gen in both words has the value
+// that was stored with it -- no fence before the store, no acquire on the load, and a relaxed load polls without
+// invalidating L1 (ld.acquire does, CCTL.IVALL).  The pair is stored as one v2 store, but nothing relies on 16-byte
+// atomicity (the PTX memory model does not promise it): the words are checked one by one.  A reader must never find
+// the generation it waits for in a word before that word is meant for it: the callers zero the buffers before a solve
+// and count gen up from 1 within it.
+__device__ __forceinline__ void flag_put(unsigned long long* p, double v, unsigned gen) {
+  const unsigned long long b = (unsigned long long)__double_as_longlong(v), g = (unsigned long long)gen << 32;
+  asm volatile("st.relaxed.gpu.global.v2.b64 [%0], {%1, %2};" ::"l"(p), "l"((b & 0xffffffffull) | g), "l"((b >> 32) | g)
+               : "memory");
+}
+__device__ __forceinline__ ulonglong2 flag_ld(const unsigned long long* p) {
+  ulonglong2 w;
+  asm volatile("ld.relaxed.gpu.global.v2.b64 {%0, %1}, [%2];" : "=l"(w.x), "=l"(w.y) : "l"(p));
+  return w;
+}
+__device__ __forceinline__ bool flag_ok(ulonglong2 w, unsigned gen) {
+  return (unsigned)(w.x >> 32) == gen && (unsigned)(w.y >> 32) == gen;
+}
+__device__ __forceinline__ double flag_val(ulonglong2 w) {
+  return __longlong_as_double((long long)((w.x & 0xffffffffull) | (w.y << 32)));
+}
+// Waits until the N loaded pairs w[i] (of addr(i)) all carry gen.  The late ones are re-loaded together, so a wait costs
+// one round trip per poll however many of them were late -- one by one, every stale pair behind the first late one
+// would cost another.  grid_reduce's clock budget.  A pair the caller has no address for is set to carry gen.
+template <int N, class Addr>
+__device__ __forceinline__ void flag_wait_all(ulonglong2 (&w)[N], Addr addr, unsigned gen) {
+  bool ok = true;
+#pragma unroll
+  for (int i = 0; i < N; ++i) ok = ok && flag_ok(w[i], gen);
+  if (ok) return;
+  const long long t0 = clock64();
+  do {
+#pragma unroll
+    for (int i = 0; i < N; ++i)
+      if (!flag_ok(w[i], gen)) w[i] = flag_ld(addr(i));
+    if (clock64() - t0 > 8000000000LL) __trap();  // a protocol bug must not hang the GPU
+    ok = true;
+#pragma unroll
+    for (int i = 0; i < N; ++i) ok = ok && flag_ok(w[i], gen);
+  } while (!ok);
+}
+
+// The two halves of the wide barrier for the loop of pcg_pipelined, with its PCG_NW doubles per CTA in flagged words
+// (st->slotf[gen & 1]).  pcg_post_wide: warp i sums column i of inrow (same order as grid_reduce_wide) and stores it;
+// no fence, no flag, no wait.  pcg_collect_wide, called later: value i is summed over the CTAs by ONE warp of the grid
+// (warp i / nblocks of CTA i % nblocks), in grid_reduce_wide's order -- lane l takes CTAs l, l + 32, ... in order, then
+// a fixed tree -- and published as a flagged total, which every CTA then reads: bit-identical totals everywhere, but
+// every CTA reads PCG_NW totals instead of every slot of the grid (132 x 132 x 160 bytes per iteration on C4, read
+// from the same few hundred lines at once, which made the collection cost more than the barrier it replaced).
+// Reuse: a slot (and a total) of gen + 2 is written only after its writer has read the totals of gen + 1; they exist
+// only once every CTA has posted gen + 1, which each does after it has read the totals of gen, and those were
+// published after every slot of gen had been read.  No reader of gen can see it overwritten.
+__device__ __noinline__ void pcg_post_wide(PcgState* st, unsigned gen, const double* inrow /* [nactive][PCG_NW] */,
+                                           int nactive) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  __syncthreads();   // inrow is complete
+  if (warp < PCG_NW) {
+    double sa = 0.0;
+    for (int r = lane; r < nactive; r += 32) sa += inrow[r * PCG_NW + warp];
+#pragma unroll
+    for (int o = 16; o; o >>= 1) sa += __shfl_xor_sync(0xffffffffu, sa, o);
+    if (lane == 0) flag_put(st->slotf[gen & 1][warp][blockIdx.x], sa, gen);
+  }
+}
+__device__ __noinline__ void pcg_collect_wide(PcgState* st, unsigned nblocks, unsigned gen, double* vals /* [PCG_NW] */) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const unsigned i = warp * nblocks + blockIdx.x;   // the value this warp sums, if any
+  if (i < PCG_NW) {
+    const unsigned long long(*sl)[2] = st->slotf[gen & 1][i];
+    const unsigned long long none = (unsigned long long)gen << 32;   // past the last CTA: nothing to wait for
+    constexpr int K = PCG_MAX_CTAS / 32;
+    ulonglong2 v[K];
+#pragma unroll
+    for (int k = 0; k < K; ++k) v[k] = lane + 32 * k < (int)nblocks ? flag_ld(sl[lane + 32 * k]) : make_ulonglong2(none, none);
+    flag_wait_all(v, [&](int k) { return sl[lane + 32 * k]; }, gen);
+    double sa = 0.0;
+#pragma unroll
+    for (int k = 0; k < K; ++k)
+      if (lane + 32 * k < (int)nblocks) sa += flag_val(v[k]);
+#pragma unroll
+    for (int o = 16; o; o >>= 1) sa += __shfl_xor_sync(0xffffffffu, sa, o);
+    if (lane == 0) flag_put(st->totf[gen & 1][i], sa, gen);
+  }
+  if (threadIdx.x < PCG_NW) {
+    ulonglong2 t[1] = {flag_ld(st->totf[gen & 1][threadIdx.x])};
+    flag_wait_all(t, [&](int) { return st->totf[gen & 1][threadIdx.x]; }, gen);
+    vals[threadIdx.x] = flag_val(t[0]);
+  }
+  __syncthreads();
+}
+static_assert(PCG_MAX_CTAS % 32 == 0 && PCG_NW <= PCG_THREADS / 32, "pcg_collect_wide: whole warps of slots, a warp per value");
+
+// grid_reduce<3> split the same way, for the loop of pcg_pipelined without deflation: the same sums in the same order
+// (bit-identical totals), the CTA's three values in flagged words of st->slotf[gen & 1] instead of a released slot.
+__device__ __forceinline__ void pcg_post3(PcgState* st, unsigned gen, double a, double b, double c, double (*red)[3]) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
+#pragma unroll
+  for (int o = 16; o; o >>= 1) {
+    a += __shfl_xor_sync(0xffffffffu, a, o);
+    b += __shfl_xor_sync(0xffffffffu, b, o);
+    c += __shfl_xor_sync(0xffffffffu, c, o);
+  }
+  if (lane == 0) { red[warp][0] = a; red[warp][1] = b; red[warp][2] = c; }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double sa = 0.0, sb = 0.0, sc = 0.0;
+    for (int w = 0; w < nwarps; ++w) { sa += red[w][0]; sb += red[w][1]; sc += red[w][2]; }
+    flag_put(st->slotf[gen & 1][0][blockIdx.x], sa, gen);
+    flag_put(st->slotf[gen & 1][1][blockIdx.x], sb, gen);
+    flag_put(st->slotf[gen & 1][2][blockIdx.x], sc, gen);
+  }
+  __syncthreads();   // red[] is read by thread 0 above and rewritten by pcg_collect3
+}
+__device__ __forceinline__ void pcg_collect3(PcgState* st, unsigned nblocks, unsigned gen, double& A, double& B, double& C,
+                                             double (*red)[3]) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  double va = 0.0, vb = 0.0, vc = 0.0;
+  if (threadIdx.x < nblocks) {
+    const auto sl = st->slotf[gen & 1];
+    ulonglong2 v[3] = {flag_ld(sl[0][threadIdx.x]), flag_ld(sl[1][threadIdx.x]), flag_ld(sl[2][threadIdx.x])};
+    flag_wait_all(v, [&](int i) { return sl[i][threadIdx.x]; }, gen);
+    va = flag_val(v[0]); vb = flag_val(v[1]); vc = flag_val(v[2]);
+  }
+#pragma unroll
+  for (int o = 16; o; o >>= 1) {
+    va += __shfl_xor_sync(0xffffffffu, va, o);
+    vb += __shfl_xor_sync(0xffffffffu, vb, o);
+    vc += __shfl_xor_sync(0xffffffffu, vc, o);
+  }
+  if (lane == 0) { red[warp][0] = va; red[warp][1] = vb; red[warp][2] = vc; }
+  __syncthreads();
+  double sa = 0.0, sb = 0.0, sc = 0.0;
+  const int wmax = (int)((nblocks + 31) >> 5);
+  for (int w = 0; w < wmax; ++w) { sa += red[w][0]; sb += red[w][1]; sc += red[w][2]; }
+  A = sa; B = sb; C = sc;
+  __syncthreads();
+}
+
 __global__ void __launch_bounds__(PCG_THREADS, 1)
     pcg_pipelined(const double* __restrict__ Spcg, PcgLayout L, BsrView h, const double* __restrict__ Minv,
-                  const double* __restrict__ rhs, double* __restrict__ x_out, double* mbuf0, double* mbuf1, PcgState* st,
+                  const double* __restrict__ rhs, double* x_out, unsigned long long* mflag, PcgState* st,
                   int nc, int max_iter, double tol2_rel, PcgPipe R) {
   extern __shared__ __align__(16) unsigned char pcg_smem[];
   __shared__ double red[PCG_THREADS / 32][3];
@@ -1719,7 +1869,6 @@ __global__ void __launch_bounds__(PCG_THREADS, 1)
   double* inrow_s = gather_s + PCG_NW * gridDim.x; // [max_rows][PCG_NW]: what the owners of the rows put on it
   double* wide_s = &redw[0][0];                    // [PCG_NW]: its totals
   const int MR = R.max_rows;
-  double* mbuf[2] = {mbuf0, mbuf1};
   unsigned bar_gen = 0;
 
   const int g_lo = R.grp_lo[blockIdx.x], g_hi = R.grp_lo[blockIdx.x + 1], ng = g_hi - g_lo;
@@ -1777,8 +1926,10 @@ __global__ void __launch_bounds__(PCG_THREADS, 1)
     for (int t = lane; t < n * n; t += 32) Minv_s[grp_moff[gl] + t] = src[(t / n) * MAXB + t % n];
   }
 
-  // group solve: n_s[rows of g] = Minv_g * w_s[rows of g]; optionally published to a global vector
-  auto group_solve = [&](double* publish) {
+  // group solve: g_s[rows of g] = Minv_g * w_s[rows of g], published as flagged words of generation gen in the m buffer
+  // of its parity (mflag[gen & 1][column][2], zeroed before the solve)
+  auto group_solve = [&](unsigned gen) {
+    unsigned long long* publish = mflag + (size_t)(gen & 1) * 2 * nc;
     for (int gl = warp; gl < ng; gl += nwarps) {
       const int r0 = grp_row0[gl], n = grp_row0[gl + 1] - r0;
       const double* M = Minv_s + grp_moff[gl];
@@ -1787,7 +1938,7 @@ __global__ void __launch_bounds__(PCG_THREADS, 1)
         for (int j = 0; j < n; ++j) sv += M[lane * n + j] * w_s[r0 + j];
       if (lane < n) {
         g_s[r0 + lane] = sv;
-        publish[row_gidx[r0 + lane]] = sv;
+        flag_put(publish + 2 * row_gidx[r0 + lane], sv, gen);
       }
     }
   };
@@ -1851,6 +2002,22 @@ __global__ void __launch_bounds__(PCG_THREADS, 1)
         if (e + k * bd < ncols) mp_s[e + k * bd] = a[k];
     }
   };
+  // the same for the m that group_solve(gen) published: each entry is waited for on its own, so the gathers of a CTA
+  // need only the CTAs that own its columns to have published, not the whole grid
+  auto stage_m = [&](unsigned gen) {
+    const unsigned long long* src = mflag + (size_t)(gen & 1) * 2 * nc;
+    const int bd = blockDim.x;
+    for (int e = tid; e < ncols; e += 8 * bd) {
+      const unsigned long long none = (unsigned long long)gen << 32;   // past the end: nothing to wait for
+      ulonglong2 a[8];
+#pragma unroll
+      for (int k = 0; k < 8; ++k) a[k] = e + k * bd < ncols ? flag_ld(src + 2 * cols_s[e + k * bd]) : make_ulonglong2(none, none);
+      flag_wait_all(a, [&](int k) { return src + 2 * cols_s[e + k * bd]; }, gen);
+#pragma unroll
+      for (int k = 0; k < 8; ++k)
+        if (e + k * bd < ncols) mp_s[e + k * bd] = flag_val(a[k]);
+    }
+  };
 
   // ---- deflation set-up: A W (PCG_ND mat-vecs, no barrier: W is known everywhere), E = W^T A W, W^T b ----
   // Deflated CG (Saad, Yeung, Erhel, Guyomarc'h 2000) in its projected form: with Q = W E^-1 W^T and P = I - A Q solve
@@ -1877,9 +2044,9 @@ __global__ void __launch_bounds__(PCG_THREADS, 1)
     }
     // 28 entries of the symmetric E, W^T b (7), b^T b: four wide reductions
     double E[PCG_ND * PCG_ND], wb[PCG_ND];
-    bb = 0.0;
-    int e_idx = 0;
-    double collected[40];
+    // the 36 totals wait in Einv_s (49 doubles, written only once thread 0 has read them): an array of them in
+    // registers, live across the grid_reduce_wide calls, does not fit the kernel's 128 registers
+    double* collected = Einv_s;
     for (int pass = 0; pass < 4; ++pass) {
 #pragma unroll
       for (int q = 0; q < PCG_NW; ++q) {
@@ -1900,11 +2067,11 @@ __global__ void __launch_bounds__(PCG_THREADS, 1)
         if (mine) inrow_s[tid * PCG_NW + q] = val;
       }
       grid_reduce_wide(st, gridDim.x, &bar_gen, wide_s, gather_s, inrow_s, nrows);
-#pragma unroll
-      for (int q = 0; q < PCG_NW; ++q) collected[pass * PCG_NW + q] = wide_s[q];
+      if (tid < PCG_NW && pass * PCG_NW + tid < 36) collected[pass * PCG_NW + tid] = wide_s[tid];
       __syncthreads();   // wide_s / inrow_s are rewritten by the next pass
     }
-    (void)e_idx;
+    bb = collected[35];
+    __syncthreads();   // every thread has read bb before thread 0 rewrites Einv_s
     if (tid == 0) {
       // every CTA factorises the same 7 x 7 matrix: identical decisions everywhere
       int idx = 0;
@@ -1951,7 +2118,6 @@ __global__ void __launch_bounds__(PCG_THREADS, 1)
       s_defl = ok ? 1 : 0;
     }
     __syncthreads();
-    bb = collected[35];
     defl = s_defl != 0;   // dependent / vanishing vectors (e.g. every rig instance fixed): plain PCG
   }
   // tc_s = E^-1 t for the PCG_ND projections the wide barrier left in wide_s[3..]: seven threads, not all 512 (49 DFMA
@@ -1978,7 +2144,10 @@ __global__ void __launch_bounds__(PCG_THREADS, 1)
   if (defl && mine) rr_ = bi - aw_dot(c0_s);
   if (mine) w_s[tid] = rr_;
   __syncthreads();
-  group_solve(mbuf[0]);
+  // Generations of the flagged exchanges: u = M^-1 r is 1, the m of loop iteration it and the dot products posted in it
+  // are it + 2.  Every flagged buffer (mflag, st->slotf, st->totf) is zeroed with the rest of PcgState before the solve, so no
+  // word left by an earlier solve, run or handle can carry a generation this solve waits for.
+  group_solve(1);
   if (defl) {
     __syncthreads();   // g_s of my row was written by the warp that solved its group
     if (mine) {
@@ -1999,18 +2168,25 @@ __global__ void __launch_bounds__(PCG_THREADS, 1)
   int it = 0, converged = 0;
   if (bb > 0.0) {
     if (mine) u = g_s[tid];
-    stage(mbuf[0]);
+    stage_m(1);   // already visible: the barrier above ordered it
     __syncthreads();
     matvec();
     __syncthreads();
     if (mine) { w = n_s[tid] - (defl ? aw_dot(tc_s) : 0.0); w_s[tid] = w; }
     __syncthreads();
-    group_solve(mbuf[1]);
+    group_solve(2);
     double gamma_prev = 1.0, alpha_prev = 1.0, best = bb;
     int since_best = 0;
+    // Ghysels-Vanroose order: an iteration posts its dot products, then stages m and runs the mat-vec -- which do not
+    // need them -- and only then collects the totals, which by then have mostly arrived.  The exit tests therefore run
+    // after a mat-vec the exiting iteration does not use; every CTA takes them on bit-identical totals, so all leave
+    // together and none waits for an m that is not coming.
+    // Reuse of the two m buffers: m of generation gen + 2 overwrites gen.  Its writer has read the totals of gen + 1
+    // first, which exist only once every CTA has posted gen + 1, and a CTA posts that only after it has staged gen, so
+    // no CTA is still reading gen.
     for (;; ++it) {
+      const unsigned gen = (unsigned)it + 2u;
       const long long tk0 = clock64();
-      double gamma, delta;
       if (defl) {
         __syncthreads();   // g_s (m of my row) comes from another warp's group solve
         if (mine) {
@@ -2019,24 +2195,28 @@ __global__ void __launch_bounds__(PCG_THREADS, 1)
 #pragma unroll
           for (int j = 0; j < PCG_ND; ++j) ir[3 + j] = AW_s[j * MR + tid] * g_s[tid];   // (A W)^T m of the m being exchanged
         }
-        grid_reduce_wide(st, gridDim.x, &bar_gen, wide_s, gather_s, inrow_s, nrows);
-        gamma = wide_s[0]; delta = wide_s[1]; rr = wide_s[2];
-        coarse();
+        pcg_post_wide(st, gen, inrow_s, nrows);
       } else
-        grid_reduce<3>(st, gridDim.x, bar_gen, mine ? rr_ * u : 0.0, mine ? w * u : 0.0, mine ? rr_ * rr_ : 0.0, gamma, delta, rr,
-                   red);
+        pcg_post3(st, gen, mine ? rr_ * u : 0.0, mine ? w * u : 0.0, mine ? rr_ * rr_ : 0.0, red);
       const long long tk1 = clock64();
-      if (!(rr == rr)) break;
-      if (rr <= tol2) { converged = 1; break; }
-      if (rr < best) { best = rr; since_best = 0; } else if (++since_best > 150) break;  // stagnation
-      if (it >= max_iter) break;
-      const double* mcur = mbuf[(it + 1) & 1];
-      stage(mcur);
+      stage_m(gen);
       __syncthreads();
       const long long tk2 = clock64();
       matvec();
       __syncthreads();
       const long long tk3 = clock64();
+      double gamma, delta;
+      if (defl) {
+        pcg_collect_wide(st, gridDim.x, gen, wide_s);
+        gamma = wide_s[0]; delta = wide_s[1]; rr = wide_s[2];
+        coarse();
+      } else
+        pcg_collect3(st, gridDim.x, gen, gamma, delta, rr, red);
+      const long long tk4 = clock64();
+      if (!(rr == rr)) break;
+      if (rr <= tol2) { converged = 1; break; }
+      if (rr < best) { best = rr; since_best = 0; } else if (++since_best > 150) break;  // stagnation
+      if (it >= max_iter) break;
       const double beta = it > 0 ? gamma / gamma_prev : 0.0;
       const double alpha = it > 0 ? gamma / (delta - beta * gamma / alpha_prev) : gamma / delta;
       if (mine) {
@@ -2052,12 +2232,13 @@ __global__ void __launch_bounds__(PCG_THREADS, 1)
         w_s[tid] = w;
       }
       __syncthreads();
-      group_solve(mbuf[it & 1]);
+      group_solve(gen + 1);
       gamma_prev = gamma;
       alpha_prev = alpha;
-      if (blockIdx.x == 0 && tid == 0) {
-        const long long tk4 = clock64();
-        st->prof[0] += tk2 - tk1; st->prof[1] += tk3 - tk2; st->prof[2] += tk1 - tk0; st->prof[3] += tk4 - tk3;
+      if (blockIdx.x == 0 && tid == 0) {   // OSFM_BA_TRACE: post, stage (with the waits for m), mat-vec, collect, update
+        const long long tk5 = clock64();
+        st->prof[0] += tk1 - tk0; st->prof[1] += tk2 - tk1; st->prof[2] += tk3 - tk2; st->prof[3] += tk4 - tk3;
+        st->prof[4] += tk5 - tk4;
       }
     }
   } else {
@@ -2084,10 +2265,9 @@ __global__ void __launch_bounds__(PCG_THREADS, 1)
   // The residual above is the recurred one, which drifts from b - S x in pipelined CG: check the true residual of the
   // returned x with one more exchange and mat-vec, and hand the solve to the classic kernel if it is not what was claimed.
   if (converged && bb > 0.0) {
-    if (mine) mbuf[0][gi] = xr;
     double d0, d1, d2;
     grid_reduce<3>(st, gridDim.x, bar_gen, 0.0, 0.0, 0.0, d0, d1, d2, red);   // x of every CTA is visible
-    stage(mbuf[0]);
+    stage(x_out);
     __syncthreads();
     matvec();
     __syncthreads();
