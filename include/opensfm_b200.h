@@ -18,8 +18,8 @@
  *
  * There is no CPU fallback: every call needs a CUDA device (H100, sm_90a).
  *
- * Handles (osfm_matcher, osfm_ba, osfm_tracks, osfm_rotransac) own a CUDA stream and workspaces on the device they
- * were created on, and every call on a handle makes that device current on the calling thread.  Calls on one handle
+ * Handles (osfm_matcher, osfm_ba, osfm_tracks, osfm_rotransac, osfm_resect) own a CUDA stream and workspaces on the
+ * device they were created on, and every call on a handle makes that device current on the calling thread.  Calls on one handle
  * are serialised and may come from any thread; calls on different handles do not wait for each other.  A callback
  * (today only the all-reduce of osfm_ba_set_distributed) must not call into the handle that called it.
  */
@@ -515,6 +515,36 @@ int osfm_rotransac_last_device_ms(osfm_rotransac* h, float* ms);
 int osfm_rotransac_set_stream_prefix(osfm_rotransac* h, int64_t length);
 int osfm_rotransac_set_trace(osfm_rotransac* h, int capacity);
 int osfm_rotransac_get_trace(osfm_rotransac* h, int32_t* count, int64_t* stream_used, int32_t* indices);
+
+/* ------------------------------------------------------------------------
+ * ABSOLUTE-POSE RANSAC OF SHOTS (RESECTION)
+ * ---------------------------------------------------------------------- */
+typedef struct osfm_resect osfm_resect;
+
+/* Resects shots against the reconstructed points: pyrobust's ransac_absolute_pose with RANSAC scoring (P3P samples,
+ * Lu's orthogonal iteration in local optimisation), as resect runs it through multiview.absolute_pose_ransac
+ * (opensfm/reconstruction.py:695-762), and the chord inliers of the resulting pose, for many shots at once.  The
+ * rules, including the deliberate differences, are stated in oracle/absolute_pose_oracle.py.  A handle owns one CUDA
+ * stream, its workspaces on `device` and the shared sample stream of mt19937(42). */
+int osfm_resect_create(int device, osfm_resect** out);
+int osfm_resect_destroy(osfm_resect* h);
+/* bearings: num_bearings x 3 fp64 (normalised on the device); points: num_points x 3 fp64 world points.  Shot s
+ * owns rows [shot_start[s], shot_start[s + 1]) (shot_start[0] = 0); row r pairs bearing row_bearing[r] with point
+ * row_point[r].  threshold is resect's angle (resection_threshold): RANSAC inliers have |1 - b . normalize(R X + t)|
+ * below 1 - cos(threshold), chord inliers ||normalize(R (X - o)) - b|| below threshold, o = -R^T t.  iterations >= 1
+ * (resect passes 1000).  Outputs: lo_model (12 per shot: [R | t] row-major, world to camera), the RANSAC inlier count
+ * and the chord inlier count of every shot, and the chord inlier mask of every row.  A shot of fewer than 3 rows, or
+ * a row naming a bearing or point outside its table, fails with OSFM_ERR_ARG naming it. */
+int osfm_resect_run(osfm_resect* h, int64_t num_bearings, const double* bearings, int64_t num_points,
+                    const double* points, int64_t num_shots, const int64_t* shot_start, const int64_t* row_bearing,
+                    const int64_t* row_point, double threshold, int iterations, double* lo_model,
+                    int32_t* ransac_inliers, int32_t* chord_inliers, uint8_t* chord_mask);
+/* Device time of the last osfm_resect_run (CUDA events around its kernels, after the uploads). */
+int osfm_resect_last_device_ms(osfm_resect* h, float* ms);
+/* Test hooks, as osfm_rotransac_set_stream_prefix / set_trace / get_trace, per shot. */
+int osfm_resect_set_stream_prefix(osfm_resect* h, int64_t length);
+int osfm_resect_set_trace(osfm_resect* h, int capacity);
+int osfm_resect_get_trace(osfm_resect* h, int32_t* count, int64_t* stream_used, int32_t* indices);
 
 #ifdef __cplusplus
 }

@@ -11,9 +11,7 @@
 // A pair of at most RR_STAGE_ROWS rows is staged in shared memory as fp64 structure-of-arrays; a larger one is read
 // through L2 via its row indices.  A last pass writes the chord-inlier mask and counts.
 //
-// The stream every pair consumes from its start is the same, so a prefix of it (RR_DEFAULT_PREFIX outputs) is made
-// once per handle and kept on the device; a pair that reaches its end continues from the generator state saved after
-// the prefix, in shared memory, so the stream stays exact.
+// The sample stream, its device prefix and the stopping bound are those of ransac_stream.cuh.
 #include <algorithm>
 #include <cfloat>
 #include <climits>
@@ -22,7 +20,9 @@
 #include <numeric>
 #include <vector>
 
+#include "absolute_pose.cuh"
 #include "common.cuh"
+#include "ransac_stream.cuh"
 
 namespace osfm {
 namespace {
@@ -33,39 +33,6 @@ constexpr int RR_STAGE_ROWS = 1024;
 constexpr int RR_MIN_SAMPLE = 3;
 constexpr int RR_MAX_SAMPLE = 12;          // local optimisation samples min(12, inliers / 2) rows (at least 3)
 constexpr int RR_LO_ITERATIONS = 10;
-constexpr double RR_PROBABILITY = 0.99;
-constexpr long long RR_DEFAULT_PREFIX = 1LL << 16;
-constexpr int RR_NEWTON_MAX = 50;
-constexpr double RR_NEWTON_UNSCALED_BELOW = 1e-2;
-constexpr double RR_NEWTON_TOLERANCE = 1e-14;
-
-// std::mt19937: the 32-bit Mersenne twister with its standard seeding.
-struct Mt {
-  static constexpr int N = 624, M = 397;
-  uint32_t s[N];
-  int i;
-  __host__ __device__ void seed(uint32_t x) {
-    s[0] = x;
-    for (int k = 1; k < N; ++k) s[k] = 1812433253u * (s[k - 1] ^ (s[k - 1] >> 30)) + (uint32_t)k;
-    i = N;
-  }
-  __host__ __device__ void twist() {
-    for (int k = 0; k < N; ++k) {
-      const uint32_t y = (s[k] & 0x80000000u) | (s[(k + 1) % N] & 0x7fffffffu);
-      s[k] = s[(k + M) % N] ^ (y >> 1) ^ ((y & 1u) ? 0x9908b0dfu : 0u);
-    }
-    i = 0;
-  }
-  __host__ __device__ uint32_t next() {
-    if (i >= N) twist();
-    uint32_t y = s[i++];
-    y ^= y >> 11;
-    y ^= (y << 7) & 0x9d2c5680u;
-    y ^= (y << 15) & 0xefc60000u;
-    y ^= y >> 18;
-    return y;
-  }
-};
 
 struct RrArgs {
   const double* bearings;        // 3 per entry
@@ -75,30 +42,23 @@ struct RrArgs {
   const int* order;              // pairs of this launch
   double chord_threshold, ransac_threshold;
   int iterations;
-  const uint32_t* prefix;
-  long long prefix_len;
-  const Mt* saved;               // the generator after prefix_len outputs
+  StreamSource src;              // trace: trace_cap drawn indices per pair, or null
   int* best_rows;                // per row: the best model's inlier rows, ascending
   double* lo_model;              // 9 per pair
   int* ransac_inliers;
   int* chord_inliers;
   unsigned char* chord_mask;     // per row
-  int* trace;                    // trace_cap per pair, or null
   int* trace_count;
   long long* stream_used;
-  int trace_cap;
 };
 
 struct RrShared {
-  Mt mt;                         // live once the pair has used the whole prefix
+  StreamState st;
   double sample[RR_MAX_SAMPLE][6];
   double cand[9];                // rotation Q of the candidate (the model is Q^T), row-major
   double best[9];
-  long long cursor;
-  int mt_live;
   int best_count, cand_count;
   int replace, lo, stop;
-  int trace_n;
   int idx[RR_MAX_SAMPLE];
   int warp_n[RR_WARPS];
 };
@@ -121,141 +81,10 @@ struct RrRows {
   }
 };
 
-// ---- thread 0: sampling -------------------------------------------------------------------------------------
-__device__ uint32_t rr_next(RrShared& s, const RrArgs& a) {
-  if (s.cursor < a.prefix_len) return __ldg(a.prefix + s.cursor++);
-  if (!s.mt_live) {
-    s.mt = *a.saved;
-    s.mt_live = 1;
-  }
-  ++s.cursor;
-  return s.mt.next();
-}
-
-// uniform_int_distribution<unsigned long>(0, n - 1) over a 32-bit generator, libstdc++ 13: Lemire's 64-bit product,
-// rejecting low words below 2^32 mod n
-__device__ int rr_draw(RrShared& s, const RrArgs& a, uint32_t n) {
-  unsigned long long prod = (unsigned long long)rr_next(s, a) * n;
-  uint32_t low = (uint32_t)prod;
-  if (low < n) {
-    const uint32_t thr = (0u - n) % n;
-    while (low < thr) {
-      prod = (unsigned long long)rr_next(s, a) * n;
-      low = (uint32_t)prod;
-    }
-  }
-  return (int)(prod >> 32);
-}
-
-// `size` distinct indices in [0, n) into s.idx, redrawing repeats
-__device__ void rr_sample(RrShared& s, const RrArgs& a, int pair, int size, int n) {
-  for (int k = 0; k < size; ++k) {
-    int v;
-    bool dup;
-    do {
-      v = rr_draw(s, a, (uint32_t)n);
-      dup = false;
-      for (int j = 0; j < k; ++j) dup |= s.idx[j] == v;
-    } while (dup);
-    s.idx[k] = v;
-    if (a.trace) {
-      if (s.trace_n < a.trace_cap) a.trace[(long long)pair * a.trace_cap + s.trace_n] = v;
-      ++s.trace_n;
-    }
-  }
-}
-
 // ---- thread 0: the rotation of a sample ---------------------------------------------------------------------
-// row-major 3x3; cof(X) has columns c1 x c2, c2 x c0, c0 x c1 (c_j the columns of X), so X^-T = cof(X) / det(X)
-__device__ __forceinline__ void rr_cof(const double* X, double* C) {
-  for (int j = 0; j < 3; ++j) {
-    const int a = (j + 1) % 3, b = (j + 2) % 3;
-    C[0 * 3 + j] = X[1 * 3 + a] * X[2 * 3 + b] - X[2 * 3 + a] * X[1 * 3 + b];
-    C[1 * 3 + j] = X[2 * 3 + a] * X[0 * 3 + b] - X[0 * 3 + a] * X[2 * 3 + b];
-    C[2 * 3 + j] = X[0 * 3 + a] * X[1 * 3 + b] - X[1 * 3 + a] * X[0 * 3 + b];
-  }
-}
-
-__device__ __forceinline__ double rr_fro(const double* X) {
-  double s = 0.0;
-  for (int k = 0; k < 9; ++k) s += X[k] * X[k];
-  return sqrt(s);
-}
-
-// orthogonal polar factor by scaled Newton (Higham); false if X is singular
-__device__ bool rr_polar(double* X) {
-  const double nx = rr_fro(X);
-  if (!isfinite(nx) || nx == 0.0) return false;
-  for (int k = 0; k < 9; ++k) X[k] /= nx;
-  bool scaled = true;
-  for (int it = 0; it < RR_NEWTON_MAX; ++it) {
-    double C[9];
-    rr_cof(X, C);
-    const double d = X[0] * C[0] + X[3] * C[3] + X[6] * C[6];
-    if (d == 0.0 || !isfinite(d)) return false;
-    for (int k = 0; k < 9; ++k) C[k] /= d;
-    const double z = scaled ? sqrt(rr_fro(C) / rr_fro(X)) : 1.0;
-    double step = 0.0;
-    for (int k = 0; k < 9; ++k) {
-      const double xn = scaled ? 0.5 * (z * X[k] + C[k] / z) : 0.5 * (X[k] + C[k]);
-      step += (xn - X[k]) * (xn - X[k]);
-      X[k] = xn;
-    }
-    step = sqrt(step);
-    if (step < RR_NEWTON_UNSCALED_BELOW) scaled = false;
-    if (step <= RR_NEWTON_TOLERANCE) break;
-  }
-  for (int k = 0; k < 9; ++k)
-    if (!isfinite(X[k])) return false;
-  return true;
-}
-
-// rotation Q (Q b2 ~ b1) of the k sample rows in s.sample, into out: the polar factor of the centred
-// cross-covariance, negated if improper; for k = 3 the proper completion (see oracle/rotation_ransac_oracle.py)
+// rotation Q (Q b2 ~ b1) of the k sample rows in s.sample, into out (absolute_pose.cuh)
 __device__ void rr_rotation(RrShared& s, int k, double* out) {
-  double m1[3], m2[3];
-  for (int c = 0; c < 3; ++c) {
-    m1[c] = s.sample[0][c];
-    m2[c] = s.sample[0][3 + c];
-  }
-  for (int i = 1; i < k; ++i)
-    for (int c = 0; c < 3; ++c) {
-      m1[c] += s.sample[i][c];
-      m2[c] += s.sample[i][3 + c];
-    }
-  for (int c = 0; c < 3; ++c) {
-    m1[c] /= k;
-    m2[c] /= k;
-  }
-  double X[9];
-  for (int q = 0; q < 9; ++q) X[q] = 0.0;
-  for (int i = 0; i < k; ++i) {
-    double dp[3], dq[3];
-    for (int c = 0; c < 3; ++c) {
-      dp[c] = s.sample[i][c] - m1[c];
-      dq[c] = s.sample[i][3 + c] - m2[c];
-    }
-    for (int r = 0; r < 3; ++r)
-      for (int c = 0; c < 3; ++c) X[r * 3 + c] += dp[r] * dq[c];
-  }
-  if (k == RR_MIN_SAMPLE) {
-    double C[9];
-    rr_cof(X, C);
-    const double nc = rr_fro(C);
-    if (nc > 0.0) {
-      const double w = rr_fro(X) / nc;
-      for (int q = 0; q < 9; ++q) X[q] = X[q] + w * C[q];
-    }
-  }
-  if (!rr_polar(X)) {
-    for (int q = 0; q < 9; ++q) out[q] = (q % 4 == 0) ? 1.0 : 0.0;
-    return;
-  }
-  double C[9];
-  rr_cof(X, C);
-  const double det = X[0] * C[0] + X[3] * C[3] + X[6] * C[6];
-  const double sgn = det < 0.0 ? -1.0 : 1.0;
-  for (int q = 0; q < 9; ++q) out[q] = sgn * X[q];
+  pose::rotation_between(k, &s.sample[0][0], &s.sample[0][3], 6, out);
 }
 
 // ---- the whole CTA ----------------------------------------------------------------------------------------
@@ -336,10 +165,8 @@ __global__ void __launch_bounds__(RR_THREADS) rr_ransac(RrArgs a, int staged) {
   int* best_rows = a.best_rows + off;
   const double t = a.ransac_threshold;
   if (threadIdx.x == 0) {
-    s.cursor = 0;
-    s.mt_live = 0;
+    s.st.reset();
     s.best_count = 0;
-    s.trace_n = 0;
     s.stop = 0;
     for (int k = 0; k < 9; ++k) s.best[k] = 0.0;
   }
@@ -347,7 +174,7 @@ __global__ void __launch_bounds__(RR_THREADS) rr_ransac(RrArgs a, int staged) {
 
   for (int it = 0; it < a.iterations; ++it) {
     if (threadIdx.x == 0) {
-      rr_sample(s, a, pair, RR_MIN_SAMPLE, n);
+      stream_sample(s.st, a.src, pair, RR_MIN_SAMPLE, n, s.idx);
       for (int k = 0; k < RR_MIN_SAMPLE; ++k) rows.get(s.idx[k], &s.sample[k][0], &s.sample[k][3]);
       rr_rotation(s, RR_MIN_SAMPLE, s.cand);
     }
@@ -367,7 +194,7 @@ __global__ void __launch_bounds__(RR_THREADS) rr_ransac(RrArgs a, int staged) {
           if (threadIdx.x == 0) {
             const int m = s.best_count;
             const int size = max(min(RR_MAX_SAMPLE, (int)(m * 0.5)), RR_MIN_SAMPLE);
-            rr_sample(s, a, pair, size, m);
+            stream_sample(s.st, a.src, pair, size, m, s.idx);
             for (int k = 0; k < size; ++k) rows.get(best_rows[s.idx[k]], &s.sample[k][0], &s.sample[k][3]);
             rr_rotation(s, size, s.cand);
           }
@@ -385,9 +212,7 @@ __global__ void __launch_bounds__(RR_THREADS) rr_ransac(RrArgs a, int staged) {
       }
     }
     if (threadIdx.x == 0) {
-      const double ratio = (double)s.best_count / n;
-      const double p1 = fmin(1.0 - DBL_EPSILON, 1.0 - pow(ratio, 3.0));
-      s.stop = log(1.0 - RR_PROBABILITY) / log(p1) < (double)it;
+      s.stop = ransac_should_stop(s.best_count, n, it);
     }
     __syncthreads();
     if (s.stop) break;
@@ -417,40 +242,25 @@ __global__ void __launch_bounds__(RR_THREADS) rr_ransac(RrArgs a, int staged) {
     a.ransac_inliers[pair] = s.best_count;
     for (int r = 0; r < 3; ++r)
       for (int k = 0; k < 3; ++k) a.lo_model[9LL * pair + r * 3 + k] = Q[k * 3 + r];
-    if (a.trace) {
-      a.trace_count[pair] = s.trace_n;
-      a.stream_used[pair] = s.cursor;
+    if (a.src.trace) {
+      a.trace_count[pair] = s.st.trace_n;
+      a.stream_used[pair] = s.st.cursor;
     }
   }
 }
 
 struct RotRansac : DeviceStream<2> {
   bool timed = false;
-  long long prefix_len = 0, prefix_want = RR_DEFAULT_PREFIX;
   int trace_cap = 0;
   long long P = 0;
 
-  DevBuf<uint32_t> d_prefix;
-  DevBuf<Mt> d_saved;
+  StreamPrefix prefix;
   DevBuf<double> d_bearings, d_lo;
   DevBuf<long long> d_pair_start, d_row_a, d_row_b, d_stream_used;
   DevBuf<int> d_order, d_best_rows, d_ransac, d_chord, d_trace, d_trace_count;
   DevBuf<unsigned char> d_mask;
 
   explicit RotRansac(int dev) : DeviceStream(dev) {}
-
-  // the first prefix_want outputs of mt19937(42) and the generator after them
-  void make_prefix() {
-    if (prefix_len == prefix_want) return;
-    auto mt = std::make_unique<Mt>();
-    mt->seed(42u);
-    std::vector<uint32_t> h((size_t)prefix_want);
-    for (auto& v : h) v = mt->next();
-    upload(d_prefix, h.data(), h.size());
-    upload(d_saved, mt.get(), 1);
-    OSFM_CUDA(cudaStreamSynchronize(stream));
-    prefix_len = prefix_want;
-  }
 
   void run(int64_t num_bearings, const double* bearings, int64_t num_pairs, const int64_t* pair_start,
            const int64_t* row_a, const int64_t* row_b, double threshold, int iterations, double* lo_model,
@@ -486,7 +296,7 @@ void RotRansac::run(int64_t num_bearings, const double* bearings, int64_t num_pa
     timed = false;
     return;
   }
-  make_prefix();
+  prefix.make(stream);
 
   // largest pairs first; the pairs too large for shared memory form their own launch
   std::vector<int> order((size_t)num_pairs);
@@ -522,18 +332,14 @@ void RotRansac::run(int64_t num_bearings, const double* bearings, int64_t num_pa
   a.chord_threshold = threshold;
   a.ransac_threshold = 1.0 - std::cos(threshold);
   a.iterations = iterations;
-  a.prefix = d_prefix.p;
-  a.prefix_len = prefix_len;
-  a.saved = d_saved.p;
+  a.src = prefix.source(trace_cap > 0 ? d_trace.p : nullptr, trace_cap);
   a.best_rows = d_best_rows.p;
   a.lo_model = d_lo.p;
   a.ransac_inliers = d_ransac.p;
   a.chord_inliers = d_chord.p;
   a.chord_mask = d_mask.p;
-  a.trace = trace_cap > 0 ? d_trace.p : nullptr;
   a.trace_count = d_trace_count.p;
   a.stream_used = d_stream_used.p;
-  a.trace_cap = trace_cap;
 
   OSFM_CUDA(cudaEventRecord(ev[0], stream));
   if (big > 0) {
@@ -584,7 +390,7 @@ int osfm_rotransac_run(osfm_rotransac* h, int64_t num_bearings, const double* be
 int osfm_rotransac_set_stream_prefix(osfm_rotransac* h, int64_t length) {
   return osfm::with_handle(h, [&](osfm::RotRansac& K) {
     if (length < 1 || length > (1LL << 28)) throw osfm::ArgError("stream prefix length must be in [1, 2^28]");
-    K.prefix_want = length;
+    K.prefix.want = length;
   });
 }
 

@@ -17,10 +17,12 @@ from . import types as T
 
 
 class Measurement:
-    """pymap.ShotMeasurementDouble / Vec3d: an optional value (has_value / value / reset)."""
+    """pymap.ShotMeasurementDouble / Vec3d (and, with `kind` int or str, ShotMeasurementInt / String): an optional
+    value (has_value / value / reset)."""
 
-    def __init__(self):
+    def __init__(self, kind=None):
         self._v = None
+        self._kind = kind
 
     @property
     def has_value(self) -> bool:
@@ -32,7 +34,10 @@ class Measurement:
 
     @value.setter
     def value(self, v) -> None:
-        self._v = np.asarray(v, dtype=np.float64).copy() if np.ndim(v) else float(v)
+        if self._kind is not None:
+            self._v = self._kind(v)
+        else:
+            self._v = np.asarray(v, dtype=np.float64).copy() if np.ndim(v) else float(v)
 
     def reset(self) -> None:
         self._v = None
@@ -46,6 +51,10 @@ class ShotMeasurements:
         self.compass_accuracy = Measurement()
         self.gravity_down = Measurement()
         self.capture_time = Measurement()
+        self.opk_angles = Measurement()
+        self.opk_accuracy = Measurement()
+        self.orientation = Measurement(int)
+        self.sequence_key = Measurement(str)
 
 
 class Depth:
@@ -100,6 +109,10 @@ class RigInstance:
         self.rig_cameras[shot.id] = rig_camera
         shot.rig_instance = self
         shot.rig_camera = rig_camera
+
+    def update_instance_pose_with_shot(self, shot_id: str, shot_pose: T.Pose) -> None:
+        """Moves the instance so that shot `shot_id` has pose `shot_pose` (RigInstance::UpdateInstancePoseWithShot)."""
+        self.shots[shot_id].pose._assign(shot_pose)
 
 
 class _ShotPose:

@@ -29,6 +29,17 @@ and the triangulation of tracks after each shot the incremental loop adds, from 
 
   triangulate_shot_features               reconstruction.py:1143-1183
   retriangulate                           reconstruction.py:1186-1226
+
+and the resection of the incremental loop, batched over every candidate image by the absolute-pose RANSAC of
+opensfm_b200/resection.py:
+
+  reconstructed_points_for_images         reconstruction.py:677-692  (ties in the order of tracks_manager.images)
+  add_shot                                reconstruction.py:247-285
+  resect                                  reconstruction.py:695-762
+  resect_candidates                       the inner `for image, _ in candidates` loop of grow_reconstruction
+                                          (:1495-1575): every candidate in one launch, the first success applied
+  exif_to_metadata, get_image_metadata    reconstruction_helpers.py:129-185
+  rig_assignments_per_image               rig.py:39-52
 """
 from __future__ import annotations
 
@@ -39,8 +50,10 @@ from typing import Any, Dict, Iterable, List, Optional, Sequence, Set, Tuple
 import numpy as np
 
 from . import bundle as _bundle
+from . import resection as _rs
 from . import rotation_ransac as _rr
 from . import types as T
+from .map_types import RigInstance, ShotMeasurements
 from .triangulation import retriangulate, triangulate_shot_features  # noqa: F401
 
 logger = logging.getLogger(__name__)
@@ -658,3 +671,183 @@ def compute_image_pairs_from_tracks(tracks_manager, cameras_by_image: Dict[Any, 
     res = _rr.ransac_pairs(bearings, pair_start, row_a, row_b, 4 * config["five_point_algo_threshold"])
     keys = [(images[a], images[b]) for a, b in zip(pa[kept].tolist(), pb[kept].tolist())]
     return _ranked_by_argsort(keys, res.scores())
+
+
+# ---------------------------------------------------------------------------------------------------------------
+# resection (reconstruction.py:247-285, 677-762; reconstruction_helpers.py:129-185; rig.py:39-52)
+# ---------------------------------------------------------------------------------------------------------------
+MAXIMUM_ALTITUDE = 1e4   # opensfm.exif.maximum_altitude
+RESECTION_MIN_ROWS = 5   # resect rejects a candidate with fewer common points before RANSAC
+
+_last_resect_times: Dict[str, float] = {}
+
+
+def rig_assignments_per_image(rig_assignments: Dict[str, List[Tuple[str, str]]]) -> Dict[str, Tuple[str, str, List[str]]]:
+    """{image: (instance id, rig camera id, the instance's images)} of {instance id: [(image, rig camera id)]}."""
+    out = {}
+    for instance_id, instance in rig_assignments.items():
+        instance_shots = [s[0] for s in instance]
+        for shot_id, rig_camera_id in instance:
+            out[shot_id] = (f"{instance_id}", rig_camera_id, instance_shots)
+    return out
+
+
+def exif_to_metadata(exif: Dict[str, Any], use_altitude: bool, reference) -> ShotMeasurements:
+    """Shot metadata from the EXIF dict: GPS position (topocentric, through `reference.to_topocentric`) and accuracy,
+    OPK angles and accuracy, orientation, gravity down, compass angle and accuracy, capture time, sequence key."""
+    metadata = ShotMeasurements()
+    gps = exif.get("gps")
+    if gps and "latitude" in gps and "longitude" in gps:
+        lat, lon = gps["latitude"], gps["longitude"]
+        alt = min([MAXIMUM_ALTITUDE, gps.get("altitude", 2.0)]) if use_altitude else 2.0
+        x, y, z = reference.to_topocentric(lat, lon, alt)
+        metadata.gps_position.value = np.array([x, y, z])
+        metadata.gps_accuracy.value = gps.get("dop", 15.0)
+        if metadata.gps_accuracy.value == 0.0:
+            metadata.gps_accuracy.value = 15.0
+    opk = exif.get("opk")
+    if opk and "omega" in opk and "phi" in opk and "kappa" in opk:
+        metadata.opk_angles.value = np.array([opk["omega"], opk["phi"], opk["kappa"]])
+        metadata.opk_accuracy.value = opk.get("accuracy", 1.0)
+    metadata.orientation.value = exif.get("orientation", 1)
+    if "accelerometer" in exif:
+        logger.warning("'accelerometer' EXIF tag is deprecated in favor of 'gravity_down', which expresses the gravity "
+                       "down direction in the image coordinate frame.")
+    if "gravity_down" in exif:
+        metadata.gravity_down.value = exif["gravity_down"]
+    if "compass" in exif:
+        metadata.compass_angle.value = exif["compass"]["angle"]
+        if exif["compass"].get("accuracy") is not None:
+            metadata.compass_accuracy.value = exif["compass"]["accuracy"]
+    if "capture_time" in exif:
+        metadata.capture_time.value = exif["capture_time"]
+    if "skey" in exif:
+        metadata.sequence_key.value = exif["skey"]
+    return metadata
+
+
+def get_image_metadata(data, image: str) -> ShotMeasurements:
+    return exif_to_metadata(data.load_exif(image), data.config["use_altitude_tag"], data.load_reference())
+
+
+def add_shot(data, reconstruction, rig_assignments: Dict[str, Tuple[str, str, List[str]]], shot_id: str,
+             pose: T.Pose) -> Set[str]:
+    """Adds a shot with the given pose; a shot of a rig brings its whole rig instance, placed so that the shot has
+    that pose.  Returns the ids of the shots added."""
+    if shot_id not in rig_assignments:
+        shot = reconstruction.create_shot(shot_id, data.load_exif(shot_id)["camera"], pose)
+        shot.metadata = get_image_metadata(data, shot_id)
+        return {shot_id}
+    instance_id, _, instance_shots = rig_assignments[shot_id]
+    rig_instance = reconstruction.add_rig_instance(RigInstance(instance_id))
+    for shot in instance_shots:
+        _, rig_camera_id, _ = rig_assignments[shot]
+        created = reconstruction.create_shot(shot, data.load_exif(shot)["camera"], T.Pose(), rig_camera_id,
+                                             instance_id)
+        created.metadata = get_image_metadata(data, shot)
+    rig_instance.update_instance_pose_with_shot(shot_id, pose)
+    return set(instance_shots)
+
+
+def _point_tracks(tracks_manager, reconstruction) -> Tuple[np.ndarray, np.ndarray]:
+    """(per track: is a point of the reconstruction, its coordinates); a point's id is its track id."""
+    T_ = tracks_manager.num_tracks()
+    is_point = np.zeros(T_, dtype=bool)
+    coords = np.zeros((T_, 3), dtype=np.float64)
+    for point_id, lm in reconstruction.points.items():
+        t = int(point_id) if isinstance(point_id, str) and point_id.isdigit() else -1
+        if 0 <= t < T_ and str(t) == point_id:
+            is_point[t] = True
+            coords[t] = lm.coordinates
+    return is_point, coords
+
+
+def reconstructed_points_for_images(tracks_manager, reconstruction, images) -> List[Tuple[Any, int]]:
+    """(image, reconstructed points it sees) of the images not in the reconstruction, by decreasing count; ties in
+    the order of tracks_manager.images (the reference's follow a set's iteration order)."""
+    images = set(images)
+    is_point = _point_tracks(tracks_manager, reconstruction)[0]
+    seen = is_point[tracks_manager.obs_track]
+    counts = np.bincount(tracks_manager.obs_image[seen], minlength=len(tracks_manager.images))
+    has_obs = np.diff(tracks_manager._shot_order()[1]) > 0
+    keep = [i for i, im in enumerate(tracks_manager.images)
+            if im in images and im not in reconstruction.shots and has_obs[i]]
+    keep.sort(key=lambda i: -counts[i])
+    return [(tracks_manager.images[i], int(counts[i])) for i in keep]
+
+
+def resect_candidates(data, tracks_manager, reconstruction, candidates, threshold: float, min_inliers: int
+                      ) -> Tuple[Optional[Any], Set[str], Optional[Dict[str, Any]], List[Dict[str, Any]]]:
+    """Resects every candidate image (ids, or (id, count) pairs as reconstructed_points_for_images returns) in one
+    launch and adds the first one, in candidate order, with at least min_inliers chord inliers, exactly as
+    `resect` called on the candidates one after another would: a failed resection changes nothing.  Returns (that
+    image or None, the shots added, its report, the report of every candidate)."""
+    t0 = time.perf_counter()
+    images = [c[0] if isinstance(c, tuple) else c for c in candidates]
+    rig_assignments = rig_assignments_per_image(data.load_rig_assignments())
+    is_point, coords = _point_tracks(tracks_manager, reconstruction)
+    order, start = tracks_manager._shot_order()
+    xy = tracks_manager._points()[0]
+    index = {im: i for i, im in enumerate(tracks_manager.images)}
+    rows_of, bearings_of = [], []
+    for im in images:
+        i = index[im]
+        rows = order[start[i]:start[i + 1]]
+        rows = rows[is_point[tracks_manager.obs_track[rows]]]
+        camera = reconstruction.cameras[data.load_exif(im)["camera"]]
+        rows_of.append(rows)
+        bearings_of.append(camera.pixel_bearing_many(xy[rows]) if len(rows) else np.zeros((0, 3)))
+    t1 = time.perf_counter()
+    launched = [k for k, r in enumerate(rows_of) if len(r) >= RESECTION_MIN_ROWS]
+    bs = [bearings_of[k] for k in launched]
+    Xs = [coords[tracks_manager.obs_track[rows_of[k]]] for k in launched]
+    packed = _rs.pack_lists(bs, Xs)
+    t2 = time.perf_counter()
+    res = _rs.ransac_shots(*packed, threshold) if launched else None
+    t3 = time.perf_counter()
+
+    reports: List[Dict[str, Any]] = [{"num_common_points": len(r)} for r in rows_of]
+    chosen = None
+    poses = res.poses() if res is not None else None
+    for s, k in enumerate(launched):
+        reports[k]["num_inliers"] = int(res.chord_inliers[s])
+        if chosen is None and res.chord_inliers[s] >= min_inliers:
+            chosen = (s, k)
+    new_shots: Set[str] = set()
+    if chosen is not None:
+        s, k = chosen
+        shot_id, rows = images[k], rows_of[k]
+        Tp = poses[s]
+        R = Tp[:, :3].T
+        pose = T.Pose()
+        pose.set_rotation_matrix(R)
+        pose.translation = -R.dot(Tp[:, 3])
+        assert shot_id not in reconstruction.shots
+        new_shots = add_shot(data, reconstruction, rig_assignments, shot_id, pose)
+        if shot_id in rig_assignments:
+            triangulate_shot_features(tracks_manager, reconstruction, new_shots, data.config)
+        ids = tracks_manager._track_ids()
+        for r in rows[res.inliers(s)].tolist():
+            reconstruction.add_observation(shot_id, ids[tracks_manager.obs_track[r]], tracks_manager._observation(r))
+        reports[k]["shots"] = list(new_shots)
+    t4 = time.perf_counter()
+    _last_resect_times.clear()
+    _last_resect_times.update(bearings=t1 - t0, packing=t2 - t1, device_call=t3 - t2, map_writes=t4 - t3,
+                              device_ms=_rs.last_device_ms() if launched else 0.0)
+    if chosen is None:
+        return None, set(), None, reports
+    return images[chosen[1]], new_shots, reports[chosen[1]], reports
+
+
+def last_resect_times() -> Dict[str, float]:
+    """Host seconds of the last resect_candidates / resect call, by part (bearings, packing, device_call,
+    map_writes), and the kernel's device milliseconds (device_ms)."""
+    return dict(_last_resect_times)
+
+
+def resect(data, tracks_manager, reconstruction, shot_id: str, threshold: float, min_inliers: int
+           ) -> Tuple[bool, Set[str], Dict[str, Any]]:
+    """Tries resecting and adding one shot: (success, shots added, report), the reference's signature and report."""
+    image, new_shots, _, reports = resect_candidates(data, tracks_manager, reconstruction, [shot_id], threshold,
+                                                     min_inliers)
+    return image is not None, new_shots, reports[0]
