@@ -18,8 +18,8 @@
  *
  * There is no CPU fallback: every call needs a CUDA device (H100, sm_90a).
  *
- * Handles (osfm_matcher, osfm_ba, osfm_tracks, osfm_rotransac, osfm_resect) own a CUDA stream and workspaces on the
- * device they were created on, and every call on a handle makes that device current on the calling thread.  Calls on one handle
+ * Handles (osfm_matcher, osfm_ba, osfm_tracks, osfm_rotransac, osfm_resect, osfm_relpose) own a CUDA stream and
+ * workspaces on the device they were created on, and every call on a handle makes that device current on the calling thread.  Calls on one handle
  * are serialised and may come from any thread; calls on different handles do not wait for each other.  A callback
  * (today only the all-reduce of osfm_ba_set_distributed) must not call into the handle that called it.
  */
@@ -545,6 +545,35 @@ int osfm_resect_last_device_ms(osfm_resect* h, float* ms);
 int osfm_resect_set_stream_prefix(osfm_resect* h, int64_t length);
 int osfm_resect_set_trace(osfm_resect* h, int capacity);
 int osfm_resect_get_trace(osfm_resect* h, int32_t* count, int64_t* stream_used, int32_t* indices);
+
+/* ------------------------------------------------------------------------
+ * FIVE-POINT RELATIVE-POSE RANSAC OF IMAGE PAIRS
+ * ---------------------------------------------------------------------- */
+typedef struct osfm_relpose osfm_relpose;
+
+/* Estimates the relative pose of image pairs: pyrobust's ransac_relative_pose with RANSAC scoring (five-point
+ * samples, EssentialNPoints in local optimisation), as two_view_reconstruction_general runs it through
+ * multiview.relative_pose_ransac, for many pairs at once.  The rules, including the deliberate differences, are
+ * stated in oracle/relative_pose_oracle.py.  A handle owns one CUDA stream, its workspaces on `device` and the shared
+ * sample stream of mt19937(42). */
+int osfm_relpose_create(int device, osfm_relpose** out);
+int osfm_relpose_destroy(osfm_relpose* h);
+/* bearings: num_bearings x 3 fp64 (normalised on the device).  Pair p owns rows [pair_start[p], pair_start[p + 1])
+ * (pair_start[0] = 0); row r pairs bearing row_a[r] of the first image with bearing row_b[r] of the second.
+ * threshold is an angle: inliers have |1 - (px . x + py . y) / 2| below 1 - cos(threshold), px and py the midpoint
+ * of the row seen from both cameras.  iterations >= 1 (two_view_reconstruction_general passes 1000).  Outputs:
+ * lo_model (12 per pair: [R | t] row-major, x2 = R x1 + t, |t| = 1), the RANSAC inlier count of every pair and the
+ * inlier mask of lo_model over every row.  A pair of fewer than 5 rows, or a row naming a bearing outside the table,
+ * fails with OSFM_ERR_ARG naming it. */
+int osfm_relpose_run(osfm_relpose* h, int64_t num_bearings, const double* bearings, int64_t num_pairs,
+                     const int64_t* pair_start, const int64_t* row_a, const int64_t* row_b, double threshold,
+                     int iterations, double* lo_model, int32_t* ransac_inliers, uint8_t* inlier_mask);
+/* Device time of the last osfm_relpose_run (CUDA events around its kernels, after the uploads). */
+int osfm_relpose_last_device_ms(osfm_relpose* h, float* ms);
+/* Test hooks, as osfm_rotransac_set_stream_prefix / set_trace / get_trace, per pair. */
+int osfm_relpose_set_stream_prefix(osfm_relpose* h, int64_t length);
+int osfm_relpose_set_trace(osfm_relpose* h, int capacity);
+int osfm_relpose_get_trace(osfm_relpose* h, int32_t* count, int64_t* stream_used, int32_t* indices);
 
 #ifdef __cplusplus
 }

@@ -13,7 +13,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIBDIR = os.path.join(HERE, "lib")
 LIB = os.path.join(LIBDIR, "libopensfm_b200.so")
-SOURCES = ["core.cu", "match.cu", "match_tc.cu", "words.cu", "vlad.cu", "bow.cu", "tracks.cu", "triangulate.cu", "rotransac.cu", "resect.cu", "ba.cu"]
+SOURCES = ["core.cu", "match.cu", "match_tc.cu", "words.cu", "vlad.cu", "bow.cu", "tracks.cu", "triangulate.cu", "rotransac.cu", "resect.cu", "relpose.cu", "ba.cu"]
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = ARCH + [ "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "-ccbin", "/usr/bin/g++"]

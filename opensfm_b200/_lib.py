@@ -172,6 +172,14 @@ SIGNATURES = {
     "osfm_resect_set_stream_prefix": (c_int, [c_void_p, c_int64]),
     "osfm_resect_set_trace": (c_int, [c_void_p, c_int]),
     "osfm_resect_get_trace": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p]),
+    "osfm_relpose_create": (c_int, [c_int, POINTER(c_void_p)]),
+    "osfm_relpose_destroy": (c_int, [c_void_p]),
+    "osfm_relpose_run": (c_int, [c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_double, c_int,
+                                 c_void_p, c_void_p, c_void_p]),
+    "osfm_relpose_last_device_ms": (c_int, [c_void_p, POINTER(c_float)]),
+    "osfm_relpose_set_stream_prefix": (c_int, [c_void_p, c_int64]),
+    "osfm_relpose_set_trace": (c_int, [c_void_p, c_int]),
+    "osfm_relpose_get_trace": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p]),
 }
 
 _lib = None
@@ -209,7 +217,7 @@ def ptr(a: Optional[np.ndarray]) -> Optional[ctypes.c_void_p]:
 
 class Handle:
     """One engine object of the C ABI, `osfm_<kind>_create(device)` .. `osfm_<kind>_destroy`, with kind one of "ba",
-    "matcher", "tracks", "rotransac" and "resect".  It keeps its stream and device workspaces between calls.  The
+    "matcher", "tracks", "rotransac", "resect" and "relpose".  It keeps its stream and device workspaces between calls.  The
     library serialises calls on one handle, so callers that should not wait for one another use handles of their own."""
 
     def __init__(self, kind: str, device: int = 0):

@@ -1,7 +1,7 @@
 // The sample stream of pyrobust's RANSAC (robust/random_sampler.h, robust_estimator.h), shared by the batched
-// estimators (rotransac.cu, resect.cu): a std::mt19937 seeded with 42 and restarted for every problem, indices drawn
-// by libstdc++'s uniform_int_distribution, repeats in a sample drawn again, and the ShouldStop bound.  The
-// restatement these follow is oracle/rotation_ransac_oracle.py.
+// estimators (rotransac.cu, resect.cu, relpose.cu): a std::mt19937 seeded with 42 and restarted for every problem,
+// indices drawn by libstdc++'s uniform_int_distribution, repeats in a sample drawn again, and the ShouldStop bound.
+// The restatement these follow is oracle/rotation_ransac_oracle.py.
 //
 // Every problem consumes the same stream from its start, so a prefix of it is made once per handle and kept on the
 // device (StreamPrefix); a problem that reaches its end continues from the generator state saved after the prefix,
@@ -114,10 +114,10 @@ __device__ inline void stream_sample(StreamState& s, const StreamSource& a, int 
   }
 }
 
-// ShouldStop with 3-row minimal samples: stop once log(1 - p) / log(min(1 - eps, 1 - ratio^3)) < iteration
-__device__ inline bool ransac_should_stop(int best_inliers, int n, int iteration) {
+// ShouldStop with `minimal`-row samples: stop once log(1 - p) / log(min(1 - eps, 1 - ratio^minimal)) < iteration
+__device__ inline bool ransac_should_stop(int best_inliers, int n, int iteration, int minimal = 3) {
   const double ratio = (double)best_inliers / n;
-  const double p1 = fmin(1.0 - DBL_EPSILON, 1.0 - pow(ratio, 3.0));
+  const double p1 = fmin(1.0 - DBL_EPSILON, 1.0 - pow(ratio, (double)minimal));
   return log(1.0 - RANSAC_PROBABILITY) / log(p1) < (double)iteration;
 }
 
