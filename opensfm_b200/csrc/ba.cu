@@ -1923,7 +1923,7 @@ void BA::linearize(int b, bool timed) {
     ba_prior_colnorm_grad<<<grid_for(npr_local, 128), 128, 0, stream>>>(rs.pv, params_of(b), d_colnorm2.p, d_grad.p);
     OSFM_LAUNCH_CHECK();
   }
-  if (NT > 0) {   // every rank keeps the terms' Jacobians (the system part is added after the all-reduce)
+  if (NT > 0) {   // every rank keeps the terms' Jacobians (rank 0 adds the system part, before the all-reduce)
     side_linearize<<<NT, SIDE_THREADS, 0, stream>>>(rs.sv, rs.v, rs.bm, params_of(b), d_sc.p, rs.add_priors ? 1 : 0);
     OSFM_LAUNCH_CHECK();
     if (rs.add_priors) {
@@ -2039,10 +2039,17 @@ void BA::build_system(const double* diag, double inv_radius, int* rank_flag, boo
     if (timed) lm_phase(LM_PH_SCHUR, -1);
   }
   if (nc > 0) {
+    // the side terms' blocks: rank 0 adds them to its partial system before the exchange.  Several terms add to one
+    // entry with atomics, in an order that changes from run to run; added on every rank after the exchange, they left
+    // each rank with a slightly different system and the ranks' camera sides apart by a few 1e-12.
+    if (rs.NT > 0 && rs.add_priors) {
+      side_system<<<rs.NT, SIDE_THREADS, 0, stream>>>(rs.sv, rs.v, rs.bm, params_of(0), rs.bsr, d_scale.p, d_S_p, d_rhs_p);
+      OSFM_LAUNCH_CHECK();
+    }
     // the one exchange step of the LM iteration: sum of the partial reduced systems over ranks
     if (world > 1) allreduce_dev(d_Sbuf.p, (long long)rs.nc_pad + rs.s_upper_total);  // rhs + upper blocks, one call
-    // S_g stays a pure partial sum through the all-reduce; every rank then adds the (replicated)
-    // prior rows and the damping to its copy of the reduced system.
+    // every rank then adds the (replicated) prior rows, one addition per entry, and the damping to its copy of the
+    // reduced system: the copies stay identical.
     PriorView pall = rs.pv;
     pall.n_cam_rows = (int)rs.pr_cam_param.size();
     pall.n_pos_rows = (int)rs.pr_pos_inst.size();
@@ -2050,10 +2057,6 @@ void BA::build_system(const double* diag, double inv_radius, int* rank_flag, boo
     if (nall > 0) {
       ba_prior_system<<<grid_for(nall, 128), 128, 0, stream>>>(pall, params_of(0), d_scale.p, d_prior_diag_off.p,
                                                               d_S_p, d_rhs_p);
-      OSFM_LAUNCH_CHECK();
-    }
-    if (rs.NT > 0) {
-      side_system<<<rs.NT, SIDE_THREADS, 0, stream>>>(rs.sv, rs.v, rs.bm, params_of(0), rs.bsr, d_scale.p, d_S_p, d_rhs_p);
       OSFM_LAUNCH_CHECK();
     }
     ba_finish_system<<<grid_for((long long)rs.n_upper * 32, 256), 256, 0, stream>>>(d_upper.p, rs.n_upper, rs.bsr, d_S_p,
@@ -2510,7 +2513,8 @@ void BA::run() {
   if (!(fallbacks & OSFM_BA_FALLBACK_UNDEFLATED_PCG) && rs.pcg_pipe_ok && rs.NI > 0 && nc > 0) {
     d_Wdef.reserve((size_t)PCG_ND * nc);
     OSFM_CUDA(cudaMemsetAsync(d_Wdef.p, 0, sizeof(double) * PCG_ND * (size_t)nc, stream));
-    pcg_gauge_vectors<<<grid_for(rs.NI, 128), 128, 0, stream>>>(rs.NI, d_inst_poff.p, params_of(0).inst, d_scale.p, nc, d_Wdef.p);
+    pcg_gauge_vectors<<<grid_for(rs.NI, 128), 128, 0, stream>>>(rs.NI, d_inst_poff.p, params_of(0).inst, d_colnorm2.p,
+                                                                    d_scale.p, nc, d_Wdef.p);
     OSFM_LAUNCH_CHECK();
     rs.pcg_pipe.Wdef = d_Wdef.p;
   }

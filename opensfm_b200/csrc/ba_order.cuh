@@ -92,9 +92,16 @@ __global__ void ord_signatures(const unsigned long long* __restrict__ keys, cons
   const long long b = g_start[p], e = g_start[p + 1];
   // pt_const: bit 0 = constant point, bit 1 = the point has a prior (kept off the segment path: only the
   // per-point kernel ba_schur adds prior rows to V_p / g_p)
-  unsigned long long h = 1469598103934665603ULL ^ (unsigned long long)((pt_const[p] & 1) ? 1 : 0);
+  unsigned long long h = 1469598103934665603ULL;
   for (long long j = b; j < e; ++j) {
     h ^= (keys[j] & 0xffffffffULL) + 0x9e3779b97f4a7c15ULL;
+    h *= 1099511628211ULL;
+  }
+  // the constant flag hashes as one more element of the list, 2^32, which no shot index takes.  (Folded into the
+  // initial value instead, it cancelled against the first shot: a constant point seen by shots (1, ...) hashed like
+  // a free point seen by (2, ...), and the two groups split each other's runs into more segments.)
+  if (pt_const[p] & 1) {
+    h ^= (1ULL << 32) + 0x9e3779b97f4a7c15ULL;
     h *= 1099511628211ULL;
   }
   const long long k = e - b;

@@ -1595,11 +1595,18 @@ struct PcgPipe {   // the layout of plan_pcg_pipelined (ba_pcg_plan.h)
 // When nothing fixes the gauge these seven directions carry the smallest eigenvalues of the reduced system
 // (only the LM damping acts on them); with priors / fixed shots they are ordinary vectors and deflating them is harmless.
 __global__ void pcg_gauge_vectors(int NI, const int* __restrict__ inst_poff, const double* __restrict__ inst,
-                                  const double* __restrict__ scale, int nc, double* __restrict__ W) {
+                                  const double* __restrict__ colnorm2, const double* __restrict__ scale, int nc,
+                                  double* __restrict__ W) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= NI) return;
   const int c0 = inst_poff[i];
   if (c0 < 0) return;
+  // an instance no residual uses (empty columns) has no gauge: its rows of the reduced system hold the LM damping
+  // only, so a deflation component there would reach its step unchecked.  Ceres drops such a block from the problem
+  // and leaves it as given; with zero rows here its step is exactly 0.
+  bool used = false;
+  for (int j = 0; j < 6; ++j) used |= colnorm2[c0 + j] != 0.0;
+  if (!used) return;
   const double r[3] = {inst[6 * (size_t)i], inst[6 * (size_t)i + 1], inst[6 * (size_t)i + 2]};
   const double t[3] = {inst[6 * (size_t)i + 3], inst[6 * (size_t)i + 4], inst[6 * (size_t)i + 5]};
   // J_l^-1 = I - K / 2 + g K^2,  K = [r]x,  g = 1 / th^2 - (1 + cos th) / (2 th sin th)

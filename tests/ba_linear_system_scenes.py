@@ -224,6 +224,66 @@ def fixed_instances():
     return pb
 
 
+def _keep_observations(pb, keep):
+    pb.obs_shot, pb.obs_point = pb.obs_shot[keep], pb.obs_point[keep]
+    pb.obs_xy, pb.obs_sigma = pb.obs_xy[keep], pb.obs_sigma[keep]
+    return pb
+
+
+def pipe_long_runs():
+    """4 cameras that all see all 400 points; 64 points (at random places of the point list) lose shot 3 and 65 lose
+    shot 2: runs of 64, 65 and 271 identical shot lists, cut into 1, 2 and 5 segments of ba_schur_pipe."""
+    pb = cube(4, 400)
+    rng = np.random.RandomState(11)
+    order = rng.permutation(len(pb.points))
+    drop = np.full(len(pb.points), -1)
+    drop[order[:64]], drop[order[64:129]] = 3, 2
+    return _keep_observations(pb, pb.obs_shot != drop[pb.obs_point])
+
+
+def pipe_k_edge():
+    """12 perspective cameras (wc = 9); 150 points keep 10 of their 12 shots (90 camera-side columns: segments of
+    ba_schur_pipe) and 150 keep 11 (99 > 96: the per-point ba_schur), on one solve."""
+    pb = cube(12, 300)
+    rng = np.random.RandomState(12)
+    keep = np.zeros(len(pb.obs_shot), dtype=bool)
+    for p in range(len(pb.points)):
+        mine = np.nonzero(pb.obs_point == p)[0]
+        keep[rng.choice(mine, 10 if p % 2 else 11, replace=False)] = True
+    return _keep_observations(pb, keep)
+
+
+def unobserved_and_idle():
+    """A cube scene with 20 free points that no shot observes, at random places of the point list, and a shot whose
+    rig instance (free, no prior) is used by nothing else and which observes nothing, in the middle of the shot and
+    instance lists.  Their parameter blocks appear in no residual (see test_ba_input_order_gpu.py)."""
+    pb = cube(10, 500, max_obs=6)
+    rng = np.random.RandomState(13)
+    P, extra = len(pb.points), 20
+    idle = np.sort(rng.choice(P + extra, extra, replace=False))
+    observed = np.setdiff1d(np.arange(P + extra), idle)
+    pts = np.zeros((P + extra, 3))
+    pts[observed] = pb.points
+    pts[idle] = rng.uniform(-0.5, 0.5, (extra, 3))
+    pb.points, pb.point_const = pts, np.zeros(P + extra, dtype=np.int32)
+    pb.obs_point = observed[pb.obs_point].astype(np.int32)
+    # the idle instance at index 3, its shot at index 4 (camera 0)
+    ins, sh = 3, 4
+    pb.inst = np.insert(pb.inst, ins, pb.inst[ins] + rng.normal(0, 0.05, 6), axis=0)
+    pb.inst_const = np.insert(pb.inst_const, ins, 0)
+    pb.inst_has_prior = np.insert(pb.inst_has_prior, ins, 0)
+    pb.inst_prior_pos = np.insert(pb.inst_prior_pos, ins, 0.0, axis=0)
+    pb.inst_prior_std = np.insert(pb.inst_prior_std, ins, 1.0, axis=0)
+    shot_inst = pb.shot_inst + (pb.shot_inst >= ins)
+    pb.shot_inst = np.insert(shot_inst, sh, ins).astype(np.int32)
+    pb.shot_cam = np.insert(pb.shot_cam, sh, 0).astype(np.int32)
+    pb.shot_rc = np.insert(pb.shot_rc, sh, 0).astype(np.int32)
+    pb.shot_use_rc = np.insert(pb.shot_use_rc, sh, 0).astype(np.int32)
+    pb.obs_shot = (pb.obs_shot + (pb.obs_shot >= sh)).astype(np.int32)
+    pb.validate()
+    return pb
+
+
 # name -> builder; CPU_SCENES are the ones the numpy restatement covers (all but side_terms, which has no simple numpy
 # restatement, and the two large cube scenes)
 SCENES = {
@@ -244,7 +304,11 @@ SCENES = {
     "huber_outliers": lambda: robust("HuberLoss"),
     "duplicate_observations": duplicate_observations,
     "fixed_instances": fixed_instances,
+    "pipe_long_runs": pipe_long_runs,
+    "pipe_k_edge": pipe_k_edge,
+    "unobserved_and_idle": unobserved_and_idle,
 }
 CPU_SCENES = ["pipe_few_chunks", "shared_intrinsics", "constant_blocks", "brown_simt_segments", "rig_free_rigcam_priors",
               "rig_segments", "spherical", "all_ten_models", "point_priors_many_obs", "camera_and_position_priors", "cauchy_outliers",
-              "huber_outliers", "duplicate_observations", "fixed_instances"]
+              "huber_outliers", "duplicate_observations", "fixed_instances", "pipe_long_runs", "pipe_k_edge",
+              "unobserved_and_idle"]

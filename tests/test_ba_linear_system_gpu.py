@@ -181,6 +181,9 @@ EXPECT = {
     "huber_outliers": dict(schur_kernel="pipe"),
     "duplicate_observations": dict(schur_kernel="pipe"),
     "fixed_instances": dict(schur_kernel="pipe", pcg_kernel="pipelined"),
+    "pipe_long_runs": dict(schur_kernel="pipe", wc=9, nres=2, nseg=8, p_slow=0),
+    "pipe_k_edge": dict(schur_kernel="pipe", wc=9, nres=2, p_fast=150, p_slow=150),
+    "unobserved_and_idle": dict(schur_kernel="pipe", wc=9, nres=2, p_slow=20),
 }
 
 

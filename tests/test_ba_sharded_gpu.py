@@ -72,7 +72,7 @@ def _single(name, max_iterations=None, fallbacks=HOST_LOOP):
 def _check_ranks(pb, world, ranks):
     """Every rank returns the same solve: identical points, reprojection errors and summary (but for the local
     observation count, which is that of its shard), camera side to 1e-12 (each rank solves its own copy of the
-    all-reduced system, and the side-term blocks are added with atomics after the exchange).  Returns that spread."""
+    all-reduced system).  Returns that spread."""
     r0 = ranks[0]
     owner = np.asarray(pb.obs_point) % world
     for r, res in enumerate(ranks):
