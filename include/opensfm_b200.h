@@ -568,8 +568,31 @@ int osfm_relpose_destroy(osfm_relpose* h);
 int osfm_relpose_run(osfm_relpose* h, int64_t num_bearings, const double* bearings, int64_t num_pairs,
                      const int64_t* pair_start, const int64_t* row_a, const int64_t* row_b, double threshold,
                      int iterations, double* lo_model, int32_t* ransac_inliers, uint8_t* inlier_mask);
-/* Device time of the last osfm_relpose_run (CUDA events around its kernels, after the uploads). */
+/* two_view_reconstruction_general's steps after the plane homography, for many pairs in one call: the RANSAC of
+ * osfm_relpose_run (same inputs, same checks, same threshold angle), then on the device, per pair, from its lo_model:
+ * the bearing inliers of the pose [R^T | -R^T t] (and, when check_reversal = 1, of its transpose), the TinySolver
+ * refinement of RelativePoseRefinement on more than 5 inliers (refine_iterations = max_num_iterations), the inliers
+ * of the refined pose, the Necker rule of two_view_reconstruction_5pt with reversal_ratio, and the inliers of the
+ * plane motion.  The rules are stated in oracle/two_view_oracle.py.
+ *   threshold         the angle of RANSAC and the chord bound of the bearing inliers (five_point_algo_threshold)
+ *   plane_pose        12 per pair: the plane motion [R_p | t_p] row-major (motion_from_plane_homography's first),
+ *                     whose inliers are those of (R_p^T, -R_p^T t_p); NaN when the pair has none
+ * Outputs: lo_model and ransac_inliers as osfm_relpose_run; pose (24 per pair: each configuration's final [R | t],
+ * row-major, in compute_inliers_bearings' convention, NaN for a configuration not run); counts (3 per pair: final
+ * inliers of each configuration, then of the plane motion); chosen (per pair: 0 or 1, the configuration the 5-point
+ * result keeps, -1 for none); mask_5pt and mask_plane (per row: the inliers of the 5-point and plane results).
+ * refine_iterations >= 1, check_reversal 0 or 1, reversal_ratio not NaN; otherwise, or on the conditions of
+ * osfm_relpose_run, OSFM_ERR_ARG. */
+int osfm_relpose_two_view(osfm_relpose* h, int64_t num_bearings, const double* bearings, int64_t num_pairs,
+                          const int64_t* pair_start, const int64_t* row_a, const int64_t* row_b, double threshold,
+                          int ransac_iterations, int refine_iterations, int check_reversal, double reversal_ratio,
+                          const double* plane_pose, double* lo_model, int32_t* ransac_inliers, double* pose,
+                          int32_t* counts, int32_t* chosen, uint8_t* mask_5pt, uint8_t* mask_plane);
+/* Device time of the last osfm_relpose_run or osfm_relpose_two_view (CUDA events around its kernels, after the
+ * uploads). */
 int osfm_relpose_last_device_ms(osfm_relpose* h, float* ms);
+/* The same split into the RANSAC kernels and the two-view kernel (0 when the last call was osfm_relpose_run). */
+int osfm_relpose_last_stage_ms(osfm_relpose* h, float* ransac_ms, float* two_view_ms);
 /* Test hooks, as osfm_rotransac_set_stream_prefix / set_trace / get_trace, per pair. */
 int osfm_relpose_set_stream_prefix(osfm_relpose* h, int64_t length);
 int osfm_relpose_set_trace(osfm_relpose* h, int capacity);

@@ -176,7 +176,11 @@ SIGNATURES = {
     "osfm_relpose_destroy": (c_int, [c_void_p]),
     "osfm_relpose_run": (c_int, [c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_double, c_int,
                                  c_void_p, c_void_p, c_void_p]),
+    "osfm_relpose_two_view": (c_int, [c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_double,
+                                      c_int, c_int, c_int, c_double, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                      c_void_p, c_void_p, c_void_p]),
     "osfm_relpose_last_device_ms": (c_int, [c_void_p, POINTER(c_float)]),
+    "osfm_relpose_last_stage_ms": (c_int, [c_void_p, POINTER(c_float), POINTER(c_float)]),
     "osfm_relpose_set_stream_prefix": (c_int, [c_void_p, c_int64]),
     "osfm_relpose_set_trace": (c_int, [c_void_p, c_int]),
     "osfm_relpose_get_trace": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p]),

@@ -684,5 +684,243 @@ OSFM_HD int five_point(const double* x1, const double* x2, double* Es, double* c
   return nr;
 }
 
+// ---------------------------------------------------------------------------------------------------------------
+// The two-view stage after RANSAC (reconstruction.two_view_reconstruction_and_refinement): bearing inliers, and the
+// cost, parametrisation and rotation helpers of RelativePoseRefinement (geometry/relative_pose.h).  Poses here are
+// in compute_inliers_bearings' convention: [R | t] maps the second image to the first, the second camera sits at t
+// and sees the world direction R y.  The restatement is oracle/two_view_oracle.py.
+// ---------------------------------------------------------------------------------------------------------------
+
+constexpr int REFINE_PICKED = 100;              // RelativePoseCost::MAX_ERRORS
+constexpr double ANGLE_AXIS_EPS = 2.220446049250313e-16;   // DBL_EPSILON: the first-order branch at or below it
+
+// matching.compute_inliers_bearings of one row: the midpoint X of the rays (0, x) and (t, R y); an inlier when
+// |X / |X| - x| and |R^T (X - t) / |.| - y| are both below thr.  A row that does not triangulate is no inlier.
+OSFM_HD bool bearing_inlier(const double* M, const double* x, const double* y, double thr) {
+  double c1[3] = {M[3], M[7], M[11]}, by[3], X[3];
+  for (int r = 0; r < 3; ++r) by[r] = M[r * 4] * y[0] + M[r * 4 + 1] * y[1] + M[r * 4 + 2] * y[2];
+  if (!midpoint(c1, x, by, X)) return false;
+  const double nx = sqrt(dot3(X, X));
+  double d1 = 0.0, d2 = 0.0, q[3];
+  for (int c = 0; c < 3; ++c) {
+    const double e = X[c] / nx - x[c];
+    d1 += e * e;
+  }
+  for (int c = 0; c < 3; ++c)
+    q[c] = M[c] * (X[0] - c1[0]) + M[4 + c] * (X[1] - c1[1]) + M[8 + c] * (X[2] - c1[2]);
+  const double nq = sqrt(dot3(q, q));
+  for (int c = 0; c < 3; ++c) {
+    const double e = q[c] / nq - y[c];
+    d2 += e * e;
+  }
+  return sqrt(d1) < thr && sqrt(d2) < thr;
+}
+
+// A forward-mode dual number over the 6 refinement parameters (what Ceres' Jet<double, 6> computes).
+struct Dual6 {
+  double v, d[6];
+  OSFM_HD Dual6() {}
+  OSFM_HD Dual6(double a) : v(a) {
+    for (int k = 0; k < 6; ++k) d[k] = 0.0;
+  }
+};
+OSFM_HD Dual6 operator+(const Dual6& a, const Dual6& b) {
+  Dual6 r;
+  r.v = a.v + b.v;
+  for (int k = 0; k < 6; ++k) r.d[k] = a.d[k] + b.d[k];
+  return r;
+}
+OSFM_HD Dual6 operator-(const Dual6& a, const Dual6& b) {
+  Dual6 r;
+  r.v = a.v - b.v;
+  for (int k = 0; k < 6; ++k) r.d[k] = a.d[k] - b.d[k];
+  return r;
+}
+OSFM_HD Dual6 operator-(const Dual6& a) {
+  Dual6 r;
+  r.v = -a.v;
+  for (int k = 0; k < 6; ++k) r.d[k] = -a.d[k];
+  return r;
+}
+OSFM_HD Dual6 operator*(const Dual6& a, const Dual6& b) {
+  Dual6 r;
+  r.v = a.v * b.v;
+  for (int k = 0; k < 6; ++k) r.d[k] = a.d[k] * b.v + a.v * b.d[k];
+  return r;
+}
+OSFM_HD Dual6 operator/(const Dual6& a, const Dual6& b) {
+  Dual6 r;
+  r.v = a.v / b.v;
+  for (int k = 0; k < 6; ++k) r.d[k] = (a.d[k] - r.v * b.d[k]) / b.v;
+  return r;
+}
+OSFM_HD double value(double a) { return a; }
+OSFM_HD double value(const Dual6& a) { return a.v; }
+OSFM_HD double sqrt_(double a) { return sqrt(a); }
+OSFM_HD double sin_(double a) { return sin(a); }
+OSFM_HD double cos_(double a) { return cos(a); }
+OSFM_HD Dual6 sqrt_(const Dual6& a) {
+  Dual6 r;
+  r.v = sqrt(a.v);
+  for (int k = 0; k < 6; ++k) r.d[k] = a.d[k] / (2.0 * r.v);
+  return r;
+}
+OSFM_HD Dual6 sin_(const Dual6& a) {
+  Dual6 r;
+  r.v = sin(a.v);
+  const double c = cos(a.v);
+  for (int k = 0; k < 6; ++k) r.d[k] = c * a.d[k];
+  return r;
+}
+OSFM_HD Dual6 cos_(const Dual6& a) {
+  Dual6 r;
+  r.v = cos(a.v);
+  const double s = -sin(a.v);
+  for (int k = 0; k < 6; ++k) r.d[k] = s * a.d[k];
+  return r;
+}
+
+// ceres::AngleAxisRotatePoint: Rodrigues' formula, or the first-order pt + aa x pt when |aa|^2 <= DBL_EPSILON (the
+// derivative is then the one of that branch)
+template <class T>
+OSFM_HD void angle_axis_rotate(const T* aa, const T* pt, T* out) {
+  const T theta2 = aa[0] * aa[0] + aa[1] * aa[1] + aa[2] * aa[2];
+  if (value(theta2) > ANGLE_AXIS_EPS) {
+    const T theta = sqrt_(theta2);
+    const T c = cos_(theta), s = sin_(theta);
+    const T inv = T(1.0) / theta;
+    const T w[3] = {aa[0] * inv, aa[1] * inv, aa[2] * inv};
+    const T wxp[3] = {w[1] * pt[2] - w[2] * pt[1], w[2] * pt[0] - w[0] * pt[2], w[0] * pt[1] - w[1] * pt[0]};
+    const T tmp = (w[0] * pt[0] + w[1] * pt[1] + w[2] * pt[2]) * (T(1.0) - c);
+    for (int i = 0; i < 3; ++i) out[i] = pt[i] * c + wxp[i] * s + w[i] * tmp;
+  } else {
+    const T wxp[3] = {aa[1] * pt[2] - aa[2] * pt[1], aa[2] * pt[0] - aa[0] * pt[2], aa[0] * pt[1] - aa[1] * pt[0]};
+    for (int i = 0; i < 3; ++i) out[i] = pt[i] + wxp[i];
+  }
+}
+
+// RelativePoseCost's residual of one picked row (x, y) at the parameters p (angle-axis of R^T, then t):
+// 1 - (px . x + py . y) / 2 of the midpoint of (0, x) and (t, R y); exactly 1 (no derivative) when it fails
+template <class T>
+OSFM_HD T refine_residual(const T* p, const double* xd, const double* yd) {
+  const T x[3] = {T(xd[0]), T(xd[1]), T(xd[2])}, y[3] = {T(yd[0]), T(yd[1]), T(yd[2])};
+  const T rt[3] = {-p[0], -p[1], -p[2]};
+  const T t[3] = {p[3], p[4], p[5]};
+  T by[3];
+  angle_axis_rotate(rt, y, by);
+  const T r0 = t[0] * x[0] + t[1] * x[1] + t[2] * x[2];
+  const T r1 = t[0] * by[0] + t[1] * by[1] + t[2] * by[2];
+  const T a00 = x[0] * x[0] + x[1] * x[1] + x[2] * x[2];
+  const T a10 = x[0] * by[0] + x[1] * by[1] + x[2] * by[2];
+  const T a01 = -a10;
+  const T a11 = -(by[0] * by[0] + by[1] * by[1] + by[2] * by[2]);
+  const T det = a00 * a11 - a01 * a10;
+  if (-MIDPOINT_DET_EPS < value(det) && value(det) < MIDPOINT_DET_EPS) return T(1.0);
+  const T l0 = (a11 * r0 - a01 * r1) / det;
+  const T l1 = (a00 * r1 - a10 * r0) / det;
+  T X[3], yc[3], q[3];
+  for (int c = 0; c < 3; ++c) {
+    X[c] = T(0.5) * (l0 * x[c] + (t[c] + l1 * by[c]));
+    yc[c] = X[c] - t[c];
+  }
+  angle_axis_rotate(p, yc, q);
+  const T nx = sqrt_(X[0] * X[0] + X[1] * X[1] + X[2] * X[2]);
+  const T nq = sqrt_(q[0] * q[0] + q[1] * q[1] + q[2] * q[2]);
+  const T ax = (X[0] / nx) * x[0] + (X[1] / nx) * x[1] + (X[2] / nx) * x[2];
+  const T ay = (q[0] / nq) * y[0] + (q[1] / nq) * y[1] + (q[2] / nq) * y[2];
+  return T(1.0) - (ax + ay) * T(0.5);
+}
+
+// RelativePoseCost's last residual, 1 - |t|
+template <class T>
+OSFM_HD T refine_norm_residual(const T* p) {
+  return T(1.0) - sqrt_(p[3] * p[3] + p[4] * p[4] + p[5] * p[5]);
+}
+
+// ceres::RotationMatrixToAngleAxis (through the quaternion) of the row-major R
+OSFM_HD void rotation_to_angle_axis(const double* R, double* aa) {
+#define R_(i, j) R[(i) * 3 + (j)]
+  double q[4];
+  const double trace = R_(0, 0) + R_(1, 1) + R_(2, 2);
+  if (trace >= 0.0) {
+    double t = sqrt(trace + 1.0);
+    q[0] = 0.5 * t;
+    t = 0.5 / t;
+    q[1] = (R_(2, 1) - R_(1, 2)) * t;
+    q[2] = (R_(0, 2) - R_(2, 0)) * t;
+    q[3] = (R_(1, 0) - R_(0, 1)) * t;
+  } else {
+    int i = 0;
+    if (R_(1, 1) > R_(0, 0)) i = 1;
+    if (R_(2, 2) > R_(i, i)) i = 2;
+    const int j = (i + 1) % 3, k = (j + 1) % 3;
+    double t = sqrt(R_(i, i) - R_(j, j) - R_(k, k) + 1.0);
+    q[i + 1] = 0.5 * t;
+    t = 0.5 / t;
+    q[0] = (R_(k, j) - R_(j, k)) * t;
+    q[j + 1] = (R_(j, i) + R_(i, j)) * t;
+    q[k + 1] = (R_(k, i) + R_(i, k)) * t;
+  }
+#undef R_
+  const double s2 = q[1] * q[1] + q[2] * q[2] + q[3] * q[3];
+  double k = 2.0;
+  if (s2 > 0.0) {
+    const double s = sqrt(s2), c = q[0];
+    k = 2.0 * (c < 0.0 ? atan2(-s, -c) : atan2(s, c)) / s;
+  }
+  for (int i = 0; i < 3; ++i) aa[i] = q[i + 1] * k;
+}
+
+// ceres::AngleAxisToRotationMatrix into the row-major R, with its first-order branch at |aa|^2 <= DBL_EPSILON
+OSFM_HD void angle_axis_to_rotation(const double* aa, double* R) {
+  const double theta2 = aa[0] * aa[0] + aa[1] * aa[1] + aa[2] * aa[2];
+  if (theta2 > ANGLE_AXIS_EPS) {
+    const double theta = sqrt(theta2);
+    const double wx = aa[0] / theta, wy = aa[1] / theta, wz = aa[2] / theta;
+    const double c = cos(theta), s = sin(theta), o = 1.0 - c;
+    R[0] = c + wx * wx * o;
+    R[3] = wz * s + wx * wy * o;
+    R[6] = -wy * s + wx * wz * o;
+    R[1] = wx * wy * o - wz * s;
+    R[4] = c + wy * wy * o;
+    R[7] = wx * s + wy * wz * o;
+    R[2] = wy * s + wx * wz * o;
+    R[5] = -wx * s + wy * wz * o;
+    R[8] = c + wz * wz * o;
+  } else {
+    R[0] = 1.0;
+    R[3] = aa[2];
+    R[6] = -aa[1];
+    R[1] = -aa[2];
+    R[4] = 1.0;
+    R[7] = aa[0];
+    R[2] = aa[1];
+    R[5] = -aa[0];
+    R[8] = 1.0;
+  }
+}
+
+// RelativePoseRefinement's parameters of the pose B = [R | t] (relative_pose_optimize_nonlinear passes
+// [R^T | -R^T t], whose angle-axis and -(R^T)^T (-R^T t) they are)
+OSFM_HD void refine_parameters(const double* B, double* p) {
+  double Rt[9], tc[3];
+  for (int i = 0; i < 3; ++i)
+    for (int j = 0; j < 3; ++j) Rt[i * 3 + j] = B[j * 4 + i];
+  for (int i = 0; i < 3; ++i) tc[i] = -(Rt[i * 3] * B[3] + Rt[i * 3 + 1] * B[7] + Rt[i * 3 + 2] * B[11]);
+  rotation_to_angle_axis(Rt, p);
+  for (int i = 0; i < 3; ++i) p[3 + i] = -(B[i * 4] * tc[0] + B[i * 4 + 1] * tc[1] + B[i * 4 + 2] * tc[2]);
+}
+
+// ... and back: R' = AngleAxisToRotationMatrix(p), t' = -R' p_t, then B = [R'^T | -R'^T t']
+OSFM_HD void refine_pose(const double* p, double* B) {
+  double R[9], tr[3];
+  angle_axis_to_rotation(p, R);
+  for (int i = 0; i < 3; ++i) tr[i] = -(R[i * 3] * p[3] + R[i * 3 + 1] * p[4] + R[i * 3 + 2] * p[5]);
+  for (int i = 0; i < 3; ++i) {
+    for (int j = 0; j < 3; ++j) B[i * 4 + j] = R[j * 3 + i];
+    B[i * 4 + 3] = -(R[i] * tr[0] + R[3 + i] * tr[1] + R[6 + i] * tr[2]);
+  }
+}
+
 }  // namespace relpose
 }  // namespace osfm

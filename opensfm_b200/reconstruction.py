@@ -25,6 +25,11 @@ by the rotation-only RANSAC of opensfm_b200/rotation_ransac.py:
   compute_image_pairs_from_tracks         this engine's fast path: bearings once per image, rows from the device's
                                           common-track lists
 
+and the two-view reconstruction that bootstraps from a ranked pair, from opensfm_b200/relative_pose.py:
+
+  two_view_reconstruction_general         reconstruction.py:488-560 (with :298-485 below it)
+  two_view_reconstructions                every listed pair's result in one call, from this engine's tracks
+
 and the triangulation of tracks after each shot the incremental loop adds, from opensfm_b200/triangulation.py:
 
   triangulate_shot_features               reconstruction.py:1143-1183
@@ -50,6 +55,7 @@ from typing import Any, Dict, Iterable, List, Optional, Sequence, Set, Tuple
 import numpy as np
 
 from . import bundle as _bundle
+from . import relative_pose as _rp
 from . import resection as _rs
 from . import rotation_ransac as _rr
 from . import types as T
@@ -586,6 +592,48 @@ def two_view_reconstruction_rotation_only(p1: np.ndarray, p2: np.ndarray, camera
     res = _rr.ransac_pairs_lists([b1], [b2], threshold)
     R = res.rotations()[0]
     return cv2.Rodrigues(R.T)[0].ravel(), res.inliers(0)
+
+
+def two_view_reconstruction_general(p1: np.ndarray, p2: np.ndarray, camera1, camera2, threshold: float,
+                                    iterations: int, check_reversal: bool = False, reversal_ratio: float = 1.0):
+    """(R as angle-axis, t, inlier rows, report) of the pair's two-view reconstruction: five-point RANSAC, the
+    refinement of the pose (and of its transpose when check_reversal), the plane-based motion and the choice between
+    them, as the reference computes them (rules in oracle/two_view_oracle.py)."""
+    b1 = camera1.pixel_bearing_many(p1)
+    b2 = camera2.pixel_bearing_many(p2)
+    return _rp.two_view_lists([b1], [b2], threshold, iterations, check_reversal, reversal_ratio).result(0)
+
+
+def two_view_reconstructions(tracks_manager, pairs: Sequence[Tuple[Any, Any]], cameras_by_image: Dict[Any, Any],
+                             config: Dict[str, Any]) -> List[Tuple[Any, Any, Any, Dict[str, Any]]]:
+    """two_view_reconstruction_general of every (im1, im2) in `pairs` on the points of their common tracks
+    (_get_common_feature_arrays), for this engine's TracksManager, in one call: pixel_bearing_many runs once per
+    image, the rows come from the device's common-track lists.  A pair's result depends only on its own rows, so the
+    incremental loop can read the results of its ranked pairs in order.  cameras_by_image: {image: camera}."""
+    if not len(pairs):
+        return []
+    xy = tracks_manager._points()[0]
+    ras, rbs = [], []
+    for im1, im2 in pairs:
+        ra, rb = tracks_manager._pair_rows(im1, im2)
+        ras.append(ra)
+        rbs.append(rb)
+    n = np.array([len(r) for r in ras], dtype=np.int64)
+    pair_start = np.zeros(len(n) + 1, dtype=np.int64)
+    np.cumsum(n, out=pair_start[1:])
+    row_a = np.concatenate(ras).astype(np.int64)
+    row_b = np.concatenate(rbs).astype(np.int64)
+    bearings = np.zeros((len(xy), 3), dtype=np.float64)
+    order, start = tracks_manager._shot_order()
+    images = list(tracks_manager.images)
+    for im in sorted({im for pair in pairs for im in pair}, key=images.index):
+        i = images.index(im)
+        rows = order[start[i]:start[i + 1]]
+        bearings[rows] = cameras_by_image[im].pixel_bearing_many(xy[rows])
+    res = _rp.two_view_pairs(bearings, pair_start, row_a, row_b, config["five_point_algo_threshold"],
+                             config["five_point_refine_rec_iterations"], config["five_point_reversal_check"],
+                             config["five_point_reversal_ratio"])
+    return [res.result(p) for p in range(len(pairs))]
 
 
 def _ranked_by_argsort(keys: List[Tuple[Any, Any]], scores: List[int]) -> List[Tuple[Any, Any]]:

@@ -12,7 +12,11 @@ Prints one JSON line: the card's name and power limit and
   * `single_pair`: per row count, the median host-clock latency of relative_pose.relative_pose_ransac on one pair
     of that size with 30 % outliers, and its kernel time;
   * `oracle_ms_per_pair`: oracle/relative_pose_oracle.py on --oracle-pairs pairs of the batch spread over its sizes,
-    on one CPU core, for scale only (pyrobust is not built with this project).
+    on one CPU core, for scale only (pyrobust is not built with this project);
+  * `two_view`: the full two-view call (relative_pose.two_view_lists) over the batch, with check_reversal off and
+    on: the kernel time of RANSAC and of the two-view stage (CUDA events, relative_pose.last_stage_ms), the host
+    time of the cv2.findHomography loop (relative_pose.plane_motion over every pair) and the call's host time,
+    medians of --reps; and the single-pair latency of reconstruction.two_view_reconstruction_general per row count.
 """
 import argparse
 import json
@@ -73,6 +77,46 @@ def main():
             ker.append(rp.last_device_ms())
         single[str(n)] = {"latency_ms": float(np.median(lat)), "kernel_ms": float(np.median(ker))}
     out["single_pair"] = single
+
+    tv = {}
+    for check in (False, True):
+        rp.two_view_lists(b1s, b2s, C.THRESHOLD, 1000, check, 0.95)
+        ker_r, ker_t, call, host = [], [], [], []
+        for _ in range(args.reps):
+            t0 = time.perf_counter()
+            rp.two_view_lists(b1s, b2s, C.THRESHOLD, 1000, check, 0.95)
+            call.append((time.perf_counter() - t0) * 1e3)
+            r_ms, t_ms = rp.last_stage_ms()
+            ker_r.append(r_ms)
+            ker_t.append(t_ms)
+            t0 = time.perf_counter()
+            for a, b in zip(b1s, b2s):
+                rp.plane_motion(a, b, C.THRESHOLD)
+            host.append((time.perf_counter() - t0) * 1e3)
+        tv["check_reversal" if check else "default"] = {
+            "ransac_kernel_ms": float(np.median(ker_r)), "two_view_kernel_ms": float(np.median(ker_t)),
+            "find_homography_loop_ms": float(np.median(host)), "call_ms": float(np.median(call))}
+    from image_pair_cases import PinholeCamera
+    from opensfm_b200 import reconstruction as rec
+
+    cam = PinholeCamera()
+    single_tv = {}
+    for n in (50, 200, 1000, 3000):
+        a, b = C.cube_pairs(8, 3000, 21, count=1, sizes=(n,), outlier_ratios=(0.3,))
+        p1, p2 = a[0][:, :2] / a[0][:, 2:], b[0][:, :2] / b[0][:, 2:]
+        rec.two_view_reconstruction_general(p1, p2, cam, cam, C.THRESHOLD, 1000)
+        lat, kr, kt = [], [], []
+        for _ in range(args.reps):
+            t0 = time.perf_counter()
+            rec.two_view_reconstruction_general(p1, p2, cam, cam, C.THRESHOLD, 1000)
+            lat.append((time.perf_counter() - t0) * 1e3)
+            r_ms, t_ms = rp.last_stage_ms()
+            kr.append(r_ms)
+            kt.append(t_ms)
+        single_tv[str(n)] = {"latency_ms": float(np.median(lat)), "ransac_kernel_ms": float(np.median(kr)),
+                             "two_view_kernel_ms": float(np.median(kt))}
+    tv["single_pair"] = single_tv
+    out["two_view"] = tv
 
     picks = np.linspace(0, len(b1s) - 1, args.oracle_pairs).astype(int).tolist()
     t0 = time.perf_counter()
