@@ -18,7 +18,7 @@
  *
  * There is no CPU fallback: every call needs a CUDA device (H100, sm_90a).
  *
- * Handles (osfm_matcher, osfm_ba, osfm_tracks, osfm_rotransac, osfm_resect, osfm_relpose) own a CUDA stream and
+ * Handles (osfm_matcher, osfm_ba, osfm_tracks, osfm_rotransac, osfm_resect, osfm_relpose, osfm_dense) own a CUDA stream and
  * workspaces on the device they were created on, and every call on a handle makes that device current on the calling thread.  Calls on one handle
  * are serialised and may come from any thread; calls on different handles do not wait for each other.  A callback
  * (today only the all-reduce of osfm_ba_set_distributed) must not call into the handle that called it.
@@ -597,6 +597,63 @@ int osfm_relpose_last_stage_ms(osfm_relpose* h, float* ransac_ms, float* two_vie
 int osfm_relpose_set_stream_prefix(osfm_relpose* h, int64_t length);
 int osfm_relpose_set_trace(osfm_relpose* h, int capacity);
 int osfm_relpose_get_trace(osfm_relpose* h, int32_t* count, int64_t* stream_used, int32_t* indices);
+
+/* ------------------------------------------------------------------------
+ * DENSE DEPTHMAPS
+ * ---------------------------------------------------------------------- */
+typedef struct osfm_dense osfm_dense;
+
+#define OSFM_DENSE_BRUTE_FORCE 0
+#define OSFM_DENSE_PATCH_MATCH 1
+#define OSFM_DENSE_PATCH_MATCH_SAMPLE 2
+#define OSFM_DENSE_MAX_PATCH 15
+#define OSFM_DENSE_MAX_VIEWS 32
+
+/* pydense's DepthmapEstimator, DepthmapCleaner and DepthmapPruner (opensfm/src/dense/src/depthmap.cc) for many
+ * reference shots per call, over views kept resident on the handle.  The rules are restated in
+ * oracle/dense_oracle.cpp; the one deliberate difference is the generator: every variate is Philox4x32-10 keyed by
+ * (seed, the reference's key) at counter (pixel, pass, draw, attempt).  A handle owns one CUDA stream and its
+ * workspaces on `device`. */
+int osfm_dense_create(int device, osfm_dense** out);
+int osfm_dense_destroy(osfm_dense* h);
+/* Replaces the handle's views (and forgets every map).  size: 2 per view (width, height); K, Kinv, R: 9 per view
+ * row-major fp64; t: 3 per view.  gray, mask, labels: every view's pixels in view order, row-major; rgb: 3 per
+ * pixel.  gray and mask are needed to estimate, rgb and labels to prune; each may be null otherwise.  Fails with
+ * OSFM_ERR_RUNTIME naming the bytes needed when the views and their maps do not fit in device memory. */
+int osfm_dense_set_views(osfm_dense* h, int num_views, const int32_t* size, const double* K, const double* Kinv,
+                         const double* R, const double* t, const uint8_t* gray, const uint8_t* mask,
+                         const uint8_t* rgb, const uint8_t* labels);
+/* Uploads maps of one view computed earlier: raw depth (as compute_depthmap saves it), plane (3 per pixel) and clean
+ * depth; each may be null.  A view has a raw map once raw depth and plane are set, a clean map once clean depth and
+ * plane are. */
+int osfm_dense_set_maps(osfm_dense* h, int view, const float* raw_depth, const float* plane, const float* clean_depth);
+/* Estimates the depthmap of num_refs references.  Reference r's views are views[list_start[r] .. list_start[r+1]),
+ * itself first, 2 to OSFM_DENSE_MAX_VIEWS of them.  Per list entry e: Q (9) = R_v R_ref^T and a (3) = Q t_ref - t_v.
+ * params: 5 per reference (method, patch_size, num_depth_planes, patchmatch_iterations, generator key);
+ * depth_range: 2 per reference (min, max); min_patch_variance: per reference; weights: the bilateral weight table,
+ * 256 x (2 ((OSFM_DENSE_MAX_PATCH - 1) / 2)^2 + 1) f32 indexed by (|dcolor|, dx^2 + dy^2).  The ungated maps (depth,
+ * plane 3 per pixel, score, nghbr as the list-local view index) are written per reference in request order, each of
+ * its view's size; any may be null.  The reference view's raw slot gets the depth gated by score > (float)min_score
+ * and depth < max, and the plane.  An even or too-large patch, an unknown method, a bad depth range, a view out of
+ * range or two references of the same view fails with OSFM_ERR_ARG; maps that do not fit in device memory fail with
+ * OSFM_ERR_RUNTIME naming the bytes needed. */
+int osfm_dense_estimate(osfm_dense* h, int num_refs, const int32_t* list_start, const int32_t* views, const double* Q,
+                        const double* a, const int32_t* params, const double* depth_range,
+                        const float* min_patch_variance, const float* weights, uint32_t seed, double min_score,
+                        float* depth, float* plane, float* score, int32_t* nghbr);
+/* DepthmapCleaner::Clean of every reference over the raw slots of its views (reference first, each with a raw map),
+ * into the reference's clean slot (two references of the same view fail with OSFM_ERR_ARG); clean_depth (nullable) receives the maps per reference in request order. */
+int osfm_dense_clean(osfm_dense* h, int num_refs, const int32_t* list_start, const int32_t* views,
+                     float same_depth_threshold, int min_consistent_views, float* clean_depth);
+/* DepthmapPruner::Prune of every reference over the clean depth and plane of its views (reference first, each with a
+ * clean map) and the reference's colour and labels.  counts: per reference, the points kept; the points themselves,
+ * in raster order per reference and references in request order, come from osfm_dense_get_pruned. */
+int osfm_dense_prune(osfm_dense* h, int num_refs, const int32_t* list_start, const int32_t* views,
+                     float same_depth_threshold, int64_t* counts);
+/* The last prune's points (3 f32 each), normals (3 f32), colours (3 u8) and labels (u8). */
+int osfm_dense_get_pruned(osfm_dense* h, float* points, float* normals, uint8_t* colors, uint8_t* labels);
+/* Device time of the last estimate, clean and prune (CUDA events around their kernels, after the uploads). */
+int osfm_dense_last_device_ms(osfm_dense* h, float* estimate_ms, float* clean_ms, float* prune_ms);
 
 #ifdef __cplusplus
 }

@@ -13,7 +13,9 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIBDIR = os.path.join(HERE, "lib")
 LIB = os.path.join(LIBDIR, "libopensfm_b200.so")
-SOURCES = ["core.cu", "match.cu", "match_tc.cu", "words.cu", "vlad.cu", "bow.cu", "tracks.cu", "triangulate.cu", "rotransac.cu", "resect.cu", "relpose.cu", "ba.cu"]
+SOURCES = ["core.cu", "match.cu", "match_tc.cu", "words.cu", "vlad.cu", "bow.cu", "tracks.cu", "triangulate.cu", "rotransac.cu", "resect.cu", "relpose.cu", "ba.cu", "dense.cu"]
+# per-source flags: dense.cu is checked bit for bit against a host restatement, so no product may become an FMA
+SOURCE_FLAGS = {"dense.cu": ["-fmad=false"]}
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = ARCH + [ "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "-ccbin", "/usr/bin/g++"]
@@ -44,7 +46,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
 
     def compile_one(src: str) -> str:
         obj = os.path.join(objdir, src.replace(".cu", ".o"))
-        cmd = [nvcc] + NVCC_FLAGS + ["-c", os.path.join(CSRC, src), "-o", obj]
+        cmd = [nvcc] + NVCC_FLAGS + SOURCE_FLAGS.get(src, []) + ["-c", os.path.join(CSRC, src), "-o", obj]
         if verbose:
             print(" ".join(cmd), file=sys.stderr)
         subprocess.check_call(cmd)

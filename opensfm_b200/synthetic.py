@@ -324,3 +324,89 @@ def relative_pose(R_wc_a, origin_a, R_wc_b, origin_b):
     R = R_wc_a @ R_wc_b.T
     t = R_wc_a @ (np.asarray(origin_b) - np.asarray(origin_a))
     return R, t
+
+
+@dataclass
+class TexturedScene:
+    """Images and exact depth maps of a piecewise-planar scene, in OpenSfM's conventions: x_cam = R X + t, pixel
+    coordinates through K, depth = z_cam (0 where a ray hits nothing)."""
+    K: np.ndarray        # (S,3,3)
+    R: np.ndarray        # (S,3,3)
+    t: np.ndarray        # (S,3)
+    gray: np.ndarray     # (S,H,W) u8
+    rgb: np.ndarray      # (S,H,W,3) u8
+    depth: np.ndarray    # (S,H,W) f32
+    flat: np.ndarray     # (S,H,W) bool: the flat-coloured face
+
+
+def _texture(X: np.ndarray, seed: int) -> np.ndarray:
+    """Procedural texture in 0..1 from world points: sines over three scales plus a hashed cell pattern."""
+    rng = np.random.RandomState(seed)
+    f = rng.uniform(3.0, 9.0, (4, 3))
+    v = sum(np.sin(X @ f[k] + k) for k in range(4)) / 8.0 + 0.5
+    cell = np.floor(X * 4.0).astype(np.int64)
+    h = (cell[..., 0] * 73856093) ^ (cell[..., 1] * 19349663) ^ (cell[..., 2] * 83492791)
+    return np.clip(0.6 * v + 0.4 * ((h % 1000) / 1000.0), 0.0, 1.0)
+
+
+def textured_scene(num_cameras: int = 4, width: int = 160, height: int = 120, seed: int = 3,
+                   arc_degrees: float = 40.0, radius: float = 6.0, focal: float = 0.9,
+                   sizes: Optional[List[Tuple[int, int]]] = None) -> TexturedScene:
+    """A ground plane (z = 0) with two boxes, seen from cameras on an arc around the origin, rendered by analytic
+    ray casting.  Every face is textured except the top of the first box, which is one flat colour.  `sizes` gives
+    each camera its own (width, height); `focal` is relative to the larger image side."""
+    boxes = [(np.array([-1.2, -0.6, 0.0]), np.array([-0.2, 0.4, 0.9])),
+             (np.array([0.4, -0.2, 0.0]), np.array([1.3, 0.9, 0.6]))]
+    S = num_cameras
+    sizes = sizes or [(width, height)] * S
+    Ks, Rs, ts, grays, rgbs, depths, flats = [], [], [], [], [], [], []
+    for c in range(S):
+        w, h = sizes[c]
+        ang = np.radians(-arc_degrees / 2 + arc_degrees * c / max(S - 1, 1))
+        C = np.array([radius * np.sin(ang), -radius * np.cos(ang), 3.0])
+        fwd = _normalized(np.array([0.0, 0.0, 0.2]) - C)
+        right = _normalized(np.cross(fwd, np.array([0.0, 0.0, 1.0])))
+        down = np.cross(fwd, right)
+        R = np.stack([right, down, fwd])
+        t = -R @ C
+        f = focal * max(w, h)
+        K = np.array([[f, 0, (w - 1) / 2.0], [0, f, (h - 1) / 2.0], [0, 0, 1.0]])
+        jj, ii = np.meshgrid(np.arange(w, dtype=np.float64), np.arange(h, dtype=np.float64))
+        pix = np.stack([jj, ii, np.ones_like(jj)], -1)
+        dcam = pix @ np.linalg.inv(K).T                    # z_cam = 1 along each ray
+        dw = dcam @ R                                      # world direction with z_cam = 1
+        best = np.full((h, w), np.inf)
+        face = np.full((h, w), -1)
+        with np.errstate(divide="ignore", invalid="ignore"):
+            s = -C[2] / dw[..., 2]                         # ground plane
+            ok = s > 0
+            best = np.where(ok, s, best)
+            face = np.where(ok, 0, face)
+            for b, (lo, hi) in enumerate(boxes):
+                for ax in range(3):
+                    for side, val in ((0, lo[ax]), (1, hi[ax])):
+                        s = (val - C[ax]) / dw[..., ax]
+                        X = C + s[..., None] * dw
+                        o1, o2 = [k for k in range(3) if k != ax]
+                        inside = ((X[..., o1] >= lo[o1]) & (X[..., o1] <= hi[o1]) & (X[..., o2] >= lo[o2]) &
+                                  (X[..., o2] <= hi[o2]) & (s > 0) & (s < best))
+                        best = np.where(inside, s, best)
+                        face = np.where(inside, 1 + 6 * b + 2 * ax + side, face)
+        hit = np.isfinite(best)
+        X = C + np.where(hit, best, 0.0)[..., None] * dw
+        tex = _texture(X, seed)
+        flat = face == 1 + 2 * 2 + 1                       # top of box 0
+        tex = np.where(flat, 0.55, tex)
+        shade = 0.6 + 0.4 * ((face % 5) / 4.0)
+        gray = np.clip(255.0 * tex * np.where(hit, shade, 0.0), 0, 255)
+        rgb = np.stack([gray, np.clip(gray * 0.8 + 30 * (face % 3), 0, 255), np.clip(255 - gray * 0.7, 0, 255)], -1)
+        Ks.append(K)
+        Rs.append(R)
+        ts.append(t)
+        grays.append(gray.astype(np.uint8))
+        rgbs.append(rgb.astype(np.uint8))
+        depths.append(np.where(hit, best, 0.0).astype(np.float32))
+        flats.append(flat)
+    stack = (lambda a: np.stack(a)) if len(set(sizes)) == 1 else (lambda a: np.array(a + [None], dtype=object)[:-1])
+    return TexturedScene(np.stack(Ks), np.stack(Rs), np.stack(ts), stack(grays), stack(rgbs), stack(depths),
+                         stack(flats))
