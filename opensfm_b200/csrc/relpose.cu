@@ -11,17 +11,14 @@
 // model (replace the best, local optimisation, stop) are replayed in model order from those counts.  A model's
 // inlier rows are listed, in ascending order, only when it becomes the best one with at least 5 inliers: local
 // optimisation samples from that list, thread 0 fits EssentialNPoints to the sample and the CTA counts its inliers.
-// A pair of at most RP_STAGE_ROWS rows is staged in shared memory as fp64 structure-of-arrays (both bearings, 48 B
-// per row); a larger one is read through L2 via its row indices.  A last pass writes the inlier mask of the result.
+// A pair of at most RANSAC_STAGE_ROWS rows is staged in shared memory (both bearings); a larger one is read through
+// L2 via its row indices.  A last pass writes the inlier mask of the result.  The sample stream, the row passes, the
+// launch plan and the argument checks are those of ransac_stream.cuh.
 #include <math_constants.h>
 
-#include <algorithm>
-#include <climits>
 #include <cmath>
 #include <cstdint>
 #include <cstdlib>
-#include <numeric>
-#include <string>
 #include <vector>
 
 #include "common.cuh"
@@ -31,9 +28,6 @@
 namespace osfm {
 namespace {
 
-constexpr int RP_THREADS = 128;
-constexpr int RP_WARPS = RP_THREADS / 32;
-constexpr int RP_STAGE_ROWS = 1024;        // 48 KB of shared memory
 constexpr int RP_MIN_SAMPLE = 5;
 constexpr int RP_MAX_SAMPLE = 12;          // local optimisation samples min(12, inliers / 2) rows (at least 5)
 constexpr int RP_MAX_MODELS = relpose::MAX_MODELS;
@@ -47,13 +41,11 @@ struct RpArgs {
   const int* order;              // pairs of this launch
   double threshold;              // 1 - cos(angle)
   int iterations;
-  StreamSource src;              // trace: trace_cap drawn indices per pair, or null
+  StreamSource src;
   int* best_rows;                // per row: the best model's inlier rows, ascending
   double* lo_model;              // 12 per pair
   int* ransac_inliers;
   unsigned char* mask;           // per row
-  int* trace_count;
-  long long* stream_used;
 };
 
 struct RpShared {
@@ -67,25 +59,7 @@ struct RpShared {
   int counts[RP_MAX_MODELS];
   int cand_count, best_count;
   int stop;
-  int warp_n[RP_MAX_MODELS][RP_WARPS];
-};
-
-struct RpRows {
-  const double* sm;              // staged SoA (ax ay az bx by bz, n each) or null
-  const double* bearings;
-  const long long *ra, *rb;
-  int n;
-  __device__ __forceinline__ void get(int i, double* x, double* y) const {
-    if (sm) {
-      x[0] = sm[i]; x[1] = sm[n + i]; x[2] = sm[2 * n + i];
-      y[0] = sm[3 * n + i]; y[1] = sm[4 * n + i]; y[2] = sm[5 * n + i];
-    } else {
-      const double* u = bearings + 3 * ra[i];
-      const double* v = bearings + 3 * rb[i];
-      x[0] = __ldg(u); x[1] = __ldg(u + 1); x[2] = __ldg(u + 2);
-      y[0] = __ldg(v); y[1] = __ldg(v + 1); y[2] = __ldg(v + 2);
-    }
-  }
+  int warp_n[RP_MAX_MODELS][RANSAC_WARPS];
 };
 
 __device__ __forceinline__ bool rp_inlier(const double* M, const double* x, const double* y, double t) {
@@ -100,60 +74,21 @@ struct RpErrorTest {
   }
 };
 
-// inliers (by `test`) of the nm models at M (12 apart, in shared memory) into counts, in one pass over the rows
+// inliers (by `test`) of the nm models at M (12 apart, in shared memory) into counts, in one pass over the rows;
+// warp_n is RP_MAX_MODELS x RANSAC_WARPS ints of shared scratch
 template <class Test>
-__device__ void rp_count(RpShared& s, const RpRows& rows, const double* M, int nm, Test test, int* counts) {
+__device__ void rp_count(int* warp_n, const RansacRows& rows, const double* M, int nm, Test test, int* counts) {
   int c[RP_MAX_MODELS];
 #pragma unroll
   for (int j = 0; j < RP_MAX_MODELS; ++j) c[j] = 0;
-  for (int i = threadIdx.x; i < rows.n; i += RP_THREADS) {
+  for (int i = threadIdx.x; i < rows.n; i += RANSAC_THREADS) {
     double x[3], y[3];
     rows.get(i, x, y);
 #pragma unroll
     for (int j = 0; j < RP_MAX_MODELS; ++j)
       if (j < nm) c[j] += test(M + 12 * j, x, y) ? 1 : 0;
   }
-#pragma unroll
-  for (int j = 0; j < RP_MAX_MODELS; ++j) {
-    if (j >= nm) break;
-    const int w = __reduce_add_sync(0xffffffffu, c[j]);
-    if ((threadIdx.x & 31) == 0) s.warp_n[j][threadIdx.x >> 5] = w;
-  }
-  __syncthreads();
-  if (threadIdx.x < nm) {
-    int total = 0;
-    for (int w = 0; w < RP_WARPS; ++w) total += s.warp_n[threadIdx.x][w];
-    counts[threadIdx.x] = total;
-  }
-  __syncthreads();
-}
-
-// the inlier rows (by `test`) of the pose M, ascending, into out; returns how many there are
-template <class Test>
-__device__ int rp_compact(RpShared& s, const RpRows& rows, const double* M, Test test, int* out) {
-  double m[12];
-  for (int k = 0; k < 12; ++k) m[k] = M[k];
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  int base = 0;
-  for (int tile = 0; tile < rows.n; tile += RP_THREADS) {
-    const int i = tile + threadIdx.x;
-    bool in = false;
-    if (i < rows.n) {
-      double x[3], y[3];
-      rows.get(i, x, y);
-      in = test(m, x, y);
-    }
-    const unsigned bal = __ballot_sync(0xffffffffu, in);
-    if (lane == 0) s.warp_n[0][warp] = __popc(bal);
-    __syncthreads();
-    int off = base;
-    for (int w = 0; w < warp; ++w) off += s.warp_n[0][w];
-    if (in) out[off + __popc(bal & ((1u << lane) - 1u))] = i;
-    for (int w = warp; w < RP_WARPS; ++w) off += s.warp_n[0][w];
-    base = off;
-    __syncthreads();
-  }
-  return base;
+  ransac_sums(c, nm, warp_n, counts);
 }
 
 // thread 0's solvers, out of line so that their registers and stack do not weigh on the CTA's passes over the rows
@@ -171,40 +106,12 @@ __device__ __noinline__ int rp_n_points(int k, const double* x1, const double* x
   return 1;
 }
 
-__global__ void rp_normalize(double* bearings, long long n) {
-  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  double* b = bearings + 3 * i;
-  const double r = sqrt(b[0] * b[0] + b[1] * b[1] + b[2] * b[2]);
-  b[0] /= r;
-  b[1] /= r;
-  b[2] /= r;
-}
-
-extern __shared__ double rp_dyn[];
-
-// a pair's rows: staged in shared memory (rp_dyn) when `staged`, else read through L2
-__device__ RpRows rp_rows(const double* bearings, const long long* ra, const long long* rb, int n, int staged) {
-  RpRows rows{nullptr, bearings, ra, rb, n};
-  if (staged) {
-    for (int i = threadIdx.x; i < n; i += RP_THREADS) {
-      const double* u = bearings + 3 * ra[i];
-      const double* v = bearings + 3 * rb[i];
-      for (int c = 0; c < 3; ++c) {
-        rp_dyn[c * n + i] = u[c];
-        rp_dyn[(3 + c) * n + i] = v[c];
-      }
-    }
-    rows.sm = rp_dyn;
-  }
-  return rows;
-}
-
-__global__ void __launch_bounds__(RP_THREADS) rp_ransac(RpArgs a, int staged) {
+__global__ void __launch_bounds__(RANSAC_THREADS) rp_ransac(RpArgs a, int staged) {
   __shared__ RpShared s;
   const int pair = a.order[blockIdx.x];
   const long long off = a.pair_start[pair];
-  const RpRows rows = rp_rows(a.bearings, a.row_a + off, a.row_b + off, (int)(a.pair_start[pair + 1] - off), staged);
+  const RansacRows rows =
+      ransac_rows(a.bearings, a.bearings, a.row_a + off, a.row_b + off, (int)(a.pair_start[pair + 1] - off), staged);
   const int n = rows.n;
   int* best_rows = a.best_rows + off;
   const double t = a.threshold;
@@ -224,7 +131,7 @@ __global__ void __launch_bounds__(RP_THREADS) rp_ransac(RpArgs a, int staged) {
     }
     __syncthreads();
     const int nm = s.nm;
-    if (nm > 0) rp_count(s, rows, &s.models[0][0], nm, RpErrorTest{t}, s.counts);
+    if (nm > 0) rp_count(&s.warp_n[0][0], rows, &s.models[0][0], nm, RpErrorTest{t}, s.counts);
     // the models in order: std::max(score, best) keeps the new one on ties, then LO, then ShouldStop
     for (int j = 0; j < nm; ++j) {
       const int c = s.counts[j];
@@ -235,7 +142,7 @@ __global__ void __launch_bounds__(RP_THREADS) rp_ransac(RpArgs a, int staged) {
           s.best_count = c;
         }
         if (c >= RP_MIN_SAMPLE) {
-          rp_compact(s, rows, s.models[j], RpErrorTest{t}, best_rows);
+          ransac_compact<12>(rows, s.models[j], RpErrorTest{t}, s.warp_n[0], best_rows);
           for (int lo = 0; lo < RP_LO_ITERATIONS; ++lo) {
             if (threadIdx.x == 0) {
               const int m = s.best_count;
@@ -246,9 +153,9 @@ __global__ void __launch_bounds__(RP_THREADS) rp_ransac(RpArgs a, int staged) {
             }
             __syncthreads();
             if (s.nm > 0) {
-              rp_count(s, rows, s.cand, 1, RpErrorTest{t}, &s.cand_count);
+              rp_count(&s.warp_n[0][0], rows, s.cand, 1, RpErrorTest{t}, &s.cand_count);
               if (s.cand_count >= s.best_count) {
-                rp_compact(s, rows, s.cand, RpErrorTest{t}, best_rows);
+                ransac_compact<12>(rows, s.cand, RpErrorTest{t}, s.warp_n[0], best_rows);
                 if (threadIdx.x == 0) {
                   for (int k = 0; k < 12; ++k) s.best[k] = s.cand[k];
                   s.best_count = s.cand_count;
@@ -274,7 +181,7 @@ __global__ void __launch_bounds__(RP_THREADS) rp_ransac(RpArgs a, int staged) {
   // the inlier mask of the result (pyrobust's inliers_indices)
   double M[12];
   for (int k = 0; k < 12; ++k) M[k] = s.best[k];
-  for (int i = threadIdx.x; i < n; i += RP_THREADS) {
+  for (int i = threadIdx.x; i < n; i += RANSAC_THREADS) {
     double x[3], y[3];
     rows.get(i, x, y);
     a.mask[off + i] = rp_inlier(M, x, y, t) ? 1 : 0;
@@ -282,10 +189,7 @@ __global__ void __launch_bounds__(RP_THREADS) rp_ransac(RpArgs a, int staged) {
   if (threadIdx.x == 0) {
     a.ransac_inliers[pair] = s.best_count;
     for (int k = 0; k < 12; ++k) a.lo_model[12LL * pair + k] = M[k];
-    if (a.src.trace) {
-      a.trace_count[pair] = s.st.trace_n;
-      a.stream_used[pair] = s.st.cursor;
-    }
+    stream_record(s.st, a.src, pair);
   }
 }
 
@@ -339,7 +243,8 @@ __device__ __forceinline__ double tv_warp_sum(double v) {
 // RelativePoseCost at p over the warp, the picked rows across lanes: returns f . f; with JAC also the unscaled
 // normal equations A = J^T J (upper triangle, row by row) and je = J^T (-f).  Every lane gets the sums.
 template <bool JAC>
-__device__ double tv_evaluate(const RpRows& rows, const int* list, int count, const double* p, double* A, double* je) {
+__device__ double tv_evaluate(const RansacRows& rows, const int* list, int count, const double* p, double* A,
+                              double* je) {
   const int lane = threadIdx.x & 31;
   double ff = 0.0;
   if (JAC) {
@@ -420,7 +325,7 @@ __device__ __forceinline__ void tv_cholesky_solve(double* M, const double* b, do
 // RelativePoseRefinement of the pose B (in shared memory) on the picked inlier rows, by one warp: TinySolver with
 // max_num_iterations = iterations (rules in oracle/two_view_oracle.py); every lane runs the same control, lane 0
 // writes the result.
-__device__ __noinline__ void tv_refine(const RpRows& rows, const int* list, int count, int iterations, double* B) {
+__device__ __noinline__ void tv_refine(const RansacRows& rows, const int* list, int count, int iterations, double* B) {
   double x[6], A[21], je[6], s[6], jtj[36], g[6];
   relpose::refine_parameters(B, x);
   double cost = 0.5 * tv_evaluate<true>(rows, list, count, x, A, je);
@@ -472,15 +377,16 @@ __device__ __noinline__ void tv_refine(const RpRows& rows, const int* list, int 
   __syncwarp();
 }
 
-__global__ void __launch_bounds__(RP_THREADS) rp_two_view(TvArgs a, int staged) {
-  __shared__ RpShared s;
+__global__ void __launch_bounds__(RANSAC_THREADS) rp_two_view(TvArgs a, int staged) {
+  __shared__ int warp_n[TV_CONFIGS + 1][RANSAC_WARPS];
   __shared__ double B[TV_CONFIGS + 1][12];   // the configurations' poses, then the plane motion's
   __shared__ int counts[TV_CONFIGS + 1];
   __shared__ int first[TV_CONFIGS];
   __shared__ int chosen;
   const int pair = a.order[blockIdx.x];
   const long long off = a.pair_start[pair];
-  const RpRows rows = rp_rows(a.bearings, a.row_a + off, a.row_b + off, (int)(a.pair_start[pair + 1] - off), staged);
+  const RansacRows rows =
+      ransac_rows(a.bearings, a.bearings, a.row_a + off, a.row_b + off, (int)(a.pair_start[pair + 1] - off), staged);
   const int n = rows.n;
   if (threadIdx.x == 0) {
     // multiview.relative_pose_ransac's [R^T | -R^T t] of lo_model = [R | t], then its transpose (R^T, -R^T t)
@@ -505,7 +411,7 @@ __global__ void __launch_bounds__(RP_THREADS) rp_two_view(TvArgs a, int staged) 
   const TvBearingTest test{a.threshold};
   int* lists = a.lists + 2 * off;
   for (int c = 0; c < a.configurations; ++c) {
-    const int m = rp_compact(s, rows, B[c], test, lists + (long long)c * n);
+    const int m = ransac_compact<12>(rows, B[c], test, warp_n[0], lists + (long long)c * n);
     if (threadIdx.x == 0) first[c] = m;
   }
   __syncthreads();
@@ -514,7 +420,7 @@ __global__ void __launch_bounds__(RP_THREADS) rp_two_view(TvArgs a, int staged) 
   if (warp < a.configurations && first[warp] >= TV_MIN_REFINE)
     tv_refine(rows, lists + (long long)warp * n, first[warp], a.refine_iterations, B[warp]);
   __syncthreads();
-  rp_count(s, rows, &B[0][0], TV_CONFIGS + 1, test, counts);
+  rp_count(&warp_n[0][0], rows, &B[0][0], TV_CONFIGS + 1, test, counts);
   if (threadIdx.x == 0) {
     // two_view_reconstruction_5pt: keep a configuration with more than 5 inliers; of two, none when
     // min / max > reversal_ratio, else the larger, the transposed one on a tie
@@ -528,7 +434,7 @@ __global__ void __launch_bounds__(RP_THREADS) rp_two_view(TvArgs a, int staged) 
   }
   __syncthreads();
   const int c = chosen;
-  for (int i = threadIdx.x; i < n; i += RP_THREADS) {
+  for (int i = threadIdx.x; i < n; i += RANSAC_THREADS) {
     double x[3], y[3];
     rows.get(i, x, y);
     a.mask5[off + i] = c >= 0 && test(B[c], x, y) ? 1 : 0;
@@ -559,15 +465,9 @@ void glibc_rand(unsigned seed, int count, std::vector<int>& out) {
 }
 
 struct RelPose : DeviceStream<3> {
-  bool timed = false;
-  int trace_cap = 0;
-  long long P = 0;
-
-  StreamPrefix prefix;
-  SmemOptIn smem_opt_in;
+  RansacBatch batch;
   DevBuf<double> d_bearings, d_lo;
-  DevBuf<long long> d_pair_start, d_row_a, d_row_b, d_stream_used;
-  DevBuf<int> d_order, d_best_rows, d_ransac, d_trace, d_trace_count;
+  DevBuf<int> d_ransac;
   DevBuf<unsigned char> d_mask;
 
   // the two-view stage
@@ -589,109 +489,53 @@ struct RelPose : DeviceStream<3> {
                 uint8_t* mask_5pt, uint8_t* mask_plane);
 
  private:
-  // the launches of one RANSAC call (after the argument checks), up to ev[1]; the launch split is kept for the
-  // stage after it
-  int big = 0, staged_rows = 0;
   void check(int64_t num_bearings, const double* bearings, int64_t num_pairs, const int64_t* pair_start,
-             const int64_t* row_a, const int64_t* row_b, double threshold, int iterations);
+             const int64_t* row_a, const int64_t* row_b, double threshold, int iterations) {
+    two_view_timed = false;
+    batch.check("relative pose", "pair", "rows", RP_MIN_SAMPLE, num_pairs, pair_start, threshold, iterations,
+                {{row_a, bearings, num_bearings, "bearing"}, {row_b, bearings, num_bearings, "bearing"}}, true);
+  }
+  // the launches of one RANSAC call (after the argument checks), up to ev[1]; the batch's plan serves the stage
+  // after it
   void launch_ransac(int64_t num_bearings, const double* bearings, int64_t num_pairs, const int64_t* pair_start,
                      const int64_t* row_a, const int64_t* row_b, double threshold, int iterations);
 };
 
-void RelPose::check(int64_t num_bearings, const double* bearings, int64_t num_pairs, const int64_t* pair_start,
-                    const int64_t* row_a, const int64_t* row_b, double threshold, int iterations) {
-  if (num_bearings < 0 || num_pairs < 0 || num_pairs > INT_MAX) throw ArgError("relative pose: bad sizes");
-  if (iterations < 1) throw ArgError("relative pose: iterations must be at least 1");
-  if (!std::isfinite(threshold) || threshold <= 0.0) throw ArgError("relative pose: threshold must be positive");
-  if (!pair_start) throw ArgError("relative pose: null pair_start");
-  if (pair_start[0] != 0) throw ArgError("relative pose: pair_start[0] must be 0");
-  for (int64_t p = 0; p < num_pairs; ++p) {
-    const int64_t n = pair_start[p + 1] - pair_start[p];
-    if (n < RP_MIN_SAMPLE)
-      throw ArgError("relative pose: pair " + std::to_string(p) + " has " + std::to_string(n) +
-                     " rows; at least 5 are needed");
-    if (n > INT_MAX) throw ArgError("relative pose: pair " + std::to_string(p) + " has more than 2^31 - 1 rows");
-  }
-  if (num_pairs > 0 && (!row_a || !row_b || !bearings)) throw ArgError("relative pose: null arrays");
-  for (int64_t p = 0; p < num_pairs; ++p)
-    for (int64_t r = pair_start[p]; r < pair_start[p + 1]; ++r)
-      if (row_a[r] < 0 || row_a[r] >= num_bearings || row_b[r] < 0 || row_b[r] >= num_bearings)
-        throw ArgError("relative pose: row " + std::to_string(r - pair_start[p]) + " of pair " + std::to_string(p) +
-                       " names a bearing outside [0, " + std::to_string(num_bearings) + ")");
-}
-
 void RelPose::launch_ransac(int64_t num_bearings, const double* bearings, int64_t num_pairs,
                             const int64_t* pair_start, const int64_t* row_a, const int64_t* row_b, double threshold,
                             int iterations) {
+  batch.plan(stream, num_pairs, pair_start, {row_a, row_b});
   const int64_t R = pair_start[num_pairs];
-  prefix.make(stream);
-
-  // largest pairs first; the pairs too large for shared memory form their own launch
-  std::vector<int> order((size_t)num_pairs);
-  std::iota(order.begin(), order.end(), 0);
-  std::stable_sort(order.begin(), order.end(), [&](int x, int y) {
-    return pair_start[x + 1] - pair_start[x] > pair_start[y + 1] - pair_start[y];
-  });
-  big = 0;
-  while (big < num_pairs && pair_start[order[big] + 1] - pair_start[order[big]] > RP_STAGE_ROWS) ++big;
-  staged_rows = big < num_pairs ? (int)(pair_start[order[big] + 1] - pair_start[order[big]]) : 0;
-
   upload(d_bearings, bearings, (size_t)num_bearings * 3);
-  upload(d_pair_start, reinterpret_cast<const long long*>(pair_start), (size_t)num_pairs + 1);
-  upload(d_row_a, reinterpret_cast<const long long*>(row_a), (size_t)R);
-  upload(d_row_b, reinterpret_cast<const long long*>(row_b), (size_t)R);
-  upload(d_order, order.data(), order.size());
-  d_best_rows.reserve((size_t)R);
   d_mask.reserve((size_t)R);
   d_lo.reserve((size_t)num_pairs * 12);
   d_ransac.reserve((size_t)num_pairs);
-  if (trace_cap > 0) {
-    d_trace.reserve((size_t)num_pairs * trace_cap);
-    d_trace_count.reserve((size_t)num_pairs);
-    d_stream_used.reserve((size_t)num_pairs);
-  }
 
   RpArgs a;
   a.bearings = d_bearings.p;
-  a.pair_start = d_pair_start.p;
-  a.row_a = d_row_a.p;
-  a.row_b = d_row_b.p;
+  a.pair_start = batch.d_start.p;
+  a.row_a = batch.d_rows[0].p;
+  a.row_b = batch.d_rows[1].p;
   a.threshold = 1.0 - std::cos(threshold);
   a.iterations = iterations;
-  a.src = prefix.source(trace_cap > 0 ? d_trace.p : nullptr, trace_cap);
-  a.best_rows = d_best_rows.p;
+  a.src = batch.source();
+  a.best_rows = batch.d_best_rows.p;
   a.lo_model = d_lo.p;
   a.ransac_inliers = d_ransac.p;
   a.mask = d_mask.p;
-  a.trace_count = d_trace_count.p;
-  a.stream_used = d_stream_used.p;
 
   OSFM_CUDA(cudaEventRecord(ev[0], stream));
   if (num_bearings > 0) {
-    rp_normalize<<<(unsigned)((num_bearings + 255) / 256), 256, 0, stream>>>(d_bearings.p, num_bearings);
+    ransac_normalize<<<(unsigned)((num_bearings + 255) / 256), 256, 0, stream>>>(d_bearings.p, num_bearings);
     OSFM_LAUNCH_CHECK();
   }
-  if (big > 0) {
-    a.order = d_order.p;
-    rp_ransac<<<big, RP_THREADS, 0, stream>>>(a, 0);
-    OSFM_LAUNCH_CHECK();
-  }
-  if (big < num_pairs) {
-    const int smem_max = (int)(sizeof(double) * 6 * RP_STAGE_ROWS);
-    smem_opt_in(rp_ransac, smem_max);
-    const size_t smem = sizeof(double) * 6 * (size_t)staged_rows;
-    a.order = d_order.p + big;
-    rp_ransac<<<(unsigned)(num_pairs - big), RP_THREADS, smem, stream>>>(a, 1);
-    OSFM_LAUNCH_CHECK();
-  }
+  batch.launch(rp_ransac, a, stream);
   OSFM_CUDA(cudaEventRecord(ev[1], stream));
 }
 
 void RelPose::run(int64_t num_bearings, const double* bearings, int64_t num_pairs, const int64_t* pair_start,
                   const int64_t* row_a, const int64_t* row_b, double threshold, int iterations, double* lo_model,
                   int32_t* ransac_inliers, uint8_t* inlier_mask) {
-  timed = two_view_timed = false;
-  P = 0;
   check(num_bearings, bearings, num_pairs, pair_start, row_a, row_b, threshold, iterations);
   if (num_pairs > 0 && (!lo_model || !ransac_inliers || !inlier_mask)) throw ArgError("relative pose: null arrays");
   if (num_pairs == 0) return;
@@ -701,8 +545,7 @@ void RelPose::run(int64_t num_bearings, const double* bearings, int64_t num_pair
   download(ransac_inliers, d_ransac.p, (size_t)num_pairs);
   download(inlier_mask, d_mask.p, (size_t)R);
   OSFM_CUDA(cudaStreamSynchronize(stream));
-  P = num_pairs;
-  timed = true;
+  batch.done = num_pairs;
 }
 
 void RelPose::two_view(int64_t num_bearings, const double* bearings, int64_t num_pairs, const int64_t* pair_start,
@@ -710,8 +553,6 @@ void RelPose::two_view(int64_t num_bearings, const double* bearings, int64_t num
                        int refine_iterations, int check_reversal, double reversal_ratio, const double* plane_pose,
                        double* lo_model, int32_t* ransac_inliers, double* pose, int32_t* counts, int32_t* chosen,
                        uint8_t* mask_5pt, uint8_t* mask_plane) {
-  timed = two_view_timed = false;
-  P = 0;
   check(num_bearings, bearings, num_pairs, pair_start, row_a, row_b, threshold, ransac_iterations);
   if (refine_iterations < 1) throw ArgError("two-view: refine_iterations must be at least 1");
   if (check_reversal != 0 && check_reversal != 1) throw ArgError("two-view: check_reversal must be 0 or 1");
@@ -740,9 +581,9 @@ void RelPose::two_view(int64_t num_bearings, const double* bearings, int64_t num
 
   TvArgs a;
   a.bearings = d_bearings.p;
-  a.pair_start = d_pair_start.p;
-  a.row_a = d_row_a.p;
-  a.row_b = d_row_b.p;
+  a.pair_start = batch.d_start.p;
+  a.row_a = batch.d_rows[0].p;
+  a.row_b = batch.d_rows[1].p;
   a.lo_model = d_lo.p;
   a.plane_pose = d_plane.p;
   a.threshold = threshold;
@@ -755,17 +596,7 @@ void RelPose::two_view(int64_t num_bearings, const double* bearings, int64_t num
   a.chosen = d_tv_chosen.p;
   a.mask5 = d_mask.p;             // rp_ransac's mask is not returned by this call
   a.maskp = d_mask_plane.p;
-  if (big > 0) {
-    a.order = d_order.p;
-    rp_two_view<<<big, RP_THREADS, 0, stream>>>(a, 0);
-    OSFM_LAUNCH_CHECK();
-  }
-  if (big < num_pairs) {
-    smem_opt_in(rp_two_view, (int)(sizeof(double) * 6 * RP_STAGE_ROWS));
-    a.order = d_order.p + big;
-    rp_two_view<<<(unsigned)(num_pairs - big), RP_THREADS, sizeof(double) * 6 * (size_t)staged_rows, stream>>>(a, 1);
-    OSFM_LAUNCH_CHECK();
-  }
+  batch.launch(rp_two_view, a, stream);
   OSFM_CUDA(cudaEventRecord(ev[2], stream));
   download(lo_model, d_lo.p, (size_t)num_pairs * 12);
   download(ransac_inliers, d_ransac.p, (size_t)num_pairs);
@@ -775,8 +606,8 @@ void RelPose::two_view(int64_t num_bearings, const double* bearings, int64_t num
   download(mask_5pt, d_mask.p, (size_t)R);
   download(mask_plane, d_mask_plane.p, (size_t)R);
   OSFM_CUDA(cudaStreamSynchronize(stream));
-  P = num_pairs;
-  timed = two_view_timed = true;
+  batch.done = num_pairs;
+  two_view_timed = true;
 }
 
 }  // namespace
@@ -817,41 +648,29 @@ int osfm_relpose_last_stage_ms(osfm_relpose* h, float* ransac_ms, float* two_vie
   return osfm::with_handle(h, [&](osfm::RelPose& K) {
     if (!ransac_ms || !two_view_ms) throw osfm::ArgError("null ms");
     *ransac_ms = *two_view_ms = 0.f;
-    if (K.timed) OSFM_CUDA(cudaEventElapsedTime(ransac_ms, K.ev[0], K.ev[1]));
+    if (K.batch.done) OSFM_CUDA(cudaEventElapsedTime(ransac_ms, K.ev[0], K.ev[1]));
     if (K.two_view_timed) OSFM_CUDA(cudaEventElapsedTime(two_view_ms, K.ev[1], K.ev[2]));
   });
 }
 
 int osfm_relpose_set_stream_prefix(osfm_relpose* h, int64_t length) {
-  return osfm::with_handle(h, [&](osfm::RelPose& K) {
-    if (length < 1 || length > (1LL << 28)) throw osfm::ArgError("stream prefix length must be in [1, 2^28]");
-    K.prefix.want = length;
-  });
+  return osfm::with_handle(h, [&](osfm::RelPose& K) { K.batch.set_stream_prefix(length); });
 }
 
 int osfm_relpose_set_trace(osfm_relpose* h, int capacity) {
-  return osfm::with_handle(h, [&](osfm::RelPose& K) {
-    if (capacity < 0) throw osfm::ArgError("negative trace capacity");
-    K.trace_cap = capacity;
-  });
+  return osfm::with_handle(h, [&](osfm::RelPose& K) { K.batch.set_trace(capacity); });
 }
 
 int osfm_relpose_get_trace(osfm_relpose* h, int32_t* count, int64_t* stream_used, int32_t* indices) {
-  return osfm::with_handle(h, [&](osfm::RelPose& K) {
-    if (!K.timed || K.trace_cap == 0) throw std::runtime_error("relative pose: no traced run");
-    if (!count || !stream_used || !indices) throw osfm::ArgError("null outputs");
-    K.download(count, K.d_trace_count.p, (size_t)K.P);
-    K.download(reinterpret_cast<long long*>(stream_used), K.d_stream_used.p, (size_t)K.P);
-    K.download(indices, K.d_trace.p, (size_t)K.P * K.trace_cap);
-    OSFM_CUDA(cudaStreamSynchronize(K.stream));
-  });
+  return osfm::with_handle(
+      h, [&](osfm::RelPose& K) { K.batch.get_trace(K.stream, "relative pose", count, stream_used, indices); });
 }
 
 int osfm_relpose_last_device_ms(osfm_relpose* h, float* ms) {
   return osfm::with_handle(h, [&](osfm::RelPose& K) {
     if (!ms) throw osfm::ArgError("null ms");
     *ms = 0.f;
-    if (K.timed) OSFM_CUDA(cudaEventElapsedTime(ms, K.ev[0], K.ev[K.two_view_timed ? 2 : 1]));
+    if (K.batch.done) OSFM_CUDA(cudaEventElapsedTime(ms, K.ev[0], K.ev[K.two_view_timed ? 2 : 1]));
   });
 }
 

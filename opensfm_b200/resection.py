@@ -8,14 +8,14 @@ shots own consecutive rows (`shot_start`).  `ransac_lists` builds that from per-
 """
 from __future__ import annotations
 
-import ctypes
 from dataclasses import dataclass
-from typing import List, Optional, Sequence
+from typing import Sequence
 
 import numpy as np
 
 from . import _lib
 from ._lib import ptr
+from .ransac import Engine, batch_rows
 
 ITERATIONS = 1000   # what resect passes
 
@@ -43,48 +43,18 @@ class ShotsResult:
         return self.chord_mask[self.shot_start[s]:self.shot_start[s + 1]]
 
 
-class Resection:
-    """osfm_resect: one stream, its workspaces and the sample stream kept on the device; a new handle, or `handle`
-    when given."""
+class Resection(Engine):
+    """osfm_resect (ransac.Engine): the problems are shots."""
 
-    def __init__(self, device: int = 0, handle: Optional[_lib.Handle] = None):
-        self.handle = handle if handle is not None else _lib.Handle("resect", device)
-        self.h, self.L, self.device = self.handle.h, self.handle.L, self.handle.device
-        self._trace_cap = 0
-        self._num_shots = 0
-
-    def set_stream_prefix(self, length: int) -> None:
-        """How many generator outputs the device keeps (a test hook: shots that use them all continue from the saved
-        generator state)."""
-        _lib.check(self.L.osfm_resect_set_stream_prefix(self.h, int(length)))
-
-    def set_trace(self, capacity: int) -> None:
-        """Record up to `capacity` drawn sample indices per shot in the following runs (0: off)."""
-        _lib.check(self.L.osfm_resect_set_trace(self.h, int(capacity)))
-        self._trace_cap = int(capacity)
-
-    def trace(self):
-        """(drawn indices per shot as a list of arrays, how many were drawn, generator outputs consumed per shot) of
-        the last run."""
-        S, cap = self._num_shots, self._trace_cap
-        count = np.zeros(S, dtype=np.int32)
-        used = np.zeros(S, dtype=np.int64)
-        idx = np.zeros(S * cap, dtype=np.int32)
-        _lib.check(self.L.osfm_resect_get_trace(self.h, ptr(count), ptr(used), ptr(idx)))
-        idx = idx.reshape(S, cap)
-        return [idx[s, :min(int(count[s]), cap)] for s in range(S)], count, used
+    kind = "resect"
 
     def run(self, bearings: np.ndarray, points: np.ndarray, shot_start: np.ndarray, row_bearing: np.ndarray,
             row_point: np.ndarray, threshold: float, iterations: int = ITERATIONS) -> ShotsResult:
         bearings = np.ascontiguousarray(bearings, dtype=np.float64).reshape(-1, 3)
         points = np.ascontiguousarray(points, dtype=np.float64).reshape(-1, 3)
-        shot_start = np.ascontiguousarray(shot_start, dtype=np.int64)
-        row_bearing = np.ascontiguousarray(row_bearing, dtype=np.int64)
-        row_point = np.ascontiguousarray(row_point, dtype=np.int64)
+        shot_start, row_bearing, row_point = batch_rows(shot_start, row_bearing, row_point,
+                                                        ("shot_start", "row_bearing", "row_point"))
         S = len(shot_start) - 1
-        if S < 0 or shot_start[-1] != len(row_bearing) or len(row_bearing) != len(row_point):
-            raise ValueError("shot_start must end at the number of rows, and row_bearing / row_point must match in "
-                             "length")
         lo = np.zeros((S, 3, 4), dtype=np.float64)
         ransac = np.zeros(S, dtype=np.int32)
         chord = np.zeros(S, dtype=np.int32)
@@ -92,10 +62,8 @@ class Resection:
         _lib.check(self.L.osfm_resect_run(self.h, len(bearings), ptr(bearings), len(points), ptr(points), S,
                                           ptr(shot_start), ptr(row_bearing), ptr(row_point), float(threshold),
                                           int(iterations), ptr(lo), ptr(ransac), ptr(chord), ptr(mask)))
-        self._num_shots = S
-        ms = ctypes.c_float(0)
-        _lib.check(self.L.osfm_resect_last_device_ms(self.h, ctypes.byref(ms)))
-        return ShotsResult(lo, ransac, chord, mask.view(bool), shot_start, float(ms.value))
+        self._num_problems = S
+        return ShotsResult(lo, ransac, chord, mask.view(bool), shot_start, self._device_ms())
 
 
 def ransac_shots(bearings: np.ndarray, points: np.ndarray, shot_start: np.ndarray, row_bearing: np.ndarray,

@@ -4,18 +4,19 @@ bootstrap.  The rules, and the one deliberate difference from pyrobust, are stat
 oracle/rotation_ransac_oracle.py.  There is no CPU path.
 
 The input is one fp64 bearing table and, per row, the bearing of the first and of the second image; pairs own
-consecutive rows (`pair_start`).  `ransac_pairs_lists` builds that from per-pair (b1, b2) arrays.
+consecutive rows (`pair_start`).  `ransac_pairs_lists` builds that from per-pair (b1, b2) arrays
+(`pack_lists`, the shared `ransac.pack_pairs`).
 """
 from __future__ import annotations
 
-import ctypes
 from dataclasses import dataclass
-from typing import List, Optional, Sequence
+from typing import List, Sequence
 
 import numpy as np
 
 from . import _lib
 from ._lib import ptr
+from .ransac import Engine, batch_rows, pack_pairs
 
 ITERATIONS = 1000   # what two_view_reconstruction_rotation_only passes
 
@@ -51,57 +52,26 @@ def reconstructability(common: np.ndarray, rotation_inliers: np.ndarray) -> List
     return np.where(outliers.astype(np.float64) / common >= 0.3, outliers, 0).tolist()
 
 
-class RotationRansac:
-    """osfm_rotransac: one stream, its workspaces and the sample stream kept on the device; a new handle, or `handle`
-    when given."""
+class RotationRansac(Engine):
+    """osfm_rotransac (ransac.Engine): the problems are image pairs."""
 
-    def __init__(self, device: int = 0, handle: Optional[_lib.Handle] = None):
-        self.handle = handle if handle is not None else _lib.Handle("rotransac", device)
-        self.h, self.L, self.device = self.handle.h, self.handle.L, self.handle.device
-        self._trace_cap = 0
-        self._num_pairs = 0
-
-    def set_stream_prefix(self, length: int) -> None:
-        """How many generator outputs the device keeps (a test hook: pairs that use them all continue from the saved
-        generator state)."""
-        _lib.check(self.L.osfm_rotransac_set_stream_prefix(self.h, int(length)))
-
-    def set_trace(self, capacity: int) -> None:
-        """Record up to `capacity` drawn sample indices per pair in the following runs (0: off)."""
-        _lib.check(self.L.osfm_rotransac_set_trace(self.h, int(capacity)))
-        self._trace_cap = int(capacity)
-
-    def trace(self):
-        """(drawn indices per pair as a list of arrays, generator outputs consumed per pair) of the last run."""
-        P, cap = self._num_pairs, self._trace_cap
-        count = np.zeros(P, dtype=np.int32)
-        used = np.zeros(P, dtype=np.int64)
-        idx = np.zeros(P * cap, dtype=np.int32)
-        _lib.check(self.L.osfm_rotransac_get_trace(self.h, ptr(count), ptr(used), ptr(idx)))
-        idx = idx.reshape(P, cap)
-        return [idx[p, :min(int(count[p]), cap)] for p in range(P)], count, used
+    kind = "rotransac"
 
     def run(self, bearings: np.ndarray, pair_start: np.ndarray, row_a: np.ndarray, row_b: np.ndarray,
             threshold: float, iterations: int = ITERATIONS) -> PairsResult:
         bearings = np.ascontiguousarray(bearings, dtype=np.float64).reshape(-1, 3)
-        pair_start = np.ascontiguousarray(pair_start, dtype=np.int64)
-        row_a = np.ascontiguousarray(row_a, dtype=np.int64)
-        row_b = np.ascontiguousarray(row_b, dtype=np.int64)
+        pair_start, row_a, row_b = batch_rows(pair_start, row_a, row_b)
         P = len(pair_start) - 1
-        if P < 0 or pair_start[-1] != len(row_a) or len(row_a) != len(row_b):
-            raise ValueError("pair_start must end at the number of rows, and row_a / row_b must match in length")
         R = len(row_a)
-        lo = np.zeros((max(P, 0), 3, 3), dtype=np.float64)
+        lo = np.zeros((P, 3, 3), dtype=np.float64)
         ransac = np.zeros(P, dtype=np.int32)
         chord = np.zeros(P, dtype=np.int32)
         mask = np.zeros(R, dtype=np.uint8)
         _lib.check(self.L.osfm_rotransac_run(self.h, len(bearings), ptr(bearings), P, ptr(pair_start), ptr(row_a),
                                              ptr(row_b), float(threshold), int(iterations), ptr(lo), ptr(ransac),
                                              ptr(chord), ptr(mask)))
-        self._num_pairs = P
-        ms = ctypes.c_float(0)
-        _lib.check(self.L.osfm_rotransac_last_device_ms(self.h, ctypes.byref(ms)))
-        return PairsResult(lo, ransac, chord, mask.view(bool), pair_start, float(ms.value))
+        self._num_problems = P
+        return PairsResult(lo, ransac, chord, mask.view(bool), pair_start, self._device_ms())
 
 
 def ransac_pairs(bearings: np.ndarray, pair_start: np.ndarray, row_a: np.ndarray, row_b: np.ndarray,
@@ -119,21 +89,7 @@ def last_device_ms() -> float:
     return _last_device_ms
 
 
-def pack_lists(b1s: Sequence[np.ndarray], b2s: Sequence[np.ndarray]):
-    """(bearing table, pair_start, row_a, row_b) of per-pair bearing arrays: pair p's b1 rows, then its b2 rows."""
-    n = np.array([len(b) for b in b1s], dtype=np.int64)
-    if any(len(a) != len(b) for a, b in zip(b1s, b2s)):
-        raise ValueError("every pair needs as many bearings in its second image as in its first")
-    pair_start = np.zeros(len(n) + 1, dtype=np.int64)
-    np.cumsum(n, out=pair_start[1:])
-    if len(n) == 0:
-        return np.zeros((0, 3)), pair_start, np.zeros(0, np.int64), np.zeros(0, np.int64)
-    table = np.concatenate([np.concatenate([np.asarray(a, np.float64).reshape(-1, 3), np.asarray(b, np.float64).reshape(-1, 3)])
-                            for a, b in zip(b1s, b2s)])
-    local = np.arange(pair_start[-1], dtype=np.int64) - np.repeat(pair_start[:-1], n)
-    row_a = np.repeat(2 * pair_start[:-1], n) + local
-    row_b = row_a + np.repeat(n, n)
-    return table, pair_start, row_a, row_b
+pack_lists = pack_pairs   # (bearing table, pair_start, row_a, row_b) of per-pair (b1, b2) arrays
 
 
 def ransac_pairs_lists(b1s: Sequence[np.ndarray], b2s: Sequence[np.ndarray], threshold: float,

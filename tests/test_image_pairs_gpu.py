@@ -23,7 +23,7 @@ from oracle import rotation_ransac_oracle as o
 pytestmark = pytest.mark.gpu
 
 THRESHOLD = 4 * 0.004          # 4 * five_point_algo_threshold, OpenSfM's default
-STAGE_ROWS = 1024              # RR_STAGE_ROWS: larger pairs are read through L2
+STAGE_ROWS = 1024              # RANSAC_STAGE_ROWS: larger pairs are read through L2
 
 
 def oracle_all(b1s, b2s, threshold):

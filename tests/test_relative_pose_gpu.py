@@ -22,7 +22,7 @@ from opensfm_b200 import synthetic as syn
 
 pytestmark = pytest.mark.gpu
 
-STAGE_ROWS = 1024              # RP_STAGE_ROWS: larger pairs are read through L2
+STAGE_ROWS = 1024              # RANSAC_STAGE_ROWS: larger pairs are read through L2
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "relative_pose_oracle.npz")
 
 

@@ -24,7 +24,7 @@ from opensfm_b200 import synthetic as syn
 pytestmark = pytest.mark.gpu
 
 THRESHOLD = C.THRESHOLD
-STAGE_ROWS = 1024              # RS_STAGE_ROWS: larger shots are read through L2
+STAGE_ROWS = 1024              # RANSAC_STAGE_ROWS: larger shots are read through L2
 SCENE_SCALE = 2.0              # cameras on a sphere of radius 2 around the unit cube
 
 
