@@ -634,9 +634,10 @@ int osfm_dense_set_maps(osfm_dense* h, int view, const float* raw_depth, const f
  * 256 x (2 ((OSFM_DENSE_MAX_PATCH - 1) / 2)^2 + 1) f32 indexed by (|dcolor|, dx^2 + dy^2).  The ungated maps (depth,
  * plane 3 per pixel, score, nghbr as the list-local view index) are written per reference in request order, each of
  * its view's size; any may be null.  The reference view's raw slot gets the depth gated by score > (float)min_score
- * and depth < max, and the plane.  An even or too-large patch, an unknown method, a bad depth range, a view out of
- * range or two references of the same view fails with OSFM_ERR_ARG; maps that do not fit in device memory fail with
- * OSFM_ERR_RUNTIME naming the bytes needed. */
+ * and depth < max, and the plane.  An even or too-large patch, patch size 1 with a PatchMatch method (its passes
+ * would read a pixel's neighbours outside the maps), an unknown method, a bad depth range, a view out of range or two
+ * references of the same view fails with OSFM_ERR_ARG, before anything is launched; maps that do not fit in device
+ * memory fail with OSFM_ERR_RUNTIME naming the bytes needed. */
 int osfm_dense_estimate(osfm_dense* h, int num_refs, const int32_t* list_start, const int32_t* views, const double* Q,
                         const double* a, const int32_t* params, const double* depth_range,
                         const float* min_patch_variance, const float* weights, uint32_t seed, double min_score,

@@ -711,6 +711,11 @@ struct Dense : DeviceStream<6> {
                        std::to_string(DN_MAX_PATCH));
       if (patch > v0.w || patch > v0.h)
         throw ArgError(who + ": patch size " + std::to_string(patch) + " exceeds the image size");
+      // PatchMatch reads the predecessors (i -/+ 1, j -/+ 1) of every interior pixel; with no border band those lie
+      // outside the reference's maps (the reference reads them through cv::Mat::at, which is undefined there)
+      if (patch == 1 && R.method != OSFM_DENSE_BRUTE_FORCE)
+        throw ArgError(who + ": patch size 1 leaves PatchMatch no border for a pixel's neighbours; use 3 or more, "
+                             "or BRUTE_FORCE");
       R.hpz = (patch - 1) / 2;
       if (R.iterations < 0) throw ArgError(who + ": negative number of PatchMatch iterations");
       if (!(R.dmin > 0.0) || !(R.dmax > 0.0) || !std::isfinite(R.dmin) || !std::isfinite(R.dmax))

@@ -8,7 +8,8 @@
 // from + - * / sqrt alone, so the engine draws the same variates.  Compiled with -ffp-contract=off.
 //
 // Differences from the reference where its behaviour is undefined: LinearInterpolation returns 0 for NaN
-// coordinates, and the pruner compares the int64 reprojection with the image bounds without narrowing it to int.
+// coordinates, the pruner compares the int64 reprojection with the image bounds without narrowing it to int, and
+// PatchMatch with patch size 1 is refused (its passes would read a pixel's neighbours outside the maps).
 #include <cmath>
 #include <cstdint>
 #include <cstring>
@@ -462,11 +463,13 @@ extern "C" {
 
 // One reference: views 0..n-1 (reference first), images and sizes per view, mask of the reference, K / Q / a per
 // view, K^-1 of the reference.  method 0 brute force, 1 PatchMatch, 2 PatchMatch-sample.  Outputs of the reference's
-// size, zero-initialised by the callee (AssignMatrices).
-void dn_estimate(int n, const int* size, const uint8_t* const* images, const uint8_t* mask, const double* K,
+// size, zero-initialised by the callee (AssignMatrices).  Returns 0, or -1 without touching the outputs for PatchMatch
+// with patch size 1.
+int dn_estimate(int n, const int* size, const uint8_t* const* images, const uint8_t* mask, const double* K,
                  const double* Kinv0, const double* Q, const double* a, int method, int patch, int planes,
                  int iterations, float min_var, double dmin, double dmax, const float* weights, uint32_t seed,
                  uint32_t key, float* depth, float* plane, float* score, int* nghbr) {
+  if (patch == 1 && method != 0) return -1;
   Estimator E;
   E.n = n;
   for (int v = 0; v < n; ++v) {
@@ -502,6 +505,7 @@ void dn_estimate(int n, const int* size, const uint8_t* const* images, const uin
     E.brute_force();
   else
     E.patch_match(method == 2);
+  return 0;
 }
 
 // DepthmapCleaner::Clean of view 0 against views 1..n-1

@@ -36,7 +36,7 @@ def _load():
     global _lib
     if _lib is None:
         L = ctypes.CDLL(build())
-        L.dn_estimate.restype = None
+        L.dn_estimate.restype = c_int
         L.dn_estimate.argtypes = [c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int,
                                   c_int, c_int, c_int, c_float, c_double, c_double, c_void_p, c_uint32, c_uint32,
                                   c_void_p, c_void_p, c_void_p, c_void_p]
@@ -102,9 +102,10 @@ def estimate(Ks, Rs, ts, images, mask, method, patch_size=7, num_depth_planes=50
     keep = _ptr_array(images)
     mask = _c(mask, np.uint8)
     Kinv0 = _c(Kinv[0], np.float64)
-    L.dn_estimate(n, _p(size), keep, _p(mask), _p(K), _p(Kinv0), _p(Q), _p(a), METHODS.get(method, method),
+    if L.dn_estimate(n, _p(size), keep, _p(mask), _p(K), _p(Kinv0), _p(Q), _p(a), METHODS.get(method, method),
                   patch_size, num_depth_planes, iterations, float(np.float32(min_patch_variance)), min_depth,
-                  max_depth, _p(w), seed, key, _p(depth), _p(plane), _p(score), _p(nghbr))
+                  max_depth, _p(w), seed, key, _p(depth), _p(plane), _p(score), _p(nghbr)) != 0:
+        raise ValueError("patch size %d: PatchMatch needs a border around every pixel" % patch_size)
     return depth, plane, score, nghbr
 
 
