@@ -18,7 +18,7 @@
  *
  * There is no CPU fallback: every call needs a CUDA device (H100, sm_90a).
  *
- * Handles (osfm_matcher, osfm_ba, osfm_tracks, osfm_rotransac, osfm_resect, osfm_relpose, osfm_dense) own a CUDA stream and
+ * Handles (osfm_matcher, osfm_ba, osfm_tracks, osfm_rotransac, osfm_resect, osfm_relpose, osfm_dense, osfm_undistort) own a CUDA stream and
  * workspaces on the device they were created on, and every call on a handle makes that device current on the calling thread.  Calls on one handle
  * are serialised and may come from any thread; calls on different handles do not wait for each other.  A callback
  * (today only the all-reduce of osfm_ba_set_distributed) must not call into the handle that called it.
@@ -655,6 +655,59 @@ int osfm_dense_prune(osfm_dense* h, int num_refs, const int32_t* list_start, con
 int osfm_dense_get_pruned(osfm_dense* h, float* points, float* normals, uint8_t* colors, uint8_t* labels);
 /* Device time of the last estimate, clean and prune (CUDA events around their kernels, after the uploads). */
 int osfm_dense_last_device_ms(osfm_dense* h, float* estimate_ms, float* clean_ms, float* prune_ms);
+
+/* ------------------------------------------------------------------------
+ * UNDISTORT
+ * ---------------------------------------------------------------------- */
+typedef struct osfm_undistort osfm_undistort;
+
+/* interpolation, as cv2's flag values (cv2.INTER_AREA is INTER_LINEAR inside cv2.remap) */
+#define OSFM_UNDISTORT_NEAREST 0
+#define OSFM_UNDISTORT_LINEAR 1
+/* border, as cv2's flag values; BORDER_CONSTANT samples 0 outside the image */
+#define OSFM_UNDISTORT_BORDER_CONSTANT 0
+#define OSFM_UNDISTORT_BORDER_WRAP 3
+/* mapping kinds */
+#define OSFM_UNDISTORT_CAMERA 0
+#define OSFM_UNDISTORT_FACE 1
+/* per job: src_width, src_height, channels, bytes_per_sample, interpolation, border, kind, camera projection type,
+ * grid_width, grid_height, out_width, out_height */
+#define OSFM_UNDISTORT_JOB_INTS 12
+/* per job: CAMERA: the source camera's parameters in the reference's order (camera.cc:9-178), the target
+ * perspective camera's focal at [12]; FACE: R_pano R_face^T, 9 row-major */
+#define OSFM_UNDISTORT_PARAMS 16
+
+/* OpenSfM's image undistortion (opensfm/undistort.py:166-232,360-403), restated in oracle/undistort_oracle.py.
+ * A job maps a remap grid onto its source image and samples it with cv2.remap's rules (f32 maps, INTER_NEAREST or
+ * INTER_LINEAR fixed point, BORDER_CONSTANT 0 or BORDER_WRAP), then keeps the grid pixels cv2.resize(INTER_NEAREST)
+ * keeps for the output size (scale_image).  The grid pixel's source coordinate is computed in fp64 and rounded to
+ * f32, as the reference stores its maps:
+ *   CAMERA  ComputeCameraMapping (geometry/src/camera.cc:319-342) from a perspective, brown, fisheye, fisheye_opencv
+ *           or fisheye62 camera to a perspective camera with k1 = k2 = 0; the grid is the source image;
+ *   FACE    a face_size^2 perspective face (focal 0.5) of a panorama image, as render_perspective_view_of_a_panorama.
+ * Images are uint8 or uint16 (bytes_per_sample 1 or 2), 1, 3 or 4 interleaved channels, row-major, each side at most
+ * 32766.  Anything else fails with OSFM_ERR_ARG before anything is launched. */
+int osfm_undistort_create(int device, osfm_undistort** out);
+int osfm_undistort_destroy(osfm_undistort* h);
+/* The f32 maps (width x height each, row-major) of a CAMERA mapping: params as one job's OSFM_UNDISTORT_PARAMS. */
+int osfm_undistort_camera_maps(osfm_undistort* h, int from_type, const double* params, int width, int height,
+                               float* map_x, float* map_y);
+/* The f32 maps (face_size^2 each) of a FACE of a pano_width x pano_height panorama; rotation: 9, row-major. */
+int osfm_undistort_face_maps(osfm_undistort* h, int face_size, const double* rotation, int pano_width,
+                             int pano_height, float* map_x, float* map_y);
+/* cv2.remap(src, map_x, map_y, interpolation, borderMode=border) with caller maps of width x height; dst receives
+ * width x height pixels. */
+int osfm_undistort_remap(osfm_undistort* h, const void* src, int src_width, int src_height, int channels,
+                         int bytes_per_sample, const float* map_x, const float* map_y, int width, int height,
+                         int interpolation, int border, void* dst);
+/* Runs num_jobs jobs (jobs: OSFM_UNDISTORT_JOB_INTS each; params: OSFM_UNDISTORT_PARAMS each) from src[j] into
+ * dst[j] (out_width x out_height pixels).  Jobs pass through page-locked staging, two in flight, so device memory
+ * holds the two largest jobs and not the batch; when that does not fit, fails with OSFM_ERR_RUNTIME naming the bytes
+ * needed. */
+int osfm_undistort_run(osfm_undistort* h, int num_jobs, const int32_t* jobs, const double* params,
+                       const void* const* src, void* const* dst);
+/* The last call's upload, kernel and download time, summed over its jobs (CUDA events). */
+int osfm_undistort_last_device_ms(osfm_undistort* h, float* upload_ms, float* kernel_ms, float* download_ms);
 
 #ifdef __cplusplus
 }

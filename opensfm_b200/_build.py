@@ -13,9 +13,10 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIBDIR = os.path.join(HERE, "lib")
 LIB = os.path.join(LIBDIR, "libopensfm_b200.so")
-SOURCES = ["core.cu", "match.cu", "match_tc.cu", "words.cu", "vlad.cu", "bow.cu", "tracks.cu", "triangulate.cu", "rotransac.cu", "resect.cu", "relpose.cu", "ba.cu", "dense.cu"]
-# per-source flags: dense.cu is checked bit for bit against a host restatement, so no product may become an FMA
-SOURCE_FLAGS = {"dense.cu": ["-fmad=false"]}
+SOURCES = ["core.cu", "match.cu", "match_tc.cu", "words.cu", "vlad.cu", "bow.cu", "tracks.cu", "triangulate.cu", "rotransac.cu", "resect.cu", "relpose.cu", "ba.cu", "dense.cu", "undistort.cu"]
+# per-source flags: dense.cu and undistort.cu are checked bit for bit against host restatements, so no product may
+# become an FMA
+SOURCE_FLAGS = {"dense.cu": ["-fmad=false"], "undistort.cu": ["-fmad=false"]}
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = ARCH + [ "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "-ccbin", "/usr/bin/g++"]

@@ -195,6 +195,14 @@ SIGNATURES = {
     "osfm_dense_prune": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_float, c_void_p]),
     "osfm_dense_get_pruned": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "osfm_dense_last_device_ms": (c_int, [c_void_p, POINTER(c_float), POINTER(c_float), POINTER(c_float)]),
+    "osfm_undistort_create": (c_int, [c_int, POINTER(c_void_p)]),
+    "osfm_undistort_destroy": (c_int, [c_void_p]),
+    "osfm_undistort_camera_maps": (c_int, [c_void_p, c_int, c_void_p, c_int, c_int, c_void_p, c_void_p]),
+    "osfm_undistort_face_maps": (c_int, [c_void_p, c_int, c_void_p, c_int, c_int, c_void_p, c_void_p]),
+    "osfm_undistort_remap": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_int,
+                                     c_int, c_int, c_void_p]),
+    "osfm_undistort_run": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "osfm_undistort_last_device_ms": (c_int, [c_void_p, POINTER(c_float), POINTER(c_float), POINTER(c_float)]),
 }
 
 _lib = None
@@ -232,7 +240,7 @@ def ptr(a: Optional[np.ndarray]) -> Optional[ctypes.c_void_p]:
 
 class Handle:
     """One engine object of the C ABI, `osfm_<kind>_create(device)` .. `osfm_<kind>_destroy`, with kind one of "ba",
-    "matcher", "tracks", "rotransac", "resect", "relpose" and "dense".  It keeps its stream and device workspaces between calls.  The
+    "matcher", "tracks", "rotransac", "resect", "relpose", "dense" and "undistort".  It keeps its stream and device workspaces between calls.  The
     library serialises calls on one handle, so callers that should not wait for one another use handles of their own."""
 
     def __init__(self, kind: str, device: int = 0):
