@@ -588,11 +588,30 @@ int osfm_relpose_two_view(osfm_relpose* h, int64_t num_bearings, const double* b
                           int ransac_iterations, int refine_iterations, int check_reversal, double reversal_ratio,
                           const double* plane_pose, double* lo_model, int32_t* ransac_inliers, double* pose,
                           int32_t* counts, int32_t* chosen, uint8_t* mask_5pt, uint8_t* mask_plane);
-/* Device time of the last osfm_relpose_run or osfm_relpose_two_view (CUDA events around its kernels, after the
- * uploads). */
+/* matching.robust_match_calibrated after its descriptor matches, for many pairs in one call: the RANSAC of
+ * osfm_relpose_run (same inputs, same threshold angle, ransac_iterations as its iterations), then on the device, per
+ * pair, from its lo_model and the pose B = [R^T | -R^T t] of it: for relax = 4, 2, 1, the bearing inliers of B at
+ * relax * threshold (compute_inliers_bearings; threshold is then a chord bound), and, when there are at least 8,
+ * the TinySolver refinement of RelativePoseRefinement on them (refine_iterations = max_num_iterations, what
+ * five_point_refine_match_iterations sets) replacing B; a round with fewer than 8 inliers ends the pair empty.  A
+ * last pass takes the inliers of B at threshold.  The rules are stated in oracle/robust_match_oracle.py.
+ * Outputs: lo_model and ransac_inliers as osfm_relpose_run; pose (12 per pair: the refined B row-major, in
+ * compute_inliers_bearings' convention, NaN for a pair that ends empty); counts (4 per pair: the inliers of the 4x,
+ * 2x and 1x rounds and of the last pass, -1 for a pass not run; the first round below 8 says where a pair emptied);
+ * mask (per row: the last pass's inliers, none for an empty pair).  A pair of fewer than 8 rows,
+ * refine_iterations < 1, null outputs, or the other conditions of osfm_relpose_run fail with OSFM_ERR_ARG, naming
+ * the pair where there is one. */
+int osfm_relpose_robust_match(osfm_relpose* h, int64_t num_bearings, const double* bearings, int64_t num_pairs,
+                              const int64_t* pair_start, const int64_t* row_a, const int64_t* row_b,
+                              double threshold, int ransac_iterations, int refine_iterations, double* lo_model,
+                              int32_t* ransac_inliers, double* pose, int32_t* counts, uint8_t* mask);
+/* Device time of the last osfm_relpose_run, osfm_relpose_two_view or osfm_relpose_robust_match (CUDA events around
+ * its kernels, after the uploads). */
 int osfm_relpose_last_device_ms(osfm_relpose* h, float* ms);
-/* The same split into the RANSAC kernels and the two-view kernel (0 when the last call was osfm_relpose_run). */
-int osfm_relpose_last_stage_ms(osfm_relpose* h, float* ransac_ms, float* two_view_ms);
+/* The same split into the RANSAC kernels and the kernel of the stage after them: the two-view kernel of
+ * osfm_relpose_two_view or the match filter of osfm_relpose_robust_match (0 when the last call was
+ * osfm_relpose_run). */
+int osfm_relpose_last_stage_ms(osfm_relpose* h, float* ransac_ms, float* stage_ms);
 /* Test hooks, as osfm_rotransac_set_stream_prefix / set_trace / get_trace, per pair. */
 int osfm_relpose_set_stream_prefix(osfm_relpose* h, int64_t length);
 int osfm_relpose_set_trace(osfm_relpose* h, int capacity);

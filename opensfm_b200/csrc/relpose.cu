@@ -447,6 +447,79 @@ __global__ void __launch_bounds__(RANSAC_THREADS) rp_two_view(TvArgs a, int stag
   }
 }
 
+// ---------------------------------------------------------------------------------------------------------------
+// rp_match_filter: robust_match_calibrated after its RANSAC, per pair, from rp_ransac's lo_model
+// ---------------------------------------------------------------------------------------------------------------
+constexpr int RM_ROUNDS = 3;               // the bearing inliers at 4, 2 and 1 times the threshold, each refined
+constexpr int RM_MIN_INLIERS = 8;          // a round with fewer inliers empties the pair
+
+struct RmArgs {
+  const double* bearings;
+  const long long* pair_start;
+  const long long* row_a;
+  const long long* row_b;
+  const int* order;
+  const double* lo_model;        // rp_ransac's, 12 per pair
+  double threshold;              // chord
+  int refine_iterations;
+  int* lists;                    // per row: the current round's inlier rows, ascending
+  double* pose;                  // 12 per pair: the refined [R | t], NaN when the pair ends empty
+  int* counts;                   // 4 per pair: inliers of each round, then of the final pass; -1 for a pass not run
+  unsigned char* mask;           // per row: the final inliers
+};
+
+__global__ void __launch_bounds__(RANSAC_THREADS) rp_match_filter(RmArgs a, int staged) {
+  __shared__ int warp_n[RANSAC_WARPS];
+  __shared__ double B[12];
+  __shared__ int final_count;
+  const int pair = a.order[blockIdx.x];
+  const long long off = a.pair_start[pair];
+  const RansacRows rows =
+      ransac_rows(a.bearings, a.bearings, a.row_a + off, a.row_b + off, (int)(a.pair_start[pair + 1] - off), staged);
+  const int n = rows.n;
+  if (threadIdx.x == 0) {
+    // multiview.relative_pose_ransac's [R^T | -R^T t] of lo_model = [R | t]
+    const double* L = a.lo_model + 12LL * pair;
+    for (int i = 0; i < 3; ++i) {
+      for (int j = 0; j < 3; ++j) B[i * 4 + j] = L[j * 4 + i];
+      B[i * 4 + 3] = -(L[i] * L[3] + L[4 + i] * L[7] + L[8 + i] * L[11]);
+    }
+  }
+  __syncthreads();
+  int* list = a.lists + off;
+  int* counts = a.counts + 4LL * pair;
+  // matching.py's relax loop; every thread gets the same count, so the CTA leaves the loop together
+  bool empty = false;
+  int round = 0;
+  for (; round < RM_ROUNDS && !empty; ++round) {
+    const int m = ransac_compact<12>(rows, B, TvBearingTest{(double)(4 >> round) * a.threshold}, warp_n, list);
+    if (threadIdx.x == 0) counts[round] = m;
+    empty = m < RM_MIN_INLIERS;
+    if (!empty) {
+      if (threadIdx.x < 32) tv_refine(rows, list, m, a.refine_iterations, B);
+      __syncthreads();
+    }
+  }
+  const TvBearingTest test{a.threshold};
+  int c[1] = {0};
+  for (int i = threadIdx.x; i < n; i += RANSAC_THREADS) {
+    bool in = false;
+    if (!empty) {
+      double x[3], y[3];
+      rows.get(i, x, y);
+      in = test(B, x, y);
+    }
+    a.mask[off + i] = in ? 1 : 0;
+    c[0] += in ? 1 : 0;
+  }
+  if (!empty) ransac_sums(c, 1, warp_n, &final_count);
+  if (threadIdx.x == 0) {
+    for (int k = 0; k < 12; ++k) a.pose[12LL * pair + k] = empty ? CUDART_NAN : B[k];
+    for (int r = round; r < RM_ROUNDS; ++r) counts[r] = -1;
+    counts[RM_ROUNDS] = empty ? -1 : final_count;
+  }
+}
+
 // the first `count` outputs of glibc's rand() after srand(seed) (random_r's TYPE_3 additive generator)
 void glibc_rand(unsigned seed, int count, std::vector<int>& out) {
   std::vector<int32_t> r(344 + (size_t)count);
@@ -470,8 +543,8 @@ struct RelPose : DeviceStream<3> {
   DevBuf<int> d_ransac;
   DevBuf<unsigned char> d_mask;
 
-  // the two-view stage
-  bool two_view_timed = false;
+  // the stage after RANSAC: two-view or match filter
+  bool stage_timed = false;
   DevBuf<double> d_plane, d_tv_pose;
   DevBuf<int> d_tv_lists, d_tv_counts, d_tv_chosen;
   DevBuf<unsigned char> d_mask_plane;
@@ -487,13 +560,29 @@ struct RelPose : DeviceStream<3> {
                 int refine_iterations, int check_reversal, double reversal_ratio, const double* plane_pose,
                 double* lo_model, int32_t* ransac_inliers, double* pose, int32_t* counts, int32_t* chosen,
                 uint8_t* mask_5pt, uint8_t* mask_plane);
+  void robust_match(int64_t num_bearings, const double* bearings, int64_t num_pairs, const int64_t* pair_start,
+                    const int64_t* row_a, const int64_t* row_b, double threshold, int ransac_iterations,
+                    int refine_iterations, double* lo_model, int32_t* ransac_inliers, double* pose, int32_t* counts,
+                    uint8_t* mask);
 
  private:
   void check(int64_t num_bearings, const double* bearings, int64_t num_pairs, const int64_t* pair_start,
-             const int64_t* row_a, const int64_t* row_b, double threshold, int iterations) {
-    two_view_timed = false;
-    batch.check("relative pose", "pair", "rows", RP_MIN_SAMPLE, num_pairs, pair_start, threshold, iterations,
+             const int64_t* row_a, const int64_t* row_b, double threshold, int iterations,
+             int min_rows = RP_MIN_SAMPLE) {
+    stage_timed = false;
+    batch.check("relative pose", "pair", "rows", min_rows, num_pairs, pair_start, threshold, iterations,
                 {{row_a, bearings, num_bearings, "bearing"}, {row_b, bearings, num_bearings, "bearing"}}, true);
+  }
+  // RelativePoseCost's row picks (tv_pick_fraction), uploaded once per handle before the first refinement
+  void upload_pick_fractions() {
+    if (fractions_ready) return;
+    std::vector<int> r;
+    glibc_rand(42, relpose::REFINE_PICKED, r);
+    float frac[relpose::REFINE_PICKED];
+    for (int k = 0; k < relpose::REFINE_PICKED; ++k) frac[k] = (float)r[k] / (float)RAND_MAX;
+    OSFM_CUDA(cudaMemcpyToSymbolAsync(tv_pick_fraction, frac, sizeof(frac), 0, cudaMemcpyHostToDevice, stream));
+    OSFM_CUDA(cudaStreamSynchronize(stream));
+    fractions_ready = true;
   }
   // the launches of one RANSAC call (after the argument checks), up to ev[1]; the batch's plan serves the stage
   // after it
@@ -561,15 +650,7 @@ void RelPose::two_view(int64_t num_bearings, const double* bearings, int64_t num
                         !mask_plane))
     throw ArgError("two-view: null arrays");
   if (num_pairs == 0) return;
-  if (!fractions_ready) {
-    std::vector<int> r;
-    glibc_rand(42, relpose::REFINE_PICKED, r);
-    float frac[relpose::REFINE_PICKED];
-    for (int k = 0; k < relpose::REFINE_PICKED; ++k) frac[k] = (float)r[k] / (float)RAND_MAX;
-    OSFM_CUDA(cudaMemcpyToSymbolAsync(tv_pick_fraction, frac, sizeof(frac), 0, cudaMemcpyHostToDevice, stream));
-    OSFM_CUDA(cudaStreamSynchronize(stream));
-    fractions_ready = true;
-  }
+  upload_pick_fractions();
   const int64_t R = pair_start[num_pairs];
   upload(d_plane, plane_pose, (size_t)num_pairs * 12);
   d_tv_lists.reserve((size_t)R * 2);
@@ -607,7 +688,47 @@ void RelPose::two_view(int64_t num_bearings, const double* bearings, int64_t num
   download(mask_plane, d_mask_plane.p, (size_t)R);
   OSFM_CUDA(cudaStreamSynchronize(stream));
   batch.done = num_pairs;
-  two_view_timed = true;
+  stage_timed = true;
+}
+
+void RelPose::robust_match(int64_t num_bearings, const double* bearings, int64_t num_pairs,
+                           const int64_t* pair_start, const int64_t* row_a, const int64_t* row_b, double threshold,
+                           int ransac_iterations, int refine_iterations, double* lo_model, int32_t* ransac_inliers,
+                           double* pose, int32_t* counts, uint8_t* mask) {
+  check(num_bearings, bearings, num_pairs, pair_start, row_a, row_b, threshold, ransac_iterations, RM_MIN_INLIERS);
+  if (refine_iterations < 1) throw ArgError("robust match: refine_iterations must be at least 1");
+  if (num_pairs > 0 && (!lo_model || !ransac_inliers || !pose || !counts || !mask))
+    throw ArgError("robust match: null arrays");
+  if (num_pairs == 0) return;
+  upload_pick_fractions();
+  const int64_t R = pair_start[num_pairs];
+  d_tv_lists.reserve((size_t)R);
+  d_tv_pose.reserve((size_t)num_pairs * 12);
+  d_tv_counts.reserve((size_t)num_pairs * 4);
+  launch_ransac(num_bearings, bearings, num_pairs, pair_start, row_a, row_b, threshold, ransac_iterations);
+
+  RmArgs a;
+  a.bearings = d_bearings.p;
+  a.pair_start = batch.d_start.p;
+  a.row_a = batch.d_rows[0].p;
+  a.row_b = batch.d_rows[1].p;
+  a.lo_model = d_lo.p;
+  a.threshold = threshold;
+  a.refine_iterations = refine_iterations;
+  a.lists = d_tv_lists.p;
+  a.pose = d_tv_pose.p;
+  a.counts = d_tv_counts.p;
+  a.mask = d_mask.p;              // rp_ransac's mask is not returned by this call
+  batch.launch(rp_match_filter, a, stream);
+  OSFM_CUDA(cudaEventRecord(ev[2], stream));
+  download(lo_model, d_lo.p, (size_t)num_pairs * 12);
+  download(ransac_inliers, d_ransac.p, (size_t)num_pairs);
+  download(pose, d_tv_pose.p, (size_t)num_pairs * 12);
+  download(counts, d_tv_counts.p, (size_t)num_pairs * 4);
+  download(mask, d_mask.p, (size_t)R);
+  OSFM_CUDA(cudaStreamSynchronize(stream));
+  batch.done = num_pairs;
+  stage_timed = true;
 }
 
 }  // namespace
@@ -644,12 +765,22 @@ int osfm_relpose_two_view(osfm_relpose* h, int64_t num_bearings, const double* b
   });
 }
 
-int osfm_relpose_last_stage_ms(osfm_relpose* h, float* ransac_ms, float* two_view_ms) {
+int osfm_relpose_robust_match(osfm_relpose* h, int64_t num_bearings, const double* bearings, int64_t num_pairs,
+                              const int64_t* pair_start, const int64_t* row_a, const int64_t* row_b,
+                              double threshold, int ransac_iterations, int refine_iterations, double* lo_model,
+                              int32_t* ransac_inliers, double* pose, int32_t* counts, uint8_t* mask) {
   return osfm::with_handle(h, [&](osfm::RelPose& K) {
-    if (!ransac_ms || !two_view_ms) throw osfm::ArgError("null ms");
-    *ransac_ms = *two_view_ms = 0.f;
+    K.robust_match(num_bearings, bearings, num_pairs, pair_start, row_a, row_b, threshold, ransac_iterations,
+                   refine_iterations, lo_model, ransac_inliers, pose, counts, mask);
+  });
+}
+
+int osfm_relpose_last_stage_ms(osfm_relpose* h, float* ransac_ms, float* stage_ms) {
+  return osfm::with_handle(h, [&](osfm::RelPose& K) {
+    if (!ransac_ms || !stage_ms) throw osfm::ArgError("null ms");
+    *ransac_ms = *stage_ms = 0.f;
     if (K.batch.done) OSFM_CUDA(cudaEventElapsedTime(ransac_ms, K.ev[0], K.ev[1]));
-    if (K.two_view_timed) OSFM_CUDA(cudaEventElapsedTime(two_view_ms, K.ev[1], K.ev[2]));
+    if (K.stage_timed) OSFM_CUDA(cudaEventElapsedTime(stage_ms, K.ev[1], K.ev[2]));
   });
 }
 
@@ -670,7 +801,7 @@ int osfm_relpose_last_device_ms(osfm_relpose* h, float* ms) {
   return osfm::with_handle(h, [&](osfm::RelPose& K) {
     if (!ms) throw osfm::ArgError("null ms");
     *ms = 0.f;
-    if (K.batch.done) OSFM_CUDA(cudaEventElapsedTime(ms, K.ev[0], K.ev[K.two_view_timed ? 2 : 1]));
+    if (K.batch.done) OSFM_CUDA(cudaEventElapsedTime(ms, K.ev[0], K.ev[K.stage_timed ? 2 : 1]));
   });
 }
 

@@ -3,6 +3,7 @@
     match_brute_force(f1, f2, config, maskij=None)            opensfm/matching.py:723-756
     match_brute_force_symmetric(fi, fj, config, maskij=None)  opensfm/matching.py:759-777
     match_images_with_pairs-style batch: `PairMatcher`        opensfm/matching.py:63-98
+    robust_match, robust_match_calibrated                     opensfm/matching.py:871-929
 
 Same argument meaning, same return types (lists of (queryIdx, trainIdx) tuples),
 same dtype dispatch (uint8 -> Hamming, else L2, matching.py:738-742).  All
@@ -472,10 +473,97 @@ def unfilter_matches(matches: np.ndarray, m1: np.ndarray, m2: np.ndarray) -> np.
     return np.stack([i1[matches[:, 0]], i2[matches[:, 1]]], axis=1) if len(matches) else np.zeros((0, 2), dtype=np.int64)
 
 
+ROBUST_MIN_MATCHES = 8   # robust_match_fundamental / robust_match_calibrated return nothing below this
+
+
+def robust_match_fundamental(p1: np.ndarray, p2: np.ndarray, matches: np.ndarray, config: Dict[str, Any]):
+    """matching.robust_match_fundamental (matching.py:780-802): (F, inlier matches) of cv2.findFundamentalMat with
+    FM_RANSAC, robust_matching_threshold and confidence 0.9999, on the host as the reference runs it."""
+    import cv2
+
+    matches = np.asarray(matches)
+    if len(matches) < ROBUST_MIN_MATCHES:
+        return np.array([]), np.array([])
+    q1 = p1[matches[:, 0]][:, :2].copy()
+    q2 = p2[matches[:, 1]][:, :2].copy()
+    F, mask = cv2.findFundamentalMat(q1, q2, cv2.FM_RANSAC, config["robust_matching_threshold"], 0.9999)
+    if F is None or F[2, 2] == 0.0:
+        return F, np.array([])
+    return F, matches[mask.ravel().nonzero()]
+
+
+def robust_match_calibrated(p1: np.ndarray, p2: np.ndarray, camera1, camera2, matches: np.ndarray,
+                            config: Dict[str, Any]) -> np.ndarray:
+    """matching.robust_match_calibrated (matching.py:871-903) on the GPU: five-point RANSAC of the matches' bearings
+    (camera.pixel_bearing_many), then the bearing inliers at 4, 2 and 1 times robust_matching_calib_threshold, each
+    refined with five_point_refine_match_iterations; returns the matches the refined pose keeps."""
+    from . import relative_pose
+
+    matches = np.asarray(matches)
+    if len(matches) < ROBUST_MIN_MATCHES:
+        return np.array([])
+    b1 = camera1.pixel_bearing_many(p1[matches[:, 0]][:, :2].copy())
+    b2 = camera2.pixel_bearing_many(p2[matches[:, 1]][:, :2].copy())
+    res = relative_pose.robust_match_lists([b1], [b2], config["robust_matching_calib_threshold"],
+                                           relative_pose.ITERATIONS, config["five_point_refine_match_iterations"])
+    return matches[res.mask(0)]
+
+
+def uses_fundamental(camera1, camera2) -> bool:
+    """robust_match's dispatch: both cameras perspective or brown with k1 = k2 = 0 (matching.py:919-926)."""
+    return all(c.projection_type in ["perspective", "brown"] and c.k1 == 0.0 and c.k2 == 0.0
+               for c in (camera1, camera2))
+
+
+def robust_match(p1: np.ndarray, p2: np.ndarray, camera1, camera2, matches: np.ndarray,
+                 config: Dict[str, Any]) -> np.ndarray:
+    """matching.robust_match (matching.py:906-929): the fundamental matrix for undistorted perspective cameras, the
+    essential matrix on the GPU for every other camera."""
+    if uses_fundamental(camera1, camera2):
+        return robust_match_fundamental(p1, p2, matches, config)[1]
+    return robust_match_calibrated(p1, p2, camera1, camera2, matches, config)
+
+
+def _verify_pairs(ms: Dict[Tuple[Any, Any], np.ndarray], verify: Dict[str, Any], config: Dict[str, Any],
+                  device: int) -> Dict[Tuple[Any, Any], np.ndarray]:
+    """robust_match of every pair in `ms` (its descriptor matches): the calibrated pairs in one device call over one
+    bearing table (each image's points' bearings computed once), the others through robust_match_fundamental."""
+    from . import relative_pose
+
+    cameras, points = verify["cameras"], verify["points"]
+    out: Dict[Tuple[Any, Any], np.ndarray] = {}
+    calibrated = []
+    for p, m in ms.items():
+        if uses_fundamental(cameras[p[0]], cameras[p[1]]):
+            out[p] = robust_match_fundamental(points[p[0]], points[p[1]], m, config)[1]
+        elif len(m) < ROBUST_MIN_MATCHES:
+            out[p] = np.array([])
+        else:
+            calibrated.append(p)
+    if not calibrated:
+        return out
+    images = list(dict.fromkeys(i for p in calibrated for i in p))
+    base, tables, n = {}, [], 0
+    for im in images:
+        base[im] = n
+        tables.append(cameras[im].pixel_bearing_many(np.asarray(points[im])[:, :2].copy()))
+        n += len(tables[-1])
+    starts = np.concatenate([[0], np.cumsum([len(ms[p]) for p in calibrated])]).astype(np.int64)
+    row_a = np.concatenate([base[p[0]] + ms[p][:, 0] for p in calibrated]).astype(np.int64)
+    row_b = np.concatenate([base[p[1]] + ms[p][:, 1] for p in calibrated]).astype(np.int64)
+    res = relative_pose.robust_match_pairs(np.concatenate(tables), starts, row_a, row_b,
+                                           config["robust_matching_calib_threshold"], relative_pose.ITERATIONS,
+                                           config["five_point_refine_match_iterations"], device)
+    for k, p in enumerate(calibrated):
+        out[p] = ms[p][res.mask(k)]
+    return out
+
+
 def match_images_with_pairs(descriptors: Dict[Any, np.ndarray], pairs: Sequence[Tuple[Any, Any]], config: Dict[str, Any],
                             robust_filter=None, feature_masks: Optional[Dict[Any, np.ndarray]] = None,
                             guided: Optional[Dict[str, Any]] = None, device: int = 0, rank: int = 0, world: int = 1,
-                            uint8_is_l2: bool = False) -> Dict[Tuple[Any, Any], np.ndarray]:
+                            uint8_is_l2: bool = False,
+                            verify: Optional[Dict[str, Any]] = None) -> Dict[Tuple[Any, Any], np.ndarray]:
     """The pair loop of `matching.match_images_with_pairs` / `matching.match` (matching.py:63-98, 563-634) as one
     batched submission: every image's descriptors are uploaded once, the pair list (this rank's shard of it) is
     matched in one launch sequence, then per pair the reference's post-processing runs on the host:
@@ -488,8 +576,13 @@ def match_images_with_pairs(descriptors: Dict[Any, np.ndarray], pairs: Sequence[
     descriptors: image -> the (masked) descriptor matrix `feature_loader.load_all_data(masked=True)` returns.
     guided: None, or {"bearings": image -> n x 3, "poses": (im1, im2) -> (R, t), "threshold": rad}: pairs with a
     pose are matched under the epipolar mask (`_match_descriptors_guided_impl`), always symmetric.
+    verify: None, or {"cameras": image -> camera, "points": image -> the (masked) feature points}: the reference's
+    own geometric verification, `robust_match`, of every pair past the first gate instead of `robust_filter`; the
+    calibrated pairs are verified in one device call (`robust_match_calibrated` for all of them at once).
     Returns {(im1, im2): int array [K, 2]} for this rank's pairs; `opensfm_b200.dist.gather_pair_results` merges
     the ranks."""
+    if robust_filter is not None and verify is not None:
+        raise ValueError("pass robust_filter or verify, not both")
     sizes = {k: len(v) for k, v in descriptors.items()}
     mine = shard_pairs(list(pairs), sizes, world)[rank] if world > 1 else list(pairs)
     pm = PairMatcher(device=device)
@@ -507,6 +600,9 @@ def match_images_with_pairs(descriptors: Dict[Any, np.ndarray], pairs: Sequence[
     min_match = int(config.get("robust_matching_min_match", 20))
     out: Dict[Tuple[Any, Any], np.ndarray] = {}
     empty = np.zeros((0, 2), dtype=np.int64)
+    verified: Dict[Tuple[Any, Any], np.ndarray] = {}
+    if verify is not None:
+        verified = _verify_pairs({p: raw[p] for p in mine if len(raw[p]) >= min_match}, verify, config, device)
     for p in mine:
         m = raw[p]
         if len(m) < min_match:
@@ -514,6 +610,8 @@ def match_images_with_pairs(descriptors: Dict[Any, np.ndarray], pairs: Sequence[
             continue
         if robust_filter is not None:
             m = np.asarray(robust_filter(p[0], p[1], m), dtype=np.int64).reshape(-1, 2)
+        if verify is not None:
+            m = np.asarray(verified[p], dtype=np.int64).reshape(-1, 2)
         if feature_masks is not None and feature_masks.get(p[0]) is not None and feature_masks.get(p[1]) is not None:
             m = unfilter_matches(m, feature_masks[p[0]], feature_masks[p[1]])
         out[p] = empty if len(m) < min_match else m

@@ -5,7 +5,8 @@ the deliberate differences from pyrobust, are stated in oracle/relative_pose_ora
 The input is one bearing table and, per row, the index of the first image's bearing and of the second image's;
 pairs own consecutive rows (`pair_start`).  `ransac_lists` builds that from per-pair (b1, b2) arrays
 (`pack_lists`, the shared `ransac.pack_pairs`), and
-`relative_pose_ransac` is the drop-in of `opensfm.multiview.relative_pose_ransac` for one pair.
+`relative_pose_ransac` is the drop-in of `opensfm.multiview.relative_pose_ransac` for one pair.  `robust_match_pairs`
+and `robust_match_lists` run the geometric verification of `matching.robust_match_calibrated` on the same batches.
 """
 from __future__ import annotations
 
@@ -251,5 +252,67 @@ def two_view_lists(b1_list: Sequence[np.ndarray], b2_list: Sequence[np.ndarray],
 
 
 def last_stage_ms():
-    """(RANSAC kernels, two-view kernel) device time of the last two_view_pairs / two_view_lists call."""
+    """(RANSAC kernels, two-view kernel or match filter) device time of the last two_view_pairs / two_view_lists /
+    robust_match_pairs / robust_match_lists call."""
     return _last_stage_ms
+
+
+# ---------------------------------------------------------------------------------------------------------------
+# robust_match_calibrated after the RANSAC: bearing inliers at 4, 2 and 1 times the threshold, each refined
+# ---------------------------------------------------------------------------------------------------------------
+MATCH_REFINE_ITERATIONS = 10   # five_point_refine_match_iterations
+MATCH_MIN_INLIERS = 8          # a relax round with fewer inliers empties the pair
+
+
+@dataclass
+class RobustMatchResult:
+    lo_model: np.ndarray          # (P, 3, 4) as PairsResult.lo_model
+    ransac_inliers: np.ndarray    # (P,) int32
+    pose: np.ndarray              # (P, 3, 4): the refined [R | t], second image to first; NaN for an empty pair
+    counts: np.ndarray            # (P, 4) int32: inliers of the 4x, 2x and 1x rounds, then of the final pass; -1: not run
+    inlier_mask: np.ndarray       # (R,) bool: the final inliers
+    pair_start: np.ndarray
+    ransac_ms: float
+    filter_ms: float
+
+    def mask(self, p: int) -> np.ndarray:
+        """Final inlier mask of pair p's rows (all False when the pair ended empty)."""
+        return self.inlier_mask[self.pair_start[p]:self.pair_start[p + 1]]
+
+    def empty_round(self, p: int) -> Optional[int]:
+        """The relax round (0: 4x, 1: 2x, 2: 1x) whose fewer than 8 inliers emptied pair p, None if none did."""
+        low = np.flatnonzero((self.counts[p, :3] >= 0) & (self.counts[p, :3] < MATCH_MIN_INLIERS))
+        return int(low[0]) if len(low) else None
+
+
+def robust_match_pairs(bearings: np.ndarray, pair_start: np.ndarray, row_a: np.ndarray, row_b: np.ndarray,
+                       threshold: float, ransac_iterations: int = ITERATIONS,
+                       refine_iterations: int = MATCH_REFINE_ITERATIONS, device: int = 0) -> RobustMatchResult:
+    """robust_match_calibrated's verification of every pair (rows index one bearing table, as ransac_pairs), RANSAC
+    and the relax rounds in one device call: `threshold` (robust_matching_calib_threshold) is RANSAC's angle and the
+    rounds' chord bound.  Every pair needs at least 8 rows."""
+    global _last_device_ms, _last_stage_ms
+    bearings = np.ascontiguousarray(bearings, dtype=np.float64).reshape(-1, 3)
+    pair_start, row_a, row_b = batch_rows(pair_start, row_a, row_b)
+    P = len(pair_start) - 1
+    lo = np.zeros((P, 3, 4))
+    ransac = np.zeros(P, dtype=np.int32)
+    pose = np.zeros((P, 3, 4))
+    counts = np.zeros((P, 4), dtype=np.int32)
+    mask = np.zeros(len(row_a), dtype=np.uint8)
+    with _lib.pooled("relpose", device) as h:
+        _lib.check(h.L.osfm_relpose_robust_match(
+            h.h, len(bearings), ptr(bearings), P, ptr(pair_start), ptr(row_a), ptr(row_b), float(threshold),
+            int(ransac_iterations), int(refine_iterations), ptr(lo), ptr(ransac), ptr(pose), ptr(counts), ptr(mask)))
+        a_ms, b_ms, total = ctypes.c_float(0), ctypes.c_float(0), ctypes.c_float(0)
+        _lib.check(h.L.osfm_relpose_last_stage_ms(h.h, ctypes.byref(a_ms), ctypes.byref(b_ms)))
+        _lib.check(h.L.osfm_relpose_last_device_ms(h.h, ctypes.byref(total)))
+    _last_device_ms = float(total.value)
+    _last_stage_ms = (float(a_ms.value), float(b_ms.value))
+    return RobustMatchResult(lo, ransac, pose, counts, mask.view(bool), pair_start, *_last_stage_ms)
+
+
+def robust_match_lists(b1_list: Sequence[np.ndarray], b2_list: Sequence[np.ndarray], threshold: float,
+                       ransac_iterations: int = ITERATIONS, refine_iterations: int = MATCH_REFINE_ITERATIONS,
+                       device: int = 0) -> RobustMatchResult:
+    return robust_match_pairs(*pack_lists(b1_list, b2_list), threshold, ransac_iterations, refine_iterations, device)
